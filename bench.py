@@ -53,6 +53,8 @@ def parse_args():
     ap.add_argument("--plaid-ndocs", type=int, default=1024, help="ndocs of the PLAID leg (reference default 1024)")
     ap.add_argument("--no-c2", action="store_true", help="skip the C2-shaped (112k ragged passages, Nq=832, k=100) record")
     ap.add_argument("--c2-passages", type=int, default=112_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's top-k scores and pids as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -67,16 +69,6 @@ def workload_config(args, world):
                   % (args.passages * args.nd * 256 / world / 1e9)}
 
 
-def kernel_source_sha():
-    """Hash of the scan kernel's sources: the committed ncu traffic figure is only reported while it matches."""
-    import hashlib
-    h = hashlib.sha256()
-    for fn in ("flmr_scan_kernel.cuh", "flmr_device.cuh"):
-        with open(os.path.join(ROOT, "retrieval-augmented-visual-question-answering_b200", "csrc", fn), "rb") as f:
-            h.update(f.read())
-    return h.hexdigest()[:16]
-
-
 def load_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
@@ -84,53 +76,17 @@ def load_peaks():
             p = json.load(f)
         return {"hbm_gbs": float(p["hbm_gbs"]), "bf16_burst": float(p["bf16_tflops"]),
                 "bf16_sustained": float(p.get("bf16_tflops_sustained", p["bf16_tflops"])), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_burst": 1590.0, "bf16_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 — an upper bound, not a measurement
+    return {"hbm_gbs": 3350.0, "bf16_burst": 989.0, "bf16_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 # --------------------------------------------------------------------------------------------------
 # reference CPU leg (oracle/_ref when the reference's segmented_maxsim.cpp was compiled, else the
 # oracle port).  TEST/BASELINE INFRASTRUCTURE: never on the product path.
 # --------------------------------------------------------------------------------------------------
-def _reference_packed_scorer():
-    """The reference's OWN ``colbert_score_packed`` (colbert.py:289-311) imported from /root/reference behind the
-    import shims of SURVEY.md Appendix A — build container only; the GPU box has no reference checkout."""
-    ref = "/root/reference/third_party/ColBERT"
-    if not os.path.isdir(ref):
-        return None
-    try:
-        import dataclasses
-        import torch
-        import transformers
-        sys.modules.setdefault("ujson", json)
-        _orig = dataclasses.dataclass
-
-        def _patched(cls=None, /, **kw):
-            def wrap(c):
-                c = _orig(c, **kw)
-                if c.__name__ == "DefaultVal":
-                    c.__hash__ = object.__hash__
-                return c
-            return wrap if cls is None else wrap(cls)
-        dataclasses.dataclass = _patched
-        if not hasattr(transformers, "AdamW"):
-            transformers.AdamW = torch.optim.AdamW
-        sys.path.insert(0, ref)
-        os.environ.setdefault("TORCH_EXTENSIONS_DIR", "/tmp/flmr_ref_torch_ext")
-        from colbert.infra.config import ColBERTConfig
-        from colbert.modeling.colbert import ColBERT, colbert_score_packed
-        ColBERT.try_load_torch_extensions(False)
-        cfg = ColBERTConfig(total_visible_gpus=0)
-        return lambda Q, D, doclens: colbert_score_packed(Q.unsqueeze(0), D, doclens, config=cfg)
-    except Exception:
-        return None
-
-
 def make_cpu_scorer():
     """Returns (kind, fn(Q [nq,d] fp32 torch, D [T,d] fp32 torch, doclens int64 torch) -> scores [n])."""
     import torch
-    fn = _reference_packed_scorer()
-    if fn is not None:
-        return "reference (colbert_score_packed imported from the reference checkout)", fn
     sys.path.insert(0, os.path.join(ROOT, "oracle"))
     try:
         import build_ref
@@ -499,6 +455,11 @@ def run_ours(args):
     # device-resident timing (value) with per-launch scan-kernel events for the roofline
     r_dev = timed(step_device, args.steps, args.warmup, profile=True)
     ms_per_step = r_dev["dev_ms"] / args.steps
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed path received in its last step: [batch, k] scores and global passage ids
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "topk_scores.npy"), r_dev["out"][0].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "topk_pids.npy"), r_dev["out"][1].cpu().numpy().astype(np.float64))
     value = B * 1e3 / ms_per_step
     # end-to-end through the reference-facing API with host buffers (wall clock spans H2D/D2H/lists)
     r_e2e = timed(step_e2e, args.steps, min(args.warmup, 2))
@@ -550,7 +511,7 @@ def run_ours(args):
             gbs = n_tok * 256.0 / (ms * 1e-3) / 1e9
             hbm_regime = {"workload": "1 query x Nq=32 per corpus pass (HBM-bound regime of the same kernel)",
                           "launch_ms": ms, "achieved": gbs, "unit": "GB/s", "queries_per_s": 1e3 / ms,
-                          "peak": peaks["hbm_gbs"], "frac": gbs / peaks["hbm_gbs"], "frac_of_8TBs": gbs / 8000.0}
+                          "peak": peaks["hbm_gbs"], "frac": gbs / peaks["hbm_gbs"]}
         # the north star's own shape: ONE query of Nq=320 per corpus pass (single-query latency path)
         ms = scan_only(Q_dev[:1].contiguous(), k, 5)
         if ms:
@@ -559,8 +520,7 @@ def run_ours(args):
             b1 = {"workload": "1 query x Nq=%d per corpus pass (batch 1: the shape the north star's HBM fraction "
                               "is defined on)" % nq,
                   "launch_ms": ms, "queries_per_s": 1e3 / ms,
-                  "hbm": {"achieved": gbs, "unit": "GB/s", "frac_of_measured_copy": gbs / peaks["hbm_gbs"],
-                          "hbm_frac_of_8TBs": gbs / 8000.0},
+                  "hbm": {"achieved": gbs, "unit": "GB/s", "frac_of_peak": gbs / peaks["hbm_gbs"]},
                   "tensor": {"achieved": tf, "unit": "TFLOP/s (algorithmic: %d query rows)" % nq,
                              "frac_of_burst": tf / peaks["bf16_burst"], "frac_of_sustained": tf / peaks["bf16_sustained"]},
                   "query_rows_resident": ((nq + 31) // 32) * 32, "mma_rows_issued": ((nq + 127) // 128) * 128}
@@ -629,36 +589,22 @@ def run_ours(args):
         info_tokens = n_tok
         # dominant kernel = flmr_scan_kernel: one launch scans this rank's shard for the queries resident
         # in that pass.  Algorithmic work per launch (DESIGN.md "Roofline"):
-        # queries resident per scan launch, from the launches actually timed (2 per normal pass at Nq = 320; 4 per
-        # CTA-pair pass, where two CTAs stream one token range with two queries each)
+        # queries resident per scan launch, from the launches actually timed (1 per normal pass at Nq = 320; 2 per
+        # CTA-pair pass, where two CTAs stream one token range with one query each)
         q_per_launch = B * args.steps / max(r_dev["scan_n"], 1)
         flops_launch = 2.0 * q_per_launch * nq * 128 * info_tokens
         bytes_launch = info_tokens * 256.0
         scan_avg_ms = r_dev["scan_ms"] / max(r_dev["scan_n"], 1)
         ach_tf = flops_launch / (scan_avg_ms * 1e-3) / 1e12 if scan_avg_ms > 0 else 0.0
         ach_gbs = bytes_launch / (scan_avg_ms * 1e-3) / 1e9 if scan_avg_ms > 0 else 0.0
-        # DRAM traffic of one launch from the committed `ncu --set full` capture at this exact size; reported
-        # only while the kernel sources still hash to what was captured (else null: stale)
-        traffic = traffic_src = None
-        sha = kernel_source_sha()
-        for tname in ("r02_traffic.json", "r01_traffic.json"):
-            tpath = os.path.join(ROOT, "profiles", tname)
-            if os.path.exists(tpath) and world == 1 and (n_total, nd, nq) == (1_000_000, 180, 320):
-                with open(tpath) as f:
-                    tj = json.load(f)
-                if tj.get("kernel_source_sha") == sha and abs(tj.get("queries_per_launch", 2) - q_per_launch) < 1e-6:
-                    traffic = tj.get("traffic_bytes_per_launch")
-                    traffic_src = "profiles/%s (ncu --set full: dram__bytes_read.sum + dram__bytes_write.sum per launch; kernel sources %s)" % (tname, sha)
-                    break
         roofline = {
             "bound": "tensor", "achieved": ach_tf, "peak": peaks["bf16_sustained"], "unit": "TFLOP/s",
-            "frac": ach_tf / peaks["bf16_sustained"], "traffic": traffic,
-            "traffic_source": traffic_src, "kernel_source_sha": sha,
-            "peak_source": peaks["source"] + " (sustained cuBLAS bf16: kernel timed inside a long step)",
+            "frac": ach_tf / peaks["bf16_sustained"],
+            "peak_source": peaks["source"],
             "kernel": "flmr_scan_kernel", "launch_ms": scan_avg_ms, "launches_timed": r_dev["scan_n"],
             "scan_share_of_step": r_dev["scan_ms"] / r_dev["dev_ms"] if r_dev["dev_ms"] > 0 else None,
             "hbm": {"achieved": ach_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                    "frac": ach_gbs / peaks["hbm_gbs"], "frac_of_8TBs": ach_gbs / 8000.0,
+                    "frac": ach_gbs / peaks["hbm_gbs"],
                     "algorithmic_bytes_per_launch": bytes_launch},
             "algorithmic_flops_per_launch": flops_launch, "queries_per_launch": q_per_launch,
         }
@@ -792,7 +738,7 @@ def c2_record(args, dev, peaks):
     corpus = R.FlatCorpus(D, doclens.numpy().astype(np.int32), device=dev)
     del D
     searcher = R.Searcher(index=corpus)
-    steps, warmup = max(3, min(args.steps, 10)), 3
+    steps, warmup = args.steps, args.warmup
     for _ in range(warmup):
         searcher._search_tensors(Q, k)
     torch.cuda.synchronize(dev)
@@ -822,7 +768,7 @@ def c2_record(args, dev, peaks):
            "recall_at_100": sum(int(t in r) for r, t in zip(rows_out, targets)) / B,
            "roofline": {"bound": "tensor", "achieved": tf, "unit": "TFLOP/s", "peak": peaks["bf16_burst"],
                         "frac": tf / peaks["bf16_burst"],
-                        "peak_source": peaks["source"] + " (burst cuBLAS bf16: a 50 ms step, not power-limited)",
+                        "peak_source": peaks["source"],
                         "scan_ms_per_step": scan_ms_step, "scan_share_of_step": scan_ms_step / ms_step,
                         "algorithmic_flops_per_step": flops_step,
                         "hbm_gbs": (cnt.value // steps) * n_tok * 256.0 / (scan_ms_step * 1e-3) / 1e9}}

@@ -3,7 +3,7 @@
 
     1. encode the passage collection           (PyTorch encoder - here a stand-in)   -> Indexer.index
     2. encode the queries                       (PyTorch encoder - here a stand-in)   -> Q [n, Nq, 128]
-    3. searcher._search_all_Q(queries, Q, k)    (the B200 scan: exhaustive, batched)  -> Ranking
+    3. searcher._search_all_Q(queries, Q, k)    (the H100 scan: exhaustive, batched)  -> Ranking
     4. Recall@K over the ranking                (as compute_DPR_scores, metrics_processors.py:481-542)
 
     python examples/retrieval_eval_flow.py [--passages 20000] [--queries 64]

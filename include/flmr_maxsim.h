@@ -1,5 +1,5 @@
 /*
- * flmr_maxsim.h — C ABI of the B200-native FLMR / ColBERT late-interaction MaxSim + top-k path.
+ * flmr_maxsim.h — C ABI of the H100-native FLMR / ColBERT late-interaction MaxSim + top-k path.
  *
  * This is the drop-in boundary for the ONE hot path this repository accelerates
  * (SURVEY.md §8b).  The reference has no FFI registry for this path: it binds four pybind11
@@ -130,7 +130,7 @@ int flmr_corpus_builder_destroy(flmr_corpus_builder_t* b);
 
 /* Scratch for searches on `corpus`.  max_queries (>= 1) sizes the per-CTA candidate buffer: a call with more
  * queries is processed in chunks of max_queries (each chunk: its scan passes + ONE merge launch).  max_nq
- * (>= 1) is the longest query expected: if it exceeds the 640 rows one pass holds, the partial-score rows of
+ * (>= 1) is the longest query expected: if it exceeds the 384 rows one pass holds, the partial-score rows of
  * row-sliced queries are allocated here instead of inside the first such search (longer queries still work,
  * the buffer then grows on demand). */
 int flmr_workspace_create(const flmr_corpus_t* corpus, int max_queries, int max_nq,
@@ -246,8 +246,8 @@ int flmr_corpus_gather(const flmr_corpus_t* corpus, const int64_t* d_pids, int64
  *                       is score[b, p], so for a training-sized batch this one launch is the forward AND
  *                       saves what the backward needs (4 B per pair instead of the Nd scores).
  *                       Two kernels behind it: a warp-MMA one for small batches (a RAG re-score of 5 passages) and,
- *                       from 16M (query row, token) pairs up, a tcgen05 one (documents compacted to their unmasked
- *                       tokens, then a TMA / TMEM pipeline with the query tile stationary).
+ *                       from 16M (query row, token) pairs up, a wgmma one (documents compacted to their unmasked
+ *                       tokens, then a TMA / wgmma pipeline with the query tile stationary).
  * flmr_maxsim_backward: given d_grad[b, p] = dLoss/dScore[b, p],
  *                         d_dq[b, i, :]                  = sum_p grad[b, p] * D[p, argmax[b, p, i], :]
  *                         d_dd[p, argmax[b, p, i], :]   += grad[b, p] * Q[b, i, :]      (d_dd zeroed first)
@@ -299,16 +299,15 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* corpus, const void* d_q, 
                                   int nq, unsigned flags, float* d_out_scores, void* stream);
 
 /* Test infrastructure: which scan kernel searches on the calling thread launch — 0 = chosen per call and pass (the
- * product behaviour: CTA-pair passes for as many queries as fill them when the shard spans every SM, else normal
- * passes, those with three resident query tiles on the three-warpgroup kernel),
- * 2 = flmr_scan_kernel (two epilogue warpgroups), normal passes only, 3 = flmr_scan3_kernel (three warpgroups,
- * static query-tile assignment), normal passes only, 4 = CTA-pair passes (clusters of two CTAs stream one token
+ * product behaviour: normal passes, those with three resident query tiles on the three-warpgroup kernel),
+ * 2 = flmr_scan_kernel<2> (two consumer warpgroups), normal passes only, 3 = flmr_scan_kernel<3> (three
+ * warpgroups), normal passes only, 4 = CTA-pair passes (clusters of two CTAs stream one token
  * range, each D tile fetched once and TMA-multicast to both) whenever a call has enough queries, on any shard —
  * so the parity suite can run against any of them at any shape. */
 int flmr_debug_set_scan_variant(int variant);
 
 /* Test infrastructure: which kernel flmr_maxsim_argmax(_grouped) runs on the calling thread — 0 = chosen by size
- * (the product behaviour), 1 = the warp-MMA kernel, 2 = the tcgen05 kernel — so tests can hold either against
+ * (the product behaviour), 1 = the warp-MMA kernel, 2 = the wgmma kernel — so tests can hold either against
  * the other and the oracle at any shape. */
 int flmr_debug_set_argmax_path(int path);
 
@@ -323,7 +322,7 @@ int flmr_debug_build_partition(const int32_t* h_doclens, int64_t n_passages, int
                                int64_t tile_capacity, int64_t* n_tiles_out);
 
 /* Test infrastructure, host-only: the corpus passes flmr_maxsim_scores / flmr_maxsim_topk run for a batch of
- * `n_queries` queries of `nq` tokens (a pass = one scan-kernel launch with up to 640 query rows resident per CTA);
+ * `n_queries` queries of `nq` tokens (a pass = one scan-kernel launch with up to 384 query rows resident per CTA);
  * allow_pair != 0 plans CTA-pair passes (clusters of two CTAs share a token range, each with its own queries) for
  * the query prefix that fills them, as the library does on shards that span every SM.
  * out_plan (may be NULL to query *n_passes_out) receives 8 int32 per pass: first query, queries resident PER CTA (a

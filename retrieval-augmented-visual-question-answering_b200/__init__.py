@@ -1,4 +1,4 @@
-"""B200-native FLMR / ColBERT late-interaction MaxSim + top-k (the one hot path of RA-VQA this
+"""H100-native (sm_90a) FLMR / ColBERT late-interaction MaxSim + top-k (the one hot path of RA-VQA this
 repository accelerates).  Import name: ``ravqa_b200`` (the directory name carries hyphens)."""
 from . import _cabi  # noqa: F401
 from .corpus import FlatCorpus  # noqa: F401

@@ -1,4 +1,4 @@
-"""Build the sm_100a shared library in-tree (``lib/libflmr_maxsim.so``).
+"""Build the sm_90a shared library in-tree (``lib/libflmr_maxsim.so``).
 
 nvcc cross-compiles without a GPU; the resulting .so is git-ignored but travels to the GPU box
 with the repository snapshot.  Used by ``__graft_entry__.build()`` and lazily by ``_cabi`` when the
@@ -19,7 +19,7 @@ SOURCES = [os.path.join(CSRC, "flmr_maxsim.cu")]
 HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + [os.path.join(PKG_DIR, "..", "include", "flmr_maxsim.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
 ]

@@ -1,6 +1,6 @@
-// flmr_device.cuh — thin inline-PTX wrappers for the sm_100a features the scan kernel uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / fences).
-// Hand-written for this repository; sm_100a only.
+// flmr_device.cuh — thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor, cluster multicast), thread-block clusters and wgmma.
+// Hand-written for this repository; sm_90a only.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -20,8 +20,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// One lane of the (fully converged) warp; the same lane every time, so tcgen05.commit, which tracks
-// the MMAs "initiated by the executing thread", sees all of them.
+// One lane of the (fully converged) warp, the same lane every time.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile(
@@ -70,10 +69,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
 // Bounded wait: a protocol bug must surface as a trapped launch, never as a hung GPU box.
 // `status` receives `code` before the trap so the host can say which role starved.
 //
-// The polling loop is written in PTX so that one iteration is the try_wait itself plus four instructions: the
-// round-1 C++ loop compiled to 15 instructions per iteration, and with waits this fine-grained (a warp is woken
-// by every partial arrival on its barrier) the polling iterations were 25 % of all warp instructions the scan
-// kernel executed (profiles/r01 source page).  The watchdog reads the timer once per kSpinBlock failed polls.
+// The polling loop is written in PTX so that one iteration is the try_wait itself plus four instructions (a C++
+// loop compiles to about 15), which keeps fine-grained waits cheap in issue slots.  The watchdog reads the timer
+// once per kSpinBlock failed polls.
 constexpr uint32_t kSpinBlock = 4096;
 __device__ __forceinline__ uint32_t mbar_poll_block(uint32_t bar, uint32_t parity) {
   uint32_t n;
@@ -157,131 +155,86 @@ __device__ __forceinline__ void cluster_sync_all() {   // every thread of every 
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// ---- tcgen05 / TMEM -------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// tcgen05.commit: arrive once on `bar` when all MMAs issued so far by this thread have completed.
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
-}
-
-// tcgen05.commit that arrives on the barrier at the same offset in every CTA of `cta_mask`.
-__device__ __forceinline__ void tc_commit_multicast(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask)
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 in / fp32 accumulate, one CTA.
-__device__ __forceinline__ void tc_mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
+// Arrive once on the mbarrier at shared-memory offset `bar` of cluster CTA `cta` (this CTA included), with
+// release semantics at cluster scope: the peer's waiter then sees every shared-memory read this thread ordered
+// before the arrive as complete.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .b32 r;\n\t"
+      "mapa.shared::cluster.u32 r, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [r];\n\t}"
+      ::"r"(bar), "r"(cta)
       : "memory");
 }
 
-// D[tmem] (+)= A[tmem] * B[smem]^T: the A operand (128 rows x 16 bf16 per MMA = 8 TMEM columns,
-// row = lane, two consecutive K elements per 32-bit column) is read from tensor memory.
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// Generic-proxy writes to shared memory (st.shared) made visible to the async proxy (wgmma operand reads).
+__device__ __forceinline__ void fence_proxy_async_smem() {
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 128 B
-// (64 bf16), 8-row groups 1024 B apart.  Field layout: start>>4 [0,14) | LBO>>4 [16,30) |
-// SBO>>4 [32,46) | version=1 [46,48) | layout type [61,64) (2 = SWIZZLE_128B).
+// ---- wgmma --------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (sm_90), K-major operand, 128-byte swizzle, rows of 128 B (64 bf16),
+// 8-row groups 1024 B apart.  Field layout: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
+// layout type [62,64) (1 = SWIZZLE_128B).  A K step of 16 elements inside the 128-byte row advances the
+// start address by 32 bytes; the hardware applies the swizzle to the final address.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;             // LBO (unused for swizzled K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;     // SBO: 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;             // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;             // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;             // SWIZZLE_128B
   return d;
 }
 
-// Instruction descriptor for kind::f16: bf16 x bf16 -> fp32, both operands K-major.
-// c_format [4,6)=1 (f32) | a_format [7,10)=1 (bf16) | b_format [10,13)=1 | N>>3 [17,23) | M>>4 [24,29).
-__host__ __device__ constexpr uint32_t make_idesc_bf16_f32(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// Pins the accumulator registers in place across the asynchronous MMA: without it the compiler may read or
+// move them between the issue and the wait.
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 32 consecutive fp32 columns of the accumulator -> 32 registers per thread
-// (thread t of the warp reads TMEM lane (lane-quadrant base + t)).
-#define FLMR_TMEM_LD32(v, taddr)                                                                   \
-  asm volatile(                                                                                    \
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                    \
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"                                    \
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"                   \
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),        \
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),    \
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), \
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), \
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])                                         \
-      : "r"(taddr)                                                                                 \
-      : "memory")
-
-// tcgen05.wait::ld with the destination registers threaded through as "+r" operands so the
-// compiler cannot hoist their uses above the wait.
-#define FLMR_TMEM_WAIT_LD32(v)                                                                     \
-  asm volatile("tcgen05.wait::ld.sync.aligned;"                                                    \
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]),           \
-                 "+r"(v[6]), "+r"(v[7]), "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]),         \
-                 "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]), "+r"(v[16]), "+r"(v[17]),     \
-                 "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]),     \
-                 "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]),     \
-                 "+r"(v[30]), "+r"(v[31])::"memory")
-
-// 32 registers per thread -> 32 lanes x 32 consecutive 32-bit TMEM columns.
-#define FLMR_TMEM_ST32(taddr, v)                                                                   \
-  asm volatile(                                                                                    \
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "                                              \
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"                                   \
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"                          \
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]),   \
-      "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]),             \
-      "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]),          \
-      "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),          \
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])                                               \
-      : "memory")
-
-__device__ __forceinline__ void tmem_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+// Accumulator fragment of m64nNk16 (per warp of the warpgroup, 16 rows): d[4 i + 2 h + e] is row
+// 16 * (warp % 4) + lane / 4 + 8 h, column 8 i + 2 * (lane % 4) + e.
+// 8 accumulator operands of the wgmma wrappers below.
+#define FLMR_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                   "+f"(d[i + 6]), "+f"(d[i + 7])
+// D (+)= A[smem] * B[smem]^T, m64n96k16, bf16 in / fp32 accumulate; d[48] per thread.
+__device__ __forceinline__ void wgmma_m64n96k16(float (&d)[48], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47"
+      "}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+      : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16), FLMR_F8(24), FLMR_F8(32), FLMR_F8(40)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
+// D (+)= A[smem] * B[smem]^T, m64n128k16, bf16 in / fp32 accumulate; d[64] per thread.
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16), FLMR_F8(24), FLMR_F8(32), FLMR_F8(40), FLMR_F8(48), FLMR_F8(56)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
+
+__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -1,9 +1,9 @@
-// flmr_maxsim.cu — C-ABI implementation (include/flmr_maxsim.h) of the B200-native FLMR/ColBERT
+// flmr_maxsim.cu — C-ABI implementation (include/flmr_maxsim.h) of the H100-native FLMR/ColBERT
 // MaxSim + top-k path.  Host logic: corpus residency + partition metadata, query staging, pass
 // planning, launches.  Device code: the fused scan kernel (flmr_scan_kernel.cuh) plus four small
 // helper kernels (query staging, candidate merge, corpus repack, SIMT cross-check).
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared -Xcompiler -fPIC
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC
 // No libcuda link dependency: cuTensorMapEncodeTiled is resolved through the runtime's
 // cudaGetDriverEntryPoint, so the library loads (and its symbols can be checked) without a GPU.
 #include <cuda.h>
@@ -30,7 +30,6 @@
 
 #include "../../include/flmr_maxsim.h"
 #include "flmr_scan_kernel.cuh"
-#include "flmr_scan3_kernel.cuh"
 #include "flmr_train_kernels.cuh"
 #include "flmr_train_tc_kernel.cuh"
 
@@ -561,7 +560,7 @@ struct flmr_workspace {
   int64_t acc_capacity = 0;            // floats allocated at d_acc
   int* h_status = nullptr;             // pinned + mapped: readable by the host even after a device trap
   int* d_status = nullptr;             // device alias of h_status
-  int dbg_mode = 0, dbg_lane_rbq = 4;  // -DFLMR_DEBUG builds: FLMR_DEBUG_MODE / FLMR_LANE_RBQ, read once at creation
+  int dbg_lane_rbq = 4;  // -DFLMR_DEBUG builds: FLMR_LANE_RBQ, read once at creation
 };
 
 // NCCL is resolved at RUN time (dlopen): the library has no link dependency on it, loads on a box without
@@ -635,8 +634,8 @@ int load_nccl(const NcclApi** out) {
 constexpr int kNcclInt64 = 4, kNcclFloat32 = 7;   // ncclDataType_t values (nccl.h: ncclInt64 = 4, ncclFloat32 = 7)
 
 thread_local bool g_profiling = false;
-// which scan kernel a search on this thread launches: 0 = chosen per pass (launch_scan), 2 = flmr_scan_kernel (two
-// epilogue warpgroups), 3 = flmr_scan3_kernel (three, static query-tile assignment); flmr_debug_set_scan_variant
+// which scan kernel a search on this thread launches: 0 = chosen per pass (launch_scan), 2 = flmr_scan_kernel<2> (two
+// consumer warpgroups), 3 = flmr_scan_kernel<3> (three), 4 = CTA-pair passes forced; flmr_debug_set_scan_variant
 thread_local int g_scan_variant = 0;
 struct EventPair {
   cudaEvent_t a, b;
@@ -712,7 +711,8 @@ struct PassPlan {
 
 // allow_pair: CTA-pair passes (run_search decides: shards that span every SM) for as many queries as fill them —
 // every CTA of a pair keeps exactly the residency a normal pass would give it, so a pair pass serves twice the
-// queries per corpus pass; with fewer than four 128-row tiles per CTA pairs measured slower and are not planned.
+// queries per corpus pass.  Whole queries are paired only when they fill all kMtMax tiles of a CTA: with less
+// residency the cross-CTA hand-back of every D stage is paid for fewer MMAs per tile.
 // Pair passes always cover a PREFIX of the queries (*n_pair_queries_out); the rest gets normal passes.
 void plan_passes(int n_queries, int nq, bool allow_pair, std::vector<PassPlan>* out, int* group_out,
                  int* n_pair_queries_out) {
@@ -721,7 +721,7 @@ void plan_passes(int n_queries, int nq, bool allow_pair, std::vector<PassPlan>* 
   const int rbq_total = (nq + 31) / 32;
   if (rbq_total <= kRbMax) {
     const int qpp_max = std::min(kNqMax, kRbMax / rbq_total);
-    if (allow_pair && qpp_max * rbq_total * 32 >= 4 * kTileM) {
+    if (allow_pair && qpp_max * rbq_total * 32 > (kMtMax - 1) * kTileM) {
       for (; n_pair_q + 2 * qpp_max <= n_queries; n_pair_q += 2 * qpp_max)
         out->push_back({n_pair_q, qpp_max, 0, nq, rbq_total, (qpp_max * rbq_total * 32 + kTileM - 1) / kTileM,
                         kPassFinal | kPassPair, n_pair_q, 0});
@@ -782,18 +782,9 @@ void plan_passes(int n_queries, int nq, bool allow_pair, std::vector<PassPlan>* 
 }
 
 int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pair, cudaStream_t st) {
-  // three epilogue warpgroups pay off exactly where they buy a third TMEM accumulator stage and one accumulator
-  // per warpgroup and D tile: passes with three resident query tiles (one Nq = 320 query: +12 % in short runs, +4 %
-  // sustained); with five tiles (2 / 2 / 1 accumulators per warpgroup, still two stages) they measured 7 % slower
-  // than strict two-warpgroup alternation, with one, two or four tiles the same (profiles/r02_scan_variant_probe.md)
-  const bool three = !pair && ((g_scan_variant == 3) || (g_scan_variant == 0 && p.n_mtiles == 3));
-#ifdef FLMR_DEBUG
-  auto kern = p.debug_mode ? flmr_scan_kernel<true> : flmr_scan_kernel<false>;
-  const bool use3 = three && !p.debug_mode;
-#else
-  auto kern = flmr_scan_kernel<false>;
-  const bool use3 = three;
-#endif
+  // three consumer warpgroups where the six 64-row query blocks of three resident tiles split evenly over them
+  // (two each), two otherwise; the instantiations compute bit-identical results
+  const bool use3 = !pair && ((g_scan_variant == 3) || (g_scan_variant == 0 && p.n_mtiles == 3));
   EventPair ev{};
   if (g_profiling) {
     FLMR_CUDA(cudaEventCreate(&ev.a));
@@ -809,7 +800,7 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
     p.tile_first_pid = c->d_pair_first_pid;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(static_cast<unsigned>(2 * c->n_pairs));
-    cfg.blockDim = dim3(kScanThreads);
+    cfg.blockDim = dim3(scan_threads(2));
     cfg.dynamicSmemBytes = ScanSmem::kBytes;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -819,11 +810,11 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    FLMR_CUDA(cudaLaunchKernelEx(&cfg, flmr_scan_kernel<false, true>, c->tmap_half, p));
+    FLMR_CUDA(cudaLaunchKernelEx(&cfg, flmr_scan_kernel<2, true>, c->tmap_half, p));
   } else if (use3) {
-    flmr_scan3_kernel<<<c->n_ctas, kScan3Threads, ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    flmr_scan_kernel<3><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
   } else {
-    kern<<<c->n_ctas, kScanThreads, ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    flmr_scan_kernel<2><<<c->n_ctas, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
   }
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
@@ -860,7 +851,7 @@ int launch_merge_keys(const flmr_corpus* c, flmr_workspace* ws, int n_lists, int
   return FLMR_OK;
 }
 
-// Partial-score rows of row-sliced (Nq > 640) queries: grown on demand, never shrunk.
+// Partial-score rows of row-sliced (Nq > kRbMax * 32) queries: grown on demand, never shrunk.
 int ensure_acc(flmr_workspace* ws, int64_t floats) {
   if (ws->acc_capacity >= floats) return FLMR_OK;
   if (ws->d_acc) cudaFree(ws->d_acc);
@@ -898,35 +889,18 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   p.cand_keys = ws->d_cand_keys;
   p.q_pad = reinterpret_cast<const uint4*>(ws->d_qpad);
   p.status = ws->d_status;
-  p.lane_mode_max_rbq = 4;   // measured (profiles/r01_debug_mode_probes.log): lane-per-query wins up to 4 row blocks per query
+  // reducer: one lane per query sums that query's row maxima when a query has at most 4 row blocks (short queries,
+  // many per pass), the whole warp per (query, passage) above; a heuristic, not tuned on this architecture
+  p.lane_mode_max_rbq = 4;
 #ifdef FLMR_DEBUG   // timing experiments exist only in -DFLMR_DEBUG builds (tools/); the release library has no env hooks
   p.lane_mode_max_rbq = ws->dbg_lane_rbq;
-  p.debug_mode = ws->dbg_mode;
-  if (p.debug_mode == 6) {  // timestamps of CTA 0's accumulator hand-offs, dumped by the caller
-    static long long* d_ts = nullptr;
-    if (!d_ts) {
-      FLMR_CUDA(cudaMallocManaged(reinterpret_cast<void**>(&d_ts), 64 * 8 * sizeof(long long)));
-      memset(d_ts, 0, 64 * 8 * sizeof(long long));
-    }
-    p.dbg_ts = d_ts;
-    if (const char* f = getenv("FLMR_DEBUG_TS_DUMP")) {   // dump what the PREVIOUS launch recorded
-      cudaDeviceSynchronize();
-      if (FILE* fp = fopen(f, "w")) {
-        for (int a = 0; a < 64; ++a) {
-          for (int i = 0; i < 8; ++i) fprintf(fp, "%lld ", d_ts[a * 8 + i]);
-          fprintf(fp, "\n");
-        }
-        fclose(fp);
-      }
-    }
-  }
 #endif
 
   // CTA-pair passes (clusters of two CTAs stream one token range, each CTA with the residency of a normal pass, every
-  // D tile fetched once and TMA-multicast into both: half the HBM / L2 traffic per query, ~6 % more sustained
-  // throughput on this power-capped part, profiles/r02_scan_variant_probe.md) are planned for as many queries as fill
-  // them when the shard spans every SM (variant 0 = product), always when forced (4), never under 2 / 3.
-  const bool allow_pair = c->n_pairs > 0 && (g_scan_variant == 4 || (g_scan_variant == 0 && c->n_pairs * 2 == c->sm_count));
+  // D tile fetched once and TMA-multicast into both: half the HBM / L2 traffic per query) are planned only when forced
+  // (variant 4): on an H100 a pair pass of two Nq = 320 queries over 1M passages took 105.9 ms against 39.4 ms for a
+  // single-CTA pass of one, so the product (variant 0) runs single-CTA passes.
+  const bool allow_pair = c->n_pairs > 0 && g_scan_variant == 4;
   // a call is processed in chunks of at most ws->max_queries queries (the candidate buffer's capacity);
   // within a chunk: every pass's scan, then the merge over the chunk's queries (one launch per kind of pass)
   std::vector<PassPlan> plan;
@@ -1023,7 +997,10 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
   }
   if ((rc = encode_rows_map(&c->tmap_d, c->d_tokens, static_cast<uint64_t>(n_rows), kTileN)))
     return bail(rc);
-  if (n_ctas >= 2 && n_passages >= n_ctas / 2) {   // CTA-pair experiment: its own partition + half-tile tensor map
+  // CTA-pair passes: their own partition + half-tile tensor map.  The product never plans pair passes (see
+  // run_search); these few KB per corpus are built so flmr_debug_set_scan_variant(4) can hold the cluster kernel
+  // against the single-CTA kernels on any corpus.
+  if (n_ctas >= 2 && n_passages >= n_ctas / 2) {
     std::vector<int32_t> row_begin, first_pid;
     std::vector<int64_t> tile_base;
     std::vector<uint32_t> end_mask;
@@ -1036,24 +1013,18 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
     if ((rc = dev_upload(&c->d_pair_end_mask, end_mask, &c->hbm_bytes))) return bail(rc);
     if ((rc = dev_upload(&c->d_pair_first_pid, first_pid, &c->hbm_bytes))) return bail(rc);
     if ((rc = encode_rows_map(&c->tmap_half, c->d_tokens, static_cast<uint64_t>(n_rows), kTileN / 2))) return bail(rc);
-    cudaError_t e3 = cudaFuncSetAttribute(flmr_scan_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e3 = cudaFuncSetAttribute(flmr_scan_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           ScanSmem::kBytes);
     if (e3 != cudaSuccess) return bail(fail(FLMR_ERR_CUDA, "pair kernel attribute: %s", cudaGetErrorString(e3)));
   }
   {  // per-device function attribute, set here (idempotent) rather than at launch time
-    cudaError_t e1 = cudaFuncSetAttribute(flmr_scan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e1 = cudaFuncSetAttribute(flmr_scan_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           ScanSmem::kBytes);
     if (e1 == cudaSuccess)
-      e1 = cudaFuncSetAttribute(flmr_scan3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes);
-#ifdef FLMR_DEBUG
-    cudaError_t e2 = cudaFuncSetAttribute(flmr_scan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          ScanSmem::kBytes);
-#else
-    cudaError_t e2 = cudaSuccess;
-#endif
-    if (e1 != cudaSuccess || e2 != cudaSuccess)
+      e1 = cudaFuncSetAttribute(flmr_scan_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes);
+    if (e1 != cudaSuccess)
       return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
-                       ScanSmem::kBytes, cudaGetErrorString(e1 != cudaSuccess ? e1 : e2)));
+                       ScanSmem::kBytes, cudaGetErrorString(e1)));
   }
   return FLMR_OK;
 }
@@ -1095,8 +1066,8 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
   cudaDeviceProp prop;
   FLMR_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(FLMR_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is sm_100a only", device,
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(FLMR_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is sm_90a only", device,
                 prop.major, prop.minor);
 
   cudaPointerAttributes attr{};
@@ -1243,8 +1214,8 @@ int flmr_corpus_builder_create(const int32_t* h_doclens, int64_t n_passages, int
   cudaDeviceProp prop;
   cudaError_t e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) return bail(fail(FLMR_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e)));
-  if (prop.major != 10)
-    return bail(fail(FLMR_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is sm_100a only", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0)
+    return bail(fail(FLMR_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is sm_90a only", device, prop.major,
                      prop.minor));
   b->sm_count = prop.multiProcessorCount;
   flmr_corpus* c = new (std::nothrow) flmr_corpus();
@@ -1446,7 +1417,6 @@ int flmr_workspace_create(const flmr_corpus_t* c, int max_queries, int max_nq,
     if (int rc = ensure_acc(ws, static_cast<int64_t>(group) * c->n_passages)) return bail(rc);
   }
 #ifdef FLMR_DEBUG
-  if (const char* e = getenv("FLMR_DEBUG_MODE")) ws->dbg_mode = atoi(e);
   if (const char* e = getenv("FLMR_LANE_RBQ")) ws->dbg_lane_rbq = atoi(e);
 #endif
   *out = ws;
@@ -1529,7 +1499,9 @@ int flmr_plaid_decode(const int32_t* d_codes, const uint8_t* d_residuals, int64_
   cudaError_t e = cudaSuccess;
   const int threads = 256;
   const int64_t want = (n_tokens * 32 + threads - 1) / threads;
-  const int blocks = static_cast<int>(std::min<int64_t>(want, 148 * 16));
+  int sms = 0;
+  FLMR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  const int blocks = static_cast<int>(std::min<int64_t>(want, static_cast<int64_t>(sms) * 16));
   if (e == cudaSuccess) {
     flmr_plaid_decode_kernel<<<blocks, threads, 0, st>>>(d_codes, d_residuals, d_centroids,
                                                        d_bucket_weights, nbits, normalize, n_tokens,
@@ -1578,8 +1550,8 @@ int flmr_corpus_gather(const flmr_corpus_t* c, const int64_t* d_pids, int64_t n_
   return FLMR_OK;
 }
 
-// ---- the tcgen05 route of the arg-max forward (flmr_train_tc_kernel.cuh) --------------------------------------
-thread_local int g_argmax_path = 0;   // 0 = by size, 1 = warp-MMA kernel, 2 = tcgen05 kernel (flmr_debug_set_argmax_path)
+// ---- the wgmma route of the arg-max forward (flmr_train_tc_kernel.cuh) ----------------------------------------
+thread_local int g_argmax_path = 0;   // 0 = by size, 1 = warp-MMA kernel, 2 = wgmma kernel (flmr_debug_set_argmax_path)
 
 // The library's own stream-ordered memory pool (one per device) for per-call scratch: it keeps what it has
 // been given (release threshold = max), so after the first call an allocation is a pointer bump in stream order —
@@ -1644,15 +1616,17 @@ static int argmax_tc(const void* d_q, int n_queries, int nq, const void* d_docs,
   if (attr_err != cudaSuccess)
     return done(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit: %s", cudaGetErrorString(attr_err)));
   const int n_tiles = (nq + kTcTile - 1) / kTcTile;
-  // documents per CTA: a CTA pays ~5 us of set-up (TMEM allocation, barriers, query tile, pipeline fill) before its
-  // first MMA and ~0.3 us per 128-token chunk after it; pick the split with the shortest modelled makespan
-  // (waves of 148 CTAs x per-CTA time): many documents per CTA unless that leaves SMs idle
+  // documents per CTA: a CTA pays a fixed set-up (barriers, query tile, pipeline fill) before its first MMA, modelled
+  // as ~17 chunks of 128 tokens; pick the split with the shortest modelled makespan (waves of one CTA per SM x
+  // per-CTA time): many documents per CTA unless that leaves SMs idle
+  int sms = 0;
+  FLMR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int64_t pairs_q = static_cast<int64_t>(n_queries) * n_tiles;
   int dpc = 1;
   double best_t = 1e30;
   for (int d = 1; d <= 32 && d <= std::max(1, n_per); ++d) {
     const int64_t ctas = pairs_q * ((n_per + d - 1) / d);
-    const double t = static_cast<double>((ctas + 147) / 148) * (5.0 + d * 0.3 * (nd_c / kTcTile));
+    const double t = static_cast<double>((ctas + sms - 1) / sms) * (5.0 + d * 0.3 * (nd_c / kTcTile));
     if (t < best_t) {
       best_t = t;
       dpc = d;
@@ -1691,7 +1665,7 @@ static int argmax_impl(const void* d_q, int n_queries, int nq, const void* d_doc
   if (n_queries == 0 || n_per == 0) return FLMR_OK;
   DeviceGuard guard(device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
-  // tcgen05 route when the contraction is worth a TMA / TMEM pipeline (>= 16M query-row x token pairs and full
+  // wgmma route when the contraction is worth a TMA pipeline (>= 16M query-row x token pairs and full
   // tiles), warp-MMA kernel below that: a RAG re-score of 5 passages stays on the small kernel
   const double pairs = static_cast<double>(n_queries) * n_per * nq * nd;
   const bool tc_ok = n_queries <= 65535 && (nq + kTcTile - 1) / kTcTile <= 65535;
@@ -1832,7 +1806,7 @@ int flmr_debug_set_scan_variant(int variant) {
 }
 
 int flmr_debug_set_argmax_path(int path) {
-  if (path < 0 || path > 2) return fail(FLMR_ERR_INVALID_ARG, "path must be 0 (by size), 1 (warp-MMA) or 2 (tcgen05)");
+  if (path < 0 || path > 2) return fail(FLMR_ERR_INVALID_ARG, "path must be 0 (by size), 1 (warp-MMA) or 2 (wgmma)");
   g_argmax_path = path;
   return FLMR_OK;
 }

@@ -9,36 +9,29 @@
 // segmented_maxsim.cpp reduction (CB/modeling/segmented_maxsim.cpp:22-93) and the per-query
 // `scores.sort()` of IndexScorer.rank (CB/search/index_storage.py:95).
 //
-// Structure (one persistent CTA per SM, 12 warps, warp-specialised; accumulators are numbered in
-// issue order, a = t * n_mtiles + j, where j-th in D tile t is query tile mt = j — except that with an
-// odd tile count the odd D tiles start with the LAST query tile, see the epilogue):
-//   warps 0..7   : epilogue, two warpgroups; warpgroup g drains the accumulators with (a & 1) == g.
-//                  TMEM lane = query token, TMEM column = passage token: the max over a passage's
-//                  tokens is a per-thread running max over columns (FMNMX3, no shuffles); at a passage
-//                  end (bit in the tile's end mask) the warp sums its 32 lanes and lane 0 stores one
-//                  partial per (32-row block, passage).  The running max of the passage straddling
-//                  two D tiles lives in shared memory per (query tile, row); when n_mtiles is odd the
-//                  last query tile's changes hands between the warpgroups through an mbarrier (all
-//                  other query tiles always meet the same warpgroup thanks to the rotated order).
-//   warp 8       : reducer.  Per D tile (mbarrier-fed, double-buffered partials): per (query, passage
-//                  ending in the tile) sums the row-block partials in fixed order (deterministic),
-//                  optionally accumulates / stores scores to HBM, and maintains the per-CTA top-k.
-//   warp 9       : TMA producer.  Streams the CTA's contiguous range of passage tokens through a
-//                  7-deep ring of D stages (96 tokens x 128 dims bf16, 128B-swizzled, 2 boxes).
-//   warps 10..11 : tcgen05.mma issuers; issuer i owns the accumulators with (a & 1) == i.  The
-//                  queries are STATIONARY IN TENSOR MEMORY (A operand from TMEM: up to 5 tiles of
-//                  128 rows x 128 dims = 5 x 64 columns), so shared memory only feeds the B operand.
-//                  Per accumulator: 8 MMAs (K = 8 x 16), acc[128 x 96] = Qtile . Dtile^T, into one of
-//                  2 or 4 TMEM accumulator stages; tcgen05.commit signals the epilogue / frees the
-//                  D stage.  With an even stage count every stage and its mbarrier pair belong to
-//                  exactly one issuer and one epilogue warpgroup.
+// Structure (one persistent CTA per SM, kWgs consumer warpgroups + 2 warps, warp-specialised):
+//   consumer warpgroups : the pass's query rows are STATIONARY IN SHARED MEMORY (up to kMtMax x 128 rows,
+//                         128B-swizzled, the wgmma A operand).  Warpgroup w owns the 64-row query blocks
+//                         j = w, w + kWgs, ...; per D tile and block it issues 8 wgmma.m64n96k16 (K = 8 x 16),
+//                         acc[64 x 96] = Qblock . Dtile^T in registers, then folds the accumulator into the
+//                         passage maxima.  A thread holds two rows and 24 columns per row; the max over a
+//                         passage's tokens is a per-thread max over its columns of the passage's 4-token groups
+//                         plus two shuffles inside the lane quad.  At a passage end (bit in the tile's end mask)
+//                         the per-row maxima (first kFastSlots ends of a tile) or the 16-row sums (later ends)
+//                         go to shared memory for the reducer.  The running max of the passage straddling two
+//                         D tiles stays in a register: a query block never changes warpgroup.
+//   warp 4 kWgs         : reducer.  Per D tile (mbarrier-fed, double-buffered partials): per (query, passage
+//                         ending in the tile) sums the row partials in fixed order (deterministic), optionally
+//                         accumulates / stores scores to HBM, and maintains the per-CTA top-k.
+//   warp 4 kWgs + 1     : TMA producer.  Streams the CTA's contiguous range of passage tokens through a
+//                         kDStages-deep ring of D stages (96 tokens x 128 dims bf16, 128B-swizzled, 2 boxes).
 //
 // Layout contracts (see DESIGN.md "Data layout"):
 //   * passages are stored back to back, each padded to a multiple of 4 tokens by repeating its last
 //     token (duplicates cannot change a max), so passage boundaries fall on 4-column groups and one
 //     mask per tile marks the groups that end a passage;
 //   * each query is padded to a multiple of 32 rows with zero rows (contribute exactly 0, like the
-//     reference's masked query tokens), so a warp's 32 TMEM lanes always belong to one query.
+//     reference's masked query tokens).
 #pragma once
 #include "../../include/flmr_maxsim.h"
 #include "flmr_device.cuh"
@@ -46,34 +39,28 @@
 namespace flmr {
 
 constexpr int kDim = 128;
-constexpr int kTileM = 128;               // query rows per MMA (UMMA M)
-constexpr int kTileN = FLMR_TILE_TOKENS;  // passage tokens per streamed tile (UMMA N)
-constexpr int kMtMax = 5;                 // resident 128-row query tiles per pass (5 x 64 TMEM cols)
+constexpr int kTileM = 128;               // query rows per staged query tile
+constexpr int kTileN = FLMR_TILE_TOKENS;  // passage tokens per streamed tile (wgmma N)
+constexpr int kMtMax = 3;                 // resident 128-row query tiles per pass (96 KB of shared memory)
 constexpr int kRbMax = kMtMax * 4;        // resident 32-row blocks
 constexpr int kNqMax = kRbMax;            // queries per pass (each has >= 1 row block)
+constexpr int kHbMax = 2 * kRbMax;        // resident 16-row blocks (one per consumer warp and 64-row block)
 constexpr int kMaxK = 128;                // fused top-k capacity (== FLMR_MAX_K)
 constexpr int kGroup = 4;                 // token padding granularity (== FLMR_TOKEN_GROUP)
 constexpr int kSlots = kTileN / kGroup;   // passage ends per tile, at most (24 <= 32 lanes)
-constexpr int kChunks = kTileN / 32;      // 32-column chunks per accumulator
-constexpr int kQCols = kDim / 2;          // TMEM columns of one query tile (bf16 pairs)
-constexpr int kMaxAccStages = 4;
-constexpr int kFastSlots = 4;             // passage ends per tile whose lane sums are left to the reducer
-constexpr int kLaneStride = 33;           // padded row of 32 lane values (conflict-free transposed reads)
-constexpr int kDStages = (kTileN == 96) ? 7 : 10;
+constexpr int kNb = kTileN / 8;           // 8-column blocks of an accumulator
+constexpr int kFastSlots = 4;             // passage ends per tile whose per-row maxima are left to the reducer
+constexpr int kLaneStride = 33;           // padded row of 32 row values (conflict-free transposed reads)
+constexpr int kDStages = 4;
 constexpr int kDTileBytes = kTileN * kDim * 2;   // 24 KiB: [2 k-blocks][96 rows][64 bf16]
 constexpr int kDKBlockBytes = kTileN * 128;      // 12 KiB
-// Warp roles (see the header comment).
-constexpr int kEpiWarps = 8;                      // warps 0..7: two warpgroups draining TMEM
-constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kRedWarps = 1;                      // warp 8: score finalisation + top-k
-constexpr int kWarpRed0 = kEpiWarps;
-constexpr int kWarpProducer = kEpiWarps + kRedWarps;   // warp 9
-constexpr int kMmaWarps = 2;                           // warps 10..11: issuer i owns accumulators a = i (mod 2)
-constexpr int kWarpMma = kWarpProducer + 1;
-constexpr int kScanThreads = (kWarpMma + kMmaWarps) * 32;
+constexpr int kQKBlockBytes = kMtMax * kTileM * 128;   // one 64-dim half of the resident queries
+constexpr int kRedWarps = 1;
 
-static_assert(kTileN == 96 || kTileN == 64, "tile width must be 96 or 64 tokens");
+static_assert(kTileN == 96, "the wgmma shape and accumulator fragment are written for 96-token tiles");
 static_assert(kDKBlockBytes % 1024 == 0, "swizzle atoms need 1024-B aligned k-blocks");
+
+__host__ __device__ constexpr int scan_threads(int wgs) { return (wgs * 4 + 2) * 32; }
 
 struct ScanParams {
   // corpus partition (built once per corpus, see build_partition() in flmr_maxsim.cu)
@@ -97,53 +84,26 @@ struct ScanParams {
   uint64_t* cand_keys;             // [n_ctas][cand_q_stride][k]  (ordered score << 32 | ~local pid)
   int32_t cand_q_stride;           // queries of the whole call chunk (one merge launch serves them all)
   int32_t cand_q_first;            // index of this pass's first query inside the chunk
-  // diagnostics
-  int32_t debug_mode;              // 0 = product.  Timing-only experiments (results are garbage):
-                                   // 1 = epilogue releases accumulators unread, 2 = TMEM reads but no
-                                   // passage ends, 3 = mode 1 + MMA issue skipped (pure TMA streaming),
-                                   // 4 = MMA issue never waits for the epilogue (epilogue idle),
-                                   // 5 = mode 4 without the per-accumulator commit
-                                   // 6 = product + clock64 timestamps of CTA 0's hand-offs -> dbg_ts
   int* status;                     // mapped pinned host word: watchdog code of a trapped launch
-  long long* dbg_ts;               // [64 accumulators][8] timestamps (debug_mode 6), else null
 };
 
-constexpr uint32_t kDbgAcc0 = 2000;  // first accumulator index recorded in debug_mode 6
-template <bool kDebug>
-__device__ __forceinline__ void dbg_stamp(const ScanParams& p, int cta, uint32_t a, int slot) {
-  if constexpr (kDebug) {
-    if (p.debug_mode == 6 && cta == 0 && a >= kDbgAcc0 && a < kDbgAcc0 + 64)
-      p.dbg_ts[(a - kDbgAcc0) * 8 + slot] = clock64();
-  }
-}
-
 struct ScanSmem {
-  static constexpr int kOffD = 0;
-  static constexpr int kOffPartial = kOffD + kDStages * kDTileBytes;
-  static constexpr int kPartialBytes = 2 * kRbMax * kSlots * 4;
-  // per-lane passage maxima of the first kFastSlots passage ends of a tile: [2][kFastSlots][kRbMax][33]
+  static constexpr int kOffQ = 0;                                     // [2 k-blocks][kMtMax * 128 rows][128 B]
+  static constexpr int kOffD = kOffQ + 2 * kQKBlockBytes;
+  static constexpr int kOffPartial = kOffD + kDStages * kDTileBytes;  // float[2][kHbMax][kSlots]
+  static constexpr int kPartialBytes = 2 * kHbMax * kSlots * 4;
+  // per-row passage maxima of the first kFastSlots passage ends of a tile: [2][kFastSlots][kRbMax][33]
   static constexpr int kOffLanePart = kOffPartial + kPartialBytes;
   static constexpr int kLanePartBytes = 2 * kFastSlots * kRbMax * kLaneStride * 4;
   static constexpr int kOffKeys = kOffLanePart + kLanePartBytes;
   static constexpr int kKeysBytes = kNqMax * kMaxK * 8;
   static constexpr int kOffMinKey = kOffKeys + kKeysBytes;           // u64[kNqMax]
   static constexpr int kOffMinPos = kOffMinKey + kNqMax * 8;         // int[kNqMax]
-  static constexpr int kOffCarry = kOffMinPos + kNqMax * 4;          // float[kMtMax * 128]
-  static constexpr int kOffBars = (kOffCarry + kMtMax * kTileM * 4 + 7) / 8 * 8;
-  static constexpr int kNumBars = 1 + 2 * kDStages + 2 * kMaxAccStages + 4 + kMtMax * 4;
-  static constexpr int kOffTmemPtr = kOffBars + kNumBars * 8;
-  static constexpr int kBytes = kOffTmemPtr + 16 + 1024;  // + slack for 1024-B alignment
+  static constexpr int kOffBars = (kOffMinPos + kNqMax * 4 + 7) / 8 * 8;
+  static constexpr int kNumBars = 2 * kDStages + 4;
+  static constexpr int kBytes = kOffBars + kNumBars * 8 + 1024;   // + slack for 1024-B alignment
   static_assert(kBytes <= 232448, "exceeds 227 KiB of shared memory per CTA");
 };
-
-// TMEM column budget: query tiles first, accumulator stages in what is left.  The stage count is
-// kept EVEN (4 or 2): accumulators alternate between two issuers / two epilogue warpgroups by index
-// parity, so with an even count every stage (and its mbarrier pair) belongs to exactly one issuer
-// and one warpgroup, which then see its phases strictly in order.  (With 3 stages an agent skips
-// phases of a shared barrier and the parity wait can alias: observed as a hang at n_mtiles = 3.)
-__host__ __device__ inline int scan_acc_stages(int n_mtiles) {
-  return (512 - kQCols * n_mtiles) / kTileN >= 4 ? 4 : 2;
-}
 
 // ---- epilogue helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float s) {
@@ -153,72 +113,6 @@ __device__ __forceinline__ float warp_sum(float s) {
   s += __shfl_xor_sync(0xffffffffu, s, 2);
   s += __shfl_xor_sync(0xffffffffu, s, 1);
   return s;
-}
-
-// 32 accumulator columns = 8 groups of 4 tokens.  `bits` bit g: a passage ends with group g.
-// Compact on purpose (few epilogue warps per SM sub-partition: instruction-cache misses, branches
-// and dependent-issue latency are paid almost in full): 16 FMNMX for the 8 group maxima, then
-// either a 4-instruction fold into the running max or, per passage END in this chunk, a selected
-// tree max + one warp sum.
-__device__ __forceinline__ void process_chunk(const uint32_t (&v)[32], uint32_t bits, float& m,
-                                              float init, float* partial_rb, float* lane_part_rb,
-                                              int& slot, int lane) {
-  if (bits == 0u) {
-    // no passage ends in this chunk: fold all 32 columns into the running max (16 FMNMX3)
-    float r[11];
-#pragma unroll
-    for (int i = 0; i < 10; ++i)
-      r[i] = fmax3(__uint_as_float(v[3 * i]), __uint_as_float(v[3 * i + 1]),
-                   __uint_as_float(v[3 * i + 2]));
-    r[10] = fmaxf(__uint_as_float(v[30]), __uint_as_float(v[31]));
-    const float a = fmax3(r[0], r[1], r[2]);
-    const float b = fmax3(r[3], r[4], r[5]);
-    const float c = fmax3(r[6], r[7], r[8]);
-    const float d = fmax3(r[9], r[10], m);
-    m = fmax3(a, b, fmaxf(c, d));
-    return;
-  }
-  float gv[8];
-#pragma unroll
-  for (int g = 0; g < 8; ++g) {
-    const float a = fmax3(__uint_as_float(v[4 * g]), __uint_as_float(v[4 * g + 1]),
-                          __uint_as_float(v[4 * g + 2]));
-    gv[g] = fmaxf(a, __uint_as_float(v[4 * g + 3]));
-  }
-  uint32_t live = 0xFFu;  // groups not yet consumed by a finished passage
-#pragma unroll 1
-  while (bits) {          // warp-uniform: one iteration per passage ending in this chunk
-    const uint32_t upto = bits ^ (bits - 1u);  // groups 0..(lowest set bit)
-    const uint32_t seg = upto & live;
-    float sel[8];
-#pragma unroll
-    for (int g = 0; g < 8; ++g) sel[g] = ((seg >> g) & 1u) ? gv[g] : -INFINITY;
-    const float x = fmax3(sel[0], sel[1], sel[2]);
-    const float y = fmax3(sel[3], sel[4], sel[5]);
-    float s = fmax3(m, x, y);
-    s = fmax3(s, sel[6], sel[7]);
-    if (slot < kFastSlots) {
-      // common case: every lane parks its maximum, the reducer warp sums the 32 lanes later
-      // (keeps the 5-step shuffle chain off the epilogue's critical path)
-      lane_part_rb[slot * (kRbMax * kLaneStride)] = s;
-    } else {
-      s = warp_sum(s);
-      if (lane == 0) partial_rb[slot] = s;
-    }
-    ++slot;
-    m = init;
-    live &= ~upto;
-    bits &= bits - 1u;
-  }
-  {
-    float sel[8];
-#pragma unroll
-    for (int g = 0; g < 8; ++g) sel[g] = ((live >> g) & 1u) ? gv[g] : -INFINITY;
-    const float x = fmax3(sel[0], sel[1], sel[2]);
-    const float y = fmax3(sel[3], sel[4], sel[5]);
-    m = fmax3(m, x, y);
-    m = fmax3(m, sel[6], sel[7]);
-  }
 }
 
 __device__ __forceinline__ uint64_t shfl64(uint64_t v, int src) {
@@ -255,21 +149,91 @@ __device__ __noinline__ void topk_replace_min(uint64_t* keys, int k, uint64_t ca
   __syncwarp();
 }
 
+// Fold one 64 x 96 accumulator (rows of query block j, the D tile's 96 tokens) into the passage maxima.
+// `m[h]` is the running max of row half h of the passage that is open at the tile start; on return, of the one
+// open at its end.  Every lane of a quad holds the same m (the quad's columns are combined by shuffles).
+__device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], uint32_t mask, float (&m)[2],
+                                                 float init, float* lane_part_buf, float* partial_buf, int j,
+                                                 int wq, int lane) {
+  const int hi = (lane >> 1) & 1;   // this thread's columns belong to the 4-token groups 2 i + hi
+  float gm[2][kNb];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < kNb; ++i) {
+      const float x = fmaxf(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+      gm[h][i] = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+    }
+  const int row0 = j * 64 + wq * 16 + (lane >> 2);   // row of h = 0 inside the pass; h = 1 is row0 + 8
+  uint32_t live = (1u << kSlots) - 1u;               // groups not yet consumed by a finished passage
+  uint32_t bits = mask;
+  int slot = 0;
+#pragma unroll 1
+  while (bits) {   // warp-uniform: one iteration per passage ending in this tile
+    const uint32_t upto = bits ^ (bits - 1u);   // groups 0..(lowest set bit)
+    const uint32_t seg = (upto & live) >> hi;
+    float s[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float x = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < kNb; ++i)
+        if ((seg >> (2 * i)) & 1u) x = fmaxf(x, gm[h][i]);
+      x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+      s[h] = fmaxf(x, m[h]);
+      m[h] = init;
+    }
+    if (slot < kFastSlots) {
+      // common case: one lane per quad parks its two rows' maxima, the reducer sums them later
+      if ((lane & 3) == 0) {
+        float* lp = lane_part_buf + slot * (kRbMax * kLaneStride);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = row0 + 8 * h;
+          lp[(r >> 5) * kLaneStride + (r & 31)] = s[h];
+        }
+      }
+    } else {
+      // this warp's 16 rows summed in a fixed order (the lanes of a quad hold equal values)
+      float v = s[0] + s[1];
+      v += __shfl_xor_sync(0xffffffffu, v, 4);
+      v += __shfl_xor_sync(0xffffffffu, v, 8);
+      v += __shfl_xor_sync(0xffffffffu, v, 16);
+      if (lane == 0) partial_buf[(j * 4 + wq) * kSlots + slot] = v;
+    }
+    ++slot;
+    live &= ~upto;
+    bits &= bits - 1u;
+  }
+  const uint32_t rest = live >> hi;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float x = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < kNb; ++i)
+      if ((rest >> (2 * i)) & 1u) x = fmaxf(x, gm[h][i]);
+    x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+    m[h] = fmaxf(m[h], x);
+  }
+}
+
 // ---- the kernel -------------------------------------------------------------------------------
-// kDebug = false is the product instantiation: no timing-experiment branches, no timestamps in the
-// hot loops (the epilogue is bound by instruction issue slots, every instruction there counts).
+// kWgs = consumer warpgroups (2 or 3): the 64-row query blocks are dealt to them round-robin, so with three
+// resident 128-row tiles (six blocks) three warpgroups take two blocks each.  The per-row arithmetic and its
+// order do not depend on kWgs: every instantiation returns bit-identical scores.
 //
-// kPair = true is the CTA-PAIR EXPERIMENT (launched as clusters of two CTAs): both CTAs of a pair stream the SAME
-// token range, each with its own resident queries (twice the queries per corpus pass); every D tile is fetched from
-// L2 / HBM once — CTA r loads rows [48 r, 48 r + 48) of the tile and TMA-multicasts them into both CTAs' shared
-// memory — and a D stage is recycled when the issuers of BOTH CTAs have committed it (multicast tcgen05.commit).
-// The MMAs stay cta_group::1: this isolates what a pair can save (half the HBM / L2 traffic per query) from what it
-// cannot (the accumulator drain), see DESIGN.md 4.1.
-template <bool kDebug, bool kPair = false>
-__global__ void __launch_bounds__(kScanThreads, 1)
+// kPair = true is the CTA-PAIR pass (launched as clusters of two CTAs): both CTAs of a pair stream the SAME
+// token range, each with its own resident queries (twice the queries per corpus pass); every D tile is fetched
+// from L2 / HBM once — CTA r loads rows [48 r, 48 r + 48) of the tile and TMA-multicasts them into both CTAs'
+// shared memory — and a D stage is recycled when the consumers of BOTH CTAs have released it (remote arrive).
+template <int kWgs, bool kPair = false>
+__global__ void __launch_bounds__(scan_threads(kWgs), 1)
 flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  const int dbg = kDebug ? p.debug_mode : 0;
   using S = ScanSmem;
+  constexpr int kConsumerWarps = kWgs * 4;
+  constexpr int kWarpRed0 = kConsumerWarps;
+  constexpr int kWarpProducer = kConsumerWarps + kRedWarps;
+  constexpr int kBlocksPerWg = (2 * kMtMax + kWgs - 1) / kWgs;   // 64-row query blocks per warpgroup, at most
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment by pointer arithmetic on the __shared__ array (keeps the shared address space
   // visible to the compiler: LDS/STS instead of generic loads/stores)
@@ -281,69 +245,53 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
   const uint32_t pair_rank = kPair ? cluster_ctarank() : 0u;
 
   const uint32_t bar_base = smem_base + S::kOffBars;
-  const uint32_t bar_q_full = bar_base;
-  auto bar_d_full = [&](int s) { return bar_base + 8u * (1 + s); };
-  auto bar_d_empty = [&](int s) { return bar_base + 8u * (1 + kDStages + s); };
-  auto bar_t_full = [&](int s) { return bar_base + 8u * (1 + 2 * kDStages + s); };
-  auto bar_t_empty = [&](int s) { return bar_base + 8u * (1 + 2 * kDStages + kMaxAccStages + s); };
-  auto bar_p_full = [&](int b) { return bar_base + 8u * (1 + 2 * kDStages + 2 * kMaxAccStages + b); };
-  auto bar_p_empty = [&](int b) {
-    return bar_base + 8u * (1 + 2 * kDStages + 2 * kMaxAccStages + 2 + b);
-  };
-  // running-max hand-over between the epilogue warpgroups, one per (query tile, lane quadrant)
-  auto bar_carry = [&](int mt, int quad) {
-    return bar_base + 8u * (1 + 2 * kDStages + 2 * kMaxAccStages + 4 + mt * 4 + quad);
-  };
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem + S::kOffTmemPtr);
+  auto bar_d_full = [&](int s) { return bar_base + 8u * s; };
+  auto bar_d_empty = [&](int s) { return bar_base + 8u * (kDStages + s); };
+  auto bar_p_full = [&](int b) { return bar_base + 8u * (2 * kDStages + b); };
+  auto bar_p_empty = [&](int b) { return bar_base + 8u * (2 * kDStages + 2 + b); };
 
   const int32_t row_begin = p.cta_row_begin[cta];
   const int64_t tile_base = p.cta_tile_base[cta];
   const int n_tiles = static_cast<int>(p.cta_tile_base[cta + 1] - tile_base);
   const int n_mtiles = p.n_mtiles;
-  const uint32_t acc_stages = static_cast<uint32_t>(scan_acc_stages(n_mtiles));   // 2 or 4
-  const uint32_t stage_mask = acc_stages - 1u, stage_shift = (acc_stages == 4u) ? 2u : 1u;
-  const uint32_t acc_col0 = static_cast<uint32_t>(kQCols * n_mtiles);
+  // warpgroups that own at least one 64-row query block (three warpgroups, one resident tile: two); only
+  // these read the D stages and release them
+  const int n_busy_wgs = min(kWgs, 2 * n_mtiles);
 
   // ---- one-time setup --------------------------------------------------------------------------
   if (warp == kWarpProducer && lane == 0) {
     tma_prefetch_desc(&tmap_d);
-    mbar_init(bar_q_full, 4);        // one arrive per query-staging warp
     for (int s = 0; s < kDStages; ++s) {
       mbar_init(bar_d_full(s), 1);
-      mbar_init(bar_d_empty(s), kPair ? 2 * kMmaWarps : kMmaWarps);   // pair: the issuers of both CTAs
-    }
-    for (int s = 0; s < kMaxAccStages; ++s) {
-      mbar_init(bar_t_full(s), 1);
-      mbar_init(bar_t_empty(s), 4);  // one arrive per warp of the draining epilogue warpgroup
+      mbar_init(bar_d_empty(s), (kPair ? 2 : 1) * n_busy_wgs);   // pair: the consumers of both CTAs
     }
     for (int b = 0; b < 2; ++b) {
-      mbar_init(bar_p_full(b), kEpiWarps);   // partial sums of a D tile complete
-      mbar_init(bar_p_empty(b), kRedWarps);  // ... and consumed by the reducer warps
+      mbar_init(bar_p_full(b), kConsumerWarps);   // partial sums of a D tile complete
+      mbar_init(bar_p_empty(b), kRedWarps);       // ... and consumed by the reducer warp
     }
-    for (int i = 0; i < kMtMax * 4; ++i) mbar_init(bar_carry(i >> 2, i & 3), 1);
     mbar_fence_init();
   }
-  if (warp == kWarpMma) {  // (the same warp deallocates at the end)
-    tmem_alloc<512>(smem_base + S::kOffTmemPtr);
-  }
-  if (warp < kWarpProducer) {
-    const int et = threadIdx.x;
-    constexpr int kInitThreads = kEpiThreads + kRedWarps * 32;
+  {
     // top-k lists start empty (key 0 sorts below every real candidate)
     uint64_t* keys = reinterpret_cast<uint64_t*>(smem + S::kOffKeys);
-    for (int i = et; i < kNqMax * kMaxK; i += kInitThreads) keys[i] = 0ull;
-    if (et < kNqMax) {
-      reinterpret_cast<uint64_t*>(smem + S::kOffMinKey)[et] = 0ull;
-      reinterpret_cast<int*>(smem + S::kOffMinPos)[et] = 0;
+    for (int i = threadIdx.x; i < kNqMax * kMaxK; i += blockDim.x) keys[i] = 0ull;
+    if (threadIdx.x < kNqMax) {
+      reinterpret_cast<uint64_t*>(smem + S::kOffMinKey)[threadIdx.x] = 0ull;
+      reinterpret_cast<int*>(smem + S::kOffMinPos)[threadIdx.x] = 0;
     }
-    float* carry0 = reinterpret_cast<float*>(smem + S::kOffCarry);
-    for (int i = et; i < kMtMax * kTileM; i += kInitThreads) carry0[i] = p.init_val;
+    // stage the resident queries in the 128B-swizzled K-major layout the wgmma descriptors describe:
+    // row r, 16-byte chunk c of dims [64 kb, 64 kb + 64) at kb * kQKBlockBytes + r * 128 + ((c ^ (r & 7)) * 16)
+    const uint4* src = p.q_pad + static_cast<int64_t>(pair_rank) * (kMtMax * kTileM * 16);   // pair: CTA r's slot
+    const int n_chunks = n_mtiles * kTileM * 16;
+    for (int i = threadIdx.x; i < n_chunks; i += blockDim.x) {
+      const int r = i >> 4, c = i & 15, kb = c >> 3;
+      *reinterpret_cast<uint4*>(smem + S::kOffQ + kb * kQKBlockBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) =
+          __ldg(src + i);
+    }
+    fence_proxy_async_smem();
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
   if constexpr (kPair) cluster_sync_all();   // the peer's barriers exist before anything is multicast to them
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (warp == kWarpProducer) {
     // ===================== TMA producer =====================
@@ -369,179 +317,69 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
       }
       __syncwarp();
     }
-  } else if (warp >= kWarpMma) {
-    // ===================== MMA issuers =====================
-    // A single thread needs ~31 cycles per tcgen05.mma issue plus ~300 cycles of wait / fence /
-    // commit per accumulator -- more than the 384 cycles the 8 MMAs of an accumulator execute
-    // (profiles/r01_handoff_timeline.md).  So TWO warps issue: issuer i owns the accumulators with
-    // a = i (mod 2) in issue order (a = t * n_mtiles + j), i.e. with two TMEM stages each
-    // issuer is bound to one stage and to the epilogue warpgroup that drains it.  Loops are
-    // warp-uniform; one elected lane (always the same one) issues tcgen05.mma / commit so the
-    // descriptors stay in uniform registers.
-    const uint32_t iw = static_cast<uint32_t>(warp - kWarpMma);
-    constexpr uint32_t idesc = make_idesc_bf16_f32(kTileM, kTileN);
-    mbar_wait(bar_q_full, 0, p.status, kDevTimeoutMma);  // queries are in TMEM
-    tc_fence_after_sync();
-    for (int t = 0; t < n_tiles; ++t) {
-      const int s = t % kDStages;
-      const uint32_t ph = (t / kDStages) & 1;
-      mbar_wait(bar_d_full(s), ph, p.status, kDevTimeoutMma);
-      tc_fence_after_sync();
-      const uint64_t b_desc0 = make_kmajor_sw128_desc(smem_base + S::kOffD + s * kDTileBytes);
-      const uint32_t a_first = static_cast<uint32_t>(t) * n_mtiles;
-      const bool rot = ((n_mtiles & t) & 1) != 0;  // odd tile, odd tile count: rotated order (see epilogue)
-#pragma unroll 1
-      for (uint32_t a = a_first + ((a_first ^ iw) & 1u); a < a_first + n_mtiles; a += 2) {
-        const uint32_t j = a - a_first;
-        const uint32_t mt = rot ? (j == 0 ? static_cast<uint32_t>(n_mtiles) - 1u : j - 1u) : j;
-        const uint32_t as = a & stage_mask, aph = (a >> stage_shift) & 1u;  // TMEM stage / phase
-        if (dbg != 4 && dbg != 5) {  // (modes 4/5: never wait for the epilogue)
-          mbar_wait(bar_t_empty(as), aph ^ 1u, p.status, kDevTimeoutMma);
-          tc_fence_after_sync();
-        }
-        const uint32_t d_tmem = tmem_base + acc_col0 + as * kTileN;
-        const uint32_t a_tmem = tmem_base + mt * kQCols;
-        if (elect_one_sync()) {
-          dbg_stamp<kDebug>(p, cta, a, 0);  // stage free, about to issue
-          if (dbg != 3) {
+  } else if (warp < kConsumerWarps) {
+    // ===================== consumers: wgmma + passage maxima =====================
+    const int wg = warp >> 2;
+    const int wq = warp & 3;           // warp inside the warpgroup: accumulator rows 16 wq .. 16 wq + 15
+    const int n_blocks = 2 * n_mtiles;
+    const float init = p.init_val;
+    float m[kBlocksPerWg][2];
 #pragma unroll
-            for (int k = 0; k < kDim / 16; ++k) {
-              // advance the start-address field (16-byte units) inside the descriptor
-              const uint64_t b_desc =
-                  b_desc0 + static_cast<uint64_t>(((k >> 2) * kDKBlockBytes + (k & 3) * 32) >> 4);
-              tc_mma_ts(d_tmem, a_tmem + k * 8, b_desc, idesc, k > 0 ? 1u : 0u);
+    for (int u = 0; u < kBlocksPerWg; ++u) m[u][0] = m[u][1] = init;
+    float* const lane_part = reinterpret_cast<float*>(smem + S::kOffLanePart);
+    float* const partial = reinterpret_cast<float*>(smem + S::kOffPartial);
+    const uint32_t q_smem = smem_base + S::kOffQ;
+    uint32_t mask_next = (n_tiles > 0) ? __ldg(p.tile_end_mask + tile_base) : 0u;
+    float acc[4 * kNb];
+    for (int t = 0; t < n_tiles; ++t) {
+      const uint32_t mask = mask_next;
+      if (t + 1 < n_tiles) mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
+      const int s = t % kDStages;
+      const int buf = t & 1;
+      const uint32_t d_smem = smem_base + S::kOffD + s * kDTileBytes;
+      if (wg < n_busy_wgs) mbar_wait(bar_d_full(s), (t / kDStages) & 1u, p.status, kDevTimeoutMma);
+      // the reducer must have consumed the partial sums of tile t-2 before this buffer is reused
+      mbar_wait(bar_p_empty(buf), ((static_cast<uint32_t>(t) >> 1) & 1u) ^ 1u, p.status, kDevTimeoutEpilogue);
+      float* lane_part_buf = lane_part + buf * (kFastSlots * kRbMax * kLaneStride);
+      float* partial_buf = partial + buf * (kHbMax * kSlots);
+#pragma unroll
+      for (int u = 0; u < kBlocksPerWg; ++u) {
+        const int j = wg + u * kWgs;
+        if (j < n_blocks) {
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kDim / 16; ++k) {
+            const uint32_t koff = (k & 3) * 32u;   // 16 elements along the 128-byte row
+            const uint64_t a_desc = make_kmajor_sw128_desc(q_smem + (k >> 2) * kQKBlockBytes + j * 64 * 128 + koff);
+            const uint64_t b_desc = make_kmajor_sw128_desc(d_smem + (k >> 2) * kDKBlockBytes + koff);
+            wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          wgmma_wait_all();
+          wgmma_fence_operands(acc);
+          // last block of this warpgroup on the D stage: every wgmma reading it has completed -> release it
+          if (j + kWgs >= n_blocks) {
+            __syncwarp();
+            if (wq == 0 && lane == 0) {
+              if constexpr (kPair) {
+                mbar_arrive_cluster(bar_d_empty(s), 0);
+                mbar_arrive_cluster(bar_d_empty(s), 1);
+              } else {
+                mbar_arrive(bar_d_empty(s));
+              }
             }
           }
-          if (dbg != 5) tc_commit(bar_t_full(as));  // accumulator complete -> epilogue
-          dbg_stamp<kDebug>(p, cta, a, 1);  // MMAs + commit issued
-        }
-        __syncwarp();
-      }
-      // this issuer's MMAs on the D stage are complete -> producer (both issuers must arrive)
-      if (elect_one_sync()) {
-        if constexpr (kPair) tc_commit_multicast(bar_d_empty(s), 3);
-        else tc_commit(bar_d_empty(s));
-      }
-      __syncwarp();
-    }
-  } else if (warp < kEpiWarps) {
-    // ===================== epilogue (TMEM drain) =====================
-    // Accumulators are numbered in MMA issue order, a = t * n_mtiles + j; warpgroup g drains the
-    // accumulators with (a & 1) == g, so the two warpgroups alternate strictly.  The running max of
-    // the passage straddling D tiles is per (query tile, row) and must follow the query tile from D
-    // tile to D tile.  With an even tile count query tile mt = j always meets the same warpgroup.
-    // With an odd count the issue order of odd D tiles is rotated (j = 0 is the LAST query tile, j > 0
-    // is tile j - 1): query tiles 0 .. n_mtiles-2 then keep their warpgroup and only the last one
-    // changes hands every D tile (shared memory + mbarrier), instead of all of them.
-    const int wg = warp >> 2;         // epilogue warp 0..7 -> warpgroup 0/1
-    const int quad = warp & 3;        // TMEM lane quadrant this warp may access
-    const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
-    float* partial = reinterpret_cast<float*>(smem + S::kOffPartial);
-    float* lane_part = reinterpret_cast<float*>(smem + S::kOffLanePart) + lane;
-    float* carry = reinterpret_cast<float*>(smem + S::kOffCarry) + quad * 32 + lane;
-    const bool carry_crosses = (n_mtiles & 1) != 0;  // odd: (t, mt) and (t+1, mt) are drained by different warpgroups
-    const float init = p.init_val;
-
-    // ---- stage the resident queries into tensor memory (warpgroup 0: one warp per lane quadrant).
-    // Row r of query tile mt lives in TMEM lane r, columns [mt*64, mt*64+64): column c holds the
-    // bf16 pair (k = 2c, 2c+1), i.e. the row's 256 bytes verbatim.
-    if (wg == 0) {
-      for (int mt = 0; mt < n_mtiles; ++mt) {
-        const uint4* src = p.q_pad + (static_cast<int64_t>(pair_rank) * (kMtMax * kTileM) +   // pair: CTA r's staging slot
-                                      static_cast<int64_t>(mt) * kTileM + quad * 32 + lane) * 16;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t w[32];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const uint4 x = __ldg(src + h * 8 + i);
-            w[4 * i] = x.x;
-            w[4 * i + 1] = x.y;
-            w[4 * i + 2] = x.z;
-            w[4 * i + 3] = x.w;
-          }
-          FLMR_TMEM_ST32(tmem_base + lane_base + mt * kQCols + h * 32, w);
+          fold_accumulator(acc, mask, m[u], init, lane_part_buf, partial_buf, j, wq, lane);
         }
       }
-      tmem_wait_st();
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_q_full);
-    }
-
-    const int n_tiles_epi = (dbg == 4 || dbg == 5) ? 0 : n_tiles;  // modes 4/5: epilogue idle
-    uint32_t mask_next = (n_tiles_epi > 0) ? __ldg(p.tile_end_mask + tile_base) : 0u;
-    for (int t = 0; t < n_tiles_epi; ++t) {
-      const uint32_t mask = (dbg == 2) ? 0u : mask_next;
-      if (t + 1 < n_tiles_epi) mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
-      const int buf = t & 1;
-      // the reducers must have consumed the partial sums of tile t-2 before this buffer is reused
-      mbar_wait(bar_p_empty(buf), ((static_cast<uint32_t>(t) >> 1) & 1u) ^ 1u, p.status,
-                kDevTimeoutEpilogue);
-      const uint32_t a_first = static_cast<uint32_t>(t) * n_mtiles;
-      const bool rot = ((n_mtiles & t) & 1) != 0;
-#pragma unroll 1
-      for (uint32_t a = a_first + ((a_first ^ static_cast<uint32_t>(wg)) & 1u); a < a_first + n_mtiles;
-           a += 2) {
-        const int j = static_cast<int>(a - a_first);
-        const int mt = rot ? (j == 0 ? n_mtiles - 1 : j - 1) : j;
-        const bool crosses = carry_crosses && mt == n_mtiles - 1;
-        const uint32_t as = a & stage_mask, aph = (a >> stage_shift) & 1u;  // TMEM stage / phase
-        // running max handed over by whoever drained (t-1, mt): with an odd number of query tiles
-        // that is the other warpgroup (mbarrier arrive/wait = release/acquire); with an even number
-        // it is this very warp, and program order suffices
-        if (crosses && t > 0)
-          mbar_wait(bar_carry(mt, quad), static_cast<uint32_t>(t - 1) & 1u, p.status,
-                    kDevTimeoutEpilogue);
-        float m = carry[mt * kTileM];
-        if (quad == 0 && lane == 0) dbg_stamp<kDebug>(p, cta, a, 2);               // epilogue ready to wait
-        mbar_wait(bar_t_full(as), aph, p.status, kDevTimeoutEpilogue);
-        tc_fence_after_sync();
-        if (quad == 0 && lane == 0) dbg_stamp<kDebug>(p, cta, a, 3);               // accumulator visible
-        if (dbg == 1 || dbg == 3) {  // timing experiment: release unread
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_t_empty(as));
-        } else {
-          const uint32_t taddr = tmem_base + lane_base + acc_col0 + as * kTileN;
-          uint32_t v[kChunks][32];
-          float* partial_rb = partial + (buf * kRbMax + mt * 4 + quad) * kSlots;
-          float* lane_part_rb = lane_part + ((buf * kFastSlots) * kRbMax + mt * 4 + quad) * kLaneStride;
-          int slot = 0;
-          // chunk 0 first; the remaining chunks stream in while chunk 0 is folded
-          FLMR_TMEM_LD32(v[0], taddr);
-          FLMR_TMEM_WAIT_LD32(v[0]);
-#pragma unroll
-          for (int c = 1; c < kChunks; ++c) FLMR_TMEM_LD32(v[c], taddr + 32 * c);
-          process_chunk(v[0], mask & 0xFFu, m, init, partial_rb, lane_part_rb, slot, lane);
-#pragma unroll
-          for (int c = 1; c < kChunks; ++c) FLMR_TMEM_WAIT_LD32(v[c]);
-          // every column is in registers: hand the TMEM stage back to the MMA warps
-          if (quad == 0 && lane == 0) dbg_stamp<kDebug>(p, cta, a, 4);             // TMEM read done
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_t_empty(as));
-          if (quad == 0 && lane == 0) dbg_stamp<kDebug>(p, cta, a, 5);             // stage handed back
-#pragma unroll
-          for (int c = 1; c < kChunks; ++c)
-            process_chunk(v[c], (mask >> (8 * c)) & 0xFFu, m, init, partial_rb, lane_part_rb, slot, lane);
-        }
-        if (quad == 0 && lane == 0) dbg_stamp<kDebug>(p, cta, a, 6);               // chunk processing done
-        carry[mt * kTileM] = m;
-        if (crosses) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_carry(mt, quad));
-        }
-      }
-      // this warp's per-lane maxima / partial sums of tile t are written: order every lane's stores
+      // this warp's row maxima / partial sums of tile t are written: order every lane's stores
       // before lane 0's arrive (release); the reducer's wait is the matching acquire
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_p_full(buf));
     }
-    tc_fence_before_sync();
   } else {
-    // ===================== reducers: score finalisation + per-CTA top-k =====================
-    // Per D tile and per (query, passage ending in the tile): sum the row-block partials in fixed
+    // ===================== reducer: score finalisation + per-CTA top-k =====================
+    // Per D tile and per (query, passage ending in the tile): sum the row partials in fixed
     // order (deterministic), add/store partial scores if requested, offer to the top-k list.
     const int rw = warp - kWarpRed0;  // reducer 0..kRedWarps-1 owns queries b = rw (mod kRedWarps)
     const int q_off = static_cast<int>(pair_rank) * p.nq_pass;   // pair: CTA r's queries follow CTA 0's in every per-query array
@@ -549,7 +387,7 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
     uint64_t* keys = reinterpret_cast<uint64_t*>(smem + S::kOffKeys);
     uint64_t* minkey_s = reinterpret_cast<uint64_t*>(smem + S::kOffMinKey);
     int* minpos_s = reinterpret_cast<int*>(smem + S::kOffMinPos);
-    const int n_tiles_red = (dbg == 4 || dbg == 5) ? 0 : n_tiles;
+    const int n_tiles_red = n_tiles;
     uint32_t mask_next = 0;
     int32_t fpid_next = 0;
     if (n_tiles_red > 0) {
@@ -623,9 +461,9 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
               for (int r = 0; r < p.rbq; ++r) sc += lp[r * kLaneStride];
               sc = warp_sum(sc);
             } else {
-              const float* pr = partial + (buf * kRbMax + b * p.rbq) * kSlots + slot;
+              const float* pr = partial + (buf * kHbMax + 2 * b * p.rbq) * kSlots + slot;
 #pragma unroll 2
-              for (int r = 0; r < p.rbq; ++r) sc += pr[r * kSlots];
+              for (int r = 0; r < 2 * p.rbq; ++r) sc += pr[r * kSlots];
             }
             const int64_t gi = static_cast<int64_t>(q_off + b) * p.n_passages + pid;
             if (p.acc_in) sc += __ldg(p.acc_in + gi);
@@ -661,12 +499,7 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
   }
 
   // ---- teardown -----------------------------------------------------------------------------------
-  __syncthreads();
   if constexpr (kPair) cluster_sync_all();   // no CTA leaves while its peer may still signal its barriers
-  if (warp == kWarpMma) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
-  }
 }
 
 }  // namespace flmr

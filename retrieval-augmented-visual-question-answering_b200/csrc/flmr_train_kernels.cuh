@@ -8,7 +8,7 @@
 //     dD[p, arg[b, p, i], :] += g[b, p] * Q[b, i, :]                       (scatter, flmr_bwd_dd_kernel)
 // Shapes are training-sized (tens of documents, hundreds of tokens): a register-tiled SIMT fp32
 // contraction over bf16 operands is within a few percent of what these sizes allow, so the kernels
-// stay simple; the corpus-sized forward is the tcgen05 scan kernel.
+// stay simple; the corpus-sized forward is the wgmma scan kernel.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -131,8 +131,8 @@ flmr_argmax_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __r
 }
 
 // ---- the same contract on the warp-level tensor-core path (mma.sync m16n8k16, bf16 -> fp32) -------------
-// Training shapes are far too small to amortise the tcgen05 machinery of the scan kernel (TMEM allocation,
-// TMA descriptors, a persistent grid), but the legacy warp MMA is still several times the SIMT FMA rate.
+// Training shapes are far too small to amortise the machinery of the scan kernel (mbarrier ring, TMA
+// descriptors, a persistent grid), but the legacy warp MMA is still several times the SIMT FMA rate.
 // CTA = 4 warps x 16 query rows; the query tile's A fragments are loaded once (ldmatrix) and stay in
 // registers for every 64-token chunk of the document.
 constexpr int kMmaThreads = 128;

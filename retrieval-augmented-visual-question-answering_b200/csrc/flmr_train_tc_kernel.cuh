@@ -1,10 +1,10 @@
-// flmr_train_tc_kernel.cuh — the training / re-scoring forward on the tcgen05 tensor cores:
+// flmr_train_tc_kernel.cuh — the training / re-scoring forward on the Hopper tensor cores (wgmma):
 //
 //   arg[b, p, i]    = argmax_{j : mask[p, j]} <Q[b, i, :], D[p, j, :]>        (lowest j on ties, -1 if none)
 //   rowmax[b, p, i] = that maximum;   sum_i rowmax = MaxSim score[b, p]
 //
 // Same contract as flmr_argmax_mma_kernel (flmr_train_kernels.cuh), which stays the path for small batches;
-// this one is for batches whose contraction is worth a TMA/TMEM pipeline — the global in-batch-negatives matrix
+// this one is for batches whose contraction is worth a TMA/wgmma pipeline — the global in-batch-negatives matrix
 // of a training step with cross-rank negatives (CB/modeling/colbert.py:64-113, 115-163: 8 queries x 832 rows
 // against 128 documents x 512 tokens per rank) or an exhaustive evaluation through ColBERT.score
 // (src/executors/FLMR_executor.py:826-833).
@@ -17,33 +17,25 @@
 //      After this no mask exists any more: the epilogue below has no per-element mask logic.
 //   2. flmr_argmax_tc_kernel: CTA = (query b, 128-row tile of its tokens, a range of documents).  The query tile
 //      is the stationary A operand (TMA -> shared memory once); the CTA streams its documents in chunks of 128
-//      tokens through a 4-stage ring.  Stage s = a 32 KB shared-memory chunk AND a 128-column TMEM accumulator:
+//      tokens through a kTcStages-deep ring of 32 KB shared-memory stages:
 //        warp 8 (producer): TMA, two 128B-swizzled boxes per chunk
-//        warp 9 (issuer)  : 8 x tcgen05.mma (M = 128, N = 128, K = 16), tcgen05.commit -> `done[s]`
-//        warps 0-7        : two epilogue warpgroups, documents alternate between them (a document's chunks stay
-//                           with one warpgroup, so its running (max, index) never changes hands).  TMEM lane =
-//                           query row: per 32 columns a compare-select TREE (strict '>' keeps the lower index on
-//                           ties) — 31 independent (FSETP, FSEL, SEL) triples of depth 5 instead of a 32-long
-//                           dependent chain, which with one warp per scheduler ran at a fifth of the MMA rate —
-//                           then one compare against the row's running best; one coalesced store per output at
-//                           the document's end.
-//      Per chunk the issuer commits twice: `free[s]` returns the shared-memory chunk to the producer, `done[g][s]`
-//      hands the accumulator to the warpgroup g that owns the document (one barrier per warpgroup and stage, so
-//      every waiter observes every phase of its barrier); `t_empty[s]` (one arrive per warp of the owner) hands
-//      the accumulator back to the issuer.
+//        warps 0-7        : two consumer warpgroups; warpgroup g owns query rows [64 g, 64 g + 64) of the tile and
+//                           issues 8 x wgmma.m64n128k16 per chunk into registers, then releases the stage.  A
+//                           thread holds two rows and 32 columns per row: a compare-select TREE over its columns
+//                           (strict '>' keeps the lower index on ties), two shuffles inside the lane quad, one
+//                           compare against the row's running best; one store per output at the document's end.
 #pragma once
 #include "flmr_device.cuh"
 
 namespace flmr {
 
 constexpr int kTcTile = 128;                 // query rows per CTA and document tokens per chunk
-constexpr int kTcStages = 4;                 // smem chunks == TMEM accumulator stages (4 x 128 columns)
+constexpr int kTcStages = 4;                 // shared-memory chunks of the document ring
 constexpr int kTcChunkBytes = kTcTile * 128 * 2;   // 32 KiB: [2 k-blocks][128 rows][64 bf16]
 constexpr int kTcKBlockBytes = kTcTile * 128;      // 16 KiB
-constexpr int kTcEpiWarps = 8;               // two epilogue warpgroups; warpgroup g owns the CTA's documents of parity g
-constexpr int kTcWarpProducer = kTcEpiWarps;
-constexpr int kTcWarpMma = kTcEpiWarps + 1;
-constexpr int kTcThreads = (kTcEpiWarps + 2) * 32;
+constexpr int kTcWgs = 2;                    // consumer warpgroups, 64 query rows each
+constexpr int kTcWarpProducer = kTcWgs * 4;
+constexpr int kTcThreads = (kTcWarpProducer + 1) * 32;
 constexpr int kTcSmemBytes = (1 + kTcStages) * kTcChunkBytes + 512 + 1024;   // A tile + ring + barriers, lengths + align
 
 // grid = total documents; one 256-thread block packs one document.
@@ -95,6 +87,14 @@ struct ArgmaxTcParams {
   int* status;                 // watchdog word (may be null)
 };
 
+// (value, column) pair that wins: the larger value, the lower column on equal values.
+__device__ __forceinline__ void argmax_take(float& v, int& c, float v2, int c2) {
+  if (v2 > v || (v2 == v && c2 < c)) {
+    v = v2;
+    c = c2;
+  }
+}
+
 __global__ void __launch_bounds__(kTcThreads, 1)
 flmr_argmax_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
                       const ArgmaxTcParams p) {
@@ -106,15 +106,9 @@ flmr_argmax_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   const uint32_t bar_base = smem_base + (1 + kTcStages) * kTcChunkBytes;
   const uint32_t bar_q = bar_base;
   auto bar_full = [&](int s) { return bar_base + 8u * (1 + s); };
-  auto bar_free = [&](int s) { return bar_base + 8u * (1 + kTcStages + s); };          // MMA -> producer
-  auto bar_tempty = [&](int s) { return bar_base + 8u * (1 + 2 * kTcStages + s); };    // owner warpgroup -> MMA
-  // accumulator ready, one barrier per (warpgroup, stage): a parity wait only tells CONSECUTIVE phases apart, and
-  // a warpgroup sees only its own documents' chunks, so it needs a barrier whose every phase it observes
-  auto bar_done = [&](int g, int s) { return bar_base + 8u * (1 + 3 * kTcStages + g * kTcStages + s); };
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem + (1 + kTcStages) * kTcChunkBytes + 8 * (1 + 5 * kTcStages));
-  // lengths of this CTA's documents, read from global memory ONCE (every role walks the same document list; a
-  // global load per document and role put ~500 cycles of latency in front of each document's first chunk)
-  int32_t* s_len = reinterpret_cast<int32_t*>(smem + (1 + kTcStages) * kTcChunkBytes + 8 * (1 + 5 * kTcStages) + 16);
+  auto bar_free = [&](int s) { return bar_base + 8u * (1 + kTcStages + s); };          // consumers -> producer
+  // lengths of this CTA's documents, read from global memory ONCE (every role walks the same document list)
+  int32_t* s_len = reinterpret_cast<int32_t*>(smem + (1 + kTcStages) * kTcChunkBytes + 8 * (1 + 2 * kTcStages));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.z, mt = blockIdx.y;
@@ -127,20 +121,13 @@ flmr_argmax_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     mbar_init(bar_q, 1);
     for (int s = 0; s < kTcStages; ++s) {
       mbar_init(bar_full(s), 1);
-      mbar_init(bar_free(s), 1);
-      mbar_init(bar_done(0, s), 1);
-      mbar_init(bar_done(1, s), 1);
-      mbar_init(bar_tempty(s), 4);
+      mbar_init(bar_free(s), kTcWgs);
     }
     mbar_fence_init();
   }
-  if (warp == kTcWarpMma) tmem_alloc<512>(smem_u32(const_cast<uint32_t*>(tmem_ptr_smem)));
   if (warp == 0 && p_begin + lane < p_end)
     s_len[lane] = __ldg(p.doc_len + static_cast<int64_t>(b) * p.stride_b + p_begin + lane);   // docs_per_cta <= 32
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (warp == kTcWarpProducer) {
     // ===================== TMA producer =====================
@@ -169,79 +156,47 @@ flmr_argmax_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         __syncwarp();
       }
     }
-  } else if (warp == kTcWarpMma) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = make_idesc_bf16_f32(kTcTile, kTcTile);
-    mbar_wait(bar_q, 0, p.status, kDevTimeoutMma);
-    tc_fence_after_sync();
-    const uint64_t a_desc0 = make_kmajor_sw128_desc(a_smem);
-    uint32_t n = 0;
-    for (int pl = p_begin; pl < p_end; ++pl) {
-      const int nch = (s_len[pl - p_begin] + kTcTile - 1) / kTcTile;
-      for (int c = 0; c < nch; ++c, ++n) {
-        const int s = n % kTcStages;
-        const uint32_t use = n / kTcStages;
-        mbar_wait(bar_full(s), use & 1u, p.status, kDevTimeoutMma);
-        if (use > 0) mbar_wait(bar_tempty(s), (use - 1) & 1u, p.status, kDevTimeoutMma);
-        tc_fence_after_sync();
-        const uint64_t b_desc0 = make_kmajor_sw128_desc(d_smem0 + s * kTcChunkBytes);
-        if (elect_one_sync()) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const uint64_t koff = static_cast<uint64_t>(((k >> 2) * kTcKBlockBytes + (k & 3) * 32) >> 4);
-            tc_mma_ss(tmem_base + s * kTcTile, a_desc0 + koff, b_desc0 + koff, idesc, k > 0 ? 1u : 0u);
-          }
-          tc_commit(bar_free(s));                               // shared-memory chunk consumed -> producer
-          tc_commit(bar_done((pl - p_begin) & 1, s));           // accumulator complete -> the document's warpgroup
-        }
-        __syncwarp();
-      }
-    }
   } else {
-    // ===================== epilogue: running (max, index) per query row =====================
-    const int wg = warp >> 2, quad = warp & 3;
-    const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
-    const int i = mt * kTcTile + quad * 32 + lane;               // this thread's query token
-    const bool live = i < p.nq;
+    // ===================== consumers: wgmma + running (max, index) per query row =====================
+    const int wg = warp >> 2, wq = warp & 3;
+    const int i0 = mt * kTcTile + wg * 64 + wq * 16 + (lane >> 2);   // this thread's query rows: i0 and i0 + 8
+    const int cq = 2 * (lane & 3);                                   // its first column inside an 8-column block
+    mbar_wait(bar_q, 0, p.status, kDevTimeoutMma);
+    float acc[64];
     uint32_t n = 0;
-    uint32_t own_parity = 0;                                     // bit s: parity of this warpgroup's next use of stage s
     for (int pl = p_begin; pl < p_end; ++pl) {
       const int64_t pg = static_cast<int64_t>(b) * p.stride_b + pl;
-      const int len = s_len[pl - p_begin];
-      const int nch = (len + kTcTile - 1) / kTcTile;
-      if (((pl - p_begin) & 1) != wg) {
-        n += nch;                                                // the other warpgroup's document
-        continue;
-      }
-      float best = -INFINITY;
-      int barg = -1;
+      const int nch = (s_len[pl - p_begin] + kTcTile - 1) / kTcTile;
+      float best[2] = {-INFINITY, -INFINITY};
+      int barg[2] = {-1, -1};
       for (int c = 0; c < nch; ++c, ++n) {
         const int s = n % kTcStages;
-        mbar_wait(bar_done(wg, s), (own_parity >> s) & 1u, p.status, kDevTimeoutEpilogue);
-        own_parity ^= 1u << s;
-        tc_fence_after_sync();
-        const uint32_t taddr = tmem_base + lane_base + s * kTcTile;
-        uint32_t v[2][32];
-        FLMR_TMEM_LD32(v[0], taddr);
+        mbar_wait(bar_full(s), (n / kTcStages) & 1u, p.status, kDevTimeoutMma);
+        const uint32_t d_smem = d_smem0 + s * kTcChunkBytes;
+        wgmma_fence();
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          FLMR_TMEM_WAIT_LD32(v[q & 1]);
-          if (q < 3) {
-            FLMR_TMEM_LD32(v[(q + 1) & 1], taddr + 32 * (q + 1));
-          } else {                                               // every column is in registers: stage back to the issuer
-            tc_fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_tempty(s));
-          }
-          // compare-select tree over the 32 columns: (value, column) pairs, the lower column wins ties
+        for (int k = 0; k < 8; ++k) {
+          const uint32_t koff = (k >> 2) * kTcKBlockBytes + (k & 3) * 32;
+          wgmma_m64n128k16(acc, make_kmajor_sw128_desc(a_smem + wg * 64 * 128 + koff),
+                           make_kmajor_sw128_desc(d_smem + koff), k > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        wgmma_fence_operands(acc);
+        __syncwarp();
+        if (wq == 0 && lane == 0) mbar_arrive(bar_free(s));         // every wgmma of this warpgroup read the chunk
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          // compare-select tree over this thread's 32 columns of row h (leaves in column order, so the
+          // left operand always has the lower column and strict '>' keeps it on ties)
           float tv[16];
           int ti[16];
 #pragma unroll
           for (int e = 0; e < 16; ++e) {
-            const float x0 = __uint_as_float(v[q & 1][2 * e]), x1 = __uint_as_float(v[q & 1][2 * e + 1]);
+            const float x0 = acc[4 * e + 2 * h], x1 = acc[4 * e + 2 * h + 1];
             const bool g1 = x1 > x0;
             tv[e] = g1 ? x1 : x0;
-            ti[e] = g1 ? 2 * e + 1 : 2 * e;
+            ti[e] = 8 * e + cq + (g1 ? 1 : 0);
           }
 #pragma unroll
           for (int w = 8; w >= 1; w >>= 1) {
@@ -252,24 +207,29 @@ flmr_argmax_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
               ti[e] = g1 ? ti[2 * e + 1] : ti[2 * e];
             }
           }
-          if (tv[0] > best) {                                    // strict: earlier chunks / columns keep ties
-            best = tv[0];
-            barg = c * kTcTile + q * 32 + ti[0];
+          float v = tv[0];
+          int col = ti[0];
+#pragma unroll
+          for (int off = 1; off <= 2; off <<= 1)
+            argmax_take(v, col, __shfl_xor_sync(0xffffffffu, v, off), __shfl_xor_sync(0xffffffffu, col, off));
+          if (v > best[h]) {                                     // strict: earlier chunks keep ties
+            best[h] = v;
+            barg[h] = c * kTcTile + col;
           }
         }
       }
-      if (live) {
-        const int64_t o = (static_cast<int64_t>(b) * p.n_per + pl) * p.nq + i;
-        p.arg[o] = barg >= 0 ? __ldg(p.idx_map + pg * p.nd_c + barg) : -1;
-        if (p.rowmax) p.rowmax[o] = best;
+      if ((lane & 3) == 0) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int i = i0 + 8 * h;
+          if (i < p.nq) {
+            const int64_t o = (static_cast<int64_t>(b) * p.n_per + pl) * p.nq + i;
+            p.arg[o] = barg[h] >= 0 ? __ldg(p.idx_map + pg * p.nd_c + barg[h]) : -1;
+            if (p.rowmax) p.rowmax[o] = best[h];
+          }
+        }
       }
     }
-    tc_fence_before_sync();
-  }
-  __syncthreads();
-  if (warp == kTcWarpMma) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 

@@ -12,7 +12,7 @@ summed over query tokens are the all-pairs scores ``[B, n]`` (the aligned ``Q_du
 builds with ``repeat_interleave`` is a gather of that matrix, the in-batch-negatives matrix IS that
 matrix), and the winners (4 bytes per pair) are what the backward needs.  Large inputs (exhaustive
 evaluation through ``score``): the ``n`` padded documents are packed into a temporary FlatCorpus and
-scored by one launch of the tcgen05 scan kernel; the backward then recomputes the winners.  Either way the
+scored by one launch of the wgmma scan kernel; the backward then recomputes the winners.  Either way the
 ``[n, Nd, Nq]`` score tensor the reference materialises (218 MB per rank at C4, SURVEY 8a) never exists.
 
 Backward: ``flmr_maxsim_backward`` routes the gradient through the winners (``dQ_i += g * D_argmax``
@@ -32,7 +32,7 @@ from .maxsim import (ib_loss_head, maxsim_argmax, maxsim_argmax_grouped, maxsim_
 
 
 # The forward is ONE arg-max launch (scores = row maxima summed) that also saves the winners for the backward —
-# a warp-MMA kernel for small batches, the tcgen05 kernel from 16M (query row, token) pairs up (chosen inside
+# a warp-MMA kernel for small batches, the wgmma kernel from 16M (query row, token) pairs up (chosen inside
 # flmr_maxsim_argmax) — as long as the winners + maxima ([B, n, Nq] x 8 bytes) stay below this budget.  Beyond
 # it (an exhaustive evaluation of one query against a whole collection through `score`) the n padded documents
 # are packed into a temporary FlatCorpus and scored by the scan kernel, which keeps nothing per pair; the

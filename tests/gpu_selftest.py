@@ -81,7 +81,7 @@ def _run_parity(n_passages, nd, n_queries, nq, k, ragged=False, relu=False, simt
     s_tc = R.maxsim_scores(corpus, Qt, relu=relu)
     torch.cuda.synchronize()
     s_tc = s_tc.cpu().numpy()
-    r = _report("tcgen05 scores vs oracle", s_tc, ref)
+    r = _report("wgmma scores vs oracle", s_tc, ref)
     ok &= r < tol
     if r >= tol:
         bad = np.argwhere(np.abs(s_tc - ref) / np.maximum(np.abs(ref), 1e-6) > tol)
@@ -161,7 +161,7 @@ def case_perf():
     s_simt = R.debug_scores_simt(corpus, Q[:1])
     torch.cuda.synchronize()
     rel = ((s_all - s_simt).abs() / s_simt.abs().clamp_min(1e-6)).max().item()
-    print("  full-size tcgen05 vs simt max_rel = %.3e" % rel)
+    print("  full-size wgmma vs simt max_rel = %.3e" % rel)
     ts, tp = R.maxsim_topk(corpus, Q[:1], 5)
     rs, rp = torch.topk(s_all, 5, dim=1)
     print("  fused topk ids == topk(all scores): %s" % bool((tp == rp).all().item()))

@@ -53,13 +53,13 @@ def test_ctypes_prototypes_match_the_header():
         assert n_list.count(",") + 1 == protos[name], "INTEGRATION.md stub of %s is out of date" % name
 
 
-def test_library_is_sm100a_tcgen05_build():
+def test_library_is_sm90a_wgmma_build():
     import subprocess
     from ravqa_b200 import build
     sass = subprocess.run(["cuobjdump", "-sass", build.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):
-        assert mnemonic in sass, mnemonic + " missing: the hot kernel is not tcgen05/TMA code"
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA.64x96x16.F32.BF16", "HGMMA.64x128x16.F32.BF16", "UTMALDG.2D.MULTICAST", "SYNCS"):
+        assert mnemonic in sass, mnemonic + " missing: the hot kernels are not wgmma/TMA/mbarrier code"
 
 
 def test_argument_validation_without_gpu():
@@ -130,6 +130,12 @@ def test_partition_invariants(seed, n, lo, hi, ctas):
     assert np.all(np.diff(rb) <= share + plen.max() + 1)
 
 
+# residency of one scan pass (flmr_scan_kernel.cuh): MT_MAX 128-row query tiles = RB_MAX 32-row blocks
+MT_MAX = 3
+RB_MAX = 4 * MT_MAX
+ROWS_MAX = 32 * RB_MAX
+
+
 def _plan(n_queries, nq, allow_pair=0):
     L = _cabi.lib()
     n = C.c_int(0)
@@ -141,10 +147,10 @@ def _plan(n_queries, nq, allow_pair=0):
 
 
 @pytest.mark.parametrize("n_queries,nq", [(1, 32), (16, 32), (64, 32), (21, 32), (16, 320), (5, 320), (3, 45),
-                                           (7, 832), (1, 832), (3, 1500), (2, 1280), (40, 641), (0, 64), (13, 640)])
+                                           (7, 832), (1, 832), (3, 1500), (2, 1280), (40, 641), (0, 64), (13, 640), (13, 384), (5, 385)])
 def test_pass_plan_invariants(n_queries, nq):
-    """flmr_debug_plan_passes: every (query, row) is resident in exactly one pass, never more than 640 rows
-    or 20 queries per pass, partial scores are read only after they were written, each query is finalised
+    """flmr_debug_plan_passes: every (query, row) is resident in exactly one pass, never more than ROWS_MAX rows
+    or RB_MAX queries per pass, partial scores are read only after they were written, each query is finalised
     exactly once and last, and the number of passes is the minimum this scheme allows."""
     plan = _plan(n_queries, nq)
     ACC_IN, ACC_OUT, FINAL = 1, 2, 4
@@ -152,8 +158,8 @@ def test_pass_plan_invariants(n_queries, nq):
     touched = np.zeros(n_queries, dtype=bool)
     finalised = np.zeros(n_queries, dtype=bool)
     for q_first, n_q, row0, rows, rbq, n_mtiles, flags, acc_first in plan:
-        assert 1 <= n_q <= 20 and rbq == (rows + 31) // 32 and n_q * rbq <= 20
-        assert n_mtiles == (n_q * rbq * 32 + 127) // 128 and 1 <= n_mtiles <= 5
+        assert 1 <= n_q <= RB_MAX and rbq == (rows + 31) // 32 and n_q * rbq <= RB_MAX
+        assert n_mtiles == (n_q * rbq * 32 + 127) // 128 and 1 <= n_mtiles <= MT_MAX
         assert 0 <= row0 and row0 + rows <= nq and row0 % 32 == 0
         qs = slice(q_first, q_first + n_q)
         assert not finalised[qs].any()                        # nothing after the final pass of a query
@@ -167,15 +173,15 @@ def test_pass_plan_invariants(n_queries, nq):
         assert acc_first == q_first                           # partial-score rows are indexed by query
     assert (covered == 1).all() and finalised.all()
     rbq_total = (nq + 31) // 32
-    if rbq_total <= 20:
-        per_pass = min(20, 20 // rbq_total)
+    if rbq_total <= RB_MAX:
+        per_pass = min(RB_MAX, RB_MAX // rbq_total)
         assert len(plan) == -(-n_queries // per_pass)
         sizes = [p[1] for p in plan]
         assert not sizes or max(sizes) - min(sizes) <= per_pass - 1 and max(sizes) == -(-n_queries // len(plan))
     else:
-        n_slices = -(-nq // 640)
-        tail_rbq = (nq - (n_slices - 1) * 640 + 31) // 32
-        group = max(1, min(20, 20 // tail_rbq, n_queries))
+        n_slices = -(-nq // ROWS_MAX)
+        tail_rbq = (nq - (n_slices - 1) * ROWS_MAX + 31) // 32
+        group = max(1, min(RB_MAX, RB_MAX // tail_rbq, n_queries))
         assert len(plan) == n_queries * (n_slices - 1) + -(-n_queries // group)
 
 
@@ -189,7 +195,7 @@ def test_pass_plan_random_shapes():
         covered = np.zeros((n_queries, nq), dtype=np.int32)
         final = np.zeros(n_queries, dtype=np.int32)
         for q_first, n_q, row0, rows, rbq, n_mtiles, flags, _acc in plan:
-            assert n_q * rbq <= 20 and n_q <= 20 and rows <= 640
+            assert n_q * rbq <= RB_MAX and n_q <= RB_MAX and rows <= ROWS_MAX
             covered[q_first:q_first + n_q, row0:row0 + rows] += 1
             if flags & 4:
                 final[q_first:q_first + n_q] += 1
@@ -201,7 +207,7 @@ def test_pass_plan_random_shapes():
                                            (8, 128), (3, 45), (0, 64), (44, 200)])
 def test_pass_plan_with_cta_pairs(n_queries, nq):
     """With CTA-pair passes allowed: pair passes (flag 8) cover a PREFIX of the queries, two blocks of n_q queries
-    each (CTA r of every pair the r-th block), each CTA with at least four 128-row tiles when whole queries are
+    each (CTA r of every pair the r-th block), each CTA with all three 128-row tiles when whole queries are
     resident; the rest of the batch is planned exactly like a batch of that size without pairs; every (query, row)
     is still resident exactly once, partial scores are read only after they were written, and within one group of
     row-sliced queries no two queries share a partial-score row."""
@@ -215,14 +221,14 @@ def test_pass_plan_with_cta_pairs(n_queries, nq):
     for q_first, n_q, row0, rows, rbq, n_mtiles, flags, acc_first in plan:
         pair = bool(flags & PAIR)
         span = 2 * n_q if pair else n_q
-        assert 1 <= n_q <= 20 and rbq == (rows + 31) // 32 and n_q * rbq <= 20
-        assert n_mtiles == (n_q * rbq * 32 + 127) // 128 and 1 <= n_mtiles <= 5
+        assert 1 <= n_q <= RB_MAX and rbq == (rows + 31) // 32 and n_q * rbq <= RB_MAX
+        assert n_mtiles == (n_q * rbq * 32 + 127) // 128 and 1 <= n_mtiles <= MT_MAX
         assert 0 <= row0 and row0 + rows <= nq and row0 % 32 == 0 and q_first + span <= n_queries
         if pair:
             assert not seen_single                            # pair passes first
             n_pair_q = max(n_pair_q, q_first + span)
-            if nq <= 640:
-                assert n_mtiles >= 4                          # pairs only where a CTA is tensor-bound on its own
+            if nq <= ROWS_MAX:
+                assert n_mtiles == MT_MAX                     # pairs only where a CTA is tensor-bound on its own
         else:
             seen_single = True
             assert q_first >= n_pair_q
@@ -251,10 +257,10 @@ def test_pass_plan_with_cta_pairs(n_queries, nq):
         assert len(tail) == 0
     # pairs halve the corpus passes of the prefix
     if n_pair_q:
-        assert len(plan) - len(tail) == len(_plan(n_pair_q, nq, 0)) // 2 or nq > 640
-        if nq > 640:
-            n_slices = -(-nq // 640)
-            g = max(1, min(20, 20 // ((nq - (n_slices - 1) * 640 + 31) // 32)))
+        assert len(plan) - len(tail) == len(_plan(n_pair_q, nq, 0)) // 2 or nq > ROWS_MAX
+        if nq > ROWS_MAX:
+            n_slices = -(-nq // ROWS_MAX)
+            g = max(1, min(RB_MAX, RB_MAX // ((nq - (n_slices - 1) * ROWS_MAX + 31) // 32)))
             assert n_pair_q % (2 * g) == 0
             assert len(plan) - len(tail) == (n_pair_q // (2 * g)) * (g * (n_slices - 1) + 1)
 

@@ -82,10 +82,10 @@ def test_config_c1_16q_1k_passages(R):
     (900, 200, 3, 96, 100, True, False, 4),      # several queries per pass, k = 100
     (600, 150, 2, 832, 20, True, False, 5),      # FLMR full query (512 text + 320 vision): row slices
     (400, 90, 1, 400, 128, True, True, 6),       # 2 slices, k = FLMR_MAX_K, relu
-    (500, 120, 7, 832, 5, True, False, 15),      # 7 long queries: tail slices share passes in groups of 3 (3+3+1)
-    (300, 60, 3, 1500, 9, True, True, 16),       # 3 slices (640+640+220): tail groups of 2, relu
-    (200, 50, 2, 1280, 4, True, False, 17),      # tail slice is itself a full pass (group of 1)
-    (257, 33, 13, 45, 3, True, False, 7),        # nq not a multiple of 32, 13 queries (2 passes)
+    (500, 120, 7, 832, 5, True, False, 15),      # 7 long queries: tail slices share passes in groups of 6 (6+1)
+    (300, 60, 3, 1500, 9, True, True, 16),       # 4 slices (384+384+384+348): tail groups of 1, relu
+    (200, 50, 2, 1280, 4, True, False, 17),      # 4 slices, 128-row tails in groups of 3 (one pass)
+    (257, 33, 13, 45, 3, True, False, 7),        # nq not a multiple of 32, 13 queries (3 passes)
     (50, 700, 2, 64, 5, True, False, 8),         # passages longer than several 128-token tiles
     (5000, 3, 2, 32, 10, True, False, 9),        # tiny passages: up to 32 passage ends per tile
 ])
@@ -287,9 +287,9 @@ def test_topk_select_kernel(R):
     # and Nq = 641 whose one-row tails fill a pair group only from 40 queries up
     (700, 50, 7, 832, True, False, 10), (600, 40, 5, 1500, True, True, 5), (400, 30, 43, 641, True, False, 4)])
 def test_three_warpgroup_scan_kernel_is_bit_identical(case):
-    """flmr_scan3_kernel (three epilogue warpgroups, static query-tile assignment, 2-4 TMEM stages; the product
-    uses it for passes with three resident query tiles) forced onto every pass shape: scores and fused top-k
-    bit-identical to flmr_scan_kernel's and within 2e-5 of the oracle."""
+    """flmr_scan_kernel<3> (three consumer warpgroups; the product uses it for passes with three resident query
+    tiles) forced onto every pass shape: scores and fused top-k bit-identical to flmr_scan_kernel<2>'s and within
+    2e-5 of the oracle."""
     import ravqa_b200 as R
     from ravqa_b200 import _cabi
     n, nd, B, nq, ragged, relu, k = case
@@ -341,10 +341,10 @@ def test_c2_shape_against_the_c_oracle():
 
 
 def test_big_cta_pair_passes_properties(R, big):
-    """120k passages, SIX Nq = 320 queries: on a shard that spans every SM the product runs the first four through
-    one CTA-pair pass (clusters of two CTAs, TMA multicast, two queries resident in each CTA) and the last two through
-    a normal pass.  Fused top-k == stable sort of all scores (same call pattern), deterministic, and equal — scores to
-    the last bits a different tile partition can move, ids exactly — to the single-CTA kernel forced onto all six."""
+    """120k passages, SIX Nq = 320 queries through three CTA-pair passes (variant 4: clusters of two CTAs, TMA
+    multicast, one query resident in each CTA).  Fused top-k == stable sort of all scores (same call pattern),
+    deterministic, and equal — scores to the last bits a different tile partition can move, ids exactly — to the
+    single-CTA kernel forced onto all six."""
     from ravqa_b200 import _cabi
     corpus, D, Q3, n_p, nd = big
     L = _cabi.lib()
@@ -352,16 +352,17 @@ def test_big_cta_pair_passes_properties(R, big):
     Q = torch.nn.functional.normalize(torch.randn((6, 320, 128), device="cuda", generator=g), dim=-1).to(torch.bfloat16)
     for b, t in enumerate([0, 1, n_p // 2, n_p - 1, 77, n_p - 2]):        # planted positives incl. both corpus ends
         Q[b, :32] = D[t * nd: t * nd + 32]
-    L.flmr_launch_count(1)
-    s_all = R.maxsim_scores(corpus, Q)
-    assert L.flmr_launch_count(1) == 3                                    # one staging launch + pair pass of 4 + normal pass of 2
-    for k in (5, 100):
-        ts, tp = R.maxsim_topk(corpus, Q, k)
-        rs, rp = torch.sort(s_all, dim=1, descending=True, stable=True)
-        assert torch.equal(tp, rp[:, :k]) and torch.equal(ts, rs[:, :k])
-    assert [int(tp[b, 0]) for b in range(6)] == [0, 1, n_p // 2, n_p - 1, 77, n_p - 2]
-    assert torch.equal(s_all, R.maxsim_scores(corpus, Q))
     try:
+        _cabi.check(L.flmr_debug_set_scan_variant(4))
+        L.flmr_launch_count(1)
+        s_all = R.maxsim_scores(corpus, Q)
+        assert L.flmr_launch_count(1) == 4                                # one staging launch + three pair passes of 2
+        for k in (5, 100):
+            ts, tp = R.maxsim_topk(corpus, Q, k)
+            rs, rp = torch.sort(s_all, dim=1, descending=True, stable=True)
+            assert torch.equal(tp, rp[:, :k]) and torch.equal(ts, rs[:, :k])
+        assert [int(tp[b, 0]) for b in range(6)] == [0, 1, n_p // 2, n_p - 1, 77, n_p - 2]
+        assert torch.equal(s_all, R.maxsim_scores(corpus, Q))
         _cabi.check(L.flmr_debug_set_scan_variant(2))
         s_single = R.maxsim_scores(corpus, Q)
         _, tp_single = R.maxsim_topk(corpus, Q, 100)

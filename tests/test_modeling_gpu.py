@@ -252,7 +252,7 @@ def test_training_path_matches_reference_autograd_golden():
 
 @pytest.fixture()
 def argmax_path():
-    """Force flmr_maxsim_argmax onto one of its two kernels for a test (1 = warp-MMA, 2 = tcgen05)."""
+    """Force flmr_maxsim_argmax onto one of its two kernels for a test (1 = warp-MMA, 2 = wgmma)."""
     from ravqa_b200 import _cabi
     L = _cabi.lib()
     yield lambda path: _cabi.check(L.flmr_debug_set_argmax_path(path))
@@ -261,7 +261,7 @@ def argmax_path():
 
 @pytest.mark.parametrize("shape", [(3, 70, 5, 83), (2, 320, 7, 300), (1, 832, 9, 512), (4, 129, 3, 128)])
 def test_tcgen05_argmax_kernel_equals_warp_mma_kernel_and_torch(shape, argmax_path):
-    """The tcgen05 arg-max kernel (documents compacted to their unmasked tokens, TMA/TMEM pipeline) against the
+    """The wgmma arg-max kernel (documents compacted to their unmasked tokens, TMA/wgmma pipeline) against the
     warp-MMA kernel and torch on the same bf16 inputs: hole-y masks, a fully masked document, a document whose
     only token sits at the end, sizes off the 128 tiles, several documents per CTA."""
     from ravqa_b200.maxsim import maxsim_argmax, maxsim_argmax_grouped
@@ -303,7 +303,7 @@ def test_tcgen05_argmax_kernel_equals_warp_mma_kernel_and_torch(shape, argmax_pa
 
 def test_training_step_on_the_tcgen05_path_matches_golden(argmax_path):
     """The reference-generated training golden (loss, scores, dQ, dD of compute_ib_loss_new) with the forward
-    forced onto the tcgen05 kernel."""
+    forced onto the wgmma kernel."""
     import ravqa_b200 as R
     from helpers import GOLDEN_DIR
     import os
@@ -322,7 +322,7 @@ def test_training_step_on_the_tcgen05_path_matches_golden(argmax_path):
 
 def test_tcgen05_argmax_many_documents_per_cta_back_to_back(argmax_path):
     """The global-batch shape (8 queries x 832 rows against 128 ragged documents of up to 512 tokens: 12 documents
-    per CTA, the two epilogue warpgroups alternating documents) launched back to back without synchronisation:
+    per CTA, each consumer warpgroup on half of the query tile) launched back to back without synchronisation:
     same winners and maxima as the warp-MMA kernel every time."""
     from ravqa_b200.maxsim import maxsim_argmax
     g = torch.Generator().manual_seed(12)
@@ -345,7 +345,7 @@ def test_tcgen05_argmax_many_documents_per_cta_back_to_back(argmax_path):
 def test_graphed_loss_step_replays_the_eager_step(argmax_path):
     """graphed_in_batch_negatives_loss (forward and backward captured as CUDA graphs): on NEW inputs of the captured
     shape the replayed loss and gradients equal the eager step's — both kernels of the forward (warp-MMA for the
-    C4 rank shape, tcgen05 forced) are capturable: no host synchronisation, stream-ordered scratch only."""
+    C4 rank shape, wgmma forced) are capturable: no host synchronisation, stream-ordered scratch only."""
     import ravqa_b200 as R
     B, nway, nq, nd = 8, 2, 832, 512
     Q, D, mask = _inputs(B, nq, B * nway, nd, seed=31)

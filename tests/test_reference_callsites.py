@@ -21,7 +21,7 @@ from helpers import GOLDEN_DIR
 
 REF = "/root/reference/third_party/ColBERT"
 CKPT_DIR = os.path.join(GOLDEN_DIR, "callsites", "ckpt")
-needs_reference = pytest.mark.skipif(not os.path.isdir(REF), reason="the reference checkout is absent (GPU box)")
+needs_reference = pytest.mark.skipif(not os.path.isdir(REF), reason="the reference checkout is absent or not readable")
 
 
 @pytest.fixture(scope="module")

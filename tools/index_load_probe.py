@@ -1,5 +1,5 @@
 """Index-load throughput (GPU box): write a synthetic flat index of `--gigabytes` to `--dir` (chunks of 25k
-passages, as the Indexer writes them), drop it from the page cache if allowed, and time FlatCorpus.from_index —
+passages, as the Indexer writes them), evict it from the page cache, and time FlatCorpus.from_index —
 the C-level streaming builder (pread into two pinned buffers with 8 threads, overlapped H2D, padded layout).
 
     python tools/index_load_probe.py --gigabytes 8 --dir /dev/shm/flmr_idx
@@ -43,10 +43,12 @@ def main():
     size = sum(os.path.getsize(os.path.join(args.dir, f)) for f in os.listdir(args.dir)) / 1e9
     print("wrote %.2f GB in %d chunks to %s (%.1f s)" % (size, c, args.dir, t_write), flush=True)
     cold = False
-    try:
+    try:   # evict this index's own pages from the page cache (a per-file hint, no system setting is touched)
         os.sync()
-        with open("/proc/sys/vm/drop_caches", "w") as f:
-            f.write("1\n")
+        for f in os.listdir(args.dir):
+            fd = os.open(os.path.join(args.dir, f), os.O_RDONLY)
+            os.posix_fadvise(fd, 0, 0, os.POSIX_FADV_DONTNEED)
+            os.close(fd)
         cold = True
     except Exception:
         pass

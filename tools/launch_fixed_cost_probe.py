@@ -3,9 +3,9 @@
     python tools/launch_fixed_cost_probe.py [--block-seconds 1.5] [--rounds 3]
 
 Strong scaling over N GPUs divides the shard (1M passages / N) but not whatever a launch costs independent of its
-size (prologue: barrier init, TMEM allocation, query tiles into TMEM; pipeline fill; tail: the slowest CTA, the
+size (prologue: barrier init, query tiles into shared memory; pipeline fill; tail: the slowest CTA, the
 reducers' last tiles, candidate lists; launch gap).  This probe runs the headline call (16 queries of Nq = 320, k = 5:
-four CTA-pair passes) against shards of 125k / 250k / 500k / 1M passages x 180 tokens on ONE GPU, interleaved in
+sixteen passes) against shards of 125k / 250k / 500k / 1M passages x 180 tokens on ONE GPU, interleaved in
 blocks of --block-seconds so every size sees the same power-capped regime, and fits
     scan launch ms = a + b * passages          (a = fixed cost per launch, b = streaming cost)
     call ms        = scans + c                 (c = staging + merge launches + gaps per call)

@@ -1,7 +1,7 @@
 """Turn an `ncu --metrics gpu__time_duration.sum --csv --log-file X.csv` launch list into the markdown
-summary kept under profiles/ (per-kernel launches, total time, share; this library's kernels apart).
+summary (per-kernel launches, total time, share; this library's kernels apart).
 
-    python tools/launch_list_md.py gpurun_out/launches_r01_final.csv "<command that produced it>" > profiles/r01_launches.md
+    python tools/launch_list_md.py launches.csv "<command that produced it>" > launches.md
 """
 import csv
 import sys
@@ -28,7 +28,7 @@ def main():
         agg[short] = (n + 1, t + ms)
     total = sum(t for _, t in agg.values())
     print("# ncu launch list\n")
-    print("Command (B200, 1 GPU): `%s`\n" % command)
+    print("Command (1 GPU): `%s`\n" % command)
     print("Per-launch times under ncu are cold-cache and serialised: compare SHARES, not absolutes. Includes corpus "
           "generation (torch randn/normalize), the bench's HBM-regime leg, its self-check and the library-GPU "
           "baseline leg (torch/cuBLAS kernels) when enabled.\n")

@@ -1,7 +1,8 @@
-"""Timing probe for the scan kernel (GPU box): q/s and per-launch scan time for a synthetic corpus,
-optionally under the kernel's timing-only debug modes (FLMR_DEBUG_MODE=1..3, results are garbage).
+"""Timing probe for the scan kernel (GPU box): q/s and per-launch scan time for a synthetic corpus, each run in a
+fresh child process (--modes 0,0,0 repeats it; the label is the FLMR_DEBUG_MODE the child sees, which the scan
+kernel ignores).
 
-    python tools/perf_probe.py --passages 200000 --modes 0,1,2,3
+    python tools/perf_probe.py --passages 200000 --modes 0,0,0
 """
 import argparse
 import ctypes as C

@@ -9,9 +9,9 @@ candidate generation, centroid-only pruning (filter_pids.cpp), residual decompre
 reference's own ResidualCodec / optimize_ivf (k-means by seeded torch Lloyd iterations: faiss is not
 installed), runs the reference's IndexScorer.rank per query, and compares its top-5 with exhaustive
 scoring of (a) the same decompressed embeddings and (b) the original embeddings — the ranking the
-B200 scan returns (tests/test_plaid.py and tests/test_gpu_parity.py pin the CUDA path to the oracle
+H100 scan returns (tests/test_plaid.py and tests/test_gpu_parity.py pin the CUDA path to the oracle
 used here).  Queries are noisy token subsets of a planted passage, so a known positive exists.
-Writes profiles/r01_recall_vs_plaid.md.
+Prints the tables as markdown.
 """
 from __future__ import annotations
 
@@ -65,8 +65,6 @@ def main():
     md += ["The CUDA path returns exactly the exhaustive ranking (parity tests pin it to the oracle used here): its "
            "Recall@5 equals the exhaustive rows, whatever the regime; the first row of each table is the reference's "
            "pruned search.  Latencies are for this container's %d CPU threads." % torch.get_num_threads()]
-    out = os.path.join(ROOT, "profiles", "r01_recall_vs_plaid.md")
-    open(out, "w").write("\n".join(md) + "\n")
     print("\n".join(md))
 
 

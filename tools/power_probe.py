@@ -1,7 +1,7 @@
 """Sustained-regime probe (GPU box): the scan kernel run back to back for `--seconds` per configuration, with
 the SM clock and board power sampled by nvidia-smi during the second half of the run.  Question it answers:
 how much of the power-capped (sustained) throughput depends on DATA MOVEMENT — compare a corpus streamed from
-HBM (1M passages, 46 GB) with one that stays in L2 (2k passages, 92 MB): same MMA / TMEM / epilogue work per
+HBM (1M passages, 46 GB) with one that stays in L2 (2k passages, 92 MB): same MMA / epilogue work per
 token, no HBM traffic.
 
     python tools/power_probe.py --passages 1000000,2000 --seconds 8

@@ -1,5 +1,5 @@
-"""GPU: flmr_scan3_kernel (three epilogue warpgroups, static query-tile assignment) against flmr_scan_kernel —
-bit-identical results over a spread of shapes, then timing of both.
+"""GPU: the scan kernel's variants — flmr_scan_kernel<2> (two consumer warpgroups), <3> (three) and CTA-pair passes —
+bit-identical results of <2> and <3> over a spread of shapes, then timing of all three.
 
     python tools/scan_variant_probe.py [--passages 200000]
 """
@@ -67,7 +67,7 @@ def main():
     for (B, nq) in [(16, 320), (2, 320), (1, 320), (20, 32), (1, 32), (3, 832), (4, 256), (2, 128)]:
         Q = torch.nn.functional.normalize(torch.randn((B, nq, 128), device=dev, generator=g), dim=-1).bfloat16()
         for variant in (2, 3, 4):
-            if variant == 4 and (B % 2 or nq > 640):
+            if variant == 4 and (B % 2 or nq > 384):   # pairs of whole queries that fit one pass
                 continue
             L.flmr_debug_set_scan_variant(variant)
             for _ in range(2):

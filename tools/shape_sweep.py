@@ -1,7 +1,7 @@
 """GPU probe: the scan path across the workload shapes BASELINE.json / SURVEY.md §8 name (not only the
 headline C3 shape): queries/s, per-launch scan time and the two roofline figures of each.
 
-    python tools/shape_sweep.py > profiles/r01_shape_sweep.md
+    python tools/shape_sweep.py > shape_sweep.md
 """
 import ctypes as C
 import os
@@ -73,8 +73,8 @@ def run(name, n_p, nd_rng, nq, B, k, iters):
 
 
 def main():
-    print("# Shape sweep of the scan path (round 1)\n")
-    print("`python tools/shape_sweep.py` on one B200; synthetic unit-norm bf16 embeddings; CUDA-event timing of "
+    print("# Shape sweep of the scan path\n")
+    print("`python tools/shape_sweep.py` on one GPU; synthetic unit-norm bf16 embeddings; CUDA-event timing of "
           "`maxsim_topk` calls (queries resident on the device); scan columns from per-launch events "
           "(`flmr_set_profiling`).  TFLOP/s counts real tokens x real query rows only (padding is overhead); GB/s "
           "counts the stored token rows one launch streams.  Corpora below 1M passages: q/s scale ~1/N.\n")

@@ -1,11 +1,11 @@
-// How many clusters of 1 / 2 / 4 / 8 CTAs with the scan kernel's footprint (384 threads, ~222 KB of dynamic shared
+// How many clusters of 1 / 2 / 4 / 8 CTAs with the scan kernel's footprint (448 threads, ~222 KB of dynamic shared
 // memory: one CTA per SM) can be resident at once?  A persistent kernel whose CTAs of a cluster share one token
 // range needs ALL its clusters resident together, so this bounds the cluster sizes the scan kernel could use.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -o cluster_occupancy cluster_occupancy.cu && ./cluster_occupancy
+//   nvcc -gencode arch=compute_90a,code=sm_90a -o cluster_occupancy cluster_occupancy.cu && ./cluster_occupancy
 #include <cstdio>
 #include <cuda_runtime.h>
 
-__global__ void __launch_bounds__(384, 1) footprint_kernel(int* out) {
+__global__ void __launch_bounds__(448, 1) footprint_kernel(int* out) {
   extern __shared__ char smem[];
   if (out && threadIdx.x == 0) out[blockIdx.x] = smem[0];
 }
@@ -20,7 +20,7 @@ int main() {
   for (int cs : {1, 2, 4, 8, 16}) {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(prop.multiProcessorCount / cs * cs);
-    cfg.blockDim = dim3(384);
+    cfg.blockDim = dim3(448);
     cfg.dynamicSmemBytes = smem_bytes;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;

@@ -7,7 +7,7 @@ Shapes (CB/modeling/colbert.py:64-113): per rank 8 queries x 16 documents (nway 
 ragged masks.  "global" = the same 8 queries against the documents of all 8 ranks (128 documents): the matrix
 cross-rank negatives produce (colbert.py:115-163).
 
-Reported: the arg-max forward alone under both of its kernels (warp-MMA / tcgen05) with TFLOP/s, the three kernels
+Reported: the arg-max forward alone under both of its kernels (warp-MMA / wgmma) with TFLOP/s, the three kernels
 of a step (forward, loss head, backward) timed alone, the whole step through `in_batch_negatives_loss(...).backward()`,
 and a torch restatement of the reference's compute_ib_loss_new (fp32, materialises [B, B*nway, Nd, Nq]).
 """
@@ -64,7 +64,7 @@ def single_gpu():
         Q, D, mask, tok = make(Bq, n, nq, nd, 0, dev)
         Qb, Db = Q.bfloat16(), D.bfloat16()
         flops = 2.0 * Bq * nq * 128 * tok
-        for path, label in ((1, "warp-MMA (mma.sync)"), (2, "tcgen05 (compact + TMA/TMEM pipeline)")):
+        for path, label in ((1, "warp-MMA (mma.sync)"), (2, "wgmma (compact + TMA/wgmma pipeline)")):
             L.flmr_debug_set_argmax_path(path)
             ms = timed(lambda: maxsim_argmax(Qb, Db, mask, return_rowmax=True))
             print("| %s | arg-max forward, %s | %.3f | %.0f |" % (name, label, ms, flops / ms / 1e9))
