@@ -91,9 +91,11 @@ __device__ __forceinline__ uint32_t mbar_poll_block(uint32_t bar, uint32_t parit
       : "memory");
   return n;   // < kSpinBlock: the phase completed
 }
-__device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity, int* status, int code) {
-  // 20 s of polling = a protocol bug, not a slow wait (time slicing, a sanitizer or a debugger can stretch a
-  // legitimate wait to seconds; the longest real wait of a scan is one tile, microseconds)
+// 20 s of polling = a protocol bug, not a slow wait (time slicing, a sanitizer or a debugger can stretch a
+// legitimate wait to seconds; the longest real wait of a scan is one tile, microseconds)
+// The same bounded wait with no function call, for waits while wgmma groups are in flight: ptxas cannot see what a
+// call does with the accumulator registers, so it retires the in-flight wgmma before it (warning C7518).
+__device__ __forceinline__ void mbar_wait_inline(uint32_t bar, uint32_t parity, int* status, int code) {
   constexpr uint64_t timeout_ns = 20000000000ull;
   uint64_t t0 = 0;
   while (mbar_poll_block(bar, parity) >= kSpinBlock) {
@@ -106,6 +108,9 @@ __device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity, int* 
       __trap();
     }
   }
+}
+__device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity, int* status, int code) {
+  mbar_wait_inline(bar, parity, status, code);
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* status, int code) {
   if (mbar_try_wait(bar, parity)) return;
@@ -189,6 +194,9 @@ __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Wait until at most N committed wgmma groups of this warpgroup are still in flight.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // Pins the accumulator registers in place across the asynchronous MMA: without it the compiler may read or
 // move them between the issue and the wait.

@@ -782,9 +782,13 @@ void plan_passes(int n_queries, int nq, bool allow_pair, std::vector<PassPlan>* 
 }
 
 int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pair, cudaStream_t st) {
-  // three consumer warpgroups where the six 64-row query blocks of three resident tiles split evenly over them
-  // (two each), two otherwise; the instantiations compute bit-identical results
-  const bool use3 = !pair && ((g_scan_variant == 3) || (g_scan_variant == 0 && p.n_mtiles == 3));
+  // by the pass's occupied 64-row blocks: from five up (Nq = 320: five, a full row slice: six) three warpgroups
+  // (2 / 2 / 1 or 2 / 2 / 2 blocks, serial loop: one warpgroup's MMAs overlap another's fold), below that two
+  // (each with two accumulators, its own MMAs overlapping its fold).  On an H100 (400 W, 200k x 180-token passages,
+  // median of 5) a 5-block pass took 9.19 ms with three and 10.34 ms with two (3 / 2 blocks), 6-block row slices
+  // 9.12 vs 9.64 ms, a 4-block pass 7.90 vs 7.39 ms (DESIGN.md 4.1).  The instantiations compute bit-identical results
+  const bool use3 = !pair && ((g_scan_variant == 3) ||
+                              (g_scan_variant == 0 && scan_blocks(p.nq_pass, p.rbq) >= 5));
   EventPair ev{};
   if (g_profiling) {
     FLMR_CUDA(cudaEventCreate(&ev.a));

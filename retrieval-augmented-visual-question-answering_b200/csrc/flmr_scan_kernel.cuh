@@ -36,6 +36,8 @@
 #include "../../include/flmr_maxsim.h"
 #include "flmr_device.cuh"
 
+#include <type_traits>
+
 namespace flmr {
 
 constexpr int kDim = 128;
@@ -61,6 +63,9 @@ static_assert(kTileN == 96, "the wgmma shape and accumulator fragment are writte
 static_assert(kDKBlockBytes % 1024 == 0, "swizzle atoms need 1024-B aligned k-blocks");
 
 __host__ __device__ constexpr int scan_threads(int wgs) { return (wgs * 4 + 2) * 32; }
+// 64-row query blocks that hold resident rows: the MMAs of a pass stop at its last occupied block (the staged tiles
+// are zero-padded to 128 rows, but nobody reads the sums of rows past nq_pass * rbq * 32)
+__host__ __device__ constexpr int scan_blocks(int nq_pass, int rbq) { return (nq_pass * rbq * 32 + 63) / 64; }
 
 struct ScanParams {
   // corpus partition (built once per corpus, see build_partition() in flmr_maxsim.cu)
@@ -103,6 +108,15 @@ struct ScanSmem {
   static constexpr int kNumBars = 2 * kDStages + 4;
   static constexpr int kBytes = kOffBars + kNumBars * 8 + 1024;   // + slack for 1024-B alignment
   static_assert(kBytes <= 232448, "exceeds 227 KiB of shared memory per CTA");
+};
+
+// Shared-memory addresses of the kernel's mbarriers.
+struct ScanBars {
+  uint32_t base;   // smem address of ScanSmem::kOffBars
+  __device__ uint32_t d_full(int s) const { return base + 8u * s; }                      // D stage s loaded
+  __device__ uint32_t d_empty(int s) const { return base + 8u * (kDStages + s); }        // ... and released
+  __device__ uint32_t p_full(int b) const { return base + 8u * (2 * kDStages + b); }     // partials of buffer b written
+  __device__ uint32_t p_empty(int b) const { return base + 8u * (2 * kDStages + 2 + b); }  // ... and consumed
 };
 
 // ---- epilogue helpers ---------------------------------------------------------------------------
@@ -149,21 +163,36 @@ __device__ __noinline__ void topk_replace_min(uint64_t* keys, int k, uint64_t ca
   __syncwarp();
 }
 
+// Max of a thread's values x over the quad's four lanes (they hold the same rows, different columns).
+__device__ __forceinline__ float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+
 // Fold one 64 x 96 accumulator (rows of query block j, the D tile's 96 tokens) into the passage maxima.
 // `m[h]` is the running max of row half h of the passage that is open at the tile start; on return, of the one
 // open at its end.  Every lane of a quad holds the same m (the quad's columns are combined by shuffles).
+// Max is exact, so the order of the maxima is free: each thread first reduces its own columns of a passage, and
+// the quad is combined once per passage end instead of once per 8-column block.  A thread's two columns of
+// 8-column block i in row half h are acc[4 i + 2 h] and acc[4 i + 2 h + 1]; lanes with the same hi (lane, lane ^ 1)
+// together cover the 4-token group 2 i + hi.  The accumulator is read in place: no per-block maxima are kept,
+// which leaves the registers for the second accumulator of the pipelined consumer loop.
 __device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], uint32_t mask, float (&m)[2],
                                                  float init, float* lane_part_buf, float* partial_buf, int j,
                                                  int wq, int lane) {
-  const int hi = (lane >> 1) & 1;   // this thread's columns belong to the 4-token groups 2 i + hi
-  float gm[2][kNb];
+  const int hi = (lane >> 1) & 1;
+  if (mask == 0) {   // warp-uniform: no passage ends in this tile (about half the tiles at Nd = 180)
 #pragma unroll
-  for (int h = 0; h < 2; ++h)
+    for (int h = 0; h < 2; ++h) {
+      float c[4];   // four independent max chains over the 24 columns
 #pragma unroll
-    for (int i = 0; i < kNb; ++i) {
-      const float x = fmaxf(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-      gm[h][i] = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+      for (int i = 0; i < 4; ++i) c[i] = fmaxf(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+#pragma unroll
+      for (int i = 4; i < kNb; ++i) c[i & 3] = fmax3(c[i & 3], acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+      m[h] = fmaxf(m[h], quad_max(fmaxf(fmaxf(c[0], c[1]), fmaxf(c[2], c[3]))));
     }
+    return;
+  }
   const int row0 = j * 64 + wq * 16 + (lane >> 2);   // row of h = 0 inside the pass; h = 1 is row0 + 8
   uint32_t live = (1u << kSlots) - 1u;               // groups not yet consumed by a finished passage
   uint32_t bits = mask;
@@ -178,9 +207,8 @@ __device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], ui
       float x = -INFINITY;
 #pragma unroll
       for (int i = 0; i < kNb; ++i)
-        if ((seg >> (2 * i)) & 1u) x = fmaxf(x, gm[h][i]);
-      x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
-      s[h] = fmaxf(x, m[h]);
+        if ((seg >> (2 * i)) & 1u) x = fmax3(x, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+      s[h] = fmaxf(quad_max(x), m[h]);
       m[h] = init;
     }
     if (slot < kFastSlots) {
@@ -211,9 +239,125 @@ __device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], ui
     float x = -INFINITY;
 #pragma unroll
     for (int i = 0; i < kNb; ++i)
-      if ((rest >> (2 * i)) & 1u) x = fmaxf(x, gm[h][i]);
-    x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
-    m[h] = fmaxf(m[h], x);
+      if ((rest >> (2 * i)) & 1u) x = fmax3(x, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+    m[h] = fmaxf(m[h], quad_max(x));
+  }
+}
+
+// acc = (64-row query block at q_block) . (D tile at d_stage)^T: 8 x wgmma.m64n96k16 over K = 128, one commit group.
+__device__ __forceinline__ void issue_block_mma(float (&acc)[4 * kNb], uint32_t q_block, uint32_t d_stage) {
+  // the query block's descriptors are loop-invariant: hidden from the compiler so that they are rebuilt here (a
+  // few integer adds) rather than hoisted out of the tile loop into 16 registers per block
+  asm volatile("" : "+r"(q_block));
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < kDim / 16; ++k) {
+    const uint32_t koff = (k & 3) * 32u;   // 16 elements along the 128-byte row
+    const uint64_t a_desc = make_kmajor_sw128_desc(q_block + (k >> 2) * kQKBlockBytes + koff);
+    const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + (k >> 2) * kDKBlockBytes + koff);
+    wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+  }
+  wgmma_commit();
+}
+
+// One consumer warpgroup that owns NB of the pass's 64-row query blocks (j = wg + u kWgs, u < NB), over all tiles.
+// Software-pipelined over the sequence of (tile, block) pairs with two accumulators: the MMAs of the next pair are
+// issued before the accumulator of the current one is folded (wait_group 1), so the tensor pipe works while the
+// warpgroup folds.  Pair q = t NB + u uses accumulator q & 1; tiles are walked two at a time so that the index is
+// a compile-time constant for every NB.  The next pair of the last block of tile t is the first block of tile t + 1,
+// which reads the next D stage: after the wait, every MMA that read stage t has completed and the stage is released.
+// ptxas tracks which accumulator is in flight only along compile-time structure: every join of the control flow
+// has the same group in flight (acc[0] at the loop head, none at the end), so the last one or two tiles, whose
+// last pair has no successor, are peeled out of the loop.
+// kOverlap = false is the serial form with one accumulator (next MMAs issued after the fold, wait_group 0), for
+// instantiations without the registers for two; the arithmetic and its order are the same.
+template <int NB, int kWgs, bool kPair, bool kOverlap>
+__device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base, ScanBars bars,
+                                              int n_tiles, int64_t tile_base, int wg, int wq, int lane) {
+  using S = ScanSmem;
+  const float init = p.init_val;
+  float m[NB][2];   // running passage maxima of block u's two rows of this thread
+#pragma unroll
+  for (int u = 0; u < NB; ++u) m[u][0] = m[u][1] = init;
+  float* const lane_part = reinterpret_cast<float*>(smem + S::kOffLanePart);
+  float* const partial = reinterpret_cast<float*>(smem + S::kOffPartial);
+  const uint32_t q_smem = smem_base + S::kOffQ;
+  auto q_block = [&](int u) { return q_smem + (wg + u * kWgs) * 64 * 128; };
+  auto d_stage = [&](int t) { return smem_base + S::kOffD + (t % kDStages) * kDTileBytes; };
+  float acc[kOverlap ? 2 : 1][4 * kNb];
+  uint32_t mask_next = 0;
+
+  // tile t, entered with the MMAs of (t, 0) in flight in acc[(kH * NB) & 1]; kNext: a tile t + 1 follows
+  auto tile = [&](int t, auto kh, auto knext) {
+    constexpr int kH = decltype(kh)::value;
+    constexpr bool kNext = decltype(knext)::value;
+    const uint32_t mask = mask_next;
+    const int buf = t & 1;
+    float* lane_part_buf = lane_part + buf * (kFastSlots * kRbMax * kLaneStride);
+    float* partial_buf = partial + buf * (kHbMax * kSlots);
+#pragma unroll
+    for (int u = 0; u < NB; ++u) {
+      const int a = kOverlap ? (kH * NB + u) & 1 : 0;   // accumulator of (t, u); the other one takes the next pair
+      const bool last = u + 1 == NB;
+      auto issue_next = [&](float (&acc_next)[4 * kNb]) {
+        if (!last) {
+          issue_block_mma(acc_next, q_block(u + 1), d_stage(t));
+        } else if (kNext) {
+          mbar_wait_inline(bars.d_full((t + 1) % kDStages), ((t + 1) / kDStages) & 1u, p.status, kDevTimeoutMma);
+          mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
+          issue_block_mma(acc_next, q_block(0), d_stage(t + 1));
+        }
+      };
+      if (kOverlap && (!last || kNext)) {
+        issue_next(acc[a ^ 1]);
+        wgmma_wait<1>();
+      } else {
+        wgmma_wait<0>();
+      }
+      wgmma_fence_operands(acc[a]);
+      if (last) {
+        // every wgmma reading D stage t has completed (the one in flight reads stage t + 1) -> release it
+        __syncwarp();
+        if (wq == 0 && lane == 0) {
+          if constexpr (kPair) {
+            mbar_arrive_cluster(bars.d_empty(t % kDStages), 0);
+            mbar_arrive_cluster(bars.d_empty(t % kDStages), 1);
+          } else {
+            mbar_arrive(bars.d_empty(t % kDStages));
+          }
+        }
+      }
+      // the reducer must have consumed the partial sums of tile t-2 before this buffer is reused
+      if (u == 0)
+        mbar_wait_inline(bars.p_empty(buf), ((static_cast<uint32_t>(t) >> 1) & 1u) ^ 1u, p.status,
+                         kDevTimeoutEpilogue);
+      fold_accumulator(acc[a], mask, m[u], init, lane_part_buf, partial_buf, wg + u * kWgs, wq, lane);
+      if (!kOverlap) issue_next(acc[0]);
+    }
+    // this warp's row maxima / partial sums of tile t are written: order every lane's stores
+    // before lane 0's arrive (release); the reducer's wait is the matching acquire
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bars.p_full(buf));
+  };
+  using H0 = std::integral_constant<int, 0>;
+  using H1 = std::integral_constant<int, 1>;
+  using Next = std::true_type;
+  using Final = std::false_type;
+
+  if (n_tiles <= 0) return;
+  mbar_wait(bars.d_full(0), 0u, p.status, kDevTimeoutMma);
+  mask_next = __ldg(p.tile_end_mask + tile_base);
+  issue_block_mma(acc[0], q_block(0), d_stage(0));
+  int t = 0;
+  for (; t + 2 < n_tiles; t += 2) {
+    tile(t, H0{}, Next{});
+    tile(t + 1, H1{}, Next{});
+  }
+  if (t + 2 == n_tiles) {
+    tile(t, H0{}, Next{});
+    tile(t + 1, H1{}, Final{});
+  } else {
+    tile(t, H0{}, Final{});
   }
 }
 
@@ -234,6 +378,12 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
   constexpr int kWarpRed0 = kConsumerWarps;
   constexpr int kWarpProducer = kConsumerWarps + kRedWarps;
   constexpr int kBlocksPerWg = (2 * kMtMax + kWgs - 1) / kWgs;   // 64-row query blocks per warpgroup, at most
+  // Two accumulators per consumer thread (the overlapped loop): ptxas allocates that loop with 166 registers and
+  // fails outright (C7600) below 168.  A sub-partition's 16K registers serve one warp of every warpgroup, so two
+  // consumer warpgroups (10 warps) get 168; three (14 warps, 4 on a sub-partition) get 128, and moving registers
+  // with setmaxnreg cannot help: 3 x 168 leaves the producer / reducer warps less than setmaxnreg's minimum of 24.
+  // Three warpgroups therefore run the serial loop.
+  constexpr bool kOverlap = kWgs == 2;
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment by pointer arithmetic on the __shared__ array (keeps the shared address space
   // visible to the compiler: LDS/STS instead of generic loads/stores)
@@ -244,30 +394,27 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
   const int cta = kPair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);   // partition / list index
   const uint32_t pair_rank = kPair ? cluster_ctarank() : 0u;
 
-  const uint32_t bar_base = smem_base + S::kOffBars;
-  auto bar_d_full = [&](int s) { return bar_base + 8u * s; };
-  auto bar_d_empty = [&](int s) { return bar_base + 8u * (kDStages + s); };
-  auto bar_p_full = [&](int b) { return bar_base + 8u * (2 * kDStages + b); };
-  auto bar_p_empty = [&](int b) { return bar_base + 8u * (2 * kDStages + 2 + b); };
+  const ScanBars bars{smem_base + S::kOffBars};
 
   const int32_t row_begin = p.cta_row_begin[cta];
   const int64_t tile_base = p.cta_tile_base[cta];
   const int n_tiles = static_cast<int>(p.cta_tile_base[cta + 1] - tile_base);
   const int n_mtiles = p.n_mtiles;
-  // warpgroups that own at least one 64-row query block (three warpgroups, one resident tile: two); only
-  // these read the D stages and release them
-  const int n_busy_wgs = min(kWgs, 2 * n_mtiles);
+  const int n_blocks = scan_blocks(p.nq_pass, p.rbq);   // 64-row query blocks with resident rows
+  // warpgroups that own at least one 64-row query block (three warpgroups, one block: one); only these read the
+  // D stages, release them and deliver partial sums; the others have nothing to do
+  const int n_busy_wgs = min(kWgs, n_blocks);
 
   // ---- one-time setup --------------------------------------------------------------------------
   if (warp == kWarpProducer && lane == 0) {
     tma_prefetch_desc(&tmap_d);
     for (int s = 0; s < kDStages; ++s) {
-      mbar_init(bar_d_full(s), 1);
-      mbar_init(bar_d_empty(s), (kPair ? 2 : 1) * n_busy_wgs);   // pair: the consumers of both CTAs
+      mbar_init(bars.d_full(s), 1);
+      mbar_init(bars.d_empty(s), (kPair ? 2 : 1) * n_busy_wgs);   // pair: the consumers of both CTAs
     }
     for (int b = 0; b < 2; ++b) {
-      mbar_init(bar_p_full(b), kConsumerWarps);   // partial sums of a D tile complete
-      mbar_init(bar_p_empty(b), kRedWarps);       // ... and consumed by the reducer warp
+      mbar_init(bars.p_full(b), 4 * n_busy_wgs);   // partial sums of a D tile complete (every busy consumer warp)
+      mbar_init(bars.p_empty(b), kRedWarps);       // ... and consumed by the reducer warp
     }
     mbar_fence_init();
   }
@@ -293,208 +440,164 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
   __syncthreads();
   if constexpr (kPair) cluster_sync_all();   // the peer's barriers exist before anything is multicast to them
 
-  if (warp == kWarpProducer) {
-    // ===================== TMA producer =====================
-    // The whole warp runs the loop (warp-uniform control flow keeps addresses in uniform
-    // registers); one elected lane issues the bulk copies.
-    for (int t = 0; t < n_tiles; ++t) {
-      const int s = t % kDStages;
-      const uint32_t ph = (t / kDStages) & 1;
-      mbar_wait(bar_d_empty(s), ph ^ 1u, p.status, kDevTimeoutProducer);
-      if (elect_one_sync()) {
-        mbar_arrive_expect_tx(bar_d_full(s), kDTileBytes);   // (pair: 12 KB from this CTA's loads + 12 KB from the peer's)
-        const uint32_t dst = smem_base + S::kOffD + s * kDTileBytes;
-        const int32_t row = row_begin + t * kTileN;
-        if constexpr (kPair) {   // tmap_d has a (kTileN / 2)-row box here
-          const uint32_t half = pair_rank * (kTileN / 2);
-          tma_load_2d_multicast(dst + half * 128, &tmap_d, bar_d_full(s), 0, row + half, 3, kPolicyEvictFirst);
-          tma_load_2d_multicast(dst + kDKBlockBytes + half * 128, &tmap_d, bar_d_full(s), 64, row + half, 3,
-                                kPolicyEvictFirst);
-        } else {
-          tma_load_2d(dst, &tmap_d, bar_d_full(s), 0, row, kPolicyEvictFirst);
-          tma_load_2d(dst + kDKBlockBytes, &tmap_d, bar_d_full(s), 64, row, kPolicyEvictFirst);
-        }
-      }
-      __syncwarp();
-    }
-  } else if (warp < kConsumerWarps) {
-    // ===================== consumers: wgmma + passage maxima =====================
-    const int wg = warp >> 2;
-    const int wq = warp & 3;           // warp inside the warpgroup: accumulator rows 16 wq .. 16 wq + 15
-    const int n_blocks = 2 * n_mtiles;
-    const float init = p.init_val;
-    float m[kBlocksPerWg][2];
-#pragma unroll
-    for (int u = 0; u < kBlocksPerWg; ++u) m[u][0] = m[u][1] = init;
-    float* const lane_part = reinterpret_cast<float*>(smem + S::kOffLanePart);
-    float* const partial = reinterpret_cast<float*>(smem + S::kOffPartial);
-    const uint32_t q_smem = smem_base + S::kOffQ;
-    uint32_t mask_next = (n_tiles > 0) ? __ldg(p.tile_end_mask + tile_base) : 0u;
-    float acc[4 * kNb];
-    for (int t = 0; t < n_tiles; ++t) {
-      const uint32_t mask = mask_next;
-      if (t + 1 < n_tiles) mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
-      const int s = t % kDStages;
-      const int buf = t & 1;
-      const uint32_t d_smem = smem_base + S::kOffD + s * kDTileBytes;
-      if (wg < n_busy_wgs) mbar_wait(bar_d_full(s), (t / kDStages) & 1u, p.status, kDevTimeoutMma);
-      // the reducer must have consumed the partial sums of tile t-2 before this buffer is reused
-      mbar_wait(bar_p_empty(buf), ((static_cast<uint32_t>(t) >> 1) & 1u) ^ 1u, p.status, kDevTimeoutEpilogue);
-      float* lane_part_buf = lane_part + buf * (kFastSlots * kRbMax * kLaneStride);
-      float* partial_buf = partial + buf * (kHbMax * kSlots);
-#pragma unroll
-      for (int u = 0; u < kBlocksPerWg; ++u) {
-        const int j = wg + u * kWgs;
-        if (j < n_blocks) {
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < kDim / 16; ++k) {
-            const uint32_t koff = (k & 3) * 32u;   // 16 elements along the 128-byte row
-            const uint64_t a_desc = make_kmajor_sw128_desc(q_smem + (k >> 2) * kQKBlockBytes + j * 64 * 128 + koff);
-            const uint64_t b_desc = make_kmajor_sw128_desc(d_smem + (k >> 2) * kDKBlockBytes + koff);
-            wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+  if (warp >= kConsumerWarps) {
+    if (warp == kWarpProducer) {
+      // ===================== TMA producer =====================
+      // The whole warp runs the loop (warp-uniform control flow keeps addresses in uniform
+      // registers); one elected lane issues the bulk copies.
+      for (int t = 0; t < n_tiles; ++t) {
+        const int s = t % kDStages;
+        const uint32_t ph = (t / kDStages) & 1;
+        mbar_wait(bars.d_empty(s), ph ^ 1u, p.status, kDevTimeoutProducer);
+        if (elect_one_sync()) {
+          mbar_arrive_expect_tx(bars.d_full(s), kDTileBytes);   // (pair: 12 KB from this CTA's loads + 12 KB from the peer's)
+          const uint32_t dst = smem_base + S::kOffD + s * kDTileBytes;
+          const int32_t row = row_begin + t * kTileN;
+          if constexpr (kPair) {   // tmap_d has a (kTileN / 2)-row box here
+            const uint32_t half = pair_rank * (kTileN / 2);
+            tma_load_2d_multicast(dst + half * 128, &tmap_d, bars.d_full(s), 0, row + half, 3, kPolicyEvictFirst);
+            tma_load_2d_multicast(dst + kDKBlockBytes + half * 128, &tmap_d, bars.d_full(s), 64, row + half, 3,
+                                  kPolicyEvictFirst);
+          } else {
+            tma_load_2d(dst, &tmap_d, bars.d_full(s), 0, row, kPolicyEvictFirst);
+            tma_load_2d(dst + kDKBlockBytes, &tmap_d, bars.d_full(s), 64, row, kPolicyEvictFirst);
           }
-          wgmma_commit();
-          wgmma_wait_all();
-          wgmma_fence_operands(acc);
-          // last block of this warpgroup on the D stage: every wgmma reading it has completed -> release it
-          if (j + kWgs >= n_blocks) {
-            __syncwarp();
-            if (wq == 0 && lane == 0) {
-              if constexpr (kPair) {
-                mbar_arrive_cluster(bar_d_empty(s), 0);
-                mbar_arrive_cluster(bar_d_empty(s), 1);
-              } else {
-                mbar_arrive(bar_d_empty(s));
+        }
+        __syncwarp();
+      }
+    } else if (warp == kWarpRed0) {
+      // ===================== reducer: score finalisation + per-CTA top-k =====================
+      // Per D tile and per (query, passage ending in the tile): sum the row partials in fixed
+      // order (deterministic), add/store partial scores if requested, offer to the top-k list.
+      const int rw = warp - kWarpRed0;  // reducer 0..kRedWarps-1 owns queries b = rw (mod kRedWarps)
+      const int q_off = static_cast<int>(pair_rank) * p.nq_pass;   // pair: CTA r's queries follow CTA 0's in every per-query array
+      const float* partial = reinterpret_cast<const float*>(smem + S::kOffPartial);
+      uint64_t* keys = reinterpret_cast<uint64_t*>(smem + S::kOffKeys);
+      uint64_t* minkey_s = reinterpret_cast<uint64_t*>(smem + S::kOffMinKey);
+      int* minpos_s = reinterpret_cast<int*>(smem + S::kOffMinPos);
+      const int n_tiles_red = n_tiles;
+      uint32_t mask_next = 0;
+      int32_t fpid_next = 0;
+      if (n_tiles_red > 0) {
+        mask_next = __ldg(p.tile_end_mask + tile_base);
+        fpid_next = __ldg(p.tile_first_pid + tile_base);
+      }
+      for (int t = 0; t < n_tiles_red; ++t) {
+        const uint32_t mask = mask_next;
+        const int32_t first_pid = fpid_next;
+        if (t + 1 < n_tiles_red) {
+          mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
+          fpid_next = __ldg(p.tile_first_pid + tile_base + t + 1);
+        }
+        const int buf = t & 1;
+        mbar_wait(bars.p_full(buf), (static_cast<uint32_t>(t) >> 1) & 1u, p.status, kDevTimeoutEpilogue);
+        const int n_slots = __popc(mask);
+        const float* lane_part0 = reinterpret_cast<const float*>(smem + S::kOffLanePart);
+  #pragma unroll 1
+        for (int slot = 0; slot < n_slots; ++slot) {
+          const int64_t pid = static_cast<int64_t>(first_pid) + slot;
+          const float* lp_slot = lane_part0 + ((buf * kFastSlots + slot) * kRbMax) * kLaneStride;
+          if (slot < kFastSlots && p.rbq <= p.lane_mode_max_rbq) {
+            // many short queries per pass: lane = query, each lane sums its query's 32 * rbq lane maxima
+            // (transposed read of the stride-33 layout: conflict-free for rbq = 1)
+  #pragma unroll 1
+            for (int b0 = 0; b0 < p.nq_pass; b0 += 32) {
+              const int b = b0 + lane;
+              const bool valid = b < p.nq_pass;
+              float sc = 0.f;
+              uint64_t key = 0ull;
+              if (valid) {
+                const float* lp = lp_slot + (b * p.rbq) * kLaneStride;
+                for (int r = 0; r < p.rbq; ++r) {
+  #pragma unroll 8
+                  for (int j = 0; j < 32; ++j) sc += lp[r * kLaneStride + j];
+                }
+                const int64_t gi = static_cast<int64_t>(q_off + b) * p.n_passages + pid;
+                if (p.acc_in) sc += __ldg(p.acc_in + gi);
+                if (p.acc_out) p.acc_out[gi] = sc;
+                key = (static_cast<uint64_t>(float_to_ordered(sc)) << 32) |
+                      static_cast<uint64_t>(0xFFFFFFFFu - static_cast<uint32_t>(pid));
+              }
+              if (p.k > 0) {
+                uint32_t hits = __ballot_sync(0xffffffffu, valid && key > minkey_s[valid ? b : 0]);
+                while (hits) {  // rare after warm-up: one list update at a time
+                  const int src = __ffs(hits) - 1;
+                  hits &= hits - 1;
+                  const uint64_t cand = shfl64(key, src);
+                  const int cb = b0 + src;
+                  uint64_t minkey = minkey_s[cb];
+                  int minpos = minpos_s[cb];
+                  if (cand > minkey) {
+                    topk_replace_min(keys + cb * kMaxK, p.k, cand, minkey, minpos, lane);
+                    if (lane == 0) {
+                      minkey_s[cb] = minkey;
+                      minpos_s[cb] = minpos;
+                    }
+                    __syncwarp();
+                  }
+                }
               }
             }
-          }
-          fold_accumulator(acc, mask, m[u], init, lane_part_buf, partial_buf, j, wq, lane);
-        }
-      }
-      // this warp's row maxima / partial sums of tile t are written: order every lane's stores
-      // before lane 0's arrive (release); the reducer's wait is the matching acquire
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p_full(buf));
-    }
-  } else {
-    // ===================== reducer: score finalisation + per-CTA top-k =====================
-    // Per D tile and per (query, passage ending in the tile): sum the row partials in fixed
-    // order (deterministic), add/store partial scores if requested, offer to the top-k list.
-    const int rw = warp - kWarpRed0;  // reducer 0..kRedWarps-1 owns queries b = rw (mod kRedWarps)
-    const int q_off = static_cast<int>(pair_rank) * p.nq_pass;   // pair: CTA r's queries follow CTA 0's in every per-query array
-    const float* partial = reinterpret_cast<const float*>(smem + S::kOffPartial);
-    uint64_t* keys = reinterpret_cast<uint64_t*>(smem + S::kOffKeys);
-    uint64_t* minkey_s = reinterpret_cast<uint64_t*>(smem + S::kOffMinKey);
-    int* minpos_s = reinterpret_cast<int*>(smem + S::kOffMinPos);
-    const int n_tiles_red = n_tiles;
-    uint32_t mask_next = 0;
-    int32_t fpid_next = 0;
-    if (n_tiles_red > 0) {
-      mask_next = __ldg(p.tile_end_mask + tile_base);
-      fpid_next = __ldg(p.tile_first_pid + tile_base);
-    }
-    for (int t = 0; t < n_tiles_red; ++t) {
-      const uint32_t mask = mask_next;
-      const int32_t first_pid = fpid_next;
-      if (t + 1 < n_tiles_red) {
-        mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
-        fpid_next = __ldg(p.tile_first_pid + tile_base + t + 1);
-      }
-      const int buf = t & 1;
-      mbar_wait(bar_p_full(buf), (static_cast<uint32_t>(t) >> 1) & 1u, p.status, kDevTimeoutEpilogue);
-      const int n_slots = __popc(mask);
-      const float* lane_part0 = reinterpret_cast<const float*>(smem + S::kOffLanePart);
-#pragma unroll 1
-      for (int slot = 0; slot < n_slots; ++slot) {
-        const int64_t pid = static_cast<int64_t>(first_pid) + slot;
-        const float* lp_slot = lane_part0 + ((buf * kFastSlots + slot) * kRbMax) * kLaneStride;
-        if (slot < kFastSlots && p.rbq <= p.lane_mode_max_rbq) {
-          // many short queries per pass: lane = query, each lane sums its query's 32 * rbq lane maxima
-          // (transposed read of the stride-33 layout: conflict-free for rbq = 1)
-#pragma unroll 1
-          for (int b0 = 0; b0 < p.nq_pass; b0 += 32) {
-            const int b = b0 + lane;
-            const bool valid = b < p.nq_pass;
-            float sc = 0.f;
-            uint64_t key = 0ull;
-            if (valid) {
-              const float* lp = lp_slot + (b * p.rbq) * kLaneStride;
-              for (int r = 0; r < p.rbq; ++r) {
-#pragma unroll 8
-                for (int j = 0; j < 32; ++j) sc += lp[r * kLaneStride + j];
+          } else {
+  #pragma unroll 1
+            for (int b = 0; b < p.nq_pass; ++b) {
+              // score of (query b, passage pid): the whole warp sums the row-block partials in fixed order
+              float sc = 0.f;
+              if (slot < kFastSlots) {
+                const float* lp = lp_slot + (b * p.rbq) * kLaneStride + lane;
+  #pragma unroll 2
+                for (int r = 0; r < p.rbq; ++r) sc += lp[r * kLaneStride];
+                sc = warp_sum(sc);
+              } else {
+                const float* pr = partial + (buf * kHbMax + 2 * b * p.rbq) * kSlots + slot;
+  #pragma unroll 2
+                for (int r = 0; r < 2 * p.rbq; ++r) sc += pr[r * kSlots];
               }
               const int64_t gi = static_cast<int64_t>(q_off + b) * p.n_passages + pid;
               if (p.acc_in) sc += __ldg(p.acc_in + gi);
-              if (p.acc_out) p.acc_out[gi] = sc;
-              key = (static_cast<uint64_t>(float_to_ordered(sc)) << 32) |
-                    static_cast<uint64_t>(0xFFFFFFFFu - static_cast<uint32_t>(pid));
-            }
-            if (p.k > 0) {
-              uint32_t hits = __ballot_sync(0xffffffffu, valid && key > minkey_s[valid ? b : 0]);
-              while (hits) {  // rare after warm-up: one list update at a time
-                const int src = __ffs(hits) - 1;
-                hits &= hits - 1;
-                const uint64_t cand = shfl64(key, src);
-                const int cb = b0 + src;
-                uint64_t minkey = minkey_s[cb];
-                int minpos = minpos_s[cb];
-                if (cand > minkey) {
-                  topk_replace_min(keys + cb * kMaxK, p.k, cand, minkey, minpos, lane);
+              if (p.acc_out && lane == 0) p.acc_out[gi] = sc;
+              if (p.k > 0) {
+                const uint64_t key = (static_cast<uint64_t>(float_to_ordered(sc)) << 32) |
+                                     static_cast<uint64_t>(0xFFFFFFFFu - static_cast<uint32_t>(pid));
+                uint64_t minkey = minkey_s[b];
+                if (key > minkey) {  // warp-uniform; rare after warm-up
+                  int minpos = minpos_s[b];
+                  topk_replace_min(keys + b * kMaxK, p.k, key, minkey, minpos, lane);
                   if (lane == 0) {
-                    minkey_s[cb] = minkey;
-                    minpos_s[cb] = minpos;
+                    minkey_s[b] = minkey;
+                    minpos_s[b] = minpos;
                   }
                   __syncwarp();
                 }
               }
             }
           }
-        } else {
-#pragma unroll 1
-          for (int b = 0; b < p.nq_pass; ++b) {
-            // score of (query b, passage pid): the whole warp sums the row-block partials in fixed order
-            float sc = 0.f;
-            if (slot < kFastSlots) {
-              const float* lp = lp_slot + (b * p.rbq) * kLaneStride + lane;
-#pragma unroll 2
-              for (int r = 0; r < p.rbq; ++r) sc += lp[r * kLaneStride];
-              sc = warp_sum(sc);
-            } else {
-              const float* pr = partial + (buf * kHbMax + 2 * b * p.rbq) * kSlots + slot;
-#pragma unroll 2
-              for (int r = 0; r < 2 * p.rbq; ++r) sc += pr[r * kSlots];
-            }
-            const int64_t gi = static_cast<int64_t>(q_off + b) * p.n_passages + pid;
-            if (p.acc_in) sc += __ldg(p.acc_in + gi);
-            if (p.acc_out && lane == 0) p.acc_out[gi] = sc;
-            if (p.k > 0) {
-              const uint64_t key = (static_cast<uint64_t>(float_to_ordered(sc)) << 32) |
-                                   static_cast<uint64_t>(0xFFFFFFFFu - static_cast<uint32_t>(pid));
-              uint64_t minkey = minkey_s[b];
-              if (key > minkey) {  // warp-uniform; rare after warm-up
-                int minpos = minpos_s[b];
-                topk_replace_min(keys + b * kMaxK, p.k, key, minkey, minpos, lane);
-                if (lane == 0) {
-                  minkey_s[b] = minkey;
-                  minpos_s[b] = minpos;
-                }
-                __syncwarp();
-              }
-            }
-          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bars.p_empty(buf));
+      }
+      // ---- publish this CTA's candidates ----
+      if (p.k > 0) {
+        __syncwarp();
+        for (int b = rw; b < p.nq_pass; b += kRedWarps) {
+          uint64_t* dst = p.cand_keys + (static_cast<int64_t>(cta) * p.cand_q_stride + p.cand_q_first + q_off + b) * p.k;
+          for (int i = lane; i < p.k; i += 32) dst[i] = keys[b * kMaxK + i];
         }
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p_empty(buf));
     }
-    // ---- publish this CTA's candidates ----
-    if (p.k > 0) {
-      __syncwarp();
-      for (int b = rw; b < p.nq_pass; b += kRedWarps) {
-        uint64_t* dst = p.cand_keys + (static_cast<int64_t>(cta) * p.cand_q_stride + p.cand_q_first + q_off + b) * p.k;
-        for (int i = lane; i < p.k; i += 32) dst[i] = keys[b * kMaxK + i];
-      }
+  } else {
+    // ===================== consumers: wgmma + passage maxima =====================
+    const int wg = warp >> 2;
+    const int wq = warp & 3;           // warp inside the warpgroup: accumulator rows 16 wq .. 16 wq + 15
+    // warp-uniform block count of this warpgroup, dispatched to a loop that knows it at compile time (with a
+    // run-time count ptxas serialises the wgmma of the two accumulators)
+    const int nb = wg < n_blocks ? (n_blocks - wg + kWgs - 1) / kWgs : 0;
+    if (nb == 1) {
+      scan_consumer<1, kWgs, kPair, kOverlap>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+    } else if (nb == 2) {
+      scan_consumer<2, kWgs, kPair, kOverlap>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+    } else if constexpr (kBlocksPerWg >= 3) {
+      if (nb == 3) scan_consumer<3, kWgs, kPair, kOverlap>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     }
   }
 

@@ -6,6 +6,7 @@ bit-identical results of <2> and <3> over a spread of shapes, then timing of all
 import argparse
 import ctypes as C
 import os
+import statistics
 import sys
 
 import numpy as np
@@ -21,6 +22,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--passages", type=int, default=200_000)
     ap.add_argument("--skip-parity", action="store_true")
+    ap.add_argument("--repeat", type=int, default=1, help="timed repetitions per shape and variant (median, spread)")
     ap.add_argument("--sustained", type=float, default=0.0, help="seconds per block of the power-capped A/B (0 = skip)")
     args = ap.parse_args()
     L = _cabi.lib()
@@ -63,8 +65,9 @@ def main():
     D = bench.build_shard(0, n_p, nd, dev)
     corpus = R.FlatCorpus(D, np.full(n_p, nd, dtype=np.int32))
     g = torch.Generator(device=dev).manual_seed(0)
-    print("| shape | variant | scan launch ms | TFLOP/s (algorithmic) | GB/s | q/s at 1M |\n|---|---|---:|---:|---:|---:|")
-    for (B, nq) in [(16, 320), (2, 320), (1, 320), (20, 32), (1, 32), (3, 832), (4, 256), (2, 128)]:
+    print("| shape | variant | scan launch ms | spread ms | TFLOP/s (algorithmic) | GB/s | q/s at 1M |\n"
+          "|---|---|---:|---:|---:|---:|---:|")
+    for (B, nq) in [(16, 320), (2, 320), (1, 320), (20, 32), (12, 32), (1, 32), (3, 832), (4, 256), (2, 128)]:
         Q = torch.nn.functional.normalize(torch.randn((B, nq, 128), device=dev, generator=g), dim=-1).bfloat16()
         for variant in (2, 3, 4):
             if variant == 4 and (B % 2 or nq > 384):   # pairs of whole queries that fit one pass
@@ -73,24 +76,28 @@ def main():
             for _ in range(2):
                 R.maxsim_topk(corpus, Q, 5)
             torch.cuda.synchronize()
-            L.flmr_scan_kernel_stats(None, None, 1)
-            L.flmr_set_profiling(1)
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            iters = 6
-            for _ in range(iters):
-                R.maxsim_topk(corpus, Q, 5)
-            e1.record()
-            torch.cuda.synchronize()
-            tot, cnt = C.c_double(0), C.c_int64(0)
-            L.flmr_scan_kernel_stats(C.byref(tot), C.byref(cnt), 1)
-            L.flmr_set_profiling(0)
-            ms_call = e0.elapsed_time(e1) / iters
-            ms_launch = tot.value / cnt.value
+            samples = []   # (ms per call, ms per scan launch, ms of scan per call)
+            for _ in range(args.repeat):
+                L.flmr_scan_kernel_stats(None, None, 1)
+                L.flmr_set_profiling(1)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                iters = 6
+                for _ in range(iters):
+                    R.maxsim_topk(corpus, Q, 5)
+                e1.record()
+                torch.cuda.synchronize()
+                tot, cnt = C.c_double(0), C.c_int64(0)
+                L.flmr_scan_kernel_stats(C.byref(tot), C.byref(cnt), 1)
+                L.flmr_set_profiling(0)
+                samples.append((e0.elapsed_time(e1) / iters, tot.value / cnt.value, tot.value / iters))
+            ms_call, ms_launch, scan_call = (statistics.median(x) for x in zip(*samples))
+            spread = max(x[1] for x in samples) - min(x[1] for x in samples)
             flops_call = 2.0 * B * nq * 128 * n_p * nd
-            print("| B=%d Nq=%d | %s | %.3f | %.0f | %.0f | %.1f |"
-                  % (B, nq, {2: "2 WGs", 3: "3 WGs", 4: "CTA pairs (multicast)"}[variant], ms_launch, flops_call / (tot.value / iters) / 1e9,
-                     n_p * nd * 256.0 / ms_launch / 1e6, B / ms_call * 1e3 * n_p / 1e6), flush=True)
+            print("| B=%d Nq=%d | %s | %.3f | %.3f | %.0f | %.0f | %.1f |"
+                  % (B, nq, {2: "2 WGs", 3: "3 WGs", 4: "CTA pairs (multicast)"}[variant], ms_launch, spread,
+                     flops_call / scan_call / 1e9, n_p * nd * 256.0 / ms_launch / 1e6, B / ms_call * 1e3 * n_p / 1e6),
+                  flush=True)
     # sustained (power-capped) A/B at the headline shape: alternate the two variants in blocks of ~2 s, three rounds
     if args.sustained:
         import time
