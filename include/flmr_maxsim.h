@@ -23,6 +23,11 @@
  *   flmr_topk_merge
  *       the only exchange step of the sharded path (SURVEY.md §8e): merges per-shard top-k lists
  *       (gathered by the host with one NCCL all-gather) into the global top-k.
+ *   FLMR_CORPUS_FP8, flmr_corpus_storage
+ *       an e4m3 corpus: the scan reads half the bytes per token and runs fp8 MMAs, so its scores are
+ *       APPROXIMATE; the exact bf16 rows stay in pinned host memory for flmr_corpus_gather.  The first stage of
+ *       a two-stage search whose exact second stage re-scores a shortlist (the Python Searcher does both), as
+ *       PLAID scores its ndocs/4 survivors exactly (CB/search/index_storage.py:160-177).
  *   flmr_debug_maxsim_scores_simt
  *       test infrastructure: an independent plain-SIMT fp32 device kernel used by tests to
  *       cross-check the tensor-core kernel at sizes where the CPU oracle is too slow.
@@ -66,6 +71,9 @@ extern "C" {
 #define FLMR_CORPUS_COPY 0u  /* always copy the token matrix into library-owned HBM            */
 #define FLMR_CORPUS_ADOPT 1u /* tokens is a device pointer; keep it (zero-copy) when every     \
                                 doclen is a multiple of FLMR_TOKEN_GROUP, else copy+repack     */
+#define FLMR_CORPUS_FP8 2u   /* HBM holds the tokens as e4m3 (round to nearest even, saturated;  \
+                                half the bytes); the library keeps a pinned host copy of the      \
+                                exact bf16 rows.  Not combinable with FLMR_CORPUS_ADOPT.         */
 
 #define FLMR_DIM 128        /* embedding dim of FLMR / ColBERT (CB/infra/config/settings.py:101) */
 #define FLMR_TOKEN_GROUP 4  /* passages are stored padded to a multiple of this many tokens     */
@@ -111,6 +119,18 @@ int flmr_corpus_destroy(flmr_corpus_t* corpus);
 int flmr_corpus_info(const flmr_corpus_t* corpus, flmr_corpus_info_t* out);
 
 /*
+ * How the corpus stores its tokens: *storage = 0 (bf16 in HBM) or 1 (FLMR_CORPUS_FP8: e4m3 in HBM, counted in
+ * hbm_bytes, plus the bf16 master in pinned host memory, *host_bytes bytes; 0 for a bf16 corpus).  Either output
+ * may be NULL.
+ *
+ * On an e4m3 corpus flmr_maxsim_scores, flmr_maxsim_topk and flmr_maxsim_topk_sharded compute MaxSim of e4m3(Q)
+ * against e4m3(D) with fp32 accumulation (Q rounded to nearest even, no scale): APPROXIMATE scores (up to about 6e-3
+ * relative on normalised embeddings), fit to shortlist candidates, not to rank them.  flmr_corpus_gather reads the
+ * exact bf16 rows of the master, and flmr_debug_maxsim_scores_simt computes the e4m3 semantics.
+ */
+int flmr_corpus_storage(const flmr_corpus_t* corpus, int* storage, int64_t* host_bytes);
+
+/*
  * Streaming construction of a corpus shard — the index LOAD path (replaces IndexLoader / ResidualEmbeddings.load_chunks,
  * CB/search/index_loader.py:24-62, CB/indexing/codecs/residual_embeddings.py:24-69): the padded token matrix is
  * allocated once from the doclens, then packed bf16 rows arrive IN ORDER, in chunks of any size, from host memory
@@ -123,6 +143,10 @@ int flmr_corpus_info(const flmr_corpus_t* corpus, flmr_corpus_info_t* out);
  */
 int flmr_corpus_builder_create(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
                                int64_t pid_base, flmr_corpus_builder_t** out);
+/* The same with corpus flags: FLMR_CORPUS_FP8 builds an e4m3 corpus (the staged rows fill the bf16 master and
+ * HBM receives e4m3); 0 is flmr_corpus_builder_create. */
+int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                  int64_t pid_base, unsigned flags, flmr_corpus_builder_t** out);
 int flmr_corpus_builder_append(flmr_corpus_builder_t* b, const void* h_tokens_bf16, int64_t n_rows);
 int flmr_corpus_builder_append_file(flmr_corpus_builder_t* b, const char* path, int64_t byte_offset, int64_t n_rows);
 int flmr_corpus_builder_finish(flmr_corpus_builder_t* b, flmr_corpus_t** out, double* host_fill_seconds);
@@ -294,7 +318,7 @@ int flmr_maxsim_backward_grouped(const void* d_q, int n_queries, int nq, const v
                                  float* d_dq, float* d_dd, int device, void* stream);
 
 /* Test infrastructure: plain SIMT fp32 MaxSim of every passage (same contract as
- * flmr_maxsim_scores), independent of the tensor-core kernel. */
+ * flmr_maxsim_scores, e4m3 semantics on an e4m3 corpus), independent of the tensor-core kernel. */
 int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* corpus, const void* d_q, int n_queries,
                                   int nq, unsigned flags, float* d_out_scores, void* stream);
 
@@ -302,8 +326,9 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* corpus, const void* d_q, 
  * product behaviour: normal passes, those with three resident query tiles on the three-warpgroup kernel),
  * 2 = flmr_scan_kernel<2> (two consumer warpgroups), normal passes only, 3 = flmr_scan_kernel<3> (three
  * warpgroups), normal passes only, 4 = CTA-pair passes (clusters of two CTAs stream one token
- * range, each D tile fetched once and TMA-multicast to both) whenever a call has enough queries, on any shard —
- * so the parity suite can run against any of them at any shape. */
+ * range, each D tile fetched once and TMA-multicast to both) whenever a call has enough queries, on any bf16 shard
+ * (a search on an e4m3 corpus returns FLMR_ERR_UNSUPPORTED) — so the parity suite can run against any of them at
+ * any shape. */
 int flmr_debug_set_scan_variant(int variant);
 
 /* Test infrastructure: which kernel flmr_maxsim_argmax(_grouped) runs on the calling thread — 0 = chosen by size

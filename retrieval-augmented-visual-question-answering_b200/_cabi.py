@@ -15,6 +15,8 @@ FLMR_OK = 0
 FLAG_RELU = 1
 CORPUS_COPY = 0
 CORPUS_ADOPT = 1
+CORPUS_FP8 = 2
+STORAGES = ("bf16", "fp8")     # flmr_corpus_storage codes 0 and 1
 DIM = 128
 TOKEN_GROUP = 4
 MAX_K = 128
@@ -33,12 +35,12 @@ TILE_TOKENS = _header_define("FLMR_TILE_TOKENS")
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
-    "flmr_corpus_create", "flmr_corpus_destroy", "flmr_corpus_info",
+    "flmr_corpus_create", "flmr_corpus_destroy", "flmr_corpus_info", "flmr_corpus_storage",
     "flmr_workspace_create", "flmr_workspace_destroy", "flmr_workspace_status",
     "flmr_maxsim_scores", "flmr_maxsim_topk", "flmr_topk_merge", "flmr_topk_select", "flmr_plaid_decode",
     "flmr_maxsim_argmax", "flmr_maxsim_backward", "flmr_corpus_gather",
     "flmr_maxsim_argmax_grouped", "flmr_maxsim_backward_grouped", "flmr_ib_loss",
-    "flmr_corpus_builder_create", "flmr_corpus_builder_append", "flmr_corpus_builder_append_file",
+    "flmr_corpus_builder_create", "flmr_corpus_builder_create_ex", "flmr_corpus_builder_append", "flmr_corpus_builder_append_file",
     "flmr_corpus_builder_finish", "flmr_corpus_builder_destroy",
     "flmr_comm_unique_id", "flmr_comm_create", "flmr_comm_adopt", "flmr_comm_destroy", "flmr_comm_info",
     "flmr_topk_exchange", "flmr_maxsim_topk_sharded",
@@ -80,6 +82,7 @@ def lib() -> C.CDLL:
     L.flmr_corpus_create.argtypes = [vp, vp, i64, i32, i32, i64, u32, C.POINTER(vp)]
     L.flmr_corpus_destroy.argtypes = [vp]
     L.flmr_corpus_info.argtypes = [vp, C.POINTER(CorpusInfo)]
+    L.flmr_corpus_storage.argtypes = [vp, C.POINTER(i32), C.POINTER(i64)]
     L.flmr_workspace_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
     L.flmr_workspace_destroy.argtypes = [vp]
     L.flmr_workspace_status.argtypes = [vp, C.POINTER(i32)]
@@ -95,6 +98,7 @@ def lib() -> C.CDLL:
     L.flmr_maxsim_argmax_grouped.argtypes = [vp, i32, i32, vp, vp, i32, i32, vp, vp, i32, vp]
     L.flmr_maxsim_backward_grouped.argtypes = [vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, i32, vp]
     L.flmr_corpus_builder_create.argtypes = [vp, i64, i32, i32, i64, C.POINTER(vp)]
+    L.flmr_corpus_builder_create_ex.argtypes = [vp, i64, i32, i32, i64, u32, C.POINTER(vp)]
     L.flmr_corpus_builder_append.argtypes = [vp, vp, i64]
     L.flmr_corpus_builder_append_file.argtypes = [vp, C.c_char_p, i64, i64]
     L.flmr_corpus_builder_finish.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_double)]

@@ -27,6 +27,18 @@ def _as_doclens(doclens) -> np.ndarray:
     return arr
 
 
+def _storage_flag(storage: str) -> int:
+    if storage not in _cabi.STORAGES:
+        raise ValueError("storage must be one of %s, got %r" % (_cabi.STORAGES, storage))
+    return _cabi.CORPUS_FP8 if storage == "fp8" else 0
+
+
+def _read_storage(handle) -> str:
+    code = C.c_int(0)
+    _cabi.check(_cabi.lib().flmr_corpus_storage(handle, C.byref(code), None))
+    return _cabi.STORAGES[code.value]
+
+
 class FlatCorpus:
     """One GPU's shard of the passage-token matrix, resident in HBM.
 
@@ -35,12 +47,16 @@ class FlatCorpus:
                adopted zero-copy (and kept alive by this object).
     doclens  : per-passage token counts (>= 1 each).
     pid_base : global id of this shard's first passage (sharded search, SURVEY.md §8e).
+    storage  : "bf16" (default) or "fp8": HBM holds the tokens as e4m3 (half the bytes; the scan's scores become
+               approximate, ``Searcher`` re-ranks a shortlist exactly) and the library keeps the exact bf16 rows
+               in pinned host memory, where ``gather_padded`` reads them.  An fp8 corpus never adopts ``tokens``.
     """
 
     def __init__(self, tokens: torch.Tensor, doclens, device: Optional[Union[int, torch.device]] = None,
-                 pid_base: int = 0, adopt: bool = True):
+                 pid_base: int = 0, adopt: bool = True, storage: str = "bf16"):
         if not torch.cuda.is_available():
             raise RuntimeError("FlatCorpus needs a CUDA device: there is no CPU fallback for this path")
+        fp8 = _storage_flag(storage)
         L = _cabi.lib()
         self.doclens = _as_doclens(doclens)
         if tokens.dim() != 2 or tokens.size(1) != _cabi.DIM:
@@ -59,7 +75,7 @@ class FlatCorpus:
         tokens = tokens.contiguous()
         if tokens.is_cuda and tokens.device != device:
             tokens = tokens.to(device)
-        flags = _cabi.CORPUS_ADOPT if (adopt and tokens.is_cuda) else _cabi.CORPUS_COPY
+        flags = fp8 or (_cabi.CORPUS_ADOPT if (adopt and tokens.is_cuda) else _cabi.CORPUS_COPY)
         if tokens.is_cuda:
             torch.cuda.current_stream(device).synchronize()  # producer kernels of `tokens` are done
         handle = C.c_void_p()
@@ -71,6 +87,7 @@ class FlatCorpus:
         info = _cabi.CorpusInfo()
         _cabi.check(L.flmr_corpus_info(self._h, C.byref(info)))
         self.info = info
+        self.storage = _read_storage(self._h)
         self._keepalive = tokens if info.adopted else None
         self._ws = None
         self.pid_base = int(pid_base)
@@ -85,6 +102,7 @@ class FlatCorpus:
         info = _cabi.CorpusInfo()
         _cabi.check(_cabi.lib().flmr_corpus_info(self._h, C.byref(info)))
         self.info = info
+        self.storage = _read_storage(self._h)
         self._keepalive = None
         self._ws = None
         self.pid_base = int(pid_base)
@@ -92,19 +110,22 @@ class FlatCorpus:
         return self
 
     @classmethod
-    def from_index(cls, path: str, device=None, rank: int = 0, world_size: int = 1) -> "FlatCorpus":
+    def from_index(cls, path: str, device=None, rank: int = 0, world_size: int = 1,
+                   storage: str = "bf16") -> "FlatCorpus":
         """Load a flat index (index_io.py) — or, with world_size > 1, only this rank's contiguous,
         token-balanced passage shard of it (SURVEY.md 8e) — into HBM.
 
         The token files are streamed by the C-level corpus builder: ``pread`` straight into two pinned staging
         buffers (8 reader threads, the fill of one buffer overlaps the DMA of the other) and from there into the
         padded layout — no numpy copy of the shard, no pageable ``cudaMemcpy``.  ``load_stats`` records seconds
-        and GB/s (replaces IndexLoader / ResidualEmbeddings.load_chunks, colbert/search/index_loader.py:24-62)."""
+        and GB/s (replaces IndexLoader / ResidualEmbeddings.load_chunks, colbert/search/index_loader.py:24-62).
+        ``storage="fp8"``: the staged rows fill the bf16 master in pinned host memory, HBM receives e4m3."""
         import time
         from .index_io import index_token_files
         from .sharded import shard_ranges
         if not torch.cuda.is_available():
             raise RuntimeError("FlatCorpus needs a CUDA device: there is no CPU fallback for this path")
+        flags = _storage_flag(storage)
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device())
         device = torch.device(device) if not isinstance(device, torch.device) else device
@@ -118,8 +139,8 @@ class FlatCorpus:
         L = _cabi.lib()
         t0 = time.perf_counter()
         b = C.c_void_p()
-        _cabi.check(L.flmr_corpus_builder_create(doclens.ctypes.data_as(C.c_void_p), len(doclens), _cabi.DIM,
-                                                 int(device.index), int(p0), C.byref(b)))
+        _cabi.check(L.flmr_corpus_builder_create_ex(doclens.ctypes.data_as(C.c_void_p), len(doclens), _cabi.DIM,
+                                                    int(device.index), int(p0), flags, C.byref(b)))
         try:
             for fname, f0, fn, _rows in files:
                 a, e = max(p0, f0), min(p1, f0 + fn)
@@ -142,20 +163,21 @@ class FlatCorpus:
         return self
 
     @classmethod
-    def from_plaid(cls, path: str, device=None, rank: int = 0, world_size: int = 1) -> "FlatCorpus":
+    def from_plaid(cls, path: str, device=None, rank: int = 0, world_size: int = 1,
+                   storage: str = "bf16") -> "FlatCorpus":
         """Decode a reference PLAID index directory on the GPU (plaid.py) and keep it resident — with
         world_size > 1 only this rank's contiguous, token-balanced passage shard (SURVEY.md 8e)."""
         from .plaid import plaid_to_flat, read_plaid_doclens, read_plaid_metadata
         from .sharded import shard_ranges
         if world_size == 1:
             tokens, doclens = plaid_to_flat(path, device)
-            return cls(tokens, doclens, device=tokens.device)
+            return cls(tokens, doclens, device=tokens.device, storage=storage)
         all_doclens = np.concatenate(read_plaid_doclens(path, read_plaid_metadata(path)["num_chunks"]))
         p0, p1 = shard_ranges(all_doclens, world_size)[rank]
         if p0 == p1:
             return None
         tokens, doclens = plaid_to_flat(path, device, passage_range=(p0, p1))
-        return cls(tokens, doclens, device=tokens.device, pid_base=p0)
+        return cls(tokens, doclens, device=tokens.device, pid_base=p0, storage=storage)
 
     # -- properties ---------------------------------------------------------------------------
     @property
@@ -181,7 +203,8 @@ class FlatCorpus:
         return self._ws
 
     def gather_padded(self, pids: torch.Tensor, nd_max: Optional[int] = None):
-        """Retrieved passages as a padded batch, straight out of HBM: ``pids`` (any shape, global ids) ->
+        """Retrieved passages as a padded batch, straight out of HBM (an fp8 corpus: the exact bf16 rows of its
+        pinned host master): ``pids`` (any shape, global ids) ->
         (tokens bf16 ``[*pids.shape, nd_max, 128]``, mask bool ``[*pids.shape, nd_max, 1]``).  ``nd_max``
         defaults to the longest requested passage.  Ids outside this shard give an all-masked zero row.
         Replaces the host-dictionary lookup + stack + H2D of rag_model_blip.py:414-425."""
@@ -217,5 +240,5 @@ class FlatCorpus:
 
     def __repr__(self) -> str:
         i = self.info
-        return ("FlatCorpus(n_passages=%d, n_tokens=%d, device=%s, pid_base=%d, n_ctas=%d, adopted=%d)"
-                % (i.n_passages, i.n_tokens, self.device, i.pid_base, i.n_ctas, i.adopted))
+        return ("FlatCorpus(n_passages=%d, n_tokens=%d, device=%s, pid_base=%d, n_ctas=%d, adopted=%d, storage=%s)"
+                % (i.n_passages, i.n_tokens, self.device, i.pid_base, i.n_ctas, i.adopted, self.storage))

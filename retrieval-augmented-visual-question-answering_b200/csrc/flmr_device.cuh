@@ -226,6 +226,23 @@ __device__ __forceinline__ void wgmma_m64n96k16(float (&d)[48], uint64_t a_desc,
       : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
+// D (+)= A[smem] * B[smem]^T, m64n96k32, e4m3 in / fp32 accumulate; d[48] per thread, the same fragment as
+// m64n96k16.  fp8 operands are K-major only and take no transpose immediates.
+__device__ __forceinline__ void wgmma_m64n96k32_e4m3(float (&d)[48], uint64_t a_desc, uint64_t b_desc,
+                                                     uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k32.f32.e4m3.e4m3 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47"
+      "}, %48, %49, p, 1, 1;\n\t}"
+      : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16), FLMR_F8(24), FLMR_F8(32), FLMR_F8(40)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
 // D (+)= A[smem] * B[smem]^T, m64n128k16, bf16 in / fp32 accumulate; d[64] per thread.
 __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(

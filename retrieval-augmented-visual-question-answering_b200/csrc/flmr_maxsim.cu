@@ -8,6 +8,7 @@
 // cudaGetDriverEntryPoint, so the library loads (and its symbols can be checked) without a GPU.
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <fcntl.h>
@@ -97,16 +98,18 @@ int get_encode_fn(EncodeTiledFn* out) {
   return FLMR_OK;
 }
 
-// bf16 [rows, 128] row-major matrix, box = 64 columns (128 B, one swizzle span) x box_rows rows.
-int encode_rows_map(CUtensorMap* map, const void* base, uint64_t rows, uint32_t box_rows) {
+// bf16 [rows, 128] row-major matrix, box = 64 columns (128 B, one swizzle span) x box_rows rows; fp8: an e4m3
+// [rows, 128] matrix (as bytes), box = 128 columns (128 B) x box_rows rows.
+int encode_rows_map(CUtensorMap* map, const void* base, uint64_t rows, uint32_t box_rows, bool fp8 = false) {
   EncodeTiledFn enc = nullptr;
   int rc = get_encode_fn(&enc);
   if (rc) return rc;
   const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(kDim), static_cast<cuuint64_t>(rows)};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(kDim) * 2};
-  const cuuint32_t box[2] = {64u, box_rows};
+  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(kDim) * (fp8 ? 1 : 2)};
+  const cuuint32_t box[2] = {fp8 ? 128u : 64u, box_rows};
   const cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride,
+  CUresult r = enc(map, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                   const_cast<void*>(base), gdim, gstride,
                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(FLMR_ERR_CUDA, "cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
@@ -115,9 +118,23 @@ int encode_rows_map(CUtensorMap* map, const void* base, uint64_t rows, uint32_t 
 
 // ---- helper kernels --------------------------------------------------------------------------------
 
+// Eight bf16 (16 bytes) -> eight e4m3 (8 bytes): bf16 -> f32 is exact, f32 -> e4m3 rounds to nearest even and
+// saturates at +-448 (cvt.rn.satfinite.e4m3x2.f32).  No scale: a zero stays exactly zero.
+__device__ __forceinline__ uint32_t bf16x4_to_e4m3x4(uint32_t a, uint32_t b) {
+  const float2 fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&a));
+  const float2 fb = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&b));
+  const uint32_t lo = __nv_cvt_float2_to_fp8x2(fa, __NV_SATFINITE, __NV_E4M3);   // element 0 in the low byte
+  const uint32_t hi = __nv_cvt_float2_to_fp8x2(fb, __NV_SATFINITE, __NV_E4M3);
+  return lo | (hi << 16);
+}
+__device__ __forceinline__ uint2 bf16x8_to_e4m3x8(uint4 v) {
+  return make_uint2(bf16x4_to_e4m3x4(v.x, v.y), bf16x4_to_e4m3x4(v.z, v.w));
+}
+
 // Stage the resident queries of EVERY pass of a call in one launch (blockIdx.y = pass): each query padded
 // with zero rows to rbq*32 rows, the pass's block padded with zero rows to n_mtiles*128 rows, pass i at
-// qpad + i * kMtMax*128 rows.  One thread per 16 bytes.
+// qpad + i * kMtMax*128 rows.  One thread per 16 bytes of output.  kFp8: the rows are written as e4m3 (128 B per
+// row, the slots keep their bf16 stride).
 constexpr int kStageMaxPasses = 64;
 struct StagePass {
   int32_t q_first, n_q, row0, rows, rbq, n_rows_pad;
@@ -125,25 +142,36 @@ struct StagePass {
 struct StageParams {
   StagePass pass[kStageMaxPasses];
 };
+template <bool kFp8>
 __global__ void flmr_stage_queries_kernel(const uint4* __restrict__ q, uint4* __restrict__ qpad,
                                           int nq_total_rows, const __grid_constant__ StageParams sp) {
+  constexpr int kChunkBits = kFp8 ? 3 : 4;   // log2 of the 16-byte output chunks per row
   const StagePass& ps = sp.pass[blockIdx.y];
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  const int r = idx >> 4, c = idx & 15;
+  const int r = idx >> kChunkBits, c = idx & ((1 << kChunkBits) - 1);
   if (r >= ps.n_rows_pad) return;
   const int rows_q = ps.rbq * 32;
   const int b = r / rows_q, i = r % rows_q;
   uint4 v = make_uint4(0u, 0u, 0u, 0u);
-  if (b < ps.n_q && i < ps.rows)
-    v = q[(static_cast<int64_t>(ps.q_first + b) * nq_total_rows + ps.row0 + i) * 16 + c];
+  if (b < ps.n_q && i < ps.rows) {
+    const uint4* row = q + (static_cast<int64_t>(ps.q_first + b) * nq_total_rows + ps.row0 + i) * 16;
+    if constexpr (kFp8) {
+      const uint2 lo = bf16x8_to_e4m3x8(row[2 * c]), hi = bf16x8_to_e4m3x8(row[2 * c + 1]);
+      v = make_uint4(lo.x, lo.y, hi.x, hi.y);
+    } else {
+      v = row[c];
+    }
+  }
   qpad[static_cast<int64_t>(blockIdx.y) * (kMtMax * kTileM * 16) + idx] = v;
 }
 
 // Copy passages into the padded layout: passage p occupies rows [poff[p], poff[p+1]) of dst, its
-// last token repeated over the padding rows.  One warp per passage, 2 rows per iteration.
+// last token repeated over the padding rows.  One warp per passage, 2 rows per iteration.  dst8 (an e4m3 corpus,
+// may be null): the same rows converted to e4m3, in the same layout with 128-byte rows.
 __global__ void flmr_repack_kernel(const uint4* __restrict__ src, const int64_t* __restrict__ soff,
                                    const int64_t* __restrict__ poff, uint4* __restrict__ dst,
-                                   int64_t p_begin, int64_t p_count, int64_t src_row_base) {
+                                   uint2* __restrict__ dst8, int64_t p_begin, int64_t p_count,
+                                   int64_t src_row_base) {
   const int64_t w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= p_count) return;
@@ -153,16 +181,19 @@ __global__ void flmr_repack_kernel(const uint4* __restrict__ src, const int64_t*
   const int half = lane >> 4, c = lane & 15;
   for (int64_t j = half; j < plen; j += 2) {
     const int64_t sj = j < len ? j : len - 1;
-    dst[(d0 + j) * 16 + c] = src[(s0 - src_row_base + sj) * 16 + c];
+    const uint4 v = src[(s0 - src_row_base + sj) * 16 + c];
+    dst[(d0 + j) * 16 + c] = v;
+    if (dst8) dst8[(d0 + j) * 16 + c] = bf16x8_to_e4m3x8(v);
   }
 }
 
 // Streamed corpus load: rows [s0, s0 + n) of the PACKED source order (staged at `src`) go to their place in the
 // padded layout; the last token of a passage is also copied over its padding rows.  Chunks need not start or end
 // on passage boundaries.  One half-warp per row; the passage of a row is found by binary search in `soff`.
+// dst8 (may be null): the rows also go to an e4m3 matrix of the same layout, as in flmr_repack_kernel.
 __global__ void flmr_scatter_rows_kernel(const uint4* __restrict__ src, const int64_t* __restrict__ soff,
                                          const int64_t* __restrict__ poff, uint4* __restrict__ dst,
-                                         int64_t s0, int64_t n, int64_t n_passages) {
+                                         uint2* __restrict__ dst8, int64_t s0, int64_t n, int64_t n_passages) {
   const int64_t r = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 4;
   const int c = threadIdx.x & 15;
   if (r >= n) return;
@@ -173,15 +204,39 @@ __global__ void flmr_scatter_rows_kernel(const uint4* __restrict__ src, const in
     if (soff[mid] <= srow) lo = mid; else hi = mid;
   }
   const uint4 v = src[r * 16 + c];
+  const uint2 v8 = dst8 ? bf16x8_to_e4m3x8(v) : make_uint2(0u, 0u);
   const int64_t d = poff[lo] + (srow - soff[lo]);
-  dst[d * 16 + c] = v;
-  if (srow == soff[lo + 1] - 1)             // last token: fill the group padding with copies
-    for (int64_t j = d + 1; j < poff[lo + 1]; ++j) dst[j * 16 + c] = v;
+  const int64_t d_end = srow == soff[lo + 1] - 1 ? poff[lo + 1] : d + 1;   // last token: fill the group padding
+  for (int64_t j = d; j < d_end; ++j) {
+    dst[j * 16 + c] = v;
+    if (dst8) dst8[j * 16 + c] = v8;
+  }
+}
+
+// Rows of bf16 rounded to e4m3 and back (exact: every e4m3 value is a bf16 value), 16 bytes per thread: the queries
+// of the SIMT cross-check on an e4m3 corpus.
+__global__ void flmr_round_e4m3_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int64_t n_chunks) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n_chunks) return;
+  const uint2 v8 = bf16x8_to_e4m3x8(src[i]);
+  const uint32_t w[2] = {v8.x, v8.y};
+  uint32_t out[4];
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {
+    const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w[h >> 1] >> (16 * (h & 1))),
+                                                     __NV_E4M3);
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+    const __nv_bfloat162 b = __floats2bfloat162_rn(f.x, f.y);
+    out[h] = *reinterpret_cast<const uint32_t*>(&b);
+  }
+  dst[i] = make_uint4(out[0], out[1], out[2], out[3]);
 }
 
 // Independent plain-SIMT MaxSim (test infrastructure): one block per (passage, query), one thread
 // per query token (looping if nq > blockDim), fp32 FMA over bf16 inputs, fixed-order block sum.
-__global__ void flmr_simt_maxsim_kernel(const __nv_bfloat16* __restrict__ d, const int64_t* poff,
+// kFp8: the corpus matrix is e4m3 (the queries come already rounded to e4m3, flmr_round_e4m3_kernel).
+template <bool kFp8>
+__global__ void flmr_simt_maxsim_kernel(const void* __restrict__ d_any, const int64_t* poff,
                                         const int32_t* doclen, const __nv_bfloat16* __restrict__ q,
                                         int nq, float init, float* __restrict__ out,
                                         int64_t n_passages) {
@@ -190,7 +245,7 @@ __global__ void flmr_simt_maxsim_kernel(const __nv_bfloat16* __restrict__ d, con
   const int64_t p = blockIdx.x;
   const int b = blockIdx.y;
   const int len = doclen[p];
-  const __nv_bfloat16* dp = d + poff[p] * kDim;
+  const int64_t d0 = poff[p] * kDim;
   float total = 0.f;
   for (int i0 = 0; i0 < nq; i0 += blockDim.x) {
     const int i = i0 + threadIdx.x;
@@ -198,7 +253,15 @@ __global__ void flmr_simt_maxsim_kernel(const __nv_bfloat16* __restrict__ d, con
     const __nv_bfloat16* qi = q + (static_cast<int64_t>(b) * nq + (i < nq ? i : 0)) * kDim;
     for (int j = 0; j < len; ++j) {
       __syncthreads();
-      if (threadIdx.x < kDim) drow[threadIdx.x] = __bfloat162float(dp[j * kDim + threadIdx.x]);
+      if (threadIdx.x < kDim) {
+        const int64_t e = d0 + j * kDim + threadIdx.x;
+        if constexpr (kFp8) {
+          const __half_raw h = __nv_cvt_fp8_to_halfraw(static_cast<const __nv_fp8_storage_t*>(d_any)[e], __NV_E4M3);
+          drow[threadIdx.x] = __half2float(__half(h));
+        } else {
+          drow[threadIdx.x] = __bfloat162float(static_cast<const __nv_bfloat16*>(d_any)[e]);
+        }
+      }
       __syncthreads();
       float acc = 0.f;
 #pragma unroll 16
@@ -510,7 +573,11 @@ struct flmr_corpus {
   int64_t n_tiles = 0;
   bool adopted = false;
   int64_t hbm_bytes = 0;
-  __nv_bfloat16* d_tokens = nullptr;   // [n_rows, 128] padded layout
+  __nv_bfloat16* d_tokens = nullptr;   // [n_rows, 128] padded layout (e4m3 corpus: device alias of h_master)
+  // FLMR_CORPUS_FP8: the scan reads an e4m3 copy in HBM; the exact bf16 rows stay in pinned, mapped host memory
+  bool fp8 = false;
+  void* h_master = nullptr;            // bf16 [n_rows, 128] padded layout, pinned + mapped (e4m3 corpus only)
+  uint8_t* d_fp8 = nullptr;            // e4m3 [n_rows, 128] padded layout (e4m3 corpus only)
   int64_t* d_poff = nullptr;           // [n_passages + 1] stored-row offsets
   int32_t* d_doclen = nullptr;         // [n_passages] real lengths
   int32_t* d_cta_row_begin = nullptr;  // [n_ctas + 1]
@@ -786,7 +853,8 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
   // (2 / 2 / 1 or 2 / 2 / 2 blocks, serial loop: one warpgroup's MMAs overlap another's fold), below that two
   // (each with two accumulators, its own MMAs overlapping its fold).  On an H100 (400 W, 200k x 180-token passages,
   // median of 5) a 5-block pass took 9.19 ms with three and 10.34 ms with two (3 / 2 blocks), 6-block row slices
-  // 9.12 vs 9.64 ms, a 4-block pass 7.90 vs 7.39 ms (DESIGN.md 4.1).  The instantiations compute bit-identical results
+  // 9.12 vs 9.64 ms, a 4-block pass 7.90 vs 7.39 ms (DESIGN.md 4.1); the e4m3 kernels follow the same threshold (1M
+  // passages, 700 W: 5 blocks 23.3 vs 31.7 ms, 4 blocks 21.4 vs 19.3 ms).  The instantiations compute bit-identical results
   const bool use3 = !pair && ((g_scan_variant == 3) ||
                               (g_scan_variant == 0 && scan_blocks(p.nq_pass, p.rbq) >= 5));
   EventPair ev{};
@@ -815,6 +883,11 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     FLMR_CUDA(cudaLaunchKernelEx(&cfg, flmr_scan_kernel<2, true>, c->tmap_half, p));
+  } else if (c->fp8) {
+    if (use3)
+      flmr_scan_kernel<3, false, true><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    else
+      flmr_scan_kernel<2, false, true><<<c->n_ctas, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
   } else if (use3) {
     flmr_scan_kernel<3><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
   } else {
@@ -832,9 +905,10 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
 // One launch stages `count` zero-padded query blocks (slot i of the workspace's staging buffer <- sp.pass[i]).
 int stage_queries(flmr_workspace* ws, const void* d_q, int nq, const StageParams& sp, int count, cudaStream_t st) {
   const int threads = 256;
-  dim3 grid((kMtMax * kTileM * 16 + threads - 1) / threads, static_cast<unsigned>(count));
-  flmr_stage_queries_kernel<<<grid, threads, 0, st>>>(reinterpret_cast<const uint4*>(d_q),
-                                                      reinterpret_cast<uint4*>(ws->d_qpad), nq, sp);
+  const bool fp8 = ws->corpus->fp8;
+  dim3 grid((kMtMax * kTileM * (fp8 ? 8 : 16) + threads - 1) / threads, static_cast<unsigned>(count));
+  (fp8 ? flmr_stage_queries_kernel<true> : flmr_stage_queries_kernel<false>)<<<grid, threads, 0, st>>>(
+      reinterpret_cast<const uint4*>(d_q), reinterpret_cast<uint4*>(ws->d_qpad), nq, sp);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;
@@ -880,6 +954,8 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
                 "an earlier scan on this workspace tripped the device watchdog (code %d: %s starved); "
                 "the CUDA context is poisoned", code,
                 code == kDevTimeoutProducer ? "TMA producer" : code == kDevTimeoutMma ? "MMA issuer" : "epilogue");
+  if (c->fp8 && g_scan_variant == 4)
+    return fail(FLMR_ERR_UNSUPPORTED, "the CTA-pair scan (variant 4) has no e4m3 kernel");
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
 
@@ -999,12 +1075,13 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
     if ((rc = dev_upload(&c->d_tile_end_mask, end_mask, &c->hbm_bytes))) return bail(rc);
     if ((rc = dev_upload(&c->d_tile_first_pid, first_pid, &c->hbm_bytes))) return bail(rc);
   }
-  if ((rc = encode_rows_map(&c->tmap_d, c->d_tokens, static_cast<uint64_t>(n_rows), kTileN)))
+  if ((rc = c->fp8 ? encode_rows_map(&c->tmap_d, c->d_fp8, static_cast<uint64_t>(n_rows), kTileN, true)
+                    : encode_rows_map(&c->tmap_d, c->d_tokens, static_cast<uint64_t>(n_rows), kTileN)))
     return bail(rc);
   // CTA-pair passes: their own partition + half-tile tensor map.  The product never plans pair passes (see
   // run_search); these few KB per corpus are built so flmr_debug_set_scan_variant(4) can hold the cluster kernel
-  // against the single-CTA kernels on any corpus.
-  if (n_ctas >= 2 && n_passages >= n_ctas / 2) {
+  // against the single-CTA kernels on any bf16 corpus.
+  if (!c->fp8 && n_ctas >= 2 && n_passages >= n_ctas / 2) {
     std::vector<int32_t> row_begin, first_pid;
     std::vector<int64_t> tile_base;
     std::vector<uint32_t> end_mask;
@@ -1022,14 +1099,44 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
     if (e3 != cudaSuccess) return bail(fail(FLMR_ERR_CUDA, "pair kernel attribute: %s", cudaGetErrorString(e3)));
   }
   {  // per-device function attribute, set here (idempotent) rather than at launch time
-    cudaError_t e1 = cudaFuncSetAttribute(flmr_scan_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          ScanSmem::kBytes);
+    cudaError_t e1 = c->fp8 ? cudaFuncSetAttribute(flmr_scan_kernel<2, false, true>,
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes)
+                            : cudaFuncSetAttribute(flmr_scan_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   ScanSmem::kBytes);
     if (e1 == cudaSuccess)
-      e1 = cudaFuncSetAttribute(flmr_scan_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes);
+      e1 = c->fp8 ? cudaFuncSetAttribute(flmr_scan_kernel<3, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         ScanSmem::kBytes)
+                  : cudaFuncSetAttribute(flmr_scan_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         ScanSmem::kBytes);
     if (e1 != cudaSuccess)
       return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
                        ScanSmem::kBytes, cudaGetErrorString(e1)));
   }
+  return FLMR_OK;
+}
+
+// The token matrix of a new corpus (n_rows set): bf16 in HBM, or (c->fp8) the e4m3 copy in HBM plus the bf16 master
+// in pinned, mapped host memory, whose device alias becomes d_tokens (the repack / scatter kernels write both).
+int alloc_token_matrix(flmr_corpus* c) {
+  const size_t rows = static_cast<size_t>(c->n_rows);
+  cudaError_t e;
+  if (c->fp8) {
+    if ((e = cudaHostAlloc(&c->h_master, rows * kDim * 2, cudaHostAllocMapped | cudaHostAllocPortable)) != cudaSuccess) {
+      c->h_master = nullptr;
+      return fail(FLMR_ERR_OOM, "cudaHostAlloc(%zu B) for the bf16 master failed: %s", rows * kDim * 2,
+                  cudaGetErrorString(e));
+    }
+    FLMR_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&c->d_tokens), c->h_master, 0));
+    if ((e = cudaMalloc(reinterpret_cast<void**>(&c->d_fp8), rows * kDim)) != cudaSuccess)
+      return fail(FLMR_ERR_OOM, "cudaMalloc(%zu B) for the e4m3 token matrix failed: %s", rows * kDim,
+                  cudaGetErrorString(e));
+    c->hbm_bytes += static_cast<int64_t>(rows * kDim);
+    return FLMR_OK;
+  }
+  if ((e = cudaMalloc(reinterpret_cast<void**>(&c->d_tokens), rows * kDim * 2)) != cudaSuccess)
+    return fail(FLMR_ERR_OOM, "cudaMalloc(%zu B) for the token matrix failed: %s", rows * kDim * 2,
+                cudaGetErrorString(e));
+  c->hbm_bytes += static_cast<int64_t>(rows * kDim * 2);
   return FLMR_OK;
 }
 
@@ -1048,6 +1155,8 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
   if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
   if (n_passages <= 0 || !tokens || !h_doclens)
     return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null tokens/doclens");
+  if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_ADOPT))
+    return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP8 keeps its own copies of the tokens and cannot adopt them");
   std::vector<int64_t> soff(n_passages + 1), poff(n_passages + 1);
   soff[0] = poff[0] = 0;
   bool aligned = true;
@@ -1091,6 +1200,7 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
   c->n_tokens = soff[n_passages];
   c->n_rows = n_rows;
   c->pid_base = pid_base;
+  c->fp8 = (flags & FLMR_CORPUS_FP8) != 0;
   int rc = FLMR_OK;
   auto bail = [&](int code) {
     flmr_corpus_destroy(c);
@@ -1103,12 +1213,9 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
     c->d_tokens = static_cast<__nv_bfloat16*>(const_cast<void*>(tokens));
     c->adopted = true;
   } else {
-    const size_t bytes = static_cast<size_t>(n_rows) * kDim * 2;
-    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&c->d_tokens), bytes);
-    if (e != cudaSuccess)
-      return bail(fail(FLMR_ERR_OOM, "cudaMalloc(%zu B) for the token matrix failed: %s", bytes,
-                       cudaGetErrorString(e)));
-    c->hbm_bytes += static_cast<int64_t>(bytes);
+    if ((rc = alloc_token_matrix(c))) return bail(rc);
+    cudaError_t e = cudaSuccess;
+    uint2* d_fp8 = reinterpret_cast<uint2*>(c->d_fp8);   // null for a bf16 corpus
     int64_t *d_soff = nullptr, *d_poff_tmp = nullptr;
     if ((rc = dev_upload(&d_soff, soff, nullptr))) return bail(rc);
     if ((rc = dev_upload(&d_poff_tmp, poff, nullptr))) {
@@ -1123,7 +1230,7 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
       const int threads = 256;
       const int64_t blocks = (n_passages * 32 + threads - 1) / threads;
       flmr_repack_kernel<<<static_cast<unsigned>(blocks), threads>>>(
-          static_cast<const uint4*>(tokens), d_soff, d_poff_tmp, reinterpret_cast<uint4*>(c->d_tokens),
+          static_cast<const uint4*>(tokens), d_soff, d_poff_tmp, reinterpret_cast<uint4*>(c->d_tokens), d_fp8,
           0, n_passages, 0);
       ++g_launches;
       e = cudaGetLastError();
@@ -1148,7 +1255,7 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
         const int64_t cnt = pb - pa;
         const int64_t blocks = (cnt * 32 + threads - 1) / threads;
         flmr_repack_kernel<<<static_cast<unsigned>(blocks), threads>>>(
-            d_stage, d_soff, d_poff_tmp, reinterpret_cast<uint4*>(c->d_tokens), pa, cnt, soff[pa]);
+            d_stage, d_soff, d_poff_tmp, reinterpret_cast<uint4*>(c->d_tokens), d_fp8, pa, cnt, soff[pa]);
         ++g_launches;
         e = cudaGetLastError();
         if (e == cudaSuccess) e = cudaDeviceSynchronize();
@@ -1169,7 +1276,11 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
 int flmr_corpus_destroy(flmr_corpus_t* c) {
   if (!c) return FLMR_OK;
   DeviceGuard guard(c->device);
-  if (!c->adopted && c->d_tokens) cudaFree(c->d_tokens);
+  if (c->h_master)
+    cudaFreeHost(c->h_master);   // d_tokens is its device alias
+  else if (!c->adopted && c->d_tokens)
+    cudaFree(c->d_tokens);
+  cudaFree(c->d_fp8);
   cudaFree(c->d_poff);
   cudaFree(c->d_doclen);
   cudaFree(c->d_cta_row_begin);
@@ -1186,8 +1297,15 @@ int flmr_corpus_destroy(flmr_corpus_t* c) {
 
 int flmr_corpus_builder_create(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
                                int64_t pid_base, flmr_corpus_builder_t** out) {
+  return flmr_corpus_builder_create_ex(h_doclens, n_passages, dim, device, pid_base, FLMR_CORPUS_COPY, out);
+}
+
+int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                  int64_t pid_base, unsigned flags, flmr_corpus_builder_t** out) {
   if (!out) return fail(FLMR_ERR_INVALID_ARG, "out is null");
   *out = nullptr;
+  if (flags & ~FLMR_CORPUS_FP8)
+    return fail(FLMR_ERR_INVALID_ARG, "builder flags 0x%x: only FLMR_CORPUS_FP8 applies to a streamed load", flags);
   if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
   if (n_passages <= 0 || !h_doclens) return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null doclens");
   flmr_corpus_builder* b = new (std::nothrow) flmr_corpus_builder();
@@ -1230,20 +1348,20 @@ int flmr_corpus_builder_create(const int32_t* h_doclens, int64_t n_passages, int
   c->n_tokens = b->soff[n_passages];
   c->n_rows = n_rows;
   c->pid_base = pid_base;
-  const size_t bytes = static_cast<size_t>(n_rows) * kDim * 2;
-  if ((e = cudaMalloc(reinterpret_cast<void**>(&c->d_tokens), bytes)) != cudaSuccess)
-    return bail(fail(FLMR_ERR_OOM, "cudaMalloc(%zu B) for the token matrix failed: %s", bytes, cudaGetErrorString(e)));
-  c->hbm_bytes += static_cast<int64_t>(bytes);
+  c->fp8 = (flags & FLMR_CORPUS_FP8) != 0;
+  if (int rc = alloc_token_matrix(c)) return bail(rc);
+  // an e4m3 corpus always goes through the scatter kernel, which writes the master and the e4m3 copy
+  const bool scatter = !b->aligned || c->fp8;
   const size_t buf_bytes = static_cast<size_t>(flmr_corpus_builder::kBufRows) * kDim * 2;
   if ((e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking)) != cudaSuccess)
     return bail(fail(FLMR_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e)));
   for (int i = 0; i < flmr_corpus_builder::kBufs; ++i) {
     if ((e = cudaHostAlloc(&b->h_pin[i], buf_bytes, cudaHostAllocDefault)) != cudaSuccess ||
         (e = cudaEventCreateWithFlags(&b->free_ev[i], cudaEventDisableTiming)) != cudaSuccess ||
-        (!b->aligned && (e = cudaMalloc(reinterpret_cast<void**>(&b->d_stage[i]), buf_bytes)) != cudaSuccess))
+        (scatter && (e = cudaMalloc(reinterpret_cast<void**>(&b->d_stage[i]), buf_bytes)) != cudaSuccess))
       return bail(fail(FLMR_ERR_OOM, "staging buffers: %s", cudaGetErrorString(e)));
   }
-  if (!b->aligned) {
+  if (scatter) {
     int rc;
     if ((rc = dev_upload(&b->d_soff, b->soff, nullptr)) || (rc = dev_upload(&b->d_poff, b->poff, nullptr)))
       return bail(rc);
@@ -1276,13 +1394,14 @@ int builder_feed(flmr_corpus_builder* b, int64_t n_rows, Fill fill) {
     b->fill_s += (t1.tv_sec - t0.tv_sec) + 1e-9 * (t1.tv_nsec - t0.tv_nsec);
     const size_t bytes = static_cast<size_t>(rows) * kDim * 2;
     const int64_t s0 = b->rows_done;
-    if (b->aligned) {                                        // packed order == stored order: straight into place
+    if (b->aligned && !c->fp8) {                             // packed order == stored order: straight into place
       FLMR_CUDA(cudaMemcpyAsync(c->d_tokens + s0 * kDim, b->h_pin[i], bytes, cudaMemcpyHostToDevice, b->stream));
     } else {
       FLMR_CUDA(cudaMemcpyAsync(b->d_stage[i], b->h_pin[i], bytes, cudaMemcpyHostToDevice, b->stream));
       const int threads = 256;
       flmr_scatter_rows_kernel<<<static_cast<unsigned>((rows * 16 + threads - 1) / threads), threads, 0, b->stream>>>(
-          b->d_stage[i], b->d_soff, b->d_poff, reinterpret_cast<uint4*>(c->d_tokens), s0, rows, c->n_passages);
+          b->d_stage[i], b->d_soff, b->d_poff, reinterpret_cast<uint4*>(c->d_tokens),
+          reinterpret_cast<uint2*>(c->d_fp8), s0, rows, c->n_passages);
       FLMR_CUDA(cudaGetLastError());
       ++g_launches;
     }
@@ -1383,6 +1502,13 @@ int flmr_corpus_info(const flmr_corpus_t* c, flmr_corpus_info_t* out) {
   out->adopted = c->adopted ? 1 : 0;
   out->n_tiles = c->n_tiles;
   out->hbm_bytes = c->hbm_bytes;
+  return FLMR_OK;
+}
+
+int flmr_corpus_storage(const flmr_corpus_t* c, int* storage, int64_t* host_bytes) {
+  if (!c) return fail(FLMR_ERR_INVALID_ARG, "null argument");
+  if (storage) *storage = c->fp8 ? 1 : 0;
+  if (host_bytes) *host_bytes = c->fp8 ? c->n_rows * kDim * 2 : 0;
   return FLMR_OK;
 }
 
@@ -1794,11 +1920,30 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
   const int threads = nq >= 256 ? 256 : (nq > 128 ? 256 : 128);
   dim3 grid(static_cast<unsigned>(c->n_passages), static_cast<unsigned>(n_queries));
-  flmr_simt_maxsim_kernel<<<grid, threads, 0, static_cast<cudaStream_t>(stream)>>>(
-      c->d_tokens, c->d_poff, c->d_doclen, static_cast<const __nv_bfloat16*>(d_q), nq,
-      (flags & FLMR_FLAG_RELU) ? 0.f : -INFINITY, d_out_scores, c->n_passages);
-  FLMR_CUDA(cudaGetLastError());
-  ++g_launches;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const float init = (flags & FLMR_FLAG_RELU) ? 0.f : -INFINITY;
+  if (!c->fp8) {
+    flmr_simt_maxsim_kernel<false><<<grid, threads, 0, st>>>(c->d_tokens, c->d_poff, c->d_doclen,
+                                                             static_cast<const __nv_bfloat16*>(d_q), nq, init,
+                                                             d_out_scores, c->n_passages);
+    FLMR_CUDA(cudaGetLastError());
+    ++g_launches;
+    return FLMR_OK;
+  }
+  // e4m3 corpus: MaxSim of e4m3(Q) against the e4m3 matrix, the queries rounded into stream-ordered scratch
+  const int64_t n_chunks = static_cast<int64_t>(n_queries) * nq * (kDim / 8);
+  cudaMemPool_t pool = nullptr;
+  if (int rc = scratch_pool(&pool)) return rc;
+  __nv_bfloat16* q8 = nullptr;
+  FLMR_CUDA(cudaMallocFromPoolAsync(reinterpret_cast<void**>(&q8), static_cast<size_t>(n_chunks) * 16, pool, st));
+  flmr_round_e4m3_kernel<<<static_cast<unsigned>((n_chunks + 255) / 256), 256, 0, st>>>(
+      static_cast<const uint4*>(d_q), reinterpret_cast<uint4*>(q8), n_chunks);
+  flmr_simt_maxsim_kernel<true><<<grid, threads, 0, st>>>(c->d_fp8, c->d_poff, c->d_doclen, q8, nq, init,
+                                                          d_out_scores, c->n_passages);
+  const cudaError_t e = cudaGetLastError();
+  cudaFreeAsync(q8, st);
+  g_launches += 2;
+  if (e != cudaSuccess) return fail(FLMR_ERR_CUDA, "SIMT cross-check launch failed: %s", cudaGetErrorString(e));
   return FLMR_OK;
 }
 

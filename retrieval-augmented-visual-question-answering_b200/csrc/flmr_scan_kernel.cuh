@@ -24,7 +24,8 @@
 //                         ending in the tile) sums the row partials in fixed order (deterministic), optionally
 //                         accumulates / stores scores to HBM, and maintains the per-CTA top-k.
 //   warp 4 kWgs + 1     : TMA producer.  Streams the CTA's contiguous range of passage tokens through a
-//                         kDStages-deep ring of D stages (96 tokens x 128 dims bf16, 128B-swizzled, 2 boxes).
+//                         kDStages-deep ring of D stages (96 tokens x 128 dims bf16, 128B-swizzled, 2 boxes;
+//                         e4m3 corpora: one box of 96 x 128 bytes).
 //
 // Layout contracts (see DESIGN.md "Data layout"):
 //   * passages are stored back to back, each padded to a multiple of 4 tokens by repeating its last
@@ -54,9 +55,12 @@ constexpr int kNb = kTileN / 8;           // 8-column blocks of an accumulator
 constexpr int kFastSlots = 4;             // passage ends per tile whose per-row maxima are left to the reducer
 constexpr int kLaneStride = 33;           // padded row of 32 row values (conflict-free transposed reads)
 constexpr int kDStages = 4;
-constexpr int kDTileBytes = kTileN * kDim * 2;   // 24 KiB: [2 k-blocks][96 rows][64 bf16]
-constexpr int kDKBlockBytes = kTileN * 128;      // 12 KiB
-constexpr int kQKBlockBytes = kMtMax * kTileM * 128;   // one 64-dim half of the resident queries
+constexpr int kDTileBytes = kTileN * kDim * 2;   // 24 KiB: [2 k-blocks][96 rows][64 bf16]; the D stage stride
+constexpr int kDKBlockBytes = kTileN * 128;      // 12 KiB; also a whole e4m3 tile: [1 k-block][96 rows][128 e4m3]
+constexpr int kQKBlockBytes = kMtMax * kTileM * 128;   // one 64-dim half of the resident bf16 queries (all of e4m3)
+// bytes one D tile brings into its stage: two 128-B k-blocks of bf16, or one of e4m3
+template <bool kFp8>
+__host__ __device__ constexpr int d_tile_bytes() { return kFp8 ? kDKBlockBytes : kDTileBytes; }
 constexpr int kRedWarps = 1;
 
 static_assert(kTileN == 96, "the wgmma shape and accumulator fragment are written for 96-token tiles");
@@ -74,7 +78,7 @@ struct ScanParams {
   const uint32_t* tile_end_mask;   // [n_tiles] bit g set <=> a passage ends with 4-token group g
   const int32_t* tile_first_pid;   // [n_tiles] local id of the first passage ending in the tile
   // resident queries of this pass
-  const uint4* q_pad;              // bf16 [n_mtiles * 128][128], zero-padded (stage_queries kernel)
+  const uint4* q_pad;              // bf16 (e4m3 kernel: e4m3) [n_mtiles * 128][128], zero-padded (stage_queries kernel)
   int32_t n_mtiles;                // 128-row query tiles (1..kMtMax)
   int32_t nq_pass;                 // queries resident in this pass (1..kNqMax)
   int32_t rbq;                     // 32-row blocks per query in this pass
@@ -244,18 +248,30 @@ __device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], ui
   }
 }
 
-// acc = (64-row query block at q_block) . (D tile at d_stage)^T: 8 x wgmma.m64n96k16 over K = 128, one commit group.
+// acc = (64-row query block at q_block) . (D tile at d_stage)^T over K = 128, one commit group: bf16, 8 x
+// wgmma.m64n96k16 over two 128-byte k-blocks; e4m3 (kFp8), 4 x wgmma.m64n96k32 over one.  Either way a k-step is 32
+// bytes along the row, and the accumulator fragment is the same.
+template <bool kFp8>
 __device__ __forceinline__ void issue_block_mma(float (&acc)[4 * kNb], uint32_t q_block, uint32_t d_stage) {
   // the query block's descriptors are loop-invariant: hidden from the compiler so that they are rebuilt here (a
   // few integer adds) rather than hoisted out of the tile loop into 16 registers per block
   asm volatile("" : "+r"(q_block));
   wgmma_fence();
+  if constexpr (kFp8) {
 #pragma unroll
-  for (int k = 0; k < kDim / 16; ++k) {
-    const uint32_t koff = (k & 3) * 32u;   // 16 elements along the 128-byte row
-    const uint64_t a_desc = make_kmajor_sw128_desc(q_block + (k >> 2) * kQKBlockBytes + koff);
-    const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + (k >> 2) * kDKBlockBytes + koff);
-    wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+    for (int k = 0; k < kDim / 32; ++k) {
+      const uint64_t a_desc = make_kmajor_sw128_desc(q_block + k * 32u);   // 32 elements along the 128-byte row
+      const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + k * 32u);
+      wgmma_m64n96k32_e4m3(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < kDim / 16; ++k) {
+      const uint32_t koff = (k & 3) * 32u;   // 16 elements along the 128-byte row
+      const uint64_t a_desc = make_kmajor_sw128_desc(q_block + (k >> 2) * kQKBlockBytes + koff);
+      const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + (k >> 2) * kDKBlockBytes + koff);
+      wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+    }
   }
   wgmma_commit();
 }
@@ -271,7 +287,7 @@ __device__ __forceinline__ void issue_block_mma(float (&acc)[4 * kNb], uint32_t 
 // last pair has no successor, are peeled out of the loop.
 // kOverlap = false is the serial form with one accumulator (next MMAs issued after the fold, wait_group 0), for
 // instantiations without the registers for two; the arithmetic and its order are the same.
-template <int NB, int kWgs, bool kPair, bool kOverlap>
+template <int NB, int kWgs, bool kPair, bool kOverlap, bool kFp8>
 __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base, ScanBars bars,
                                               int n_tiles, int64_t tile_base, int wg, int wq, int lane) {
   using S = ScanSmem;
@@ -301,11 +317,11 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
       const bool last = u + 1 == NB;
       auto issue_next = [&](float (&acc_next)[4 * kNb]) {
         if (!last) {
-          issue_block_mma(acc_next, q_block(u + 1), d_stage(t));
+          issue_block_mma<kFp8>(acc_next, q_block(u + 1), d_stage(t));
         } else if (kNext) {
           mbar_wait_inline(bars.d_full((t + 1) % kDStages), ((t + 1) / kDStages) & 1u, p.status, kDevTimeoutMma);
           mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
-          issue_block_mma(acc_next, q_block(0), d_stage(t + 1));
+          issue_block_mma<kFp8>(acc_next, q_block(0), d_stage(t + 1));
         }
       };
       if (kOverlap && (!last || kNext)) {
@@ -347,7 +363,7 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
   if (n_tiles <= 0) return;
   mbar_wait(bars.d_full(0), 0u, p.status, kDevTimeoutMma);
   mask_next = __ldg(p.tile_end_mask + tile_base);
-  issue_block_mma(acc[0], q_block(0), d_stage(0));
+  issue_block_mma<kFp8>(acc[0], q_block(0), d_stage(0));
   int t = 0;
   for (; t + 2 < n_tiles; t += 2) {
     tile(t, H0{}, Next{});
@@ -370,9 +386,15 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
 // token range, each with its own resident queries (twice the queries per corpus pass); every D tile is fetched
 // from L2 / HBM once — CTA r loads rows [48 r, 48 r + 48) of the tile and TMA-multicasts them into both CTAs'
 // shared memory — and a D stage is recycled when the consumers of BOTH CTAs have released it (remote arrive).
-template <int kWgs, bool kPair = false>
+//
+// kFp8 = true is the e4m3 corpus (FLMR_CORPUS_FP8): the staged queries and the D tiles hold one 128-byte e4m3
+// k-block per row (a D tile is one 96-row TMA box of 12 KiB) and the MMAs are wgmma.m64n96k32 e4m3.  Tiles, masks,
+// the shared-memory layout (each stage and the query area keep their bf16 size, half used), the fold, the reducer and
+// the top-k are those of the bf16 kernel.  There is no CTA-pair fp8 kernel.
+template <int kWgs, bool kPair = false, bool kFp8 = false>
 __global__ void __launch_bounds__(scan_threads(kWgs), 1)
 flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  static_assert(!(kPair && kFp8), "the CTA-pair kernel is bf16 only");
   using S = ScanSmem;
   constexpr int kConsumerWarps = kWgs * 4;
   constexpr int kWarpRed0 = kConsumerWarps;
@@ -428,10 +450,12 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
     }
     // stage the resident queries in the 128B-swizzled K-major layout the wgmma descriptors describe:
     // row r, 16-byte chunk c of dims [64 kb, 64 kb + 64) at kb * kQKBlockBytes + r * 128 + ((c ^ (r & 7)) * 16)
+    // (e4m3: 8 chunks per row, all in k-block 0)
+    constexpr int kChunkBits = kFp8 ? 3 : 4;   // log2 of the 16-byte chunks of a staged row
     const uint4* src = p.q_pad + static_cast<int64_t>(pair_rank) * (kMtMax * kTileM * 16);   // pair: CTA r's slot
-    const int n_chunks = n_mtiles * kTileM * 16;
+    const int n_chunks = n_mtiles * kTileM << kChunkBits;
     for (int i = threadIdx.x; i < n_chunks; i += blockDim.x) {
-      const int r = i >> 4, c = i & 15, kb = c >> 3;
+      const int r = i >> kChunkBits, c = i & ((1 << kChunkBits) - 1), kb = c >> 3;
       *reinterpret_cast<uint4*>(smem + S::kOffQ + kb * kQKBlockBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) =
           __ldg(src + i);
     }
@@ -450,7 +474,7 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
         const uint32_t ph = (t / kDStages) & 1;
         mbar_wait(bars.d_empty(s), ph ^ 1u, p.status, kDevTimeoutProducer);
         if (elect_one_sync()) {
-          mbar_arrive_expect_tx(bars.d_full(s), kDTileBytes);   // (pair: 12 KB from this CTA's loads + 12 KB from the peer's)
+          mbar_arrive_expect_tx(bars.d_full(s), d_tile_bytes<kFp8>());   // (pair: 12 KB from this CTA's loads + 12 KB from the peer's)
           const uint32_t dst = smem_base + S::kOffD + s * kDTileBytes;
           const int32_t row = row_begin + t * kTileN;
           if constexpr (kPair) {   // tmap_d has a (kTileN / 2)-row box here
@@ -458,6 +482,8 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
             tma_load_2d_multicast(dst + half * 128, &tmap_d, bars.d_full(s), 0, row + half, 3, kPolicyEvictFirst);
             tma_load_2d_multicast(dst + kDKBlockBytes + half * 128, &tmap_d, bars.d_full(s), 64, row + half, 3,
                                   kPolicyEvictFirst);
+          } else if constexpr (kFp8) {   // tmap_d: e4m3 rows, one 128-column box
+            tma_load_2d(dst, &tmap_d, bars.d_full(s), 0, row, kPolicyEvictFirst);
           } else {
             tma_load_2d(dst, &tmap_d, bars.d_full(s), 0, row, kPolicyEvictFirst);
             tma_load_2d(dst + kDKBlockBytes, &tmap_d, bars.d_full(s), 64, row, kPolicyEvictFirst);
@@ -593,11 +619,11 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
     // run-time count ptxas serialises the wgmma of the two accumulators)
     const int nb = wg < n_blocks ? (n_blocks - wg + kWgs - 1) / kWgs : 0;
     if (nb == 1) {
-      scan_consumer<1, kWgs, kPair, kOverlap>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      scan_consumer<1, kWgs, kPair, kOverlap, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     } else if (nb == 2) {
-      scan_consumer<2, kWgs, kPair, kOverlap>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      scan_consumer<2, kWgs, kPair, kOverlap, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     } else if constexpr (kBlocksPerWg >= 3) {
-      if (nb == 3) scan_consumer<3, kWgs, kPair, kOverlap>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      if (nb == 3) scan_consumer<3, kWgs, kPair, kOverlap, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     }
   }
 

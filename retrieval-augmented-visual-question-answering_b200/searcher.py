@@ -21,6 +21,12 @@ a Python loop of per-query ``rank`` calls, and results always hold exactly ``min
 hits.  ``shard_across_ranks=True`` (an extension; needs an initialised ``torch.distributed`` group) keeps
 only this rank's passage shard resident and merges the per-shard top-k with one all-gather, where the
 reference repeats the whole search on every rank (FLMR_executor.py:778-781).
+
+``storage="fp8"`` keeps the corpus as e4m3 in HBM (half the bytes; the exact bf16 rows stay in pinned host memory)
+and searches in two stages, as PLAID does (colbert/search/index_storage.py:160-177): the exhaustive e4m3 scan
+shortlists ``ndocs / 4`` candidates per query (the reference's exact-scoring depth, filter_pids.cpp:148), which are
+gathered from the bf16 master and re-scored exactly.  Returned scores are exact; an id can differ from the bf16
+search only where the exact top-k was not inside the shortlist.
 """
 from __future__ import annotations
 
@@ -34,7 +40,27 @@ from . import _cabi
 from .corpus import FlatCorpus
 from .index_io import FORMAT as FLAT_FORMAT
 from .infra import ColBERTConfig, active_run_config, resolve_index_path
-from .maxsim import maxsim_scores, maxsim_topk, topk_select
+from .maxsim import maxsim_argmax_grouped, maxsim_scores, maxsim_topk, topk_select
+
+# bytes of gathered bf16 candidate tokens one re-rank launch may hold: larger batches are split by queries
+RERANK_GATHER_BYTES = 1 << 30
+
+
+def _default_knobs(k: int) -> Tuple[int, float, int]:
+    """(ncells, centroid_score_threshold, ndocs) the reference's Searcher.dense_search fills in from k
+    (searcher.py:92-118)."""
+    return (2, 0.45, 1024) if k <= 100 else (4, 0.4, max(k * 4, 4096))
+
+
+def shortlist_depth(k: int, ndocs: Optional[int], n_candidates: int) -> int:
+    """Candidates per query the e4m3 scan hands to the exact re-rank: ``ndocs / 4``, the depth PLAID scores exactly
+    (filter_pids.cpp:148), with ``ndocs`` as the reference derives it from k when unset; never below k, at most the
+    select kernel's capacity and the candidates there are."""
+    if k > _cabi.SELECT_MAX_K:
+        raise ValueError("fp8 storage re-ranks at most %d candidates per query; k=%d" % (_cabi.SELECT_MAX_K, k))
+    if ndocs is None:
+        ndocs = _default_knobs(k)[2]
+    return min(max(int(ndocs) // 4, k), _cabi.SELECT_MAX_K, n_candidates)
 
 
 class Ranking:
@@ -141,7 +167,8 @@ class Searcher:
     def __init__(self, index: Union[str, FlatCorpus], checkpoint=None, collection=None, config=None,
                  disable_gpu: bool = True, device: Optional[Union[int, torch.device]] = None,
                  encode_fn: Optional[Callable] = None, index_root: Optional[str] = None,
-                 query_batch: int = 64, shard_across_ranks: bool = False, group=None):
+                 query_batch: int = 64, shard_across_ranks: bool = False, group=None,
+                 storage: Optional[str] = None):
         # `disable_gpu` is part of the reference signature (default True) but dead there: colbert/searcher.py:23
         # never reads it, the device is chosen by config.total_visible_gpus (:40-43), which FLMR_executor.py:778-781
         # zeroes under DDP to force CPU search.  Here the search always runs on the GPU (no CPU path exists);
@@ -157,6 +184,8 @@ class Searcher:
         self.index_config = None
         run_cfg = active_run_config(config)
         if isinstance(index, FlatCorpus):
+            if storage is not None and storage != index.storage:
+                raise ValueError("storage=%r, but the corpus given is stored as %r" % (storage, index.storage))
             self.corpus = index
             self.index = None
             self.index_kind = "resident"
@@ -171,10 +200,11 @@ class Searcher:
                 if not (dist.is_available() and dist.is_initialized()):
                     raise RuntimeError("shard_across_ranks needs an initialised torch.distributed process group")
                 rank, world = dist.get_rank(group), dist.get_world_size(group)
-            if self.index_kind == "flat":
-                self.corpus = FlatCorpus.from_index(self.index, device=device, rank=rank, world_size=world)
-            else:
-                self.corpus = FlatCorpus.from_plaid(self.index, device=device, rank=rank, world_size=world)
+            load = FlatCorpus.from_index if self.index_kind == "flat" else FlatCorpus.from_plaid
+            extra = {"storage": storage} if storage not in (None, "bf16") else {}
+            self.corpus = load(self.index, device=device, rank=rank, world_size=world, **extra)
+        self.storage = getattr(self.corpus, "storage", None) or storage or "bf16"
+        self._last_depth = None
         # searcher.py:35: checkpoint config < index config < (config + Run().config); kept for callers that
         # read searcher.config — none of its PLAID knobs influence the exhaustive scan.
         cfg_type = type(config) if (config is not None and hasattr(type(config), "from_existing")) else ColBERTConfig
@@ -208,7 +238,7 @@ class Searcher:
     def configure(self, **kw):
         """colbert.Searcher.configure (searcher.py:49-50).  PLAID knobs (ncells,
         centroid_score_threshold, ndocs) are recorded on ``config`` and otherwise ignored: the scan is
-        exhaustive."""
+        exhaustive.  On an fp8 corpus ``ndocs / 4`` sets the depth of the exact re-rank."""
         self._relu = bool(kw.pop("relu", self._relu))
         if kw and self.config is not None and hasattr(self.config, "configure"):
             self.config.configure(**kw)
@@ -274,6 +304,8 @@ class Searcher:
         if corpus is None:                               # this rank's shard is empty (more ranks than passages)
             return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=self.device),
                     torch.empty((Q.size(0), 0), dtype=torch.int64, device=self.device))
+        if self.storage == "fp8":
+            return self._reranked_topk(Q, kk, keep)
         if keep is None and kk <= _cabi.MAX_K:
             kq = min(kk, corpus.n_passages)
             outs, outp = [], []
@@ -302,6 +334,53 @@ class Searcher:
             outp.append((keep[idx] if keep is not None else idx) + corpus.pid_base)
         return torch.cat(outs), torch.cat(outp)
 
+    def _reranked_topk(self, Q: torch.Tensor, kk: int, keep: Optional[torch.Tensor]
+                       ) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``_local_topk`` of an fp8 corpus: all e4m3 scores, a shortlist of ``shortlist_depth`` candidates (after
+        ``keep``), their exact bf16 tokens gathered from the master and re-scored by the grouped rowmax kernel,
+        the top ``kk`` of those exact scores (ties: lower pid)."""
+        corpus = self.corpus
+        n_cand = corpus.n_passages if keep is None else int(keep.numel())
+        kq = min(kk, n_cand)
+        if kq == 0:
+            return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=corpus.device),
+                    torch.empty((Q.size(0), 0), dtype=torch.int64, device=corpus.device))
+        depth = shortlist_depth(kk, getattr(self.config, "ndocs", None), n_cand)
+        self._last_depth = depth
+        outs, outp = [], []
+        for b0 in range(0, Q.size(0), self.query_batch):
+            Qb = Q[b0:b0 + self.query_batch].to(corpus.device).to(torch.bfloat16)
+            s = maxsim_scores(corpus, Qb, relu=self._relu)
+            if keep is not None:
+                s = s[:, keep]
+            _, idx = topk_select(s, depth)
+            cand = keep[idx] if keep is not None else idx
+            # candidates in pid order, so that the select below breaks exact ties towards the lower pid
+            cand = torch.sort(cand, dim=1).values + corpus.pid_base
+            exact = self._exact_scores(Qb, cand)
+            vals, col = topk_select(exact, kq)
+            outs.append(vals)
+            outp.append(cand.gather(1, col))
+        return torch.cat(outs), torch.cat(outp)
+
+    def _exact_scores(self, Q: torch.Tensor, cand: torch.Tensor) -> torch.Tensor:
+        """Exact MaxSim ``[B, depth]`` of query b against its candidates ``cand[b]`` (global pids), from the bf16
+        rows of the corpus; the gather is split by queries to hold at most RERANK_GATHER_BYTES of tokens."""
+        corpus = self.corpus
+        depth = cand.size(1)
+        nd_max = int(corpus.doclens[(cand - corpus.pid_base).cpu().numpy()].max())
+        per_query = depth * nd_max * _cabi.DIM * 2
+        step = max(1, RERANK_GATHER_BYTES // per_query)
+        out = []
+        for q0 in range(0, Q.size(0), step):
+            D, mask = corpus.gather_padded(cand[q0:q0 + step], nd_max)          # [b, depth, nd_max, d]
+            _, rowmax = maxsim_argmax_grouped(Q[q0:q0 + step], D.flatten(0, 1), mask.flatten(0, 1), depth,
+                                              return_rowmax=True)
+            if self._relu:
+                rowmax = rowmax.clamp_min(0.0)
+            out.append(rowmax.sum(dim=-1))
+        return torch.cat(out)
+
     def _search_tensors(self, Q: torch.Tensor, k: int, filter_fn=None,
                         remove_zero_tensors: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
         """(scores [B,k'], pids [B,k']) on the GPU, k' = min(k, passages that pass ``filter_fn``)."""
@@ -316,8 +395,9 @@ class Searcher:
             keep = torch.as_tensor(filter_fn(all_pids), device=corpus.device).long() - corpus.pid_base
         if self._sharded is not None and int(k) > _cabi.MAX_K:
             raise ValueError("sharded search merges at most k=%d results per query" % _cabi.MAX_K)
-        if self._nccl is not None and keep is None and corpus is not None:
+        if self._nccl is not None and keep is None and corpus is not None and self.storage != "fp8":
             # the C-level sharded search: scan + one grouped all-gather + merge per call, no torch glue
+            # (fp8 shards re-rank their shortlists first, then exchange exact scores below)
             outs = [self._nccl.search(corpus, Q[b0:b0 + self.query_batch], int(k), relu=self._relu)
                     for b0 in range(0, Q.size(0), self.query_batch)]
             s, p = torch.cat([o[0] for o in outs]), torch.cat([o[1] for o in outs])
@@ -369,12 +449,13 @@ class Searcher:
 
     def _fill_search_knobs(self, k: int) -> None:
         """searcher.py:92-118: the first search fills the PLAID knobs still unset on ``config`` from ``k`` (and later
-        searches keep them).  They steer nothing here — the scan is exhaustive — but callers that read
-        ``searcher.config.ncells`` etc. after a search find what the reference would have left there."""
+        searches keep them).  The scan is exhaustive, so they steer nothing on a bf16 corpus — but callers that read
+        ``searcher.config.ncells`` etc. after a search find what the reference would have left there.  On an fp8
+        corpus ``ndocs / 4`` is the depth of the exact re-rank (``shortlist_depth``)."""
         cfg = self.config
         if cfg is None or not hasattr(cfg, "configure") or not hasattr(cfg, "ncells"):
             return
-        ncells, thr, ndocs = (2, 0.45, 1024) if k <= 100 else (4, 0.4, max(k * 4, 4096))
+        ncells, thr, ndocs = _default_knobs(k)
         if cfg.ncells is None:
             cfg.configure(ncells=ncells)
         if cfg.centroid_score_threshold is None:
@@ -408,5 +489,8 @@ class Searcher:
                 "config": self.config.export() if hasattr(self.config, "export") else None,
                 "backend": "ravqa_b200 exhaustive fused scan", "index": self.index,
                 "index_kind": self.index_kind, "exhaustive": True,
-                "n_passages": self.corpus.n_passages if self.corpus is not None else 0}
+                "n_passages": self.corpus.n_passages if self.corpus is not None else 0,
+                "storage": self.storage}
+        if self.storage == "fp8":
+            prov["shortlist_depth"] = self._last_depth
         return Ranking(data=data, provenance=prov)
