@@ -28,6 +28,9 @@
  *       APPROXIMATE; the exact bf16 rows stay in pinned host memory for flmr_corpus_gather.  The first stage of
  *       a two-stage search whose exact second stage re-scores a shortlist (the Python Searcher does both), as
  *       PLAID scores its ndocs/4 survivors exactly (CB/search/index_storage.py:160-177).
+ *   flmr_corpus_append / _delete / _deleted
+ *       the add / remove of ColBERT's later IndexUpdater (the vendored release has no update path): passages are
+ *       appended to a resident shard in place and deleted ones are tombstoned, tested in the scan's reducer.
  *   flmr_debug_maxsim_scores_simt
  *       test infrastructure: an independent plain-SIMT fp32 device kernel used by tests to
  *       cross-check the tensor-core kernel at sizes where the CPU oracle is too slow.
@@ -40,8 +43,14 @@
  *     corpus' device, "h_" parameters are HOST pointers;
  *   - compute entry points are asynchronous on the supplied CUDA stream (passed as void* so the
  *     header needs no CUDA include; NULL = default stream);
- *   - a corpus handle is immutable after creation and may be shared by threads; concurrent
- *     searches on one handle must use distinct flmr_workspace handles.
+ *   - a corpus changes only through flmr_corpus_append and flmr_corpus_delete.  Between those calls a handle
+ *     may be shared by threads; concurrent searches on one handle must use distinct flmr_workspace handles.
+ *     The two mutating calls must not run concurrently with any other call on the handle or on its workspaces;
+ *     they wait for the device themselves, so work already enqueued on any stream sees the corpus as it was.
+ *   - a DELETED passage keeps its id (ids are never reused) and its rows (they are still scanned); it yields
+ *     -inf from flmr_maxsim_scores and flmr_debug_maxsim_scores_simt, never appears in the lists of
+ *     flmr_maxsim_topk / flmr_maxsim_topk_sharded (short lists are filled with -1 / -inf), and
+ *     flmr_corpus_gather returns an all-masked zero row for it, as for an id outside the shard.
  */
 #ifndef FLMR_MAXSIM_H_
 #define FLMR_MAXSIM_H_
@@ -86,7 +95,7 @@ typedef struct flmr_comm flmr_comm_t;           /* this rank's end of the shard 
 typedef struct flmr_corpus_builder flmr_corpus_builder_t; /* streaming index load          */
 
 typedef struct flmr_corpus_info {
-  int64_t n_passages;     /* passages in this shard                                           */
+  int64_t n_passages;     /* passages stored in this shard, deleted ones included             */
   int64_t n_tokens;       /* real tokens (sum of doclens)                                     */
   int64_t n_rows;         /* stored rows (tokens incl. group padding)                         */
   int64_t pid_base;       /* global id of passage 0 of this shard                             */
@@ -129,6 +138,31 @@ int flmr_corpus_info(const flmr_corpus_t* corpus, flmr_corpus_info_t* out);
  * exact bf16 rows of the master, and flmr_debug_maxsim_scores_simt computes the e4m3 semantics.
  */
 int flmr_corpus_storage(const flmr_corpus_t* corpus, int* storage, int64_t* host_bytes);
+
+/*
+ * Updating a resident corpus (replaces rebuilding and reloading it: the surface of ColBERT's IndexUpdater add /
+ * remove).  Both calls are synchronous: they wait for the device before they free or swap anything and return when
+ * the change is complete.  See the conventions above for what may run alongside them.
+ *
+ * flmr_corpus_append   passages behind the stored ones, of either storage.  tokens: packed bf16 rows
+ *                      [sum(h_doclens), dim], host or device pointer (detected as in flmr_corpus_create); every
+ *                      doclen >= 1.  The new passages get the ids pid_base + (old n_passages ...); *first_pid (may
+ *                      be NULL) receives the first.  A library-owned matrix lives in a reserved virtual address
+ *                      range and grows in place (no copy, no second matrix).  An adopted matrix is copied into
+ *                      library memory by the first append, which then no longer references the caller's buffer.
+ *                      The bf16 master of an FLMR_CORPUS_FP8 corpus is pinned host memory and is reallocated:
+ *                      old and new master are held together for the copy.  A shard is limited to 2^31 passages
+ *                      and 2^31 stored rows.
+ * flmr_corpus_delete   tombstones the GLOBAL ids h_pids[0..n).  The whole list is checked first: an id outside the
+ *                      shard gives FLMR_ERR_INVALID_ARG and nothing changes.  Deleting a deleted id does nothing.
+ *                      The first delete allocates the shard's bitmap (1 bit per passage, counted in hbm_bytes).
+ * flmr_corpus_deleted  *n_deleted = how many ids are deleted; if h_pids is not NULL it receives them (global,
+ *                      ascending), capacity >= *n_deleted entries.
+ */
+int flmr_corpus_append(flmr_corpus_t* corpus, const void* tokens, const int32_t* h_doclens, int64_t n_passages,
+                       int64_t* first_pid);
+int flmr_corpus_delete(flmr_corpus_t* corpus, const int64_t* h_pids, int64_t n);
+int flmr_corpus_deleted(const flmr_corpus_t* corpus, int64_t* n_deleted, int64_t* h_pids, int64_t capacity);
 
 /*
  * Streaming construction of a corpus shard — the index LOAD path (replaces IndexLoader / ResidualEmbeddings.load_chunks,

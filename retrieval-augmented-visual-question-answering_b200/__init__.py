@@ -9,10 +9,11 @@ from .searcher import Searcher, Ranking  # noqa: F401,E402
 from .sharded import ShardedSearcher, shard_ranges  # noqa: F401,E402
 from .index_io import save_flat_index, load_flat_index  # noqa: F401,E402
 from .indexer import Indexer  # noqa: F401,E402
+from .updater import IndexUpdater  # noqa: F401,E402
 from .modeling import (FLMRModelForRetrieval, all_pairs_maxsim, colbert_score, grouped_maxsim,  # noqa: F401,E402
                        graphed_in_batch_negatives_loss, in_batch_negatives_loss)
 from .infra import ColBERTConfig, Queries, Run, RunConfig, resolve_index_path  # noqa: F401,E402
 
-__all__ += ["Searcher", "Ranking", "ShardedSearcher", "shard_ranges", "save_flat_index", "load_flat_index", "Indexer",
+__all__ += ["Searcher", "Ranking", "ShardedSearcher", "shard_ranges", "save_flat_index", "load_flat_index", "Indexer", "IndexUpdater",
             "FLMRModelForRetrieval", "all_pairs_maxsim", "colbert_score", "grouped_maxsim",
             "in_batch_negatives_loss", "graphed_in_batch_negatives_loss", "ColBERTConfig", "Queries", "Run", "RunConfig", "resolve_index_path"]

@@ -32,10 +32,12 @@ def _header_define(name: str) -> int:
 
 TILE_TOKENS = _header_define("FLMR_TILE_TOKENS")
 
+UPDATE_SYMBOLS = ("flmr_corpus_append", "flmr_corpus_delete", "flmr_corpus_deleted")
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
     "flmr_corpus_create", "flmr_corpus_destroy", "flmr_corpus_info", "flmr_corpus_storage",
+    *UPDATE_SYMBOLS,
     "flmr_workspace_create", "flmr_workspace_destroy", "flmr_workspace_status",
     "flmr_maxsim_scores", "flmr_maxsim_topk", "flmr_topk_merge", "flmr_topk_select", "flmr_plaid_decode",
     "flmr_maxsim_argmax", "flmr_maxsim_backward", "flmr_corpus_gather",
@@ -83,6 +85,12 @@ def lib() -> C.CDLL:
     L.flmr_corpus_destroy.argtypes = [vp]
     L.flmr_corpus_info.argtypes = [vp, C.POINTER(CorpusInfo)]
     L.flmr_corpus_storage.argtypes = [vp, C.POINTER(i32), C.POINTER(i64)]
+    # the corpus-update entry points are declared only where the library has them: tools/scan_ab.py drives a
+    # library built from an earlier revision through this binding (build() checks that ours exports every symbol)
+    if hasattr(L, "flmr_corpus_append"):
+        L.flmr_corpus_append.argtypes = [vp, vp, vp, i64, C.POINTER(i64)]
+        L.flmr_corpus_delete.argtypes = [vp, vp, i64]
+        L.flmr_corpus_deleted.argtypes = [vp, C.POINTER(i64), vp, i64]
     L.flmr_workspace_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
     L.flmr_workspace_destroy.argtypes = [vp]
     L.flmr_workspace_status.argtypes = [vp, C.POINTER(i32)]
@@ -120,6 +128,8 @@ def lib() -> C.CDLL:
     L.flmr_set_profiling.argtypes = [i32]
     L.flmr_scan_kernel_stats.argtypes = [C.POINTER(C.c_double), C.POINTER(i64), i32]
     for name in SYMBOLS:
+        if name in UPDATE_SYMBOLS and not hasattr(L, name):
+            continue
         fn = getattr(L, name)
         if name not in ("flmr_last_error", "flmr_launch_count"):
             fn.restype = i32

@@ -119,9 +119,10 @@ class FlatCorpus:
         buffers (8 reader threads, the fill of one buffer overlaps the DMA of the other) and from there into the
         padded layout — no numpy copy of the shard, no pageable ``cudaMemcpy``.  ``load_stats`` records seconds
         and GB/s (replaces IndexLoader / ResidualEmbeddings.load_chunks, colbert/search/index_loader.py:24-62).
-        ``storage="fp8"``: the staged rows fill the bf16 master in pinned host memory, HBM receives e4m3."""
+        ``storage="fp8"``: the staged rows fill the bf16 master in pinned host memory, HBM receives e4m3.
+        The deletions an index records (``deleted.npy``, format v2) are applied to the passages of this shard."""
         import time
-        from .index_io import index_token_files
+        from .index_io import deleted_in_range, index_token_files, read_deleted
         from .sharded import shard_ranges
         if not torch.cuda.is_available():
             raise RuntimeError("FlatCorpus needs a CUDA device: there is no CPU fallback for this path")
@@ -156,6 +157,9 @@ class FlatCorpus:
             if b is not None:
                 L.flmr_corpus_builder_destroy(b)
         self = cls._from_handle(handle, doclens, device, p0)
+        dead = deleted_in_range(read_deleted(path), p0, p1)    # this shard's share of the index's deletions
+        if dead.size:
+            self.delete(dead)
         dt = time.perf_counter() - t0
         gb = float(doclens.sum()) * _cabi.DIM * 2 / 1e9
         self.load_stats = {"seconds": dt, "gigabytes": gb, "gb_per_s": gb / dt, "host_fill_seconds": fill_s.value,
@@ -194,6 +198,78 @@ class FlatCorpus:
             raise RuntimeError("corpus was closed")
         return self._h
 
+    @property
+    def n_deleted(self) -> int:
+        n = C.c_int64(0)
+        _cabi.check(_cabi.lib().flmr_corpus_deleted(self.handle, C.byref(n), None, 0))
+        return int(n.value)
+
+    @property
+    def n_live(self) -> int:
+        """Passages a search can return: every stored passage but the deleted ones."""
+        return self.n_passages - self.n_deleted
+
+    def deleted_pids(self) -> np.ndarray:
+        """Global ids of the deleted passages, ascending (int64)."""
+        n = C.c_int64(0)
+        L = _cabi.lib()
+        _cabi.check(L.flmr_corpus_deleted(self.handle, C.byref(n), None, 0))
+        out = np.empty(n.value, dtype=np.int64)
+        _cabi.check(L.flmr_corpus_deleted(self.handle, C.byref(n), out.ctypes.data_as(C.c_void_p), out.size))
+        return out
+
+    def live_pids(self) -> torch.Tensor:
+        """Global ids of the passages that are not deleted, ascending, on the corpus' device."""
+        pids = torch.arange(self.n_passages, dtype=torch.int64) + self.pid_base
+        dead = self.deleted_pids()
+        if dead.size:
+            keep = torch.ones(self.n_passages, dtype=torch.bool)
+            keep[torch.from_numpy(dead - self.pid_base)] = False
+            pids = pids[keep]
+        return pids.to(self.device)
+
+    def append(self, tokens: torch.Tensor, doclens) -> np.ndarray:
+        """Append passages (``tokens [sum(doclens), 128]``, on the CPU or on the corpus' GPU; ``doclens`` >= 1 each)
+        behind the stored ones, in place; returns their global ids (int64), which continue the shard's ids.  An
+        adopted token tensor is copied into library memory by the first append and released."""
+        doclens = _as_doclens(doclens)
+        if tokens.dim() != 2 or tokens.size(1) != _cabi.DIM:
+            raise ValueError("tokens must be [sum(doclens), %d], got %s" % (_cabi.DIM, tuple(tokens.shape)))
+        if int(doclens.sum()) != tokens.size(0):
+            raise ValueError("sum(doclens)=%d != tokens rows=%d" % (int(doclens.sum()), tokens.size(0)))
+        tokens = tokens.detach()
+        if tokens.dtype != torch.bfloat16:
+            tokens = tokens.to(torch.bfloat16)
+        tokens = tokens.contiguous()
+        if tokens.is_cuda and tokens.device != self.device:
+            tokens = tokens.to(self.device)
+        if tokens.is_cuda:
+            torch.cuda.current_stream(self.device).synchronize()   # producer kernels of `tokens` are done
+        first = C.c_int64(0)
+        _cabi.check(_cabi.lib().flmr_corpus_append(self.handle, C.c_void_p(tokens.data_ptr()),
+                                                   doclens.ctypes.data_as(C.c_void_p), int(doclens.shape[0]),
+                                                   C.byref(first)))
+        self.doclens = np.concatenate([self.doclens, doclens])
+        self._refresh()
+        return np.arange(first.value, first.value + doclens.shape[0], dtype=np.int64)
+
+    def delete(self, pids) -> None:
+        """Delete passages by global id: they are never returned by a search again and gather as all-masked rows.
+        Every id must belong to this shard (else nothing is deleted and ``FlmrError`` is raised); deleting a deleted
+        id does nothing."""
+        if isinstance(pids, torch.Tensor):
+            pids = pids.detach().cpu().numpy()
+        arr = np.ascontiguousarray(np.asarray(pids, dtype=np.int64).reshape(-1))
+        _cabi.check(_cabi.lib().flmr_corpus_delete(self.handle, arr.ctypes.data_as(C.c_void_p), int(arr.size)))
+        self._refresh()
+
+    def _refresh(self) -> None:
+        info = _cabi.CorpusInfo()
+        _cabi.check(_cabi.lib().flmr_corpus_info(self.handle, C.byref(info)))
+        self.info = info
+        if not info.adopted:
+            self._keepalive = None
+
     def workspace(self) -> C.c_void_p:
         """Default per-corpus scratch (single-threaded use, like the reference Searcher)."""
         if self._ws is None:
@@ -206,7 +282,8 @@ class FlatCorpus:
         """Retrieved passages as a padded batch, straight out of HBM (an fp8 corpus: the exact bf16 rows of its
         pinned host master): ``pids`` (any shape, global ids) ->
         (tokens bf16 ``[*pids.shape, nd_max, 128]``, mask bool ``[*pids.shape, nd_max, 1]``).  ``nd_max``
-        defaults to the longest requested passage.  Ids outside this shard give an all-masked zero row.
+        defaults to the longest requested passage.  Ids outside this shard and deleted ids give an all-masked zero
+        row.
         Replaces the host-dictionary lookup + stack + H2D of rag_model_blip.py:414-425."""
         shape = tuple(pids.shape)
         flat = pids.detach().reshape(-1).to(device=self.device, dtype=torch.int64).contiguous()

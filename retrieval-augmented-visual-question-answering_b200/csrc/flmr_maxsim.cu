@@ -98,6 +98,121 @@ int get_encode_fn(EncodeTiledFn* out) {
   return FLMR_OK;
 }
 
+// ---- growable device matrices: driver virtual memory management, resolved like cuTensorMapEncodeTiled -------------
+// A library-owned token matrix lives in a virtual address range reserved once, as large as the device's memory, and
+// backed by physical allocations mapped behind its end as it grows.  An append therefore never copies the matrix and
+// never needs room for two of it, and the matrix stays one contiguous 2-D tensor for the scan's TMA descriptor.
+struct VmmApi {
+  CUresult (*AddressReserve)(CUdeviceptr*, size_t, size_t, CUdeviceptr, unsigned long long) = nullptr;
+  CUresult (*AddressFree)(CUdeviceptr, size_t) = nullptr;
+  CUresult (*Create)(CUmemGenericAllocationHandle*, size_t, const CUmemAllocationProp*, unsigned long long) = nullptr;
+  CUresult (*Release)(CUmemGenericAllocationHandle) = nullptr;
+  CUresult (*Map)(CUdeviceptr, size_t, size_t, CUmemGenericAllocationHandle, unsigned long long) = nullptr;
+  CUresult (*Unmap)(CUdeviceptr, size_t) = nullptr;
+  CUresult (*SetAccess)(CUdeviceptr, size_t, const CUmemAccessDesc*, size_t) = nullptr;
+  CUresult (*Granularity)(size_t*, const CUmemAllocationProp*, CUmemAllocationGranularity_flags) = nullptr;
+};
+
+int get_vmm_api(const VmmApi** out) {
+  static VmmApi api;
+  static bool ok = false;
+  static std::mutex mu;
+  std::lock_guard<std::mutex> lock(mu);
+  if (!ok) {
+    VmmApi a;
+    const std::pair<const char*, void**> names[] = {
+        {"cuMemAddressReserve", reinterpret_cast<void**>(&a.AddressReserve)},
+        {"cuMemAddressFree", reinterpret_cast<void**>(&a.AddressFree)},
+        {"cuMemCreate", reinterpret_cast<void**>(&a.Create)},
+        {"cuMemRelease", reinterpret_cast<void**>(&a.Release)},
+        {"cuMemMap", reinterpret_cast<void**>(&a.Map)},
+        {"cuMemUnmap", reinterpret_cast<void**>(&a.Unmap)},
+        {"cuMemSetAccess", reinterpret_cast<void**>(&a.SetAccess)},
+        {"cuMemGetAllocationGranularity", reinterpret_cast<void**>(&a.Granularity)}};
+    for (const auto& n : names) {
+      cudaDriverEntryPointQueryResult qres;
+      FLMR_CUDA(cudaGetDriverEntryPoint(n.first, n.second, cudaEnableDefault, &qres));
+      if (qres != cudaDriverEntryPointSuccess || !*n.second)
+        return fail(FLMR_ERR_CUDA, "%s not available from the driver", n.first);
+    }
+    api = a;
+    ok = true;
+  }
+  *out = &api;
+  return FLMR_OK;
+}
+
+struct GrowableMatrix {
+  CUdeviceptr base = 0;         // start of the reserved range (0: none)
+  size_t reserved = 0;          // bytes of address space
+  size_t mapped = 0;            // bytes backed by physical memory, from base
+  size_t gran = 0;              // allocation granularity
+  std::vector<std::pair<CUmemGenericAllocationHandle, size_t>> chunks;   // (allocation, bytes) in address order
+};
+
+#define FLMR_CU(expr)                                                                                   \
+  do {                                                                                                  \
+    CUresult r__ = (expr);                                                                              \
+    if (r__ != CUDA_SUCCESS)                                                                            \
+      return fail(r__ == CUDA_ERROR_OUT_OF_MEMORY ? FLMR_ERR_OOM : FLMR_ERR_CUDA, "%s failed (CUresult %d)", \
+                  #expr, (int)r__);                                                                     \
+  } while (0)
+
+void gm_free(GrowableMatrix* g) {
+  const VmmApi* api = nullptr;
+  if (!g->base || get_vmm_api(&api)) return;
+  size_t off = 0;
+  for (auto& ch : g->chunks) {
+    api->Unmap(g->base + off, ch.second);
+    api->Release(ch.first);
+    off += ch.second;
+  }
+  api->AddressFree(g->base, g->reserved);
+  *g = GrowableMatrix();
+}
+
+// Back at least `bytes` of g with physical memory on `device` (reserving the range first if g has none).  Only the
+// new tail is mapped: rows already there stay where they are.
+int gm_grow(GrowableMatrix* g, int device, size_t bytes) {
+  const VmmApi* api = nullptr;
+  if (int rc = get_vmm_api(&api)) return rc;
+  CUmemAllocationProp prop{};
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = device;
+  if (!g->base) {
+    FLMR_CUDA(cudaFree(nullptr));   // the device's primary context is current for the driver calls
+    size_t free_b = 0, total_b = 0;
+    FLMR_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    FLMR_CU(api->Granularity(&g->gran, &prop, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED));
+    const size_t reserve = (total_b + g->gran - 1) / g->gran * g->gran;
+    FLMR_CU(api->AddressReserve(&g->base, reserve, g->gran, 0, 0));
+    g->reserved = reserve;
+  }
+  if (bytes <= g->mapped) return FLMR_OK;
+  const size_t add = (bytes - g->mapped + g->gran - 1) / g->gran * g->gran;
+  if (g->mapped + add > g->reserved)
+    return fail(FLMR_ERR_OOM, "a token matrix of %zu bytes exceeds the device's %zu bytes", bytes, g->reserved);
+  CUmemGenericAllocationHandle h;
+  FLMR_CU(api->Create(&h, add, &prop, 0));
+  CUresult r = api->Map(g->base + g->mapped, add, 0, h, 0);
+  if (r == CUDA_SUCCESS) {
+    CUmemAccessDesc acc{};
+    acc.location = prop.location;
+    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+    r = api->SetAccess(g->base + g->mapped, add, &acc, 1);
+    if (r != CUDA_SUCCESS) api->Unmap(g->base + g->mapped, add);
+  }
+  if (r != CUDA_SUCCESS) {
+    api->Release(h);
+    return fail(r == CUDA_ERROR_OUT_OF_MEMORY ? FLMR_ERR_OOM : FLMR_ERR_CUDA,
+                "mapping %zu bytes behind the token matrix failed (CUresult %d)", add, (int)r);
+  }
+  g->chunks.emplace_back(h, add);
+  g->mapped += add;
+  return FLMR_OK;
+}
+
 // bf16 [rows, 128] row-major matrix, box = 64 columns (128 B, one swizzle span) x box_rows rows; fp8: an e4m3
 // [rows, 128] matrix (as bytes), box = 128 columns (128 B) x box_rows rows.
 int encode_rows_map(CUtensorMap* map, const void* base, uint64_t rows, uint32_t box_rows, bool fp8 = false) {
@@ -234,16 +349,22 @@ __global__ void flmr_round_e4m3_kernel(const uint4* __restrict__ src, uint4* __r
 
 // Independent plain-SIMT MaxSim (test infrastructure): one block per (passage, query), one thread
 // per query token (looping if nq > blockDim), fp32 FMA over bf16 inputs, fixed-order block sum.
-// kFp8: the corpus matrix is e4m3 (the queries come already rounded to e4m3, flmr_round_e4m3_kernel).
+// kFp8: the corpus matrix is e4m3 (the queries come already rounded to e4m3, flmr_round_e4m3_kernel).  A deleted
+// passage (bit set in `dead`, which may be null) scores -inf.
 template <bool kFp8>
 __global__ void flmr_simt_maxsim_kernel(const void* __restrict__ d_any, const int64_t* poff,
-                                        const int32_t* doclen, const __nv_bfloat16* __restrict__ q,
+                                        const int32_t* doclen, const uint32_t* __restrict__ dead,
+                                        const __nv_bfloat16* __restrict__ q,
                                         int nq, float init, float* __restrict__ out,
                                         int64_t n_passages) {
   __shared__ float drow[kDim];
   __shared__ float red[256];
   const int64_t p = blockIdx.x;
   const int b = blockIdx.y;
+  if (dead && ((dead[p >> 5] >> (p & 31)) & 1u)) {   // block-uniform, before any barrier
+    if (threadIdx.x == 0) out[static_cast<int64_t>(b) * n_passages + p] = -INFINITY;
+    return;
+  }
   const int len = doclen[p];
   const int64_t d0 = poff[p] * kDim;
   float total = 0.f;
@@ -574,12 +695,22 @@ struct flmr_corpus {
   bool adopted = false;
   int64_t hbm_bytes = 0;
   __nv_bfloat16* d_tokens = nullptr;   // [n_rows, 128] padded layout (e4m3 corpus: device alias of h_master)
+  GrowableMatrix vm_tokens;            // backs d_tokens of a library-owned bf16 corpus
   // FLMR_CORPUS_FP8: the scan reads an e4m3 copy in HBM; the exact bf16 rows stay in pinned, mapped host memory
   bool fp8 = false;
   void* h_master = nullptr;            // bf16 [n_rows, 128] padded layout, pinned + mapped (e4m3 corpus only)
-  uint8_t* d_fp8 = nullptr;            // e4m3 [n_rows, 128] padded layout (e4m3 corpus only)
+  uint8_t* d_fp8 = nullptr;            // e4m3 [n_rows, 128] padded layout (e4m3 corpus only), backed by vm_fp8
+  GrowableMatrix vm_fp8;
   int64_t* d_poff = nullptr;           // [n_passages + 1] stored-row offsets
   int32_t* d_doclen = nullptr;         // [n_passages] real lengths
+  std::vector<int64_t> h_poff;         // host copies of the two above (an append extends them)
+  std::vector<int32_t> h_doclen;
+  // tombstones: bit p & 31 of word p >> 5 set <=> local passage p is deleted; d_dead stays null until the first
+  // delete, so a corpus without deletions runs the scan exactly as before
+  uint32_t* d_dead = nullptr;
+  std::vector<uint32_t> h_dead;
+  int64_t n_deleted = 0;
+  int sm_total = 0;                    // SMs of the device (n_ctas = min(sm_total, n_passages))
   int32_t* d_cta_row_begin = nullptr;  // [n_ctas + 1]
   int64_t* d_cta_tile_base = nullptr;  // [n_ctas + 1]
   uint32_t* d_tile_end_mask = nullptr; // [n_tiles]
@@ -623,6 +754,7 @@ struct flmr_workspace {
   int max_queries = 0, max_nq = 0;
   __nv_bfloat16* d_qpad = nullptr;     // [kStageMaxPasses][kMtMax*128, 128] staged (zero-padded) queries, one slot per pass
   uint64_t* d_cand_keys = nullptr;     // [n_ctas][max_queries][k] candidate keys of one call chunk
+  int cand_lists = 0;                  // CTAs d_cand_keys is sized for (grown when an append raises n_ctas)
   float* d_acc = nullptr;              // [group][n_passages] lazily allocated (row-sliced queries)
   int64_t acc_capacity = 0;            // floats allocated at d_acc
   int* h_status = nullptr;             // pinned + mapped: readable by the host even after a device trap
@@ -966,6 +1098,17 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   p.tile_first_pid = c->d_tile_first_pid;
   p.init_val = (flags & FLMR_FLAG_RELU) ? 0.f : -INFINITY;
   p.n_passages = c->n_passages;
+  p.dead = c->d_dead;   // null until the first delete: the reducer then makes no extra load
+  if (ws->cand_lists < c->n_ctas) {
+    // the corpus grew past the CTA count this workspace was sized for (a corpus of fewer passages than SMs launches
+    // one CTA per passage); cudaFree waits for the searches still using the old buffer
+    cudaFree(ws->d_cand_keys);
+    ws->d_cand_keys = nullptr;
+    ws->cand_lists = 0;
+    FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&ws->d_cand_keys),
+                         static_cast<size_t>(c->n_ctas) * ws->max_queries * kMaxK * 8));
+    ws->cand_lists = c->n_ctas;
+  }
   p.cand_keys = ws->d_cand_keys;
   p.q_pad = reinterpret_cast<const uint4*>(ws->d_qpad);
   p.status = ws->d_status;
@@ -1055,6 +1198,9 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
     std::vector<int32_t> lens(h_doclens, h_doclens + n_passages);
     if ((rc = dev_upload(&c->d_poff, poff, &c->hbm_bytes))) return bail(rc);
     if ((rc = dev_upload(&c->d_doclen, lens, &c->hbm_bytes))) return bail(rc);
+    c->h_poff = poff;
+    c->h_doclen.swap(lens);
+    c->sm_total = sm_count;
   }
 
   // --- partition + tile metadata ---
@@ -1127,17 +1273,88 @@ int alloc_token_matrix(flmr_corpus* c) {
                   cudaGetErrorString(e));
     }
     FLMR_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&c->d_tokens), c->h_master, 0));
-    if ((e = cudaMalloc(reinterpret_cast<void**>(&c->d_fp8), rows * kDim)) != cudaSuccess)
-      return fail(FLMR_ERR_OOM, "cudaMalloc(%zu B) for the e4m3 token matrix failed: %s", rows * kDim,
-                  cudaGetErrorString(e));
+    if (int rc = gm_grow(&c->vm_fp8, c->device, rows * kDim)) return rc;
+    c->d_fp8 = reinterpret_cast<uint8_t*>(c->vm_fp8.base);
     c->hbm_bytes += static_cast<int64_t>(rows * kDim);
     return FLMR_OK;
   }
-  if ((e = cudaMalloc(reinterpret_cast<void**>(&c->d_tokens), rows * kDim * 2)) != cudaSuccess)
-    return fail(FLMR_ERR_OOM, "cudaMalloc(%zu B) for the token matrix failed: %s", rows * kDim * 2,
-                cudaGetErrorString(e));
+  if (int rc = gm_grow(&c->vm_tokens, c->device, rows * kDim * 2)) return rc;
+  c->d_tokens = reinterpret_cast<__nv_bfloat16*>(c->vm_tokens.base);
   c->hbm_bytes += static_cast<int64_t>(rows * kDim * 2);
   return FLMR_OK;
+}
+
+// Packed bf16 rows of n passages (soff / poff relative to the first; host or device source) into the padded layout
+// at dst, and (dst8 non-null) as e4m3 at dst8.  Synchronous.
+cudaError_t pack_passages(const void* tokens, bool is_device_ptr, const std::vector<int64_t>& soff,
+                          const std::vector<int64_t>& poff, const int32_t* h_doclens, int64_t n_passages, uint4* dst,
+                          uint2* dst8) {
+  int64_t *d_soff = nullptr, *d_poff = nullptr;
+  cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&d_soff), soff.size() * sizeof(int64_t));
+  if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d_poff), poff.size() * sizeof(int64_t));
+  if (e == cudaSuccess) e = cudaMemcpy(d_soff, soff.data(), soff.size() * sizeof(int64_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(d_poff, poff.data(), poff.size() * sizeof(int64_t), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && is_device_ptr) {
+    const int threads = 256;
+    const int64_t blocks = (n_passages * 32 + threads - 1) / threads;
+    flmr_repack_kernel<<<static_cast<unsigned>(blocks), threads>>>(static_cast<const uint4*>(tokens), d_soff, d_poff,
+                                                                   dst, dst8, 0, n_passages, 0);
+    ++g_launches;
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  } else if (e == cudaSuccess) {
+    // host source: stage through a bounded device buffer, chunk by chunk of whole passages
+    const int64_t chunk_rows = std::min<int64_t>(soff[n_passages], (256ll << 20) / (kDim * 2));
+    int64_t max_len = 0;
+    for (int64_t p = 0; p < n_passages; ++p) max_len = std::max<int64_t>(max_len, h_doclens[p]);
+    const int64_t buf_rows = std::max(chunk_rows, max_len);
+    uint4* d_stage = nullptr;
+    e = cudaMalloc(reinterpret_cast<void**>(&d_stage), static_cast<size_t>(buf_rows) * kDim * 2);
+    int64_t pa = 0;
+    while (e == cudaSuccess && pa < n_passages) {
+      int64_t pb = std::upper_bound(soff.begin() + pa, soff.end(), soff[pa] + buf_rows) - soff.begin() - 1;
+      pb = std::max(pb, pa + 1);
+      const int64_t rows = soff[pb] - soff[pa];
+      e = cudaMemcpy(d_stage, static_cast<const char*>(tokens) + soff[pa] * kDim * 2,
+                     static_cast<size_t>(rows) * kDim * 2, cudaMemcpyHostToDevice);
+      if (e != cudaSuccess) break;
+      const int threads = 256;
+      const int64_t cnt = pb - pa;
+      const int64_t blocks = (cnt * 32 + threads - 1) / threads;
+      flmr_repack_kernel<<<static_cast<unsigned>(blocks), threads>>>(d_stage, d_soff, d_poff, dst, dst8, pa, cnt,
+                                                                     soff[pa]);
+      ++g_launches;
+      e = cudaGetLastError();
+      if (e == cudaSuccess) e = cudaDeviceSynchronize();
+      pa = pb;
+    }
+    cudaFree(d_stage);
+  }
+  cudaFree(d_soff);
+  cudaFree(d_poff);
+  return e;
+}
+
+// The per-passage arrays, partition and tensor maps finish_corpus builds (the token matrices are not touched).
+void free_metadata(flmr_corpus* c) {
+  for (void* p : {static_cast<void*>(c->d_poff), static_cast<void*>(c->d_doclen),
+                  static_cast<void*>(c->d_cta_row_begin), static_cast<void*>(c->d_cta_tile_base),
+                  static_cast<void*>(c->d_tile_end_mask), static_cast<void*>(c->d_tile_first_pid),
+                  static_cast<void*>(c->d_pair_row_begin), static_cast<void*>(c->d_pair_tile_base),
+                  static_cast<void*>(c->d_pair_end_mask), static_cast<void*>(c->d_pair_first_pid)})
+    cudaFree(p);
+  c->d_poff = nullptr;
+  c->d_doclen = nullptr;
+  c->d_cta_row_begin = nullptr;
+  c->d_cta_tile_base = nullptr;
+  c->d_tile_end_mask = nullptr;
+  c->d_tile_first_pid = nullptr;
+  c->d_pair_row_begin = nullptr;
+  c->d_pair_tile_base = nullptr;
+  c->d_pair_end_mask = nullptr;
+  c->d_pair_first_pid = nullptr;
+  c->n_pairs = 0;
+  c->n_tiles_pair = 0;
 }
 
 }  // namespace
@@ -1214,56 +1431,9 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
     c->adopted = true;
   } else {
     if ((rc = alloc_token_matrix(c))) return bail(rc);
-    cudaError_t e = cudaSuccess;
-    uint2* d_fp8 = reinterpret_cast<uint2*>(c->d_fp8);   // null for a bf16 corpus
-    int64_t *d_soff = nullptr, *d_poff_tmp = nullptr;
-    if ((rc = dev_upload(&d_soff, soff, nullptr))) return bail(rc);
-    if ((rc = dev_upload(&d_poff_tmp, poff, nullptr))) {
-      cudaFree(d_soff);
-      return bail(rc);
-    }
-    auto cleanup = [&]() {
-      cudaFree(d_soff);
-      cudaFree(d_poff_tmp);
-    };
-    if (is_device_ptr) {
-      const int threads = 256;
-      const int64_t blocks = (n_passages * 32 + threads - 1) / threads;
-      flmr_repack_kernel<<<static_cast<unsigned>(blocks), threads>>>(
-          static_cast<const uint4*>(tokens), d_soff, d_poff_tmp, reinterpret_cast<uint4*>(c->d_tokens), d_fp8,
-          0, n_passages, 0);
-      ++g_launches;
-      e = cudaGetLastError();
-      if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    } else {
-      // host source: stage through a bounded device buffer, chunk by chunk of whole passages
-      const int64_t chunk_rows = std::min<int64_t>(c->n_tokens, (256ll << 20) / (kDim * 2));
-      int64_t max_len = 0;
-      for (int64_t p = 0; p < n_passages; ++p) max_len = std::max<int64_t>(max_len, h_doclens[p]);
-      const int64_t buf_rows = std::max(chunk_rows, max_len);
-      uint4* d_stage = nullptr;
-      e = cudaMalloc(reinterpret_cast<void**>(&d_stage), static_cast<size_t>(buf_rows) * kDim * 2);
-      int64_t pa = 0;
-      while (e == cudaSuccess && pa < n_passages) {
-        int64_t pb = std::upper_bound(soff.begin() + pa, soff.end(), soff[pa] + buf_rows) - soff.begin() - 1;
-        pb = std::max(pb, pa + 1);
-        const int64_t rows = soff[pb] - soff[pa];
-        e = cudaMemcpy(d_stage, static_cast<const char*>(tokens) + soff[pa] * kDim * 2,
-                       static_cast<size_t>(rows) * kDim * 2, cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) break;
-        const int threads = 256;
-        const int64_t cnt = pb - pa;
-        const int64_t blocks = (cnt * 32 + threads - 1) / threads;
-        flmr_repack_kernel<<<static_cast<unsigned>(blocks), threads>>>(
-            d_stage, d_soff, d_poff_tmp, reinterpret_cast<uint4*>(c->d_tokens), d_fp8, pa, cnt, soff[pa]);
-        ++g_launches;
-        e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaDeviceSynchronize();
-        pa = pb;
-      }
-      cudaFree(d_stage);
-    }
-    cleanup();
+    const cudaError_t e = pack_passages(tokens, is_device_ptr, soff, poff, h_doclens, n_passages,
+                                        reinterpret_cast<uint4*>(c->d_tokens),
+                                        reinterpret_cast<uint2*>(c->d_fp8));   // d_fp8: null for a bf16 corpus
     if (e != cudaSuccess)
       return bail(fail(FLMR_ERR_CUDA, "corpus repack failed: %s", cudaGetErrorString(e)));
   }
@@ -1276,21 +1446,12 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
 int flmr_corpus_destroy(flmr_corpus_t* c) {
   if (!c) return FLMR_OK;
   DeviceGuard guard(c->device);
-  if (c->h_master)
-    cudaFreeHost(c->h_master);   // d_tokens is its device alias
-  else if (!c->adopted && c->d_tokens)
-    cudaFree(c->d_tokens);
-  cudaFree(c->d_fp8);
-  cudaFree(c->d_poff);
-  cudaFree(c->d_doclen);
-  cudaFree(c->d_cta_row_begin);
-  cudaFree(c->d_cta_tile_base);
-  cudaFree(c->d_tile_end_mask);
-  cudaFree(c->d_tile_first_pid);
-  cudaFree(c->d_pair_row_begin);
-  cudaFree(c->d_pair_tile_base);
-  cudaFree(c->d_pair_end_mask);
-  cudaFree(c->d_pair_first_pid);
+  if (c->vm_tokens.base || c->vm_fp8.base) cudaDeviceSynchronize();   // no search still reads the matrices
+  if (c->h_master) cudaFreeHost(c->h_master);   // d_tokens is its device alias
+  gm_free(&c->vm_tokens);                       // (an adopted matrix is the caller's and has no mapping here)
+  gm_free(&c->vm_fp8);
+  free_metadata(c);
+  cudaFree(c->d_dead);
   delete c;
   return FLMR_OK;
 }
@@ -1512,6 +1673,174 @@ int flmr_corpus_storage(const flmr_corpus_t* c, int* storage, int64_t* host_byte
   return FLMR_OK;
 }
 
+int flmr_corpus_append(flmr_corpus_t* c, const void* tokens, const int32_t* h_doclens, int64_t n_passages,
+                       int64_t* first_pid) {
+  if (!c || !tokens || !h_doclens) return fail(FLMR_ERR_INVALID_ARG, "null argument");
+  if (n_passages <= 0) return fail(FLMR_ERR_INVALID_ARG, "n_passages=%lld must be >= 1", (long long)n_passages);
+  const int64_t old_n = c->n_passages, old_rows = c->n_rows;
+  // the new passages, relative to their first: packed (soff) and padded (poff) row offsets
+  std::vector<int64_t> soff(n_passages + 1), poff(n_passages + 1);
+  soff[0] = poff[0] = 0;
+  for (int64_t p = 0; p < n_passages; ++p) {
+    const int32_t len = h_doclens[p];
+    if (len < 1)
+      return fail(FLMR_ERR_INVALID_ARG, "passage %lld has length %d; zero-length passages have no defined MaxSim score",
+                  (long long)p, len);
+    soff[p + 1] = soff[p] + len;
+    poff[p + 1] = poff[p] + (len + kGroup - 1) / kGroup * kGroup;
+  }
+  const int64_t new_n = old_n + n_passages, new_rows = old_rows + poff[n_passages];
+  // the partition stores first passage ids and CTA row starts as int32, the scan's top-k key a 32-bit ~local id
+  if (new_n > 0x7fffffffll)
+    return fail(FLMR_ERR_UNSUPPORTED, "%lld passages exceed the 2^31 per-shard limit; shard the corpus", (long long)new_n);
+  if (new_rows + kTileN >= (1ll << 31))
+    return fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
+                (long long)new_rows);
+  DeviceGuard guard(c->device);
+  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
+  cudaPointerAttributes attr{};
+  const bool is_device_ptr = (cudaPointerGetAttributes(&attr, tokens) == cudaSuccess) &&
+                             (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+  cudaGetLastError();
+  if (is_device_ptr && attr.type == cudaMemoryTypeDevice && attr.device != c->device)
+    return fail(FLMR_ERR_INVALID_ARG, "token matrix lives on device %d, corpus on %d", attr.device, c->device);
+  // searches enqueued before this call (any stream) finish on the corpus as it was
+  FLMR_CUDA(cudaDeviceSynchronize());
+
+  // --- 1. room for the new rows: mapped behind the library-owned matrices, which stay where they are ---
+  const size_t row_bytes = static_cast<size_t>(kDim) * 2;
+  if (c->fp8) {
+    if (int rc = gm_grow(&c->vm_fp8, c->device, static_cast<size_t>(new_rows) * kDim)) return rc;
+    // the bf16 master is pinned host memory: reallocated and copied (old + new size are held for the copy)
+    void* h = nullptr;
+    cudaError_t e = cudaHostAlloc(&h, static_cast<size_t>(new_rows) * row_bytes,
+                                  cudaHostAllocMapped | cudaHostAllocPortable);
+    if (e != cudaSuccess)
+      return fail(FLMR_ERR_OOM, "cudaHostAlloc(%zu B) for the bf16 master failed: %s",
+                  static_cast<size_t>(new_rows) * row_bytes, cudaGetErrorString(e));
+    __nv_bfloat16* d_alias = nullptr;
+    if ((e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&d_alias), h, 0)) != cudaSuccess) {
+      cudaFreeHost(h);
+      return fail(FLMR_ERR_CUDA, "cudaHostGetDevicePointer: %s", cudaGetErrorString(e));
+    }
+    memcpy(h, c->h_master, static_cast<size_t>(old_rows) * row_bytes);
+    cudaFreeHost(c->h_master);
+    c->h_master = h;
+    c->d_tokens = d_alias;
+  } else if (c->adopted) {
+    // the caller's buffer is copied into library memory once; from here on it is no longer referenced
+    GrowableMatrix g;
+    int rc = gm_grow(&g, c->device, static_cast<size_t>(new_rows) * row_bytes);
+    cudaError_t e = cudaSuccess;
+    if (!rc && (e = cudaMemcpy(reinterpret_cast<void*>(g.base), c->d_tokens, static_cast<size_t>(old_rows) * row_bytes,
+                               cudaMemcpyDeviceToDevice)) != cudaSuccess)
+      rc = fail(FLMR_ERR_CUDA, "copying the adopted token matrix failed: %s", cudaGetErrorString(e));
+    if (rc) {
+      gm_free(&g);
+      return rc;
+    }
+    c->vm_tokens = g;
+    c->d_tokens = reinterpret_cast<__nv_bfloat16*>(g.base);
+    c->adopted = false;
+  } else {
+    if (int rc = gm_grow(&c->vm_tokens, c->device, static_cast<size_t>(new_rows) * row_bytes)) return rc;
+  }
+
+  // --- 2. the new rows into place (bf16, and e4m3 for an fp8 corpus), behind the old ones ---
+  cudaError_t e = pack_passages(tokens, is_device_ptr, soff, poff, h_doclens, n_passages,
+                                reinterpret_cast<uint4*>(c->d_tokens + old_rows * kDim),
+                                c->fp8 ? reinterpret_cast<uint2*>(c->d_fp8 + old_rows * kDim) : nullptr);
+  if (e != cudaSuccess) return fail(FLMR_ERR_CUDA, "packing the appended passages failed: %s", cudaGetErrorString(e));
+
+  // --- 3. offsets, lengths, partition, tensor maps and tombstones for the grown corpus, then swapped in ---
+  flmr_corpus nc = *c;
+  nc.d_poff = nullptr;
+  nc.d_doclen = nullptr;
+  nc.d_cta_row_begin = nullptr;
+  nc.d_cta_tile_base = nullptr;
+  nc.d_tile_end_mask = nullptr;
+  nc.d_tile_first_pid = nullptr;
+  nc.d_pair_row_begin = nullptr;
+  nc.d_pair_tile_base = nullptr;
+  nc.d_pair_end_mask = nullptr;
+  nc.d_pair_first_pid = nullptr;
+  nc.n_pairs = 0;
+  nc.n_tiles_pair = 0;
+  nc.d_dead = nullptr;
+  nc.n_passages = new_n;
+  nc.n_tokens = c->n_tokens + soff[n_passages];
+  nc.n_rows = new_rows;
+  nc.hbm_bytes = new_rows * (c->fp8 ? kDim : kDim * 2);
+  std::vector<int64_t> all_poff(c->h_poff);
+  all_poff.reserve(new_n + 1);
+  for (int64_t p = 1; p <= n_passages; ++p) all_poff.push_back(old_rows + poff[p]);
+  std::vector<int32_t> all_len(c->h_doclen);
+  all_len.insert(all_len.end(), h_doclens, h_doclens + n_passages);
+  int rc = FLMR_OK;
+  if (!c->h_dead.empty()) {
+    nc.h_dead.resize((new_n + 31) / 32, 0u);
+    rc = dev_upload(&nc.d_dead, nc.h_dead, &nc.hbm_bytes);
+  }
+  if (!rc) rc = finish_corpus(&nc, all_poff, all_len.data(), c->sm_total);
+  if (rc) {
+    free_metadata(&nc);
+    cudaFree(nc.d_dead);
+    return rc;
+  }
+  free_metadata(c);
+  cudaFree(c->d_dead);
+  *c = std::move(nc);
+  if (first_pid) *first_pid = c->pid_base + old_n;
+  return FLMR_OK;
+}
+
+int flmr_corpus_delete(flmr_corpus_t* c, const int64_t* h_pids, int64_t n) {
+  if (!c || n < 0 || (n > 0 && !h_pids)) return fail(FLMR_ERR_INVALID_ARG, "null argument or negative count");
+  for (int64_t i = 0; i < n; ++i) {   // the whole list is checked before anything changes
+    const int64_t p = h_pids[i] - c->pid_base;
+    if (p < 0 || p >= c->n_passages)
+      return fail(FLMR_ERR_INVALID_ARG, "passage id %lld is outside this shard [%lld, %lld)", (long long)h_pids[i],
+                  (long long)c->pid_base, (long long)(c->pid_base + c->n_passages));
+  }
+  std::vector<uint32_t> dead(c->h_dead);
+  dead.resize((c->n_passages + 31) / 32, 0u);
+  int64_t added = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    const int64_t p = h_pids[i] - c->pid_base;
+    const uint32_t bit = 1u << (p & 31);
+    added += (dead[p >> 5] & bit) == 0;
+    dead[p >> 5] |= bit;
+  }
+  if (added == 0) return FLMR_OK;   // already deleted (or nothing to do): no change, no bitmap allocated
+  DeviceGuard guard(c->device);
+  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
+  // searches enqueued before this call (any stream) finish with the old bitmap
+  FLMR_CUDA(cudaDeviceSynchronize());
+  const size_t bytes = dead.size() * sizeof(uint32_t);
+  if (!c->d_dead) {
+    FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&c->d_dead), bytes));
+    c->hbm_bytes += static_cast<int64_t>(bytes);
+  }
+  FLMR_CUDA(cudaMemcpy(c->d_dead, dead.data(), bytes, cudaMemcpyHostToDevice));
+  c->h_dead.swap(dead);
+  c->n_deleted += added;
+  return FLMR_OK;
+}
+
+int flmr_corpus_deleted(const flmr_corpus_t* c, int64_t* n_deleted, int64_t* h_pids, int64_t capacity) {
+  if (!c || !n_deleted) return fail(FLMR_ERR_INVALID_ARG, "null argument");
+  *n_deleted = c->n_deleted;
+  if (!h_pids) return FLMR_OK;
+  if (capacity < c->n_deleted)
+    return fail(FLMR_ERR_INVALID_ARG, "capacity %lld < %lld deleted ids", (long long)capacity,
+                (long long)c->n_deleted);
+  int64_t j = 0;
+  for (size_t w = 0; w < c->h_dead.size(); ++w)
+    for (uint32_t bits = c->h_dead[w]; bits; bits &= bits - 1)
+      h_pids[j++] = c->pid_base + static_cast<int64_t>(w) * 32 + __builtin_ctz(bits);
+  return FLMR_OK;
+}
+
 int flmr_workspace_create(const flmr_corpus_t* c, int max_queries, int max_nq,
                           flmr_workspace_t** out) {
   if (!c || !out) return fail(FLMR_ERR_INVALID_ARG, "null argument");
@@ -1539,6 +1868,7 @@ int flmr_workspace_create(const flmr_corpus_t* c, int max_queries, int max_nq,
       (e = cudaHostAlloc(reinterpret_cast<void**>(&ws->h_status), sizeof(int), cudaHostAllocMapped)) != cudaSuccess ||
       (e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&ws->d_status), ws->h_status, 0)) != cudaSuccess)
     return bail(fail(FLMR_ERR_CUDA, "workspace allocation failed: %s", cudaGetErrorString(e)));
+  ws->cand_lists = c->n_ctas;
   *ws->h_status = 0;
   if (max_nq > kRbMax * 32) {   // row-sliced queries expected: size their partial-score rows now
     std::vector<PassPlan> plan;
@@ -1673,7 +2003,7 @@ int flmr_corpus_gather(const flmr_corpus_t* c, const int64_t* d_pids, int64_t n_
   const int64_t blocks = (n_pids * nd_max * 32 + threads - 1) / threads;
   if (blocks > 0x7fffffffll) return fail(FLMR_ERR_UNSUPPORTED, "gather of %lld x %d rows is too large", (long long)n_pids, nd_max);
   flmr_gather_kernel<<<static_cast<unsigned>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const uint2*>(c->d_tokens), c->d_poff, c->d_doclen, d_pids, n_pids, nd_max,
+      reinterpret_cast<const uint2*>(c->d_tokens), c->d_poff, c->d_doclen, c->d_dead, d_pids, n_pids, nd_max,
       c->n_passages, c->pid_base, static_cast<uint2*>(d_out_bf16), d_mask);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
@@ -1923,7 +2253,7 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const float init = (flags & FLMR_FLAG_RELU) ? 0.f : -INFINITY;
   if (!c->fp8) {
-    flmr_simt_maxsim_kernel<false><<<grid, threads, 0, st>>>(c->d_tokens, c->d_poff, c->d_doclen,
+    flmr_simt_maxsim_kernel<false><<<grid, threads, 0, st>>>(c->d_tokens, c->d_poff, c->d_doclen, c->d_dead,
                                                              static_cast<const __nv_bfloat16*>(d_q), nq, init,
                                                              d_out_scores, c->n_passages);
     FLMR_CUDA(cudaGetLastError());
@@ -1938,7 +2268,7 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
   FLMR_CUDA(cudaMallocFromPoolAsync(reinterpret_cast<void**>(&q8), static_cast<size_t>(n_chunks) * 16, pool, st));
   flmr_round_e4m3_kernel<<<static_cast<unsigned>((n_chunks + 255) / 256), 256, 0, st>>>(
       static_cast<const uint4*>(d_q), reinterpret_cast<uint4*>(q8), n_chunks);
-  flmr_simt_maxsim_kernel<true><<<grid, threads, 0, st>>>(c->d_fp8, c->d_poff, c->d_doclen, q8, nq, init,
+  flmr_simt_maxsim_kernel<true><<<grid, threads, 0, st>>>(c->d_fp8, c->d_poff, c->d_doclen, c->d_dead, q8, nq, init,
                                                           d_out_scores, c->n_passages);
   const cudaError_t e = cudaGetLastError();
   cudaFreeAsync(q8, st);

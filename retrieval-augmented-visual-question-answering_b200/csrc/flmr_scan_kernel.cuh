@@ -22,7 +22,8 @@
 //                         D tiles stays in a register: a query block never changes warpgroup.
 //   warp 4 kWgs         : reducer.  Per D tile (mbarrier-fed, double-buffered partials): per (query, passage
 //                         ending in the tile) sums the row partials in fixed order (deterministic), optionally
-//                         accumulates / stores scores to HBM, and maintains the per-CTA top-k.
+//                         accumulates / stores scores to HBM, and maintains the per-CTA top-k.  A passage marked
+//                         in the corpus' tombstone bitmap (ScanParams::dead) is skipped: -inf score, no top-k offer.
 //   warp 4 kWgs + 1     : TMA producer.  Streams the CTA's contiguous range of passage tokens through a
 //                         kDStages-deep ring of D stages (96 tokens x 128 dims bf16, 128B-swizzled, 2 boxes;
 //                         e4m3 corpora: one box of 96 x 128 bytes).
@@ -88,6 +89,7 @@ struct ScanParams {
   const float* acc_in;             // [nq_pass][n_passages] partial scores of earlier row slices, or null
   float* acc_out;                  // [nq_pass][n_passages] scores (or partial scores) out, or null
   int64_t n_passages;
+  const uint32_t* dead;            // [ceil(n_passages / 32)] tombstones (bit p & 31 of word p >> 5), or null: none
   // fused top-k
   int32_t k;                       // 0 = disabled
   uint64_t* cand_keys;             // [n_ctas][cand_q_stride][k]  (ordered score << 32 | ~local pid)
@@ -165,6 +167,12 @@ __device__ __noinline__ void topk_replace_min(uint64_t* keys, int k, uint64_t ca
   minkey = mk;
   minpos = mp;
   __syncwarp();
+}
+
+// -inf into column `out` of the nq rows (stride n) of a score output: a deleted passage.  Out of line: the reducer's
+// cold path, kept from adding to the kernel's register allocation.
+__device__ __noinline__ void store_dead_scores(float* out, int64_t n, int nq, int lane) {
+  for (int b = lane; b < nq; b += 32) out[b * n] = -INFINITY;
 }
 
 // Max of a thread's values x over the quad's four lanes (they hold the same rows, different columns).
@@ -523,6 +531,13 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
         for (int slot = 0; slot < n_slots; ++slot) {
           const int64_t pid = static_cast<int64_t>(first_pid) + slot;
           const float* lp_slot = lane_part0 + ((buf * kFastSlots + slot) * kRbMax) * kLaneStride;
+          // a deleted passage (warp-uniform test, once per slot): never offered to the top-k, -inf in the score
+          // output.  Its rows were still streamed and folded; only its partial sums are left unread.
+          if (p.dead != nullptr && ((__ldg(p.dead + (pid >> 5)) >> (pid & 31)) & 1u)) {
+            if (p.acc_out) store_dead_scores(p.acc_out + static_cast<int64_t>(q_off) * p.n_passages + pid,
+                                             p.n_passages, p.nq_pass, lane);
+            continue;
+          }
           if (slot < kFastSlots && p.rbq <= p.lane_mode_max_rbq) {
             // many short queries per pass: lane = query, each lane sums its query's 32 * rbq lane maxima
             // (transposed read of the stride-33 layout: conflict-free for rbq = 1)

@@ -341,9 +341,11 @@ flmr_ib_loss_kernel(const float* __restrict__ rowmax, int B, int n, int nq, int 
     dscores[static_cast<int64_t>(b) * n + p] = (expf(s_sc[p] - lse) - (p == label ? 1.f : 0.f)) * inv_b;
 }
 
-// Padded batch of retrieved passages out of the resident corpus.  One warp per (slot, token row).
+// Padded batch of retrieved passages out of the resident corpus.  One warp per (slot, token row).  A deleted passage
+// (bit set in `dead`, which may be null) gives the all-masked zero row of an id outside the shard.
 __global__ void flmr_gather_kernel(const uint2* __restrict__ tokens, const int64_t* __restrict__ poff,
-                                   const int32_t* __restrict__ doclen, const int64_t* __restrict__ pids,
+                                   const int32_t* __restrict__ doclen, const uint32_t* __restrict__ dead,
+                                   const int64_t* __restrict__ pids,
                                    int64_t n_pids, int nd_max, int64_t n_passages, int64_t pid_base,
                                    uint2* __restrict__ out, uint8_t* __restrict__ mask) {
   const int64_t w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
@@ -354,7 +356,7 @@ __global__ void flmr_gather_kernel(const uint2* __restrict__ tokens, const int64
   const int64_t p = pids[slot] - pid_base;
   uint2 v = make_uint2(0u, 0u);
   bool real = false;
-  if (p >= 0 && p < n_passages && j < doclen[p]) {
+  if (p >= 0 && p < n_passages && j < doclen[p] && !(dead && ((dead[p >> 5] >> (p & 31)) & 1u))) {
     v = tokens[(poff[p] + j) * 32 + lane];
     real = true;
   }

@@ -10,17 +10,47 @@ A flat index is simply what the scan kernel streams, in one piece or in chunks o
     single file layout     doclens.npy (int32 [n_passages]) + tokens.bf16 (raw bf16 [n_tokens, dim])
     chunked layout         doclens.<c>.npy + tokens.<c>.bf16 + <c>.metadata.json
                            {"passage_offset", "num_passages", "num_embeddings"}   for c < C
+
+An index whose corpus lost passages after it was built (``IndexUpdater.remove``) is written as "flmr-flat-v2": the
+same files plus ``deleted.npy`` (int64, the sorted ids of the deleted passages, which keep their rows and ids).
+Readers of v1 refuse a v2 index instead of bringing the deleted passages back; v2 is written only when there are
+deletions.
 """
 from __future__ import annotations
 
 import json
 import os
+import shutil
 from typing import Optional, Tuple
 
 import numpy as np
 import torch
 
 FORMAT = "flmr-flat-v1"
+FORMAT_V2 = "flmr-flat-v2"        # FORMAT + deleted.npy
+FORMATS = (FORMAT, FORMAT_V2)
+
+
+def read_metadata(path: str) -> dict:
+    """metadata.json of a flat index of either format version."""
+    with open(os.path.join(path, "metadata.json")) as f:
+        meta = json.load(f)
+    if meta.get("format") not in FORMATS:
+        raise ValueError("%s is not a %s index" % (path, " / ".join(FORMATS)))
+    return meta
+
+
+def read_deleted(path: str) -> np.ndarray:
+    """Sorted global ids of the passages deleted from the index at ``path`` (empty for a v1 index)."""
+    if read_metadata(path)["format"] != FORMAT_V2:
+        return np.empty(0, dtype=np.int64)
+    return np.load(os.path.join(path, "deleted.npy")).astype(np.int64)
+
+
+def deleted_in_range(deleted: np.ndarray, p0: int, p1: int) -> np.ndarray:
+    """The deleted ids that fall in the passage shard ``[p0, p1)``."""
+    deleted = np.asarray(deleted, dtype=np.int64)
+    return deleted[(deleted >= p0) & (deleted < p1)]
 
 
 def _write_tokens(path: str, tokens: torch.Tensor) -> None:
@@ -66,7 +96,7 @@ def chunk_exists(path: str, chunk_idx: int) -> bool:
                for n in ("%d.metadata.json", "doclens.%d.npy", "tokens.%d.bf16"))
 
 
-def finalize_chunked_index(path: str, num_chunks: int) -> dict:
+def finalize_chunked_index(path: str, num_chunks: int, fmt: str = FORMAT) -> dict:
     """Check the chunks tile the passage range and write the index-level metadata.json
     (cf. CollectionIndexer.finalize, collection_indexer.py:341-444, minus codec/IVF)."""
     offset = n_tokens = 0
@@ -79,20 +109,80 @@ def finalize_chunked_index(path: str, num_chunks: int) -> dict:
         offset += m["num_passages"]
         n_tokens += m["num_embeddings"]
         dim = m["dim"] if dim is None else dim
-    meta = {"format": FORMAT, "n_passages": offset, "n_tokens": n_tokens, "dim": dim,
+    meta = {"format": fmt, "n_passages": offset, "n_tokens": n_tokens, "dim": dim,
             "dtype": "bfloat16", "num_chunks": num_chunks}
-    with open(os.path.join(path, "metadata.json"), "w") as f:
+    tmp = os.path.join(path, "metadata.json.tmp")
+    with open(tmp, "w") as f:
         json.dump(meta, f)
+    os.replace(tmp, os.path.join(path, "metadata.json"))
+    return meta
+
+
+def persist_updates(path: str, new_tokens: Optional[torch.Tensor], new_doclens, deleted,
+                    chunksize: int = 25_000) -> dict:
+    """Bring the flat index at ``path`` up to date with a corpus that was appended to and / or lost passages:
+    ``new_tokens [sum(new_doclens), dim]`` are the passages behind the ``n_passages`` the index holds (may be empty),
+    ``deleted`` every deleted id.  Appended passages become new chunks of at most ``chunksize`` passages; a
+    single-file index is first turned into chunk 0 (its files are linked under the chunk names and the old names
+    removed only after the new metadata.json is in place).  ``deleted.npy`` is written when there are deletions,
+    and metadata.json last, as "flmr-flat-v2" when there are deletions and "flmr-flat-v1" otherwise."""
+    meta = read_metadata(path)
+    n_old = int(meta["n_passages"])
+    num_chunks = int(meta.get("num_chunks", 0))
+    new_doclens = np.ascontiguousarray(np.asarray(new_doclens if new_doclens is not None else [], dtype=np.int32))
+    n_new = int(new_doclens.shape[0])
+    deleted = np.unique(np.asarray(deleted if deleted is not None else [], dtype=np.int64))
+    if deleted.size and (deleted[0] < 0 or deleted[-1] >= n_old + n_new):
+        raise ValueError("deleted ids must lie in [0, %d)" % (n_old + n_new))
+    stale = []
+    if n_new:
+        if new_tokens is None or new_tokens.dim() != 2 or int(new_doclens.sum()) != new_tokens.size(0):
+            raise ValueError("new_tokens must be [sum(new_doclens), dim]")
+        if num_chunks == 0:                                  # single file -> chunk 0
+            for old, new in (("tokens.bf16", "tokens.0.bf16"), ("doclens.npy", "doclens.0.npy")):
+                src, dst = os.path.join(path, old), os.path.join(path, new)
+                if os.path.exists(dst):
+                    os.remove(dst)
+                try:
+                    os.link(src, dst)
+                except OSError:
+                    shutil.copyfile(src, dst)
+                stale.append(src)
+            m0 = {"passage_offset": 0, "num_passages": n_old, "num_embeddings": int(meta["n_tokens"]),
+                  "dim": int(meta["dim"])}
+            with open(os.path.join(path, "0.metadata.json"), "w") as f:
+                json.dump(m0, f)
+            num_chunks = 1
+        off = np.concatenate([[0], np.cumsum(new_doclens, dtype=np.int64)])
+        for a in range(0, n_new, chunksize):
+            b = min(n_new, a + chunksize)
+            save_flat_chunk(path, num_chunks, n_old + a, new_tokens[int(off[a]):int(off[b])], new_doclens[a:b])
+            num_chunks += 1
+    fmt = FORMAT_V2 if deleted.size else FORMAT
+    dpath = os.path.join(path, "deleted.npy")
+    if deleted.size:
+        with open(dpath + ".tmp", "wb") as f:
+            np.save(f, deleted)
+        os.replace(dpath + ".tmp", dpath)
+    if num_chunks:
+        meta = finalize_chunked_index(path, num_chunks, fmt)
+    else:
+        meta = dict(meta, format=fmt)
+        tmp = os.path.join(path, "metadata.json.tmp")
+        with open(tmp, "w") as f:
+            json.dump(meta, f)
+        os.replace(tmp, os.path.join(path, "metadata.json"))
+    for f in stale:
+        os.remove(f)
+    if not deleted.size and os.path.exists(dpath):
+        os.remove(dpath)
     return meta
 
 
 def index_token_files(path: str):
     """(doclens of the whole index int32 [n_passages], [(token file, first passage, passages, rows), ...]) —
     what a streaming loader needs to pick the byte ranges of a passage shard without reading any token."""
-    with open(os.path.join(path, "metadata.json")) as f:
-        meta = json.load(f)
-    if meta.get("format") != FORMAT:
-        raise ValueError("%s is not a %s index" % (path, FORMAT))
+    meta = read_metadata(path)
     if meta.get("num_chunks", 0) == 0:
         doclens = np.load(os.path.join(path, "doclens.npy")).astype(np.int32)
         return doclens, [(os.path.join(path, "tokens.bf16"), 0, len(doclens), int(doclens.sum()))]
@@ -114,11 +204,9 @@ def _read_tokens(fname: str, n_rows: int, dim: int, row0: int = 0, row1: Optiona
 def load_flat_index(path: str, passage_range: Optional[Tuple[int, int]] = None
                     ) -> Tuple[torch.Tensor, np.ndarray, dict]:
     """Returns (tokens bf16 [n_tok, dim] on CPU, doclens int32, metadata) of the whole index or of the
-    passages ``[p0, p1)`` only (a GPU's shard, SURVEY.md 8e) — only the chunks that overlap are read."""
-    with open(os.path.join(path, "metadata.json")) as f:
-        meta = json.load(f)
-    if meta.get("format") != FORMAT:
-        raise ValueError("%s is not a %s index" % (path, FORMAT))
+    passages ``[p0, p1)`` only (a GPU's shard, SURVEY.md 8e) — only the chunks that overlap are read.  Deleted
+    passages of a v2 index are included (their ids stay valid); ``read_deleted`` lists them."""
+    meta = read_metadata(path)
     dim = meta["dim"]
     p0, p1 = passage_range if passage_range is not None else (0, meta["n_passages"])
     if not 0 <= p0 <= p1 <= meta["n_passages"]:

@@ -38,7 +38,7 @@ import torch
 
 from . import _cabi
 from .corpus import FlatCorpus
-from .index_io import FORMAT as FLAT_FORMAT
+from .index_io import FORMATS as FLAT_FORMATS
 from .infra import ColBERTConfig, active_run_config, resolve_index_path
 from .maxsim import maxsim_argmax_grouped, maxsim_scores, maxsim_topk, topk_select
 
@@ -61,6 +61,17 @@ def shortlist_depth(k: int, ndocs: Optional[int], n_candidates: int) -> int:
     if ndocs is None:
         ndocs = _default_knobs(k)[2]
     return min(max(int(ndocs) // 4, k), _cabi.SELECT_MAX_K, n_candidates)
+
+
+def _n_live(corpus) -> int:
+    """Passages a search on ``corpus`` can return: all but the deleted ones (a corpus type without updates: all)."""
+    return corpus.n_live if hasattr(corpus, "n_live") else corpus.n_passages
+
+
+def _live_pids(corpus) -> torch.Tensor:
+    if hasattr(corpus, "live_pids"):
+        return corpus.live_pids()
+    return torch.arange(corpus.n_passages, device=corpus.device) + corpus.pid_base
 
 
 class Ranking:
@@ -151,12 +162,12 @@ def detect_index_kind(path: str) -> str:
     if os.path.exists(meta_path):
         with open(meta_path) as f:
             meta = json.load(f)
-        if meta.get("format") == FLAT_FORMAT:
+        if meta.get("format") in FLAT_FORMATS:
             return "flat"
         if "nbits" in meta.get("config", {}) and os.path.exists(os.path.join(path, "centroids.pt")):
             return "plaid"
         raise ValueError("%s holds a metadata.json that is neither a %s index nor a PLAID index "
-                         "(config.nbits + centroids.pt)" % (path, FLAT_FORMAT))
+                         "(config.nbits + centroids.pt)" % (path, " / ".join(FLAT_FORMATS)))
     if os.path.exists(os.path.join(path, "plan.json")):
         raise ValueError("%s holds only plan.json: the PLAID index build did not finish "
                          "(collection_indexer.py:428-444 writes metadata.json last)" % path)
@@ -307,16 +318,17 @@ class Searcher:
         if self.storage == "fp8":
             return self._reranked_topk(Q, kk, keep)
         if keep is None and kk <= _cabi.MAX_K:
-            kq = min(kk, corpus.n_passages)
+            kq = min(kk, _n_live(corpus))                # deleted passages are never offered to the fused top-k
             outs, outp = [], []
             for b0 in range(0, Q.size(0), self.query_batch):
                 s, p = maxsim_topk(corpus, Q[b0:b0 + self.query_batch], kq, relu=self._relu)
                 outs.append(s)
                 outp.append(p)
             return torch.cat(outs), torch.cat(outp)
-        # filtered or very large k: all scores from the fused scan, selection as plain plumbing
+        # filtered or very large k: all scores from the fused scan, selection as plain plumbing (deleted passages
+        # score -inf, so at most n_live candidates are selected)
         outs, outp = [], []
-        n_cand = corpus.n_passages if keep is None else int(keep.numel())
+        n_cand = _n_live(corpus) if keep is None else int(keep.numel())
         kq = min(kk, n_cand)
         if kq == 0:
             return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=corpus.device),
@@ -340,7 +352,7 @@ class Searcher:
         ``keep``), their exact bf16 tokens gathered from the master and re-scored by the grouped rowmax kernel,
         the top ``kk`` of those exact scores (ties: lower pid)."""
         corpus = self.corpus
-        n_cand = corpus.n_passages if keep is None else int(keep.numel())
+        n_cand = _n_live(corpus) if keep is None else int(keep.numel())
         kq = min(kk, n_cand)
         if kq == 0:
             return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=corpus.device),
@@ -391,8 +403,8 @@ class Searcher:
         corpus = self.corpus
         keep = None
         if filter_fn is not None and corpus is not None:
-            all_pids = torch.arange(corpus.n_passages, device=corpus.device) + corpus.pid_base
-            keep = torch.as_tensor(filter_fn(all_pids), device=corpus.device).long() - corpus.pid_base
+            # the filter sees the live candidates only, as the reference's filter only ever sees candidates
+            keep = torch.as_tensor(filter_fn(_live_pids(corpus)), device=corpus.device).long() - corpus.pid_base
         if self._sharded is not None and int(k) > _cabi.MAX_K:
             raise ValueError("sharded search merges at most k=%d results per query" % _cabi.MAX_K)
         if self._nccl is not None and keep is None and corpus is not None and self.storage != "fp8":
@@ -433,6 +445,8 @@ class Searcher:
         if self._sharded is not None:
             raise RuntimeError("retrieve_and_rescore gathers embeddings from the local shard only; "
                                "use an unsharded Searcher for the RAG block")
+        if _n_live(self.corpus) < n_docs:
+            raise ValueError("the corpus holds %d live passages, fewer than n_docs=%d" % (_n_live(self.corpus), n_docs))
         n_retrieve = max(5, int(n_docs))
         Qd = Q.to(self.corpus.device)
         s, p = self._search_tensors(Qd.detach(), n_retrieve)
@@ -490,6 +504,8 @@ class Searcher:
                 "backend": "ravqa_b200 exhaustive fused scan", "index": self.index,
                 "index_kind": self.index_kind, "exhaustive": True,
                 "n_passages": self.corpus.n_passages if self.corpus is not None else 0,
+                "n_live": _n_live(self.corpus) if self.corpus is not None else 0,
+                "n_deleted": getattr(self.corpus, "n_deleted", 0) if self.corpus is not None else 0,
                 "storage": self.storage}
         if self.storage == "fp8":
             prov["shortlist_depth"] = self._last_depth
