@@ -503,7 +503,7 @@ flmr_merge_kernel(const uint64_t* __restrict__ keys, const float* __restrict__ i
       } else {
         const int64_t pid = in_pids[g];
         if (pid >= 0) {
-          c[i].ord = float_to_ordered(in_scores[g]);
+          c[i].ord = float_to_ordered(in_scores[g] + 0.0f);   // -0 -> +0: equal scores tie on pid (as in select)
           c[i].pid = pid;
         }
       }

@@ -21,7 +21,8 @@
 //                         go to shared memory for the reducer.  The running max of the passage straddling two
 //                         D tiles stays in a register: a query block never changes warpgroup.
 //   warp 4 kWgs         : reducer.  Per D tile (mbarrier-fed, double-buffered partials): per (query, passage
-//                         ending in the tile) sums the row partials in fixed order (deterministic), optionally
+//                         ending in the tile) sums the row partials in one fixed order (chunk_sum16: the same for
+//                         every passage end, so a score does not depend on where the passage is stored), optionally
 //                         accumulates / stores scores to HBM, and maintains the per-CTA top-k.  A passage marked
 //                         in the corpus' tombstone bitmap (ScanParams::dead) is skipped: -inf score, no top-k offer.
 //   warp 4 kWgs + 1     : TMA producer.  Streams the CTA's contiguous range of passage tokens through a
@@ -126,15 +127,6 @@ struct ScanBars {
 };
 
 // ---- epilogue helpers ---------------------------------------------------------------------------
-__device__ __forceinline__ float warp_sum(float s) {
-  s += __shfl_xor_sync(0xffffffffu, s, 16);
-  s += __shfl_xor_sync(0xffffffffu, s, 8);
-  s += __shfl_xor_sync(0xffffffffu, s, 4);
-  s += __shfl_xor_sync(0xffffffffu, s, 2);
-  s += __shfl_xor_sync(0xffffffffu, s, 1);
-  return s;
-}
-
 __device__ __forceinline__ uint64_t shfl64(uint64_t v, int src) {
   const uint32_t lo = __shfl_sync(0xffffffffu, static_cast<uint32_t>(v), src);
   const uint32_t hi = __shfl_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), src);
@@ -173,6 +165,20 @@ __device__ __noinline__ void topk_replace_min(uint64_t* keys, int k, uint64_t ca
 // cold path, kept from adding to the kernel's register allocation.
 __device__ __noinline__ void store_dead_scores(float* out, int64_t n, int nq, int lane) {
   for (int b = lane; b < nq; b += 32) out[b * n] = -INFINITY;
+}
+
+// THE summation order of a passage's score, whichever path computes it (so the score depends on the query and the
+// passage's tokens only, not on where the passage is stored).  The rows of a pass are cut into 16-row chunks; chunk c
+// is summed as ((v0 + v1) + (v2 + v3)) + ((v4 + v5) + (v6 + v7)) with v_q = r[16 c + q] + r[16 c + q + 8], and a query's
+// chunks are then added in row order starting from 0.f (acc_in of earlier row slices last).  A passage that is the
+// 5th or later to end in its tile is chunk-summed by the consumer warp that holds the rows (fold_accumulator's
+// shuffle tree), the first kFastSlots by the reducer from the parked row maxima (chunk_sum16).
+// chunk_sum16: the sum of one chunk whose 16 row values are x[0..15], in that order.
+__device__ __forceinline__ float chunk_sum16(const float* x) {
+  float v[8];
+#pragma unroll
+  for (int q = 0; q < 8; ++q) v[q] = x[q] + x[q + 8];
+  return ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]));
 }
 
 // Max of a thread's values x over the quad's four lanes (they hold the same rows, different columns).
@@ -234,7 +240,8 @@ __device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], ui
         }
       }
     } else {
-      // this warp's 16 rows summed in a fixed order (the lanes of a quad hold equal values)
+      // this warp's 16 rows summed in chunk_sum16's order (the lanes of a quad hold equal values; lane group g holds
+      // rows g and g + 8, and the xor-4 / 8 / 16 shuffles pair g with g ^ 1, g ^ 2, g ^ 4)
       float v = s[0] + s[1];
       v += __shfl_xor_sync(0xffffffffu, v, 4);
       v += __shfl_xor_sync(0xffffffffu, v, 8);
@@ -539,7 +546,7 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
             continue;
           }
           if (slot < kFastSlots && p.rbq <= p.lane_mode_max_rbq) {
-            // many short queries per pass: lane = query, each lane sums its query's 32 * rbq lane maxima
+            // many short queries per pass: lane = query, each lane sums its query's 2 * rbq row chunks in order
             // (transposed read of the stride-33 layout: conflict-free for rbq = 1)
   #pragma unroll 1
             for (int b0 = 0; b0 < p.nq_pass; b0 += 32) {
@@ -550,8 +557,8 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
               if (valid) {
                 const float* lp = lp_slot + (b * p.rbq) * kLaneStride;
                 for (int r = 0; r < p.rbq; ++r) {
-  #pragma unroll 8
-                  for (int j = 0; j < 32; ++j) sc += lp[r * kLaneStride + j];
+                  sc += chunk_sum16(lp + r * kLaneStride);
+                  sc += chunk_sum16(lp + r * kLaneStride + 16);
                 }
                 const int64_t gi = static_cast<int64_t>(q_off + b) * p.n_passages + pid;
                 if (p.acc_in) sc += __ldg(p.acc_in + gi);
@@ -582,13 +589,17 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
           } else {
   #pragma unroll 1
             for (int b = 0; b < p.nq_pass; ++b) {
-              // score of (query b, passage pid): the whole warp sums the row-block partials in fixed order
+              // score of (query b, passage pid): the whole warp adds the query's row chunks in row order
               float sc = 0.f;
               if (slot < kFastSlots) {
-                const float* lp = lp_slot + (b * p.rbq) * kLaneStride + lane;
-  #pragma unroll 2
-                for (int r = 0; r < p.rbq; ++r) sc += lp[r * kLaneStride];
-                sc = warp_sum(sc);
+                // lane c < 2 rbq <= 24 sums chunk c (rows of lane c at bank (c >> 1) + 16 (c & 1) + q: conflict-free),
+                // then every lane adds the chunks in order
+                const int n_chunks = 2 * p.rbq;
+                float ch = 0.f;
+                if (lane < n_chunks)
+                  ch = chunk_sum16(lp_slot + (b * p.rbq + (lane >> 1)) * kLaneStride + (lane & 1) * 16);
+  #pragma unroll 4
+                for (int c = 0; c < n_chunks; ++c) sc += __shfl_sync(0xffffffffu, ch, c);
               } else {
                 const float* pr = partial + (buf * kHbMax + 2 * b * p.rbq) * kSlots + slot;
   #pragma unroll 2

@@ -30,6 +30,45 @@ def golden_names():
     return sorted(os.path.basename(p)[:-4] for p in glob.glob(os.path.join(GOLDEN_DIR, "g[0-9]*.npz")))
 
 
+def placement_doclens(n: int = 20_000, seed: int = 0) -> np.ndarray:
+    """Passage lengths of the placement fixture: most passages 1-23 tokens, so that a 96-token scan tile holds more
+    than the 4 passage ends whose row maxima the reducer sums itself; one in 16 is 24-200 tokens long."""
+    rng = np.random.default_rng(seed)
+    dl = rng.integers(1, 24, size=n)
+    long = rng.random(n) < 1 / 16
+    dl[long] = rng.integers(24, 201, size=int(long.sum()))
+    return dl.astype(np.int32)
+
+
+def placement_tracked(n: int) -> np.ndarray:
+    """Tracked passages of the placement fixture: the front of the corpus (the first two of 132 CTAs, where a
+    prepended passage shifts every passage) and every 97th passage after it."""
+    return np.concatenate([np.arange(300), np.arange(300, n, 97)])
+
+
+def scan_slots(doclens, n_ctas: int = 132) -> np.ndarray:
+    """Slot of every passage in the scan's partition for `n_ctas` CTAs (host-only flmr_debug_build_partition): the
+    passage is the slot-th passage to end in its 96-token tile.  The reducer sums slots 0-3 from parked row maxima
+    and later slots from the consumer warps' 16-row sums."""
+    from ravqa_b200 import _cabi
+    L = _cabi.lib()
+    dl = np.ascontiguousarray(doclens, dtype=np.int32)
+    rb = np.zeros(n_ctas + 1, np.int32)
+    tb = np.zeros(n_ctas + 1, np.int64)
+    cap = int(((dl.astype(np.int64) + 3) // 4 * 4).sum() // 96 + n_ctas + 1)
+    em = np.zeros(cap, np.uint32)
+    fp = np.zeros(cap, np.int32)
+    nt = C.c_int64()
+    _cabi.check(L.flmr_debug_build_partition(dl.ctypes.data, len(dl), n_ctas, rb.ctypes.data, tb.ctypes.data,
+                                             em.ctypes.data, fp.ctypes.data, cap, C.byref(nt)))
+    slot = np.full(len(dl), -1, np.int64)
+    for mask, first in zip(em[:nt.value].tolist(), fp[:nt.value].tolist()):
+        n_end = bin(mask).count("1")
+        slot[first:first + n_end] = np.arange(n_end)
+    assert (slot >= 0).all()
+    return slot
+
+
 def c_oracle():
     """Build (if needed) and load oracle/_ref/libmaxsim_oracle.so."""
     path = os.path.join(ROOT, "oracle", "_ref", "libmaxsim_oracle.so")

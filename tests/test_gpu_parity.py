@@ -216,9 +216,20 @@ def test_big_planted_positive_recall(R, big):
 
 
 def test_shard_concatenation_invariance(R):
-    """Sharding property (SURVEY 8e): top-k over the whole corpus == merge of per-shard top-k."""
+    """Sharding property (SURVEY 8e): top-k over the whole corpus == merge of per-shard top-k, bitwise.
+    30-60-token passages: at most 4 passage ends per 96-token tile."""
+    _check_shard_concatenation(R, 4000, 60, 21)
+
+
+def test_shard_concatenation_invariance_short_passages(R):
+    """The same property on 12-23-token passages: a tile holds more than 4 passage ends, so sharding moves passages
+    between the reducer's two forms of partial sums (parked row maxima and the consumer warps' 16-row sums)."""
+    _check_shard_concatenation(R, 8000, 23, 22)
+
+
+def _check_shard_concatenation(R, n, nd, seed):
     from ravqa_b200.sharded import shard_ranges
-    Q, D, dl = O.synth(4000, 60, 4, 64, seed=21, ragged=True)
+    Q, D, dl = O.synth(n, nd, 4, 64, seed=seed, ragged=True)
     whole = _corpus(R, D, dl)
     ws, wp = R.maxsim_topk(whole, torch.from_numpy(Q), 10)
     off = np.concatenate([[0], np.cumsum(dl)])
@@ -306,13 +317,11 @@ def test_three_warpgroup_scan_kernel_is_bit_identical(case):
         L.flmr_debug_set_scan_variant(0)
     for x, y in zip(outs[2], outs[3]):
         assert torch.equal(x, y)
-    # CTA-pair passes (variant 4; the product uses them on shards that span every SM): another partition of the
-    # passages, so a passage that is the 5th or later to end inside its tile is summed lanes-first instead of
-    # row-blocks-first — last-bit differences in the scores, the same ranking
+    # CTA-pair passes (variant 4) partition the passages differently; every passage end is summed in the same order,
+    # so the scores are bitwise those of the single-CTA kernel too
     for variant in (4, 0):
-        np.testing.assert_allclose(outs[variant][0].cpu().numpy(), outs[2][0].cpu().numpy(), rtol=2e-6)
-        assert torch.equal(outs[variant][2], outs[2][2])
-        np.testing.assert_allclose(outs[variant][1].cpu().numpy(), outs[2][1].cpu().numpy(), rtol=2e-6)
+        for x, y in zip(outs[variant], outs[2]):
+            assert torch.equal(x, y), variant
     ref = O.maxsim_scores(Q, D, dl, relu=relu)
     np.testing.assert_allclose(outs[3][0].cpu().numpy(), ref, rtol=2e-5)
 
@@ -343,8 +352,8 @@ def test_c2_shape_against_the_c_oracle():
 def test_big_cta_pair_passes_properties(R, big):
     """120k passages, SIX Nq = 320 queries through three CTA-pair passes (variant 4: clusters of two CTAs, TMA
     multicast, one query resident in each CTA).  Fused top-k == stable sort of all scores (same call pattern),
-    deterministic, and equal — scores to the last bits a different tile partition can move, ids exactly — to the
-    single-CTA kernel forced onto all six."""
+    deterministic, and bitwise equal to the single-CTA kernel forced onto all six (another tile partition, the same
+    summation order)."""
     from ravqa_b200 import _cabi
     corpus, D, Q3, n_p, nd = big
     L = _cabi.lib()
@@ -368,7 +377,7 @@ def test_big_cta_pair_passes_properties(R, big):
         _, tp_single = R.maxsim_topk(corpus, Q, 100)
     finally:
         L.flmr_debug_set_scan_variant(0)
-    np.testing.assert_allclose(s_all.cpu().numpy(), s_single.cpu().numpy(), rtol=2e-6)
+    assert torch.equal(s_all, s_single)
     assert torch.equal(tp, tp_single)
 
 
