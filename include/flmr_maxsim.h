@@ -31,6 +31,9 @@
  *   flmr_corpus_append / _delete / _deleted
  *       the add / remove of ColBERT's later IndexUpdater (the vendored release has no update path): passages are
  *       appended to a resident shard in place and deleted ones are tombstoned, tested in the scan's reducer.
+ *   flmr_maxsim_scores_allowed / flmr_maxsim_topk_allowed / flmr_maxsim_topk_sharded_allowed
+ *       the pids= / qid_to_pids= restriction of later ColBERT Searchers: a per-query allow bitmap tested in the
+ *       scan's reducer (the vendored release filters scores with filter_fn, CB/searcher.py:61-132).
  *   flmr_debug_maxsim_scores_simt
  *       test infrastructure: an independent plain-SIMT fp32 device kernel used by tests to
  *       cross-check the tensor-core kernel at sizes where the CPU oracle is too slow.
@@ -218,6 +221,29 @@ int flmr_maxsim_topk(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const vo
                      int64_t* d_out_pids, void* stream);
 
 /*
+ * Restricted search: each query is scored against its own set of passages (the pids= / qid_to_pids= of later
+ * ColBERT Searchers: re-ranking a first stage's candidates, one entity's or tenant's passages, a training query
+ * without its positives).  The restriction is tested inside the scan's reducer, so no score matrix is written; the
+ * scan still streams the whole shard, so a restricted search costs what an unrestricted one does.
+ *   d_allow             uint32 device bitmaps, one per query: bit p & 31 of word p >> 5 set <=> query b may return
+ *                       LOCAL passage p (global id pid_base + p).  Query b's bitmap starts at
+ *                       d_allow + b * allow_stride_words.  Bits at or beyond n_passages are ignored.
+ *   allow_stride_words  0 (every query uses the one bitmap at d_allow) or >= ceil(n_passages / 32); any other value
+ *                       gives FLMR_ERR_INVALID_ARG.  d_allow == NULL is the unrestricted call.
+ * A bitmap describes the shard as it is at call time: after flmr_corpus_append a bitmap must be rebuilt (with the
+ * new stride) to reach the new passages.  A disallowed pair behaves like a deleted passage for that query only: -inf
+ * from flmr_maxsim_scores_allowed; never in the lists of the two top-k calls, which are filled with (-inf, -1) when
+ * fewer than k passages are allowed and live.  Allowed scores are bitwise those of the unrestricted call.
+ * flmr_maxsim_topk_sharded_allowed (see below) takes each rank's bitmaps of its own shard.
+ */
+int flmr_maxsim_scores_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries,
+                               int nq, unsigned flags, const uint32_t* d_allow, int64_t allow_stride_words,
+                               float* d_out_scores, void* stream);
+int flmr_maxsim_topk_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries,
+                             int nq, int k, unsigned flags, const uint32_t* d_allow, int64_t allow_stride_words,
+                             float* d_out_scores, int64_t* d_out_pids, void* stream);
+
+/*
  * Merge n_lists candidate lists per query into one top-k (the post-all-gather step of the
  * sharded path).  Entries with pid < 0 are ignored.
  *   d_in_scores fp32  [n_lists, n_queries, k_in]     d_in_pids int64 [n_lists, n_queries, k_in]
@@ -241,6 +267,8 @@ int flmr_topk_merge(const float* d_in_scores, const int64_t* d_in_pids, int n_li
  *   flmr_topk_exchange    all-gather + merge of lists the caller already has (d_scores / d_pids [n_queries, k_in],
  *                         entries with pid < 0 ignored) -> [n_queries, k_out] on EVERY rank
  *   flmr_maxsim_topk_sharded   flmr_maxsim_topk on this rank's shard + flmr_topk_exchange, one call
+ *   flmr_maxsim_topk_sharded_allowed   the same with flmr_maxsim_topk_allowed: every rank passes the bitmaps of its
+ *                         own shard (indexed by local passage)
  */
 int flmr_comm_unique_id(void* out_id_128_bytes);
 int flmr_comm_create(const void* id_128_bytes, int rank, int world_size, int device, flmr_comm_t** out);
@@ -252,6 +280,10 @@ int flmr_topk_exchange(flmr_comm_t* comm, const float* d_scores, const int64_t* 
 int flmr_maxsim_topk_sharded(const flmr_corpus_t* corpus, flmr_workspace_t* ws, flmr_comm_t* comm, const void* d_q,
                              int n_queries, int nq, int k, unsigned flags, float* d_out_scores,
                              int64_t* d_out_pids, void* stream);
+int flmr_maxsim_topk_sharded_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, flmr_comm_t* comm,
+                                     const void* d_q, int n_queries, int nq, int k, unsigned flags,
+                                     const uint32_t* d_allow, int64_t allow_stride_words, float* d_out_scores,
+                                     int64_t* d_out_pids, void* stream);
 
 /*
  * Top-k of dense score rows for k beyond FLMR_MAX_K (Searcher.dense_search accepts any k,

@@ -33,6 +33,9 @@ def _header_define(name: str) -> int:
 TILE_TOKENS = _header_define("FLMR_TILE_TOKENS")
 
 UPDATE_SYMBOLS = ("flmr_corpus_append", "flmr_corpus_delete", "flmr_corpus_deleted")
+ALLOWED_SYMBOLS = ("flmr_maxsim_scores_allowed", "flmr_maxsim_topk_allowed", "flmr_maxsim_topk_sharded_allowed")
+# symbols an earlier revision's library may lack (tools/scan_ab.py drives one through this binding)
+OPTIONAL_SYMBOLS = UPDATE_SYMBOLS + ALLOWED_SYMBOLS
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
@@ -45,7 +48,7 @@ SYMBOLS = [
     "flmr_corpus_builder_create", "flmr_corpus_builder_create_ex", "flmr_corpus_builder_append", "flmr_corpus_builder_append_file",
     "flmr_corpus_builder_finish", "flmr_corpus_builder_destroy",
     "flmr_comm_unique_id", "flmr_comm_create", "flmr_comm_adopt", "flmr_comm_destroy", "flmr_comm_info",
-    "flmr_topk_exchange", "flmr_maxsim_topk_sharded",
+    "flmr_topk_exchange", "flmr_maxsim_topk_sharded", *ALLOWED_SYMBOLS,
     "flmr_debug_maxsim_scores_simt", "flmr_debug_set_argmax_path", "flmr_debug_set_scan_variant", "flmr_debug_build_partition", "flmr_debug_plan_passes",
     "flmr_launch_count", "flmr_set_profiling", "flmr_scan_kernel_stats",
 ]
@@ -91,6 +94,10 @@ def lib() -> C.CDLL:
         L.flmr_corpus_append.argtypes = [vp, vp, vp, i64, C.POINTER(i64)]
         L.flmr_corpus_delete.argtypes = [vp, vp, i64]
         L.flmr_corpus_deleted.argtypes = [vp, C.POINTER(i64), vp, i64]
+    if hasattr(L, "flmr_maxsim_topk_allowed"):
+        L.flmr_maxsim_scores_allowed.argtypes = [vp, vp, vp, i32, i32, u32, vp, i64, vp, vp]
+        L.flmr_maxsim_topk_allowed.argtypes = [vp, vp, vp, i32, i32, i32, u32, vp, i64, vp, vp, vp]
+        L.flmr_maxsim_topk_sharded_allowed.argtypes = [vp, vp, vp, vp, i32, i32, i32, u32, vp, i64, vp, vp, vp]
     L.flmr_workspace_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
     L.flmr_workspace_destroy.argtypes = [vp]
     L.flmr_workspace_status.argtypes = [vp, C.POINTER(i32)]
@@ -128,7 +135,7 @@ def lib() -> C.CDLL:
     L.flmr_set_profiling.argtypes = [i32]
     L.flmr_scan_kernel_stats.argtypes = [C.POINTER(C.c_double), C.POINTER(i64), i32]
     for name in SYMBOLS:
-        if name in UPDATE_SYMBOLS and not hasattr(L, name):
+        if name in OPTIONAL_SYMBOLS and not hasattr(L, name):
             continue
         fn = getattr(L, name)
         if name not in ("flmr_last_error", "flmr_launch_count"):

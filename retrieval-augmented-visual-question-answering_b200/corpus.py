@@ -39,6 +39,37 @@ def _read_storage(handle) -> str:
     return _cabi.STORAGES[code.value]
 
 
+def allow_bitmaps(pid_lists: Sequence, n_passages: int, pid_base: int = 0,
+                  device: Optional[Union[str, torch.device]] = None) -> torch.Tensor:
+    """Per-query allow bitmaps of a shard for ``maxsim_scores`` / ``maxsim_topk`` / ``NcclExchange.search``: int32
+    ``[len(pid_lists), ceil(n_passages / 32)]``, bit ``p & 31`` of word ``p >> 5`` of row b set <=> query b may return
+    the shard's local passage ``p`` (global id ``pid_base + p``).
+
+    ``pid_lists[b]`` is a sequence or tensor of GLOBAL ids, or None (the whole shard: an all-ones row).  Ids outside
+    ``[pid_base, pid_base + n_passages)`` are dropped, so every rank of a sharded search can pass the same global lists;
+    duplicates collapse.  Plain torch, on ``device`` (CPU by default), with one byte of scratch per (query, passage)
+    and no host synchronisation on a GPU."""
+    dev = torch.device(device) if device is not None else torch.device("cpu")
+    n, words, B = int(n_passages), (int(n_passages) + 31) // 32, len(pid_lists)
+    lists = [torch.as_tensor(ids if ids is not None else [], dtype=torch.int64).reshape(-1) for ids in pid_lists]
+    lens = torch.tensor([x.numel() for x in lists], dtype=torch.int64)
+    total = int(lens.sum())
+    flat = torch.cat([x.to(dev) for x in lists]) if total else torch.empty(0, dtype=torch.int64, device=dev)
+    rows = torch.repeat_interleave(torch.arange(B, device=dev), lens.to(dev), output_size=total)
+    local = flat - int(pid_base)
+    inside = (local >= 0) & (local < n)
+    # one bool per (query, passage); ids outside the shard land in a spare row B, so nothing waits for the device
+    dense = torch.zeros((B + 1, words * 32), dtype=torch.bool, device=dev)
+    dense[torch.where(inside, rows, B), torch.where(inside, local, 0)] = True
+    none_rows = [b for b, ids in enumerate(pid_lists) if ids is None]
+    if none_rows:
+        dense[torch.tensor(none_rows, device=dev)] = True
+    # 8 bools -> one byte (bit q = passage 8 j + q), four little-endian bytes -> one int32 word
+    shifts = torch.arange(8, dtype=torch.uint8, device=dev)
+    packed = (dense[:B].view(B, words * 4, 8).to(torch.uint8) << shifts).sum(-1, dtype=torch.uint8)
+    return packed.view(torch.int32)
+
+
 class FlatCorpus:
     """One GPU's shard of the passage-token matrix, resident in HBM.
 
@@ -217,6 +248,11 @@ class FlatCorpus:
         out = np.empty(n.value, dtype=np.int64)
         _cabi.check(L.flmr_corpus_deleted(self.handle, C.byref(n), out.ctypes.data_as(C.c_void_p), out.size))
         return out
+
+    def allow_bitmaps(self, pid_lists: Sequence) -> torch.Tensor:
+        """``allow_bitmaps`` of this shard (its ``n_passages`` and ``pid_base``), on the corpus' device.  A bitmap
+        describes the shard as it is now: after ``append`` build a new one to reach the new passages."""
+        return allow_bitmaps(pid_lists, self.n_passages, self.pid_base, self.device)
 
     def live_pids(self) -> torch.Tensor:
         """Global ids of the passages that are not deleted, ascending, on the corpus' device."""

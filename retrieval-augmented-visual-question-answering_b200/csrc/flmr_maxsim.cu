@@ -1072,14 +1072,18 @@ int ensure_acc(flmr_workspace* ws, int64_t floats) {
   return FLMR_OK;
 }
 
-// Shared driver of flmr_maxsim_scores / flmr_maxsim_topk.
+// Shared driver of flmr_maxsim_scores / flmr_maxsim_topk (and their _allowed forms: `allow` null = unrestricted,
+// else query b's bitmap starts at allow + b * allow_stride).
 int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_queries, int nq,
-               unsigned flags, int k, float* d_all_scores, float* d_topk_scores,
-               int64_t* d_topk_pids, cudaStream_t st) {
+               unsigned flags, int k, const uint32_t* allow, int64_t allow_stride, float* d_all_scores,
+               float* d_topk_scores, int64_t* d_topk_pids, cudaStream_t st) {
   if (!c || !ws || !d_q) return fail(FLMR_ERR_INVALID_ARG, "null corpus / workspace / query pointer");
   if (ws->corpus != c) return fail(FLMR_ERR_INVALID_ARG, "workspace belongs to a different corpus");
   if (n_queries < 0 || nq <= 0) return fail(FLMR_ERR_INVALID_ARG, "bad n_queries=%d nq=%d", n_queries, nq);
   if (k < 0 || k > kMaxK) return fail(FLMR_ERR_UNSUPPORTED, "k=%d outside [1, %d]", k, kMaxK);
+  if (allow && allow_stride != 0 && allow_stride < (c->n_passages + 31) / 32)
+    return fail(FLMR_ERR_INVALID_ARG, "allow_stride_words=%lld: must be 0 or >= %lld", (long long)allow_stride,
+                (long long)((c->n_passages + 31) / 32));
   if (n_queries == 0) return FLMR_OK;
   if (const int code = *reinterpret_cast<volatile int*>(ws->h_status))
     return fail(FLMR_ERR_KERNEL,
@@ -1170,6 +1174,8 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
       p.acc_out = ((pp.flags & kPassAccOut) || ((pp.flags & kPassFinal) && d_all_c)) ? acc : nullptr;
       p.k = (pp.flags & kPassFinal) ? k : 0;
       p.cand_q_first = pp.q_first;
+      p.allow = allow ? allow + static_cast<int64_t>(c0 + pp.q_first) * allow_stride : nullptr;
+      p.allow_stride = allow_stride;
       if ((rc = launch_scan(c, ws, p, (pp.flags & kPassPair) != 0, st))) return rc;
     }
     if (k > 0) {
@@ -1902,18 +1908,31 @@ int flmr_workspace_status(const flmr_workspace_t* ws, int* out) {
 
 int flmr_maxsim_scores(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q,
                        int n_queries, int nq, unsigned flags, float* d_out_scores, void* stream) {
+  return flmr_maxsim_scores_allowed(corpus, ws, d_q, n_queries, nq, flags, nullptr, 0, d_out_scores, stream);
+}
+
+int flmr_maxsim_scores_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries,
+                               int nq, unsigned flags, const uint32_t* d_allow, int64_t allow_stride_words,
+                               float* d_out_scores, void* stream) {
   if (!d_out_scores) return fail(FLMR_ERR_INVALID_ARG, "d_out_scores is null");
-  return run_search(corpus, ws, d_q, n_queries, nq, flags, 0, d_out_scores, nullptr, nullptr,
-                    static_cast<cudaStream_t>(stream));
+  return run_search(corpus, ws, d_q, n_queries, nq, flags, 0, d_allow, allow_stride_words, d_out_scores, nullptr,
+                    nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int flmr_maxsim_topk(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q,
                      int n_queries, int nq, int k, unsigned flags, float* d_out_scores,
                      int64_t* d_out_pids, void* stream) {
+  return flmr_maxsim_topk_allowed(corpus, ws, d_q, n_queries, nq, k, flags, nullptr, 0, d_out_scores, d_out_pids,
+                                  stream);
+}
+
+int flmr_maxsim_topk_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries,
+                             int nq, int k, unsigned flags, const uint32_t* d_allow, int64_t allow_stride_words,
+                             float* d_out_scores, int64_t* d_out_pids, void* stream) {
   if (!d_out_scores || !d_out_pids) return fail(FLMR_ERR_INVALID_ARG, "output pointer is null");
   if (k < 1) return fail(FLMR_ERR_INVALID_ARG, "k=%d must be >= 1", k);
-  return run_search(corpus, ws, d_q, n_queries, nq, flags, k, nullptr, d_out_scores, d_out_pids,
-                    static_cast<cudaStream_t>(stream));
+  return run_search(corpus, ws, d_q, n_queries, nq, flags, k, d_allow, allow_stride_words, nullptr, d_out_scores,
+                    d_out_pids, static_cast<cudaStream_t>(stream));
 }
 
 int flmr_topk_merge(const float* d_in_scores, const int64_t* d_in_pids, int n_lists, int n_queries,
@@ -2454,6 +2473,14 @@ int flmr_topk_exchange(flmr_comm_t* c, const float* d_scores, const int64_t* d_p
 int flmr_maxsim_topk_sharded(const flmr_corpus_t* corpus, flmr_workspace_t* ws, flmr_comm_t* comm, const void* d_q,
                              int n_queries, int nq, int k, unsigned flags, float* d_out_scores,
                              int64_t* d_out_pids, void* stream) {
+  return flmr_maxsim_topk_sharded_allowed(corpus, ws, comm, d_q, n_queries, nq, k, flags, nullptr, 0, d_out_scores,
+                                          d_out_pids, stream);
+}
+
+int flmr_maxsim_topk_sharded_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, flmr_comm_t* comm,
+                                     const void* d_q, int n_queries, int nq, int k, unsigned flags,
+                                     const uint32_t* d_allow, int64_t allow_stride_words, float* d_out_scores,
+                                     int64_t* d_out_pids, void* stream) {
   if (!comm) return fail(FLMR_ERR_INVALID_ARG, "comm is null");
   if (!d_out_scores || !d_out_pids) return fail(FLMR_ERR_INVALID_ARG, "output pointer is null");
   if (k < 1 || k > kMaxK) return fail(FLMR_ERR_INVALID_ARG, "k=%d outside [1, %d]", k, kMaxK);
@@ -2473,7 +2500,8 @@ int flmr_maxsim_topk_sharded(const flmr_corpus_t* corpus, flmr_workspace_t* ws, 
     FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&comm->d_send_p), static_cast<size_t>(n) * sizeof(int64_t)));
   }
   // this rank's shard (the fused scan fills short lists with (-inf, -1), which the merge ignores)
-  if (int rc = run_search(corpus, ws, d_q, n_queries, nq, flags, k, nullptr, comm->d_send_s, comm->d_send_p, st))
+  if (int rc = run_search(corpus, ws, d_q, n_queries, nq, flags, k, d_allow, allow_stride_words, nullptr,
+                          comm->d_send_s, comm->d_send_p, st))
     return rc;
   return flmr_topk_exchange(comm, comm->d_send_s, comm->d_send_p, n_queries, k, k, d_out_scores, d_out_pids, stream);
 }

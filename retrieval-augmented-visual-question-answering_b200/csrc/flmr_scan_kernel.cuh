@@ -25,6 +25,8 @@
 //                         every passage end, so a score does not depend on where the passage is stored), optionally
 //                         accumulates / stores scores to HBM, and maintains the per-CTA top-k.  A passage marked
 //                         in the corpus' tombstone bitmap (ScanParams::dead) is skipped: -inf score, no top-k offer.
+//                         A (query, passage) pair whose bit is clear in the query's allow bitmap (ScanParams::allow)
+//                         is treated the same way for that query only.
 //   warp 4 kWgs + 1     : TMA producer.  Streams the CTA's contiguous range of passage tokens through a
 //                         kDStages-deep ring of D stages (96 tokens x 128 dims bf16, 128B-swizzled, 2 boxes;
 //                         e4m3 corpora: one box of 96 x 128 bytes).
@@ -91,6 +93,10 @@ struct ScanParams {
   float* acc_out;                  // [nq_pass][n_passages] scores (or partial scores) out, or null
   int64_t n_passages;
   const uint32_t* dead;            // [ceil(n_passages / 32)] tombstones (bit p & 31 of word p >> 5), or null: none
+  // per-query allow bitmaps (layout of `dead`): the pass's query b may return passage p only if bit p of
+  // allow[(q_off + b) * allow_stride ...] is set (q_off: the CTA-pair offset); null: every passage allowed
+  const uint32_t* allow;
+  int64_t allow_stride;            // words between consecutive queries' bitmaps; 0 = one bitmap for all
   // fused top-k
   int32_t k;                       // 0 = disabled
   uint64_t* cand_keys;             // [n_ctas][cand_q_stride][k]  (ordered score << 32 | ~local pid)
@@ -165,6 +171,12 @@ __device__ __noinline__ void topk_replace_min(uint64_t* keys, int k, uint64_t ca
 // cold path, kept from adding to the kernel's register allocation.
 __device__ __noinline__ void store_dead_scores(float* out, int64_t n, int nq, int lane) {
   for (int b = lane; b < nq; b += 32) out[b * n] = -INFINITY;
+}
+
+// May query qb of the pass (its index in the per-query arrays, CTA-pair offset included) return local passage pid?
+__device__ __forceinline__ bool pair_allowed(const ScanParams& p, int qb, int64_t pid) {
+  return p.allow == nullptr ||
+         ((__ldg(p.allow + static_cast<int64_t>(qb) * p.allow_stride + (pid >> 5)) >> (pid & 31)) & 1u);
 }
 
 // THE summation order of a passage's score, whichever path computes it (so the score depends on the query and the
@@ -552,6 +564,8 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
             for (int b0 = 0; b0 < p.nq_pass; b0 += 32) {
               const int b = b0 + lane;
               const bool valid = b < p.nq_pass;
+              // this lane's query may return the passage (a disallowed lane stores -inf and makes no offer)
+              const bool allowed = valid && pair_allowed(p, q_off + b, pid);
               float sc = 0.f;
               uint64_t key = 0ull;
               if (valid) {
@@ -562,12 +576,13 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
                 }
                 const int64_t gi = static_cast<int64_t>(q_off + b) * p.n_passages + pid;
                 if (p.acc_in) sc += __ldg(p.acc_in + gi);
+                if (!allowed) sc = -INFINITY;
                 if (p.acc_out) p.acc_out[gi] = sc;
                 key = (static_cast<uint64_t>(float_to_ordered(sc)) << 32) |
                       static_cast<uint64_t>(0xFFFFFFFFu - static_cast<uint32_t>(pid));
               }
               if (p.k > 0) {
-                uint32_t hits = __ballot_sync(0xffffffffu, valid && key > minkey_s[valid ? b : 0]);
+                uint32_t hits = __ballot_sync(0xffffffffu, allowed && key > minkey_s[valid ? b : 0]);
                 while (hits) {  // rare after warm-up: one list update at a time
                   const int src = __ffs(hits) - 1;
                   hits &= hits - 1;
@@ -589,6 +604,13 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
           } else {
   #pragma unroll 1
             for (int b = 0; b < p.nq_pass; ++b) {
+              // a pair the query's allow bitmap excludes (warp-uniform test): -inf in the score output, no offer
+              if (!pair_allowed(p, q_off + b, pid)) {
+                if (p.acc_out)
+                  store_dead_scores(p.acc_out + static_cast<int64_t>(q_off + b) * p.n_passages + pid, p.n_passages, 1,
+                                    lane);
+                continue;
+              }
               // score of (query b, passage pid): the whole warp adds the query's row chunks in row order
               float sc = 0.f;
               if (slot < kFastSlots) {

@@ -28,11 +28,28 @@ def _stream(corpus: FlatCorpus) -> C.c_void_p:
     return C.c_void_p(torch.cuda.current_stream(corpus.device).cuda_stream)
 
 
+def _prep_allow(corpus: FlatCorpus, allow: Optional[torch.Tensor], B: int) -> Tuple[Optional[torch.Tensor], int]:
+    """(bitmaps on the corpus' device, stride in words) for ``allow`` = int32 ``[B, words]`` (one bitmap per query) or
+    ``[words]`` (shared, stride 0), ``words = ceil(n_passages / 32)``; ``(None, 0)`` for no restriction."""
+    if allow is None:
+        return None, 0
+    words = (corpus.n_passages + 31) // 32
+    if allow.dtype != torch.int32 or allow.shape not in ((B, words), (words,)):
+        raise ValueError("allow must be int32 [%d, %d] or [%d] (see allow_bitmaps), got %s %s"
+                         % (B, words, words, allow.dtype, tuple(allow.shape)))
+    allow = allow.to(corpus.device).contiguous()
+    return allow, (words if allow.dim() == 2 else 0)
+
+
 def maxsim_scores(corpus: FlatCorpus, Q: torch.Tensor, relu: bool = False,
-                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``out[b, p] = sum_i max_j <Q[b,i], D_p[j]>`` for every passage of the shard (fp32, on GPU)."""
+                  out: Optional[torch.Tensor] = None, allow: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``out[b, p] = sum_i max_j <Q[b,i], D_p[j]>`` for every passage of the shard (fp32, on GPU).
+
+    ``allow`` (see ``allow_bitmaps``) restricts query b to the local passages whose bit is set in its bitmap: the
+    others score -inf, as deleted passages do; allowed scores are bitwise those of the unrestricted call."""
     Qd = _prep_queries(corpus, Q)
     B, nq = Qd.size(0), Qd.size(1)
+    allow, stride = _prep_allow(corpus, allow, B)
     if out is None:
         out = torch.empty((B, corpus.n_passages), dtype=torch.float32, device=corpus.device)
     elif out.shape != (B, corpus.n_passages) or out.dtype != torch.float32 or not out.is_contiguous():
@@ -40,28 +57,44 @@ def maxsim_scores(corpus: FlatCorpus, Q: torch.Tensor, relu: bool = False,
     if B == 0:
         return out
     with torch.cuda.device(corpus.device):
-        _cabi.check(_cabi.lib().flmr_maxsim_scores(
-            corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq,
-            _cabi.FLAG_RELU if relu else 0, C.c_void_p(out.data_ptr()), _stream(corpus)))
+        flags = _cabi.FLAG_RELU if relu else 0
+        if allow is None:
+            _cabi.check(_cabi.lib().flmr_maxsim_scores(
+                corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq, flags,
+                C.c_void_p(out.data_ptr()), _stream(corpus)))
+        else:
+            _cabi.check(_cabi.lib().flmr_maxsim_scores_allowed(
+                corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq, flags,
+                C.c_void_p(allow.data_ptr()), stride, C.c_void_p(out.data_ptr()), _stream(corpus)))
     return out
 
 
-def maxsim_topk(corpus: FlatCorpus, Q: torch.Tensor, k: int, relu: bool = False
-                ) -> Tuple[torch.Tensor, torch.Tensor]:
-    """Fused scan + top-k: ``(scores fp32 [B,k], pids int64 [B,k])`` sorted by descending score."""
+def maxsim_topk(corpus: FlatCorpus, Q: torch.Tensor, k: int, relu: bool = False,
+                allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Fused scan + top-k: ``(scores fp32 [B,k], pids int64 [B,k])`` sorted by descending score.
+
+    ``allow`` (see ``maxsim_scores``): query b ranks only its allowed live passages; a list with fewer than k of them
+    is filled with (-inf, -1)."""
     if not 1 <= k <= _cabi.MAX_K:
         raise ValueError("k=%d outside [1, %d]" % (k, _cabi.MAX_K))
     Qd = _prep_queries(corpus, Q)
     B, nq = Qd.size(0), Qd.size(1)
+    allow, stride = _prep_allow(corpus, allow, B)
     scores = torch.empty((B, k), dtype=torch.float32, device=corpus.device)
     pids = torch.empty((B, k), dtype=torch.int64, device=corpus.device)
     if B == 0:
         return scores, pids
     with torch.cuda.device(corpus.device):
-        _cabi.check(_cabi.lib().flmr_maxsim_topk(
-            corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq, k,
-            _cabi.FLAG_RELU if relu else 0, C.c_void_p(scores.data_ptr()),
-            C.c_void_p(pids.data_ptr()), _stream(corpus)))
+        flags = _cabi.FLAG_RELU if relu else 0
+        if allow is None:
+            _cabi.check(_cabi.lib().flmr_maxsim_topk(
+                corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq, k, flags,
+                C.c_void_p(scores.data_ptr()), C.c_void_p(pids.data_ptr()), _stream(corpus)))
+        else:
+            _cabi.check(_cabi.lib().flmr_maxsim_topk_allowed(
+                corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq, k, flags,
+                C.c_void_p(allow.data_ptr()), stride, C.c_void_p(scores.data_ptr()),
+                C.c_void_p(pids.data_ptr()), _stream(corpus)))
     return scores, pids
 
 

@@ -18,7 +18,8 @@ GPU into the flat bf16 store (plaid.py).
 What differs, by design (SURVEY.md §0): scoring is exhaustive and exact (no PLAID candidate
 generation / centroid pruning), all queries of a call go through one batched fused scan instead of
 a Python loop of per-query ``rank`` calls, and results always hold exactly ``min(k, n_passages)``
-hits.  ``shard_across_ranks=True`` (an extension; needs an initialised ``torch.distributed`` group) keeps
+hits (a restricted search, ``pids=`` / ``qid_to_pids=``: ``min(k, allowed live passages)`` per
+query).  ``shard_across_ranks=True`` (an extension; needs an initialised ``torch.distributed`` group) keeps
 only this rank's passage shard resident and merges the per-shard top-k with one all-gather, where the
 reference repeats the whole search on every rank (FLMR_executor.py:778-781).
 
@@ -37,7 +38,7 @@ from typing import Callable, Dict, List, Optional, Tuple, Union
 import torch
 
 from . import _cabi
-from .corpus import FlatCorpus
+from .corpus import FlatCorpus, allow_bitmaps
 from .index_io import FORMATS as FLAT_FORMATS
 from .infra import ColBERTConfig, active_run_config, resolve_index_path
 from .maxsim import maxsim_argmax_grouped, maxsim_scores, maxsim_topk, topk_select
@@ -72,6 +73,25 @@ def _live_pids(corpus) -> torch.Tensor:
     if hasattr(corpus, "live_pids"):
         return corpus.live_pids()
     return torch.arange(corpus.n_passages, device=corpus.device) + corpus.pid_base
+
+
+def _popcount_rows(words: torch.Tensor) -> torch.Tensor:
+    """Set bits per row of an int32 bitmap ``[B, words]`` (int64 ``[B]``)."""
+    x = words.to(torch.int64) & 0xFFFFFFFF
+    x = x - ((x >> 1) & 0x55555555)
+    x = (x & 0x33333333) + ((x >> 2) & 0x33333333)
+    x = (x + (x >> 4)) & 0x0F0F0F0F
+    return (((x * 0x01010101) & 0xFFFFFFFF) >> 24).sum(dim=-1)
+
+
+def _live_words(corpus) -> torch.Tensor:
+    """Bitmap ``[words]`` of the passages of ``corpus`` a search can return (not deleted; no bits past the end)."""
+    n = corpus.n_passages
+    dead = corpus.deleted_pids() if hasattr(corpus, "deleted_pids") else []
+    live = ~allow_bitmaps([dead], n, corpus.pid_base, corpus.device)[0]
+    if n % 32:
+        live[-1] &= (1 << (n % 32)) - 1
+    return live
 
 
 class Ranking:
@@ -243,6 +263,14 @@ class Searcher:
         if self._sharded is not None and self._want_nccl:
             from .sharded import NcclExchange
             self._nccl = NcclExchange(self.device, self._group)       # collective: every rank constructs it
+        if self._sharded is not None:
+            # passages of the whole index, for checking the ids of restricted searches; collective, and fixed: a
+            # sharded Searcher cannot be updated
+            import torch.distributed as dist
+            n = self.corpus.pid_base + self.corpus.n_passages if self.corpus is not None else 0
+            t = torch.tensor([n], dtype=torch.int64, device=self.device if self._want_nccl else "cpu")
+            dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self._group)
+            self._sharded_index_size = int(t.item())
         self._relu = False
 
     # -- reference-compatible surface ------------------------------------------------------------
@@ -286,15 +314,15 @@ class Searcher:
             model.query_tokenizer.query_maxlen = maxlen
         return model.queryFromText(queries, bsize=bsize, to_cpu=False)
 
-    def search(self, text: str, k: int = 10, filter_fn=None):
-        return self.dense_search(self.encode(text), k, filter_fn=filter_fn)
+    def search(self, text: str, k: int = 10, filter_fn=None, pids=None):
+        return self.dense_search(self.encode(text), k, filter_fn=filter_fn, pids=pids)
 
-    def search_all(self, queries, k: int = 10, filter_fn=None):
+    def search_all(self, queries, k: int = 10, filter_fn=None, qid_to_pids=None):
         texts = list(queries.values()) if hasattr(queries, "values") else list(queries)
         Q = self.encode(texts)
         if isinstance(Q, (list, tuple)):               # queryFromText with a batch size returns per-batch tensors
             Q = torch.cat(list(Q))
-        return self._search_all_Q(queries, Q, k, filter_fn=filter_fn)
+        return self._search_all_Q(queries, Q, k, filter_fn=filter_fn, qid_to_pids=qid_to_pids)
 
     @staticmethod
     def _drop_zero_rows(Q: torch.Tensor) -> torch.Tensor:
@@ -380,7 +408,8 @@ class Searcher:
         rows of the corpus; the gather is split by queries to hold at most RERANK_GATHER_BYTES of tokens."""
         corpus = self.corpus
         depth = cand.size(1)
-        nd_max = int(corpus.doclens[(cand - corpus.pid_base).cpu().numpy()].max())
+        c = cand[cand >= 0]                              # (-1: an empty entry, gathered as an all-masked row)
+        nd_max = int(corpus.doclens[(c - corpus.pid_base).cpu().numpy()].max()) if c.numel() else 1
         per_query = depth * nd_max * _cabi.DIM * 2
         step = max(1, RERANK_GATHER_BYTES // per_query)
         out = []
@@ -393,13 +422,113 @@ class Searcher:
             out.append(rowmax.sum(dim=-1))
         return torch.cat(out)
 
+    def _index_size(self) -> int:
+        """Passages of the whole index (every shard, deleted ones included): ids a search may name are below it."""
+        if self._sharded is not None:
+            return self._sharded_index_size
+        return self.corpus.pid_base + self.corpus.n_passages
+
+    def _restricted_tensors(self, Q: torch.Tensor, k: int, filter_fn, pid_lists: List
+                            ) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``_search_tensors`` with query b restricted to the SET of global ids ``pid_lists[b]`` (None: the whole
+        index).  The whole batch is checked before anything is searched.  Each query's allowed ids become a bitmap
+        the scan's reducer tests, so there is no score matrix on the fused path.  Rows are padded with (-inf, -1)."""
+        n_index = self._index_size()
+        lists = []
+        for ids in pid_lists:
+            if ids is not None:
+                ids = torch.as_tensor(ids, dtype=torch.int64).reshape(-1).cpu()
+                if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= n_index):
+                    raise ValueError("passage id %d outside the index [0, %d)"
+                                     % (int(ids.min()) if int(ids.min()) < 0 else int(ids.max()), n_index))
+            lists.append(ids)
+        if self._sharded is not None and k > _cabi.MAX_K:
+            raise ValueError("sharded search merges at most k=%d results per query" % _cabi.MAX_K)
+        corpus = self.corpus
+        B = Q.size(0)
+        if filter_fn is not None:
+            # applied to each query's own list, as the reference applies it to the pids it was given
+            everything = _live_pids(corpus) if corpus is not None else torch.empty(0, dtype=torch.int64)
+            lists = [torch.as_tensor(filter_fn(ids.to(everything.device) if ids is not None else everything)).long()
+                     for ids in lists]
+        # the C-level sharded search (scan + exchange in one call) takes bf16 shards; the others exchange below
+        c_level = self._nccl is not None and corpus is not None and self.storage != "fp8"
+        parts = []
+        if corpus is not None:
+            for b0 in range(0, B, self.query_batch):
+                Qb = Q[b0:b0 + self.query_batch]
+                allow = corpus.allow_bitmaps(lists[b0:b0 + self.query_batch])     # built on the device
+                if c_level:
+                    parts.append(self._nccl.search(corpus, Qb, k, relu=self._relu, allow=allow))
+                else:
+                    parts.append(self._allowed_topk(Qb, k, allow))
+        width = k if self._sharded is not None else max([ps.size(1) for ps, _ in parts], default=0)
+        s = torch.full((B, width), float("-inf"), dtype=torch.float32, device=self.device)
+        p = torch.full((B, width), -1, dtype=torch.int64, device=self.device)
+        b0 = 0
+        for ps, pp in parts:
+            s[b0:b0 + ps.size(0), :ps.size(1)] = ps
+            p[b0:b0 + pp.size(0), :pp.size(1)] = pp
+            b0 += ps.size(0)
+        if self._sharded is not None and not c_level:
+            # one exchange per query batch, as the ranks on the C-level path make (a rank without a shard takes this
+            # branch while the others may not)
+            ex = self._nccl or self._sharded
+            merged = [ex.exchange(s[b0:b0 + self.query_batch], p[b0:b0 + self.query_batch], k)
+                      for b0 in range(0, B, self.query_batch)]
+            s, p = torch.cat([m[0] for m in merged]), torch.cat([m[1] for m in merged])
+        n_valid = int((p >= 0).sum(dim=1).max()) if p.numel() else 0
+        return s[:, :n_valid], p[:, :n_valid]
+
+    def _allowed_topk(self, Q: torch.Tensor, k: int, allow: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Top-k of this shard for queries restricted by ``allow`` (``[B, words]``): (scores, global pids)
+        ``[B, min(k, live passages)]`` (fp8: at most the most allowed live passages of a query), short rows ending in
+        (-inf, -1)."""
+        corpus = self.corpus
+        kq = min(k, _n_live(corpus))
+        n_allowed = None
+        if self.storage == "fp8" and kq > 0:
+            # the shortlist depth follows the allowed count (the one host synchronisation of a restricted search
+            # before its results)
+            n_allowed = int(_popcount_rows(allow & _live_words(corpus)).max())
+            kq = min(kq, n_allowed)
+        if kq == 0:
+            return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=corpus.device),
+                    torch.empty((Q.size(0), 0), dtype=torch.int64, device=corpus.device))
+        if self.storage == "fp8":
+            depth = shortlist_depth(kq, getattr(self.config, "ndocs", None), n_allowed)
+            self._last_depth = depth
+            Qb = Q.to(corpus.device).to(torch.bfloat16)
+            vals, idx = topk_select(maxsim_scores(corpus, Qb, relu=self._relu, allow=allow), depth)
+            # a -inf e4m3 score is a disallowed or deleted passage: it never reaches the exact re-rank
+            cand = torch.where(vals == float("-inf"), -1, idx + corpus.pid_base)
+            cand = torch.sort(cand, dim=1).values        # pid order: the select below breaks exact ties by lower pid
+            exact = self._exact_scores(Qb, cand).masked_fill(cand < 0, float("-inf"))
+            vals, col = topk_select(exact, kq)
+            pids = cand.gather(1, col)
+        elif kq <= _cabi.MAX_K:
+            return maxsim_topk(corpus, Q, kq, relu=self._relu, allow=allow)
+        else:
+            s = maxsim_scores(corpus, Q, relu=self._relu, allow=allow)
+            if kq <= _cabi.SELECT_MAX_K:
+                vals, pids = topk_select(s, kq, corpus.pid_base)
+            else:
+                vals, idx = torch.sort(s, dim=1, descending=True, stable=True)
+                vals, pids = vals[:, :kq], idx[:, :kq] + corpus.pid_base
+        return vals, pids.masked_fill(vals == float("-inf"), -1)
+
     def _search_tensors(self, Q: torch.Tensor, k: int, filter_fn=None,
-                        remove_zero_tensors: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
-        """(scores [B,k'], pids [B,k']) on the GPU, k' = min(k, passages that pass ``filter_fn``)."""
+                        remove_zero_tensors: bool = False, pid_lists: Optional[List] = None
+                        ) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(scores [B,k'], pids [B,k']) on the GPU, k' = min(k, passages that pass ``filter_fn``).  With
+        ``pid_lists`` (one list of global ids, or None, per query) each query searches its own set, and rows with fewer
+        hits end in (-inf, -1) entries."""
         if Q.dim() == 2:
             Q = Q.unsqueeze(0)
         if remove_zero_tensors:
             Q = self._drop_zero_rows(Q)
+        if pid_lists is not None:
+            return self._restricted_tensors(Q, int(k), filter_fn, pid_lists)
         corpus = self.corpus
         keep = None
         if filter_fn is not None and corpus is not None:
@@ -477,26 +606,36 @@ class Searcher:
         if cfg.ndocs is None:
             cfg.configure(ndocs=ndocs)
 
-    def dense_search(self, Q: torch.Tensor, k: int = 10, filter_fn=None, remove_zero_tensors: bool = False):
-        """searcher.py:91-132 -> ``(pids[:k], [1..k], scores[:k])`` for ONE query ``Q [1, Nq, d]``."""
+    def dense_search(self, Q: torch.Tensor, k: int = 10, filter_fn=None, remove_zero_tensors: bool = False,
+                     pids=None):
+        """searcher.py:91-132 -> ``(pids[:k], [1..k], scores[:k])`` for ONE query ``Q [1, Nq, d]``.
+
+        ``pids`` (later ColBERT's argument): search only this set of global ids (``filter_fn``, if given, is applied
+        to it); an id outside the index raises ValueError, deleted ids are never returned."""
         if Q.dim() == 2:
             Q = Q.unsqueeze(0)
         assert Q.size(0) == 1, "dense_search takes a single query (use _search_all_Q for batches)"
         self._fill_search_knobs(k)
-        s, p = self._search_tensors(Q, k, filter_fn, remove_zero_tensors)
-        pids, scores = p[0].tolist(), s[0].tolist()
+        s, p = self._search_tensors(Q, k, filter_fn, remove_zero_tensors, None if pids is None else [pids])
+        hit = p[0] >= 0
+        pids, scores = p[0][hit].tolist(), s[0][hit].tolist()
         return pids, list(range(1, len(pids) + 1)), scores
 
     def _search_all_Q(self, queries, Q: torch.Tensor, k: int, filter_fn=None, progress: bool = True,
-                      remove_zero_tensors: bool = False) -> Ranking:
+                      remove_zero_tensors: bool = False, qid_to_pids=None) -> Ranking:
         """searcher.py:73-89, batched: one fused scan per ``query_batch`` queries instead of a Python
-        loop of per-query ``dense_search`` calls."""
+        loop of per-query ``dense_search`` calls.
+
+        ``qid_to_pids`` (later ColBERT's argument) maps every qid to the global ids its query may return (None: the
+        whole index); a qid missing from it raises KeyError.  Queries may then return fewer than k hits."""
         del progress
         self._fill_search_knobs(k)
         keys = _query_keys(queries, Q.size(0))
-        s, p = self._search_tensors(Q, k, filter_fn, remove_zero_tensors)
+        lists = [qid_to_pids[qid] for qid in keys] if qid_to_pids is not None else None
+        s, p = self._search_tensors(Q, k, filter_fn, remove_zero_tensors, lists)
         s, p = s.cpu().tolist(), p.cpu().tolist()
-        data = {qid: [(pid, rank + 1, score) for rank, (pid, score) in enumerate(zip(pp, ss))]
+        data = {qid: [(pid, rank + 1, score) for rank, (pid, score) in enumerate((pid, sc) for pid, sc in zip(pp, ss)
+                                                                                 if pid >= 0)]
                 for qid, pp, ss in zip(keys, p, s)}
         prov = {"source": "Searcher::search_all", "k": k,
                 "queries": queries.provenance() if hasattr(queries, "provenance") else None,
@@ -506,7 +645,7 @@ class Searcher:
                 "n_passages": self.corpus.n_passages if self.corpus is not None else 0,
                 "n_live": _n_live(self.corpus) if self.corpus is not None else 0,
                 "n_deleted": getattr(self.corpus, "n_deleted", 0) if self.corpus is not None else 0,
-                "storage": self.storage}
+                "storage": self.storage, "restricted": qid_to_pids is not None}
         if self.storage == "fp8":
             prov["shortlist_depth"] = self._last_depth
         return Ranking(data=data, provenance=prov)

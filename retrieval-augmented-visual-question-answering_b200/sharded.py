@@ -54,20 +54,31 @@ class NcclExchange:
         with torch.cuda.device(device):
             _cabi.check(L.flmr_comm_create(C.c_char_p(raw), self.rank, self.world, int(device.index), C.byref(self._h)))
 
-    def search(self, corpus, Q: torch.Tensor, k: int, relu: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``flmr_maxsim_topk_sharded``: (scores [B, k], global pids [B, k]) of the MERGED ranking, on every rank."""
+    def search(self, corpus, Q: torch.Tensor, k: int, relu: bool = False,
+               allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``flmr_maxsim_topk_sharded``: (scores [B, k], global pids [B, k]) of the MERGED ranking, on every rank.
+        ``allow``: this rank's bitmaps of its own shard (``maxsim_topk``'s argument; ``allow_bitmaps`` with the
+        shard's ``n_passages`` and ``pid_base`` builds them from global id lists); short lists end in (-inf, -1)."""
         import ctypes as C
         from . import _cabi
-        from .maxsim import _prep_queries
+        from .maxsim import _prep_allow, _prep_queries
         Qd = _prep_queries(corpus, Q)
         B, nq = Qd.size(0), Qd.size(1)
+        allow, stride = _prep_allow(corpus, allow, B)
         s = torch.empty((B, k), dtype=torch.float32, device=self.device)
         p = torch.empty((B, k), dtype=torch.int64, device=self.device)
+        flags = _cabi.FLAG_RELU if relu else 0
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
         with torch.cuda.device(self.device):
-            _cabi.check(_cabi.lib().flmr_maxsim_topk_sharded(
-                corpus.handle, corpus.workspace(), self._h, C.c_void_p(Qd.data_ptr()), B, nq, k,
-                _cabi.FLAG_RELU if relu else 0, C.c_void_p(s.data_ptr()), C.c_void_p(p.data_ptr()),
-                C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)))
+            if allow is None:
+                _cabi.check(_cabi.lib().flmr_maxsim_topk_sharded(
+                    corpus.handle, corpus.workspace(), self._h, C.c_void_p(Qd.data_ptr()), B, nq, k, flags,
+                    C.c_void_p(s.data_ptr()), C.c_void_p(p.data_ptr()), stream))
+            else:
+                _cabi.check(_cabi.lib().flmr_maxsim_topk_sharded_allowed(
+                    corpus.handle, corpus.workspace(), self._h, C.c_void_p(Qd.data_ptr()), B, nq, k, flags,
+                    C.c_void_p(allow.data_ptr()), stride, C.c_void_p(s.data_ptr()), C.c_void_p(p.data_ptr()),
+                    stream))
         return s, p
 
     def exchange(self, s: torch.Tensor, p: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
