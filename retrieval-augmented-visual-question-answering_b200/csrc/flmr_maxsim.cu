@@ -2176,9 +2176,12 @@ static int argmax_impl(const void* d_q, int n_queries, int nq, const void* d_doc
 static int backward_impl(const void* d_q, int n_queries, int nq, const void* d_docs, int n_per, int stride_b,
                          int nd, const int32_t* d_argmax, const float* d_grad, float* d_dq, float* d_dd,
                          int device, void* stream) {
-  if (!d_q || !d_docs || !d_argmax || !d_grad) return fail(FLMR_ERR_INVALID_ARG, "null pointer");
   if (n_queries < 0 || n_per < 0 || nq <= 0 || nd <= 0)
     return fail(FLMR_ERR_INVALID_ARG, "bad shape n_queries=%d nq=%d n_docs=%d nd=%d", n_queries, nq, n_per, nd);
+  // without documents dQ is zeroed and nothing else is read: empty operands may come as null pointers (an empty
+  // torch tensor has none)
+  if (n_queries > 0 && n_per > 0 && (!d_q || !d_docs || !d_argmax || !d_grad))
+    return fail(FLMR_ERR_INVALID_ARG, "null pointer");
   DeviceGuard guard(device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2234,8 +2237,11 @@ int flmr_ib_loss(const float* d_rowmax, int n_queries, int n_docs, int nq, int n
   DeviceGuard guard(device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
   const size_t smem = static_cast<size_t>(n_docs) * sizeof(float);
-  if (smem > 48 * 1024)
-    FLMR_CUDA(cudaFuncSetAttribute(flmr_ib_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  // the 48 KiB a launch may use without opting in covers static + dynamic shared memory: the kernel's static
+  // reduction buffer counts too (12,288 documents = exactly 48 KiB of scores failed to launch).  Opt in to the whole
+  // 200 KiB the check above admits, so that concurrent callers never lower the limit under each other's launches.
+  if (smem + kIbThreads / 32 * sizeof(float) > 48 * 1024)
+    FLMR_CUDA(cudaFuncSetAttribute(flmr_ib_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   flmr_ib_loss_kernel<<<n_queries, kIbThreads, smem, static_cast<cudaStream_t>(stream)>>>(
       d_rowmax, n_queries, n_docs, nq, nway, label0, d_scores, d_loss_per_query, d_dscores);
   FLMR_CUDA(cudaGetLastError());
