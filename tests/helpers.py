@@ -46,25 +46,44 @@ def placement_tracked(n: int) -> np.ndarray:
     return np.concatenate([np.arange(300), np.arange(300, n, 97)])
 
 
-def scan_slots(doclens, n_ctas: int = 132) -> np.ndarray:
-    """Slot of every passage in the scan's partition for `n_ctas` CTAs (host-only flmr_debug_build_partition): the
-    passage is the slot-th passage to end in its 96-token tile.  The reducer sums slots 0-3 from parked row maxima
-    and later slots from the consumer warps' 16-row sums."""
+def scan_partition(doclens, n_ctas: int = 132) -> dict:
+    """The scan's partition for ``min(n_ctas, n)`` CTAs (host-only ``flmr_debug_build_partition``; passages padded to
+    multiples of 4 rows, 96-row tiles) and what the tests read off it: per-CTA rows and tile ranges, per-tile end masks,
+    and per passage its first / last tile (global tile index) and its slot (the how-manyth passage to end in its
+    tile)."""
     from ravqa_b200 import _cabi
     L = _cabi.lib()
     dl = np.ascontiguousarray(doclens, dtype=np.int32)
-    rb = np.zeros(n_ctas + 1, np.int32)
-    tb = np.zeros(n_ctas + 1, np.int64)
-    cap = int(((dl.astype(np.int64) + 3) // 4 * 4).sum() // 96 + n_ctas + 1)
+    n = len(dl)
+    nc = min(n_ctas, n)
+    rows = (dl.astype(np.int64) + 3) // 4 * 4
+    poff = np.concatenate([[0], np.cumsum(rows)])
+    rb = np.zeros(nc + 1, np.int32)
+    tb = np.zeros(nc + 1, np.int64)
+    cap = int(poff[-1] // 96 + nc + 1)
     em = np.zeros(cap, np.uint32)
     fp = np.zeros(cap, np.int32)
     nt = C.c_int64()
-    _cabi.check(L.flmr_debug_build_partition(dl.ctypes.data, len(dl), n_ctas, rb.ctypes.data, tb.ctypes.data,
-                                             em.ctypes.data, fp.ctypes.data, cap, C.byref(nt)))
-    slot = np.full(len(dl), -1, np.int64)
-    for mask, first in zip(em[:nt.value].tolist(), fp[:nt.value].tolist()):
-        n_end = bin(mask).count("1")
-        slot[first:first + n_end] = np.arange(n_end)
+    _cabi.check(L.flmr_debug_build_partition(dl.ctypes.data, n, nc, rb.ctypes.data, tb.ctypes.data, em.ctypes.data,
+                                             fp.ctypes.data, cap, C.byref(nt)))
+    em, fp = em[:nt.value], fp[:nt.value]
+    cta_of_row = np.searchsorted(rb[1:], poff[:-1], side="right")          # CTA of each passage's first row
+    first_tile = tb[cta_of_row] + (poff[:-1] - rb[cta_of_row]) // 96
+    last_tile = tb[cta_of_row] + (poff[1:] - 1 - rb[cta_of_row]) // 96
+    slot = np.full(n, -1, np.int64)
+    for mask, first in zip(em.tolist(), fp.tolist()):
+        k = bin(mask).count("1")
+        slot[first:first + k] = np.arange(k)
+    return {"n_ctas": nc, "row_begin": rb, "tile_base": tb, "end_mask": em, "first_pid": fp, "rows": rows,
+            "n_rows": int(poff[-1]), "first_tile": first_tile, "last_tile": last_tile, "slot": slot,
+            "cta_rows": np.diff(rb.astype(np.int64)), "cta_tiles": np.diff(tb)}
+
+
+def scan_slots(doclens, n_ctas: int = 132) -> np.ndarray:
+    """Slot of every passage in the scan's partition for `n_ctas` CTAs: the passage is the slot-th passage to end in
+    its 96-token tile.  The reducer sums slots 0-3 from parked row maxima and later slots from the consumer warps'
+    16-row sums."""
+    slot = scan_partition(doclens, n_ctas)["slot"]
     assert (slot >= 0).all()
     return slot
 
