@@ -243,6 +243,36 @@ __device__ __forceinline__ void wgmma_m64n96k32_e4m3(float (&d)[48], uint64_t a_
       : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
+// D (+)= A[smem] * B[smem]^T, m64n48k16, bf16 in / fp32 accumulate; d[24] per thread (the fragment of m64n96k16
+// restricted to its first six 8-column blocks).
+__device__ __forceinline__ void wgmma_m64n48k16(float (&d)[24], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23"
+      "}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+      : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// D (+)= A[smem] * B[smem]^T, m64n48k32, e4m3 in / fp32 accumulate; d[24] per thread, the fragment of m64n48k16.
+__device__ __forceinline__ void wgmma_m64n48k32_e4m3(float (&d)[24], uint64_t a_desc, uint64_t b_desc,
+                                                     uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k32.f32.e4m3.e4m3 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23"
+      "}, %24, %25, p, 1, 1;\n\t}"
+      : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
 // D (+)= A[smem] * B[smem]^T, m64n128k16, bf16 in / fp32 accumulate; d[64] per thread.
 __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(

@@ -834,7 +834,8 @@ constexpr int kNcclInt64 = 4, kNcclFloat32 = 7;   // ncclDataType_t values (nccl
 
 thread_local bool g_profiling = false;
 // which scan kernel a search on this thread launches: 0 = chosen per pass (launch_scan), 2 = flmr_scan_kernel<2> (two
-// consumer warpgroups), 3 = flmr_scan_kernel<3> (three), 4 = CTA-pair passes forced; flmr_debug_set_scan_variant
+// consumer warpgroups), 3 = flmr_scan_kernel<3> (three), 4 = CTA-pair passes forced, 6 = flmr_scan_split_kernel
+// (three, split-tile loop; 5 stays unassigned); flmr_debug_set_scan_variant
 thread_local int g_scan_variant = 0;
 struct EventPair {
   cudaEvent_t a, b;
@@ -981,14 +982,16 @@ void plan_passes(int n_queries, int nq, bool allow_pair, std::vector<PassPlan>* 
 }
 
 int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pair, cudaStream_t st) {
-  // by the pass's occupied 64-row blocks: from five up (Nq = 320: five, a full row slice: six) three warpgroups
-  // (2 / 2 / 1 or 2 / 2 / 2 blocks, serial loop: one warpgroup's MMAs overlap another's fold), below that two
-  // (each with two accumulators, its own MMAs overlapping its fold).  On an H100 (400 W, 200k x 180-token passages,
-  // median of 5) a 5-block pass took 9.19 ms with three and 10.34 ms with two (3 / 2 blocks), 6-block row slices
-  // 9.12 vs 9.64 ms, a 4-block pass 7.90 vs 7.39 ms (DESIGN.md 4.1); the e4m3 kernels follow the same threshold (1M
-  // passages, 700 W: 5 blocks 23.3 vs 31.7 ms, 4 blocks 21.4 vs 19.3 ms).  The instantiations compute bit-identical results
-  const bool use3 = !pair && ((g_scan_variant == 3) ||
-                              (g_scan_variant == 0 && scan_blocks(p.nq_pass, p.rbq) >= 5));
+  // by the pass's occupied 64-row blocks: from five up (Nq = 320: five, a full row slice: six) three warpgroups with
+  // the split-tile loop (2 / 2 / 1 or 2 / 2 / 2 blocks, each warpgroup folding one half of a tile under the MMAs of
+  // the other), below that two (each with two accumulators, its own MMAs overlapping its fold).  On an H100 80GB HBM3
+  // (700 W, 200k x 180-token passages, median of 5, DESIGN.md 4.1) 16 x Nq = 320 took 6.27 ms split, 6.72 ms with
+  // the serial three-warpgroup loop and 7.98 ms with two warpgroups; 3 x Nq = 832 row slices 6.63 / 6.73 / 7.19 ms;
+  // a 4-block pass (4 x Nq = 256) 5.55 / 5.91 / 5.46 ms.  e4m3 follows the same threshold (5 blocks: 3.95 ms split,
+  // 5.00 ms serial).  Every instantiation computes bit-identical results
+  const bool split = !pair && ((g_scan_variant == 6) ||
+                               (g_scan_variant == 0 && scan_blocks(p.nq_pass, p.rbq) >= 5));
+  const bool use3 = !pair && g_scan_variant == 3;
   EventPair ev{};
   if (g_profiling) {
     FLMR_CUDA(cudaEventCreate(&ev.a));
@@ -1015,6 +1018,11 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     FLMR_CUDA(cudaLaunchKernelEx(&cfg, flmr_scan_kernel<2, true>, c->tmap_half, p));
+  } else if (split) {
+    if (c->fp8)
+      flmr_scan_split_kernel<true><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    else
+      flmr_scan_split_kernel<false><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
   } else if (c->fp8) {
     if (use3)
       flmr_scan_kernel<3, false, true><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
@@ -1259,6 +1267,11 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
       e1 = c->fp8 ? cudaFuncSetAttribute(flmr_scan_kernel<3, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          ScanSmem::kBytes)
                   : cudaFuncSetAttribute(flmr_scan_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         ScanSmem::kBytes);
+    if (e1 == cudaSuccess)
+      e1 = c->fp8 ? cudaFuncSetAttribute(flmr_scan_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         ScanSmem::kBytes)
+                  : cudaFuncSetAttribute(flmr_scan_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          ScanSmem::kBytes);
     if (e1 != cudaSuccess)
       return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
@@ -2303,8 +2316,9 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
 }
 
 int flmr_debug_set_scan_variant(int variant) {
-  if (variant != 0 && variant != 2 && variant != 3 && variant != 4)
-    return fail(FLMR_ERR_INVALID_ARG, "variant must be 0 (default), 2 or 3 (epilogue warpgroups) or 4 (CTA-pair experiment)");
+  if (variant != 0 && variant != 2 && variant != 3 && variant != 4 && variant != 6)
+    return fail(FLMR_ERR_INVALID_ARG, "variant must be 0 (default), 2 or 3 (epilogue warpgroups), 4 (CTA-pair "
+                "experiment) or 6 (three warpgroups, split-tile loop)");
   g_scan_variant = variant;
   return FLMR_OK;
 }

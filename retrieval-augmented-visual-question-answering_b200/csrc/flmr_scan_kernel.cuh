@@ -207,26 +207,42 @@ __device__ __forceinline__ float quad_max(float x) {
 // 8-column block i in row half h are acc[4 i + 2 h] and acc[4 i + 2 h + 1]; lanes with the same hi (lane, lane ^ 1)
 // together cover the 4-token group 2 i + hi.  The accumulator is read in place: no per-block maxima are kept,
 // which leaves the registers for the second accumulator of the pipelined consumer loop.
-__device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], uint32_t mask, float (&m)[2],
-                                                 float init, float* lane_part_buf, float* partial_buf, int j,
-                                                 int wq, int lane) {
+// kPart = 0 folds a whole tile (kCb = kNb).  The split loop folds a tile as two halves of kCb = kNb / 2 blocks (its
+// m64n48 accumulators: 4-token groups 12 hf .. 12 hf + 11, `mask` shifted down to them), kPart = 1 and 2.  `slot` is
+// the tile's passage-end count before these columns (0, or half 0's ends for half 1) and the count after them is
+// returned, so the halves park their ends in the slots a whole-tile fold gives them.  Half 0 leaves the maxima of the
+// passage open at its end in `pend`, per thread (not yet combined over the quad), and half 1 starts from them: the
+// quad is combined once per passage end and once per tile, as in the whole-tile fold.  `pend` is unused for kPart = 0.
+template <int kCb = kNb, int kPart = 0>
+__device__ __forceinline__ int fold_accumulator(const float (&acc)[4 * kCb], uint32_t mask, float (&m)[2],
+                                                float (&pend)[2], float init, float* lane_part_buf,
+                                                float* partial_buf, int j, int wq, int lane, int slot = 0) {
+  static_assert(kPart == 0 ? kCb == kNb : kCb == kNb / 2, "a whole tile or one of its halves");
   const int hi = (lane >> 1) & 1;
-  if (mask == 0) {   // warp-uniform: no passage ends in this tile (about half the tiles at Nd = 180)
+  float carry[2];   // this thread's max over the open passage's columns before these ones (half 1 only)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) carry[h] = kPart == 2 ? pend[h] : -INFINITY;
+  if (mask == 0) {   // warp-uniform: no passage ends in these columns (about half the tiles at Nd = 180)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      float c[4];   // four independent max chains over the 24 columns
+      float c[4];   // four independent max chains over the thread's columns
 #pragma unroll
       for (int i = 0; i < 4; ++i) c[i] = fmaxf(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
 #pragma unroll
-      for (int i = 4; i < kNb; ++i) c[i & 3] = fmax3(c[i & 3], acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-      m[h] = fmaxf(m[h], quad_max(fmaxf(fmaxf(c[0], c[1]), fmaxf(c[2], c[3]))));
+      for (int i = 4; i < kCb; ++i) c[i & 3] = fmax3(c[i & 3], acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+      const float x = fmaxf(fmaxf(c[0], c[1]), fmaxf(c[2], c[3]));
+      if constexpr (kPart == 1)
+        pend[h] = x;
+      else if constexpr (kPart == 2)
+        m[h] = fmaxf(m[h], quad_max(fmaxf(carry[h], x)));
+      else
+        m[h] = fmaxf(m[h], quad_max(x));
     }
-    return;
+    return slot;
   }
   const int row0 = j * 64 + wq * 16 + (lane >> 2);   // row of h = 0 inside the pass; h = 1 is row0 + 8
-  uint32_t live = (1u << kSlots) - 1u;               // groups not yet consumed by a finished passage
+  uint32_t live = (1u << (2 * kCb)) - 1u;            // groups not yet consumed by a finished passage
   uint32_t bits = mask;
-  int slot = 0;
 #pragma unroll 1
   while (bits) {   // warp-uniform: one iteration per passage ending in this tile
     const uint32_t upto = bits ^ (bits - 1u);   // groups 0..(lowest set bit)
@@ -234,12 +250,13 @@ __device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], ui
     float s[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      float x = -INFINITY;
+      float x = carry[h];
 #pragma unroll
-      for (int i = 0; i < kNb; ++i)
+      for (int i = 0; i < kCb; ++i)
         if ((seg >> (2 * i)) & 1u) x = fmax3(x, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
       s[h] = fmaxf(quad_max(x), m[h]);
       m[h] = init;
+      carry[h] = -INFINITY;
     }
     if (slot < kFastSlots) {
       // common case: one lane per quad parks its two rows' maxima, the reducer sums them later
@@ -267,19 +284,26 @@ __device__ __forceinline__ void fold_accumulator(const float (&acc)[4 * kNb], ui
   const uint32_t rest = live >> hi;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    float x = -INFINITY;
+    float x = carry[h];
 #pragma unroll
-    for (int i = 0; i < kNb; ++i)
+    for (int i = 0; i < kCb; ++i)
       if ((rest >> (2 * i)) & 1u) x = fmax3(x, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-    m[h] = fmaxf(m[h], quad_max(x));
+    if constexpr (kPart == 1)
+      pend[h] = x;
+    else
+      m[h] = fmaxf(m[h], quad_max(x));
   }
+  return slot;
 }
 
 // acc = (64-row query block at q_block) . (D tile at d_stage)^T over K = 128, one commit group: bf16, 8 x
 // wgmma.m64n96k16 over two 128-byte k-blocks; e4m3 (kFp8), 4 x wgmma.m64n96k32 over one.  Either way a k-step is 32
 // bytes along the row, and the accumulator fragment is the same.
-template <bool kFp8>
-__device__ __forceinline__ void issue_block_mma(float (&acc)[4 * kNb], uint32_t q_block, uint32_t d_stage) {
+// A 24-register accumulator takes 48 tokens instead (m64n48, the split loop's tile halves): `d_stage` then points
+// 48 rows (6 KiB, whole swizzle atoms) into the stage for half 1, and the k-steps and their order are unchanged.
+template <bool kFp8, int kAcc>
+__device__ __forceinline__ void issue_block_mma(float (&acc)[kAcc], uint32_t q_block, uint32_t d_stage) {
+  static_assert(kAcc == 4 * kNb || kAcc == 2 * kNb, "a whole 96-token tile or one 48-token half");
   // the query block's descriptors are loop-invariant: hidden from the compiler so that they are rebuilt here (a
   // few integer adds) rather than hoisted out of the tile loop into 16 registers per block
   asm volatile("" : "+r"(q_block));
@@ -289,7 +313,10 @@ __device__ __forceinline__ void issue_block_mma(float (&acc)[4 * kNb], uint32_t 
     for (int k = 0; k < kDim / 32; ++k) {
       const uint64_t a_desc = make_kmajor_sw128_desc(q_block + k * 32u);   // 32 elements along the 128-byte row
       const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + k * 32u);
-      wgmma_m64n96k32_e4m3(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+      if constexpr (kAcc == 4 * kNb)
+        wgmma_m64n96k32_e4m3(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+      else
+        wgmma_m64n48k32_e4m3(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
     }
   } else {
 #pragma unroll
@@ -297,7 +324,10 @@ __device__ __forceinline__ void issue_block_mma(float (&acc)[4 * kNb], uint32_t 
       const uint32_t koff = (k & 3) * 32u;   // 16 elements along the 128-byte row
       const uint64_t a_desc = make_kmajor_sw128_desc(q_block + (k >> 2) * kQKBlockBytes + koff);
       const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + (k >> 2) * kDKBlockBytes + koff);
-      wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+      if constexpr (kAcc == 4 * kNb)
+        wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+      else
+        wgmma_m64n48k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
     }
   }
   wgmma_commit();
@@ -314,6 +344,16 @@ __device__ __forceinline__ void issue_block_mma(float (&acc)[4 * kNb], uint32_t 
 // last pair has no successor, are peeled out of the loop.
 // kOverlap = false is the serial form with one accumulator (next MMAs issued after the fold, wait_group 0), for
 // instantiations without the registers for two; the arithmetic and its order are the same.
+//
+// -DFLMR_SCAN_SKELETON (a timing build of tools/scan_split_probe.py, never the library's): the three-warpgroup
+// consumer loops, serial and split, issue their MMAs and keep every wait and barrier but fold nothing, so they time
+// the MMA pipe and the loop's synchronisation alone.  Their scores are meaningless.
+#ifdef FLMR_SCAN_SKELETON
+constexpr bool kScanSkeleton = true;
+#else
+constexpr bool kScanSkeleton = false;
+#endif
+
 template <int NB, int kWgs, bool kPair, bool kOverlap, bool kFp8>
 __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base, ScanBars bars,
                                               int n_tiles, int64_t tile_base, int wg, int wq, int lane) {
@@ -374,7 +414,9 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
       if (u == 0)
         mbar_wait_inline(bars.p_empty(buf), ((static_cast<uint32_t>(t) >> 1) & 1u) ^ 1u, p.status,
                          kDevTimeoutEpilogue);
-      fold_accumulator(acc[a], mask, m[u], init, lane_part_buf, partial_buf, wg + u * kWgs, wq, lane);
+      float unused[2];
+      if (!(kScanSkeleton && kWgs == 3))
+        fold_accumulator(acc[a], mask, m[u], unused, init, lane_part_buf, partial_buf, wg + u * kWgs, wq, lane);
       if (!kOverlap) issue_next(acc[0]);
     }
     // this warp's row maxima / partial sums of tile t are written: order every lane's stores
@@ -404,6 +446,96 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
   }
 }
 
+// The consumer loop of flmr_scan_split_kernel: one of three warpgroups, NB (1 or 2) query blocks, with the registers of
+// the serial loop (two 24-register half accumulators) but its fold overlapped with its own MMAs.  Each (tile, block)
+// pair is split along N into two commit groups of m64n48 MMAs: half 0 = tokens 0..47 (4-token groups 0..11) in
+// acc[0], half 1 = tokens 48..95 (groups 12..23) in acc[1].  The sequence of (tile, block, half) triples is
+// software-pipelined: the next triple is issued, wait_group 1, the current one is folded — half 0 under the MMAs of
+// half 1, half 1 under those of half 0 of the next block (or of the first block of the next tile).  The half index is
+// the accumulator index, so every tile is entered with half 0 of its first block in flight in acc[0] and only the
+// last tile is peeled.  The fold carries the open passage's maxima and the passage-end slot from half 0 to half 1 in
+// the same thread: a passage's row maxima and chunk sums are the values, in the order, of the whole-tile fold (max is
+// exact, whatever order it is taken in), and the scores bitwise those of flmr_scan_kernel.
+template <int NB, bool kFp8>
+__device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base,
+                                                    ScanBars bars, int n_tiles, int64_t tile_base, int wg, int wq,
+                                                    int lane) {
+  using S = ScanSmem;
+  constexpr int kWgs = 3;
+  constexpr int kHalfGroups = kSlots / 2;                  // 4-token groups of a half tile
+  constexpr uint32_t kHalfBytes = (kTileN / 2) * 128;      // 48 rows of a k-block: the B offset of half 1
+  static_assert(kHalfBytes % 1024 == 0, "half 1 must start on a swizzle atom");
+  const float init = p.init_val;
+  float m[NB][2];   // running passage maxima of block u's two rows of this thread
+#pragma unroll
+  for (int u = 0; u < NB; ++u) m[u][0] = m[u][1] = init;
+  float* const lane_part = reinterpret_cast<float*>(smem + S::kOffLanePart);
+  float* const partial = reinterpret_cast<float*>(smem + S::kOffPartial);
+  const uint32_t q_smem = smem_base + S::kOffQ;
+  auto q_block = [&](int u) { return q_smem + (wg + u * kWgs) * 64 * 128; };
+  auto d_half = [&](int t, int hf) { return smem_base + S::kOffD + (t % kDStages) * kDTileBytes + hf * kHalfBytes; };
+  float acc[2][2 * kNb];
+  uint32_t mask_next = 0;
+
+  // tile t, entered with the MMAs of (t, 0, half 0) in flight in acc[0]; kNext: a tile t + 1 follows
+  auto tile = [&](int t, auto knext) {
+    constexpr bool kNext = decltype(knext)::value;
+    const uint32_t mask = mask_next;
+    const int buf = t & 1;
+    float* lane_part_buf = lane_part + buf * (kFastSlots * kRbMax * kLaneStride);
+    float* partial_buf = partial + buf * (kHbMax * kSlots);
+#pragma unroll
+    for (int u = 0; u < NB; ++u) {
+      const bool last = u + 1 == NB;
+      const int j = wg + u * kWgs;
+      issue_block_mma<kFp8>(acc[1], q_block(u), d_half(t, 1));
+      wgmma_wait<1>();
+      wgmma_fence_operands(acc[0]);
+      // the reducer must have consumed the partial sums of tile t-2 before this buffer is reused
+      if (u == 0)
+        mbar_wait_inline(bars.p_empty(buf), ((static_cast<uint32_t>(t) >> 1) & 1u) ^ 1u, p.status,
+                         kDevTimeoutEpilogue);
+      int slot = 0;
+      float pend[2];   // half 0's per-thread maxima of the passage open at its end, for half 1
+      if (!kScanSkeleton)
+        slot = fold_accumulator<kNb / 2, 1>(acc[0], mask & ((1u << kHalfGroups) - 1u), m[u], pend, init,
+                                            lane_part_buf, partial_buf, j, wq, lane);
+      if (!last) {
+        issue_block_mma<kFp8>(acc[0], q_block(u + 1), d_half(t, 0));
+        wgmma_wait<1>();
+      } else if (kNext) {
+        mbar_wait_inline(bars.d_full((t + 1) % kDStages), ((t + 1) / kDStages) & 1u, p.status, kDevTimeoutMma);
+        mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
+        issue_block_mma<kFp8>(acc[0], q_block(0), d_half(t + 1, 0));
+        wgmma_wait<1>();
+      } else {
+        wgmma_wait<0>();
+      }
+      wgmma_fence_operands(acc[1]);
+      if (last) {
+        // every wgmma reading D stage t has completed (the one in flight reads stage t + 1) -> release it
+        __syncwarp();
+        if (wq == 0 && lane == 0) mbar_arrive(bars.d_empty(t % kDStages));
+      }
+      if (!kScanSkeleton)
+        fold_accumulator<kNb / 2, 2>(acc[1], mask >> kHalfGroups, m[u], pend, init, lane_part_buf, partial_buf, j,
+                                     wq, lane, slot);
+    }
+    // this warp's row maxima / partial sums of tile t are written: order every lane's stores
+    // before lane 0's arrive (release); the reducer's wait is the matching acquire
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bars.p_full(buf));
+  };
+
+  if (n_tiles <= 0) return;
+  mbar_wait(bars.d_full(0), 0u, p.status, kDevTimeoutMma);
+  mask_next = __ldg(p.tile_end_mask + tile_base);
+  issue_block_mma<kFp8>(acc[0], q_block(0), d_half(0, 0));
+  int t = 0;
+  for (; t + 1 < n_tiles; ++t) tile(t, std::true_type{});
+  tile(t, std::false_type{});
+}
+
 // ---- the kernel -------------------------------------------------------------------------------
 // kWgs = consumer warpgroups (2 or 3): the 64-row query blocks are dealt to them round-robin, so with three
 // resident 128-row tiles (six blocks) three warpgroups take two blocks each.  The per-row arithmetic and its
@@ -418,10 +550,13 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
 // k-block per row (a D tile is one 96-row TMA box of 12 KiB) and the MMAs are wgmma.m64n96k32 e4m3.  Tiles, masks,
 // the shared-memory layout (each stage and the query area keep their bf16 size, half used), the fold, the reducer and
 // the top-k are those of the bf16 kernel.  There is no CTA-pair fp8 kernel.
-template <int kWgs, bool kPair = false, bool kFp8 = false>
-__global__ void __launch_bounds__(scan_threads(kWgs), 1)
-flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+//
+// kSplit = true (flmr_scan_split_kernel, three warpgroups) runs scan_split_consumer instead of scan_consumer; the
+// producer, the reducer, the barriers and the shared-memory layout are the same code.
+template <int kWgs, bool kPair, bool kFp8, bool kSplit>
+__device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, const ScanParams& p) {
   static_assert(!(kPair && kFp8), "the CTA-pair kernel is bf16 only");
+  static_assert(!kSplit || (kWgs == 3 && !kPair), "the split consumer loop is written for three single-CTA warpgroups");
   using S = ScanSmem;
   constexpr int kConsumerWarps = kWgs * 4;
   constexpr int kWarpRed0 = kConsumerWarps;
@@ -666,7 +801,13 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
     // warp-uniform block count of this warpgroup, dispatched to a loop that knows it at compile time (with a
     // run-time count ptxas serialises the wgmma of the two accumulators)
     const int nb = wg < n_blocks ? (n_blocks - wg + kWgs - 1) / kWgs : 0;
-    if (nb == 1) {
+    if constexpr (kSplit) {
+      if (nb == 1) {
+        scan_split_consumer<1, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      } else if (nb == 2) {
+        scan_split_consumer<2, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      }
+    } else if (nb == 1) {
       scan_consumer<1, kWgs, kPair, kOverlap, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     } else if (nb == 2) {
       scan_consumer<2, kWgs, kPair, kOverlap, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
@@ -677,6 +818,20 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
 
   // ---- teardown -----------------------------------------------------------------------------------
   if constexpr (kPair) cluster_sync_all();   // no CTA leaves while its peer may still signal its barriers
+}
+
+template <int kWgs, bool kPair = false, bool kFp8 = false>
+__global__ void __launch_bounds__(scan_threads(kWgs), 1)
+flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<kWgs, kPair, kFp8, false>(tmap_d, p);
+}
+
+// Three consumer warpgroups whose loop folds one half of each tile while the MMAs of the other half run
+// (scan_split_consumer); bit-identical to flmr_scan_kernel<3, false, kFp8>.
+template <bool kFp8>
+__global__ void __launch_bounds__(scan_threads(3), 1)
+flmr_scan_split_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<3, false, kFp8, true>(tmap_d, p);
 }
 
 }  // namespace flmr
