@@ -28,6 +28,10 @@
  *       APPROXIMATE; the exact bf16 rows stay in pinned host memory for flmr_corpus_gather.  The first stage of
  *       a two-stage search whose exact second stage re-scores a shortlist (the Python Searcher does both), as
  *       PLAID scores its ndocs/4 survivors exactly (CB/search/index_storage.py:160-177).
+ *   FLMR_CORPUS_FP16, flmr_plaid_decode_fp16
+ *       an fp16 corpus: the precision the reference keeps and scores its embeddings in (ColBERT.doc returns
+ *       D.half(), colbert_score multiplies in D's dtype, CB/modeling/colbert.py:205-206, 284; the residual codec
+ *       decodes to fp16, CB/indexing/codecs/residual.py:273), scanned with fp16 MMAs instead of being rounded to bf16.
  *   flmr_corpus_append / _delete / _deleted
  *       the add / remove of ColBERT's later IndexUpdater (the vendored release has no update path): passages are
  *       appended to a resident shard in place and deleted ones are tombstoned, tested in the scan's reducer.
@@ -86,6 +90,17 @@ extern "C" {
 #define FLMR_CORPUS_FP8 2u   /* HBM holds the tokens as e4m3 (round to nearest even, saturated;  \
                                 half the bytes); the library keeps a pinned host copy of the      \
                                 exact bf16 rows.  Not combinable with FLMR_CORPUS_ADOPT.         */
+#define FLMR_CORPUS_FP16 4u  /* HBM holds the tokens as fp16 (same bytes and layout as bf16; the  \
+                                scan runs fp16 MMAs).  Combines with FLMR_CORPUS_ADOPT; not with  \
+                                FLMR_CORPUS_FP8 (FLMR_ERR_INVALID_ARG).                          */
+
+/*
+ * INPUT ELEMENT TYPE (one rule for every call below): token rows and query rows arrive in the corpus' element
+ * type.  An FLMR_CORPUS_FP16 corpus takes fp16 rows — the tokens of flmr_corpus_create, flmr_corpus_append,
+ * flmr_corpus_builder_append(_file) and the d_q of every search call — and flmr_corpus_gather writes fp16 rows
+ * from it.  A bf16 corpus and an FLMR_CORPUS_FP8 corpus take (and gather) bf16 rows.  Where a comment below says
+ * "bf16" for such an operand, it means this type.
+ */
 
 #define FLMR_DIM 128        /* embedding dim of FLMR / ColBERT (CB/infra/config/settings.py:101) */
 #define FLMR_TOKEN_GROUP 4  /* passages are stored padded to a multiple of this many tokens     */
@@ -131,9 +146,9 @@ int flmr_corpus_destroy(flmr_corpus_t* corpus);
 int flmr_corpus_info(const flmr_corpus_t* corpus, flmr_corpus_info_t* out);
 
 /*
- * How the corpus stores its tokens: *storage = 0 (bf16 in HBM) or 1 (FLMR_CORPUS_FP8: e4m3 in HBM, counted in
- * hbm_bytes, plus the bf16 master in pinned host memory, *host_bytes bytes; 0 for a bf16 corpus).  Either output
- * may be NULL.
+ * How the corpus stores its tokens: *storage = 0 (bf16 in HBM), 1 (FLMR_CORPUS_FP8: e4m3 in HBM, counted in
+ * hbm_bytes, plus the bf16 master in pinned host memory, *host_bytes bytes; 0 for the other storages) or 2
+ * (FLMR_CORPUS_FP16: fp16 in HBM).  Either output may be NULL.
  *
  * On an e4m3 corpus flmr_maxsim_scores, flmr_maxsim_topk and flmr_maxsim_topk_sharded compute MaxSim of e4m3(Q)
  * against e4m3(D) with fp32 accumulation (Q rounded to nearest even, no scale): APPROXIMATE scores (up to about 6e-3
@@ -181,7 +196,8 @@ int flmr_corpus_deleted(const flmr_corpus_t* corpus, int64_t* n_deleted, int64_t
 int flmr_corpus_builder_create(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
                                int64_t pid_base, flmr_corpus_builder_t** out);
 /* The same with corpus flags: FLMR_CORPUS_FP8 builds an e4m3 corpus (the staged rows fill the bf16 master and
- * HBM receives e4m3); 0 is flmr_corpus_builder_create. */
+ * HBM receives e4m3); FLMR_CORPUS_FP16 an fp16 corpus (the rows appended are fp16); 0 is
+ * flmr_corpus_builder_create. */
 int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
                                   int64_t pid_base, unsigned flags, flmr_corpus_builder_t** out);
 int flmr_corpus_builder_append(flmr_corpus_builder_t* b, const void* h_tokens_bf16, int64_t n_rows);
@@ -310,6 +326,11 @@ int flmr_topk_select(const float* d_scores, int n_queries, int64_t n, int k, int
 int flmr_plaid_decode(const int32_t* d_codes, const uint8_t* d_residuals, int64_t n_tokens,
                       const float* d_centroids, int64_t n_centroids, const float* d_bucket_weights,
                       int nbits, int dim, int normalize, void* d_out_bf16, int device, void* stream);
+/* The same decode into fp16 (d_out_fp16 fp16 [n_tokens, dim]): computed in fp32, normalised, rounded once to fp16
+ * (nearest even), as the bf16 output is rounded to bf16 — the rows an FLMR_CORPUS_FP16 corpus takes. */
+int flmr_plaid_decode_fp16(const int32_t* d_codes, const uint8_t* d_residuals, int64_t n_tokens,
+                           const float* d_centroids, int64_t n_centroids, const float* d_bucket_weights,
+                           int nbits, int dim, int normalize, void* d_out_fp16, int device, void* stream);
 
 /*
  * Gather retrieved passages out of the resident corpus into a padded batch — the operand of the RAG
@@ -384,7 +405,8 @@ int flmr_maxsim_backward_grouped(const void* d_q, int n_queries, int nq, const v
                                  float* d_dq, float* d_dd, int device, void* stream);
 
 /* Test infrastructure: plain SIMT fp32 MaxSim of every passage (same contract as
- * flmr_maxsim_scores, e4m3 semantics on an e4m3 corpus), independent of the tensor-core kernel. */
+ * flmr_maxsim_scores, e4m3 semantics on an e4m3 corpus, fp16 operands on an fp16 corpus), independent of the
+ * tensor-core kernel. */
 int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* corpus, const void* d_q, int n_queries,
                                   int nq, unsigned flags, float* d_out_scores, void* stream);
 
@@ -393,8 +415,9 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* corpus, const void* d_q, 
  * 2 = flmr_scan_kernel<2> (two consumer warpgroups), normal passes only, 3 = flmr_scan_kernel<3> (three
  * warpgroups), normal passes only, 4 = CTA-pair passes (clusters of two CTAs stream one token
  * range, each D tile fetched once and TMA-multicast to both) whenever a call has enough queries, on any bf16 shard
- * (a search on an e4m3 corpus returns FLMR_ERR_UNSUPPORTED) — so the parity suite can run against any of them at
- * any shape. */
+ * (a search on an e4m3 corpus returns FLMR_ERR_UNSUPPORTED), 6 = flmr_scan_split_kernel (three warpgroups,
+ * split-tile loop) — so the parity suite can run against any of them at any shape.  An FLMR_CORPUS_FP16 corpus has
+ * fp16 forms of variants 2 and 6 only: a search on it under variant 3 or 4 returns FLMR_ERR_UNSUPPORTED. */
 int flmr_debug_set_scan_variant(int variant);
 
 /* Test infrastructure: which kernel flmr_maxsim_argmax(_grouped) runs on the calling thread — 0 = chosen by size

@@ -16,7 +16,8 @@ FLAG_RELU = 1
 CORPUS_COPY = 0
 CORPUS_ADOPT = 1
 CORPUS_FP8 = 2
-STORAGES = ("bf16", "fp8")     # flmr_corpus_storage codes 0 and 1
+CORPUS_FP16 = 4
+STORAGES = ("bf16", "fp8", "fp16")     # flmr_corpus_storage codes 0, 1 and 2
 DIM = 128
 TOKEN_GROUP = 4
 MAX_K = 128
@@ -34,8 +35,9 @@ TILE_TOKENS = _header_define("FLMR_TILE_TOKENS")
 
 UPDATE_SYMBOLS = ("flmr_corpus_append", "flmr_corpus_delete", "flmr_corpus_deleted")
 ALLOWED_SYMBOLS = ("flmr_maxsim_scores_allowed", "flmr_maxsim_topk_allowed", "flmr_maxsim_topk_sharded_allowed")
+FP16_SYMBOLS = ("flmr_plaid_decode_fp16",)
 # symbols an earlier revision's library may lack (tools/scan_ab.py drives one through this binding)
-OPTIONAL_SYMBOLS = UPDATE_SYMBOLS + ALLOWED_SYMBOLS
+OPTIONAL_SYMBOLS = UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
@@ -43,6 +45,7 @@ SYMBOLS = [
     *UPDATE_SYMBOLS,
     "flmr_workspace_create", "flmr_workspace_destroy", "flmr_workspace_status",
     "flmr_maxsim_scores", "flmr_maxsim_topk", "flmr_topk_merge", "flmr_topk_select", "flmr_plaid_decode",
+    *FP16_SYMBOLS,
     "flmr_maxsim_argmax", "flmr_maxsim_backward", "flmr_corpus_gather",
     "flmr_maxsim_argmax_grouped", "flmr_maxsim_backward_grouped", "flmr_ib_loss",
     "flmr_corpus_builder_create", "flmr_corpus_builder_create_ex", "flmr_corpus_builder_append", "flmr_corpus_builder_append_file",
@@ -106,6 +109,8 @@ def lib() -> C.CDLL:
     L.flmr_topk_merge.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, i32, vp]
     L.flmr_topk_select.argtypes = [vp, i32, i64, i32, i64, vp, vp, i32, vp]
     L.flmr_plaid_decode.argtypes = [vp, vp, i64, vp, i64, vp, i32, i32, i32, vp, i32, vp]
+    if hasattr(L, "flmr_plaid_decode_fp16"):
+        L.flmr_plaid_decode_fp16.argtypes = [vp, vp, i64, vp, i64, vp, i32, i32, i32, vp, i32, vp]
     L.flmr_corpus_gather.argtypes = [vp, vp, i64, i32, vp, vp, vp]
     L.flmr_maxsim_argmax.argtypes = [vp, i32, i32, vp, vp, i32, i32, vp, vp, i32, vp]
     L.flmr_maxsim_backward.argtypes = [vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, i32, vp]

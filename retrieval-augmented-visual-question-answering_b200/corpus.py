@@ -30,7 +30,14 @@ def _as_doclens(doclens) -> np.ndarray:
 def _storage_flag(storage: str) -> int:
     if storage not in _cabi.STORAGES:
         raise ValueError("storage must be one of %s, got %r" % (_cabi.STORAGES, storage))
-    return _cabi.CORPUS_FP8 if storage == "fp8" else 0
+    return {"bf16": 0, "fp8": _cabi.CORPUS_FP8, "fp16": _cabi.CORPUS_FP16}[storage]
+
+
+def element_dtype(storage: str) -> torch.dtype:
+    """The element type of the rows a corpus of ``storage`` takes and gathers, and of the queries it is searched
+    with: fp16 for "fp16", bf16 for "bf16" and "fp8" (whose exact rows are bf16)."""
+    _storage_flag(storage)
+    return torch.float16 if storage == "fp16" else torch.bfloat16
 
 
 def _read_storage(handle) -> str:
@@ -73,21 +80,27 @@ def allow_bitmaps(pid_lists: Sequence, n_passages: int, pid_base: int = 0,
 class FlatCorpus:
     """One GPU's shard of the passage-token matrix, resident in HBM.
 
-    tokens   : ``[sum(doclens), 128]`` tensor (bf16 preferred; fp16/fp32 are rounded to bf16), on CPU
-               or on the target GPU.  A CUDA bf16 tensor whose doclens are all multiples of 4 is
-               adopted zero-copy (and kept alive by this object).
+    tokens   : ``[sum(doclens), 128]`` tensor in the storage's element type (``element_dtype``: bf16, or fp16 for
+               ``storage="fp16"``; other dtypes are converted once), on CPU or on the target GPU.  A CUDA tensor
+               of that type whose doclens are all multiples of 4 is adopted zero-copy (and kept alive by this
+               object).
     doclens  : per-passage token counts (>= 1 each).
     pid_base : global id of this shard's first passage (sharded search, SURVEY.md §8e).
     storage  : "bf16" (default) or "fp8": HBM holds the tokens as e4m3 (half the bytes; the scan's scores become
                approximate, ``Searcher`` re-ranks a shortlist exactly) and the library keeps the exact bf16 rows
                in pinned host memory, where ``gather_padded`` reads them.  An fp8 corpus never adopts ``tokens``.
+               Or "fp16": HBM holds fp16 tokens (the reference's own precision: ``ColBERT.doc`` returns ``D.half()``)
+               and the scan runs fp16 MMAs, at the bytes and layout of bf16.  fp32 / bf16 sources are converted
+               with torch's ``.half()`` as the reference does (beyond +-65504 they become +-inf); queries are
+               converted to fp16 for the search, and ``gather_padded`` returns fp16 rows.
     """
 
     def __init__(self, tokens: torch.Tensor, doclens, device: Optional[Union[int, torch.device]] = None,
                  pid_base: int = 0, adopt: bool = True, storage: str = "bf16"):
         if not torch.cuda.is_available():
             raise RuntimeError("FlatCorpus needs a CUDA device: there is no CPU fallback for this path")
-        fp8 = _storage_flag(storage)
+        sflag = _storage_flag(storage)
+        dtype = element_dtype(storage)
         L = _cabi.lib()
         self.doclens = _as_doclens(doclens)
         if tokens.dim() != 2 or tokens.size(1) != _cabi.DIM:
@@ -101,12 +114,13 @@ class FlatCorpus:
             device = torch.device("cuda", torch.cuda.current_device())
         self.device = device
         tokens = tokens.detach()
-        if tokens.dtype != torch.bfloat16:
-            tokens = tokens.to(torch.bfloat16)
+        if tokens.dtype != dtype:
+            tokens = tokens.to(dtype)
         tokens = tokens.contiguous()
         if tokens.is_cuda and tokens.device != device:
             tokens = tokens.to(device)
-        flags = fp8 or (_cabi.CORPUS_ADOPT if (adopt and tokens.is_cuda) else _cabi.CORPUS_COPY)
+        # an fp8 corpus keeps its own copies; bf16 and fp16 adopt a CUDA tensor of their element type
+        flags = sflag | (_cabi.CORPUS_ADOPT if (adopt and tokens.is_cuda and storage != "fp8") else _cabi.CORPUS_COPY)
         if tokens.is_cuda:
             torch.cuda.current_stream(device).synchronize()  # producer kernels of `tokens` are done
         handle = C.c_void_p()
@@ -140,9 +154,14 @@ class FlatCorpus:
         self.load_stats = None
         return self
 
+    @property
+    def dtype(self) -> torch.dtype:
+        """Element type of the rows this corpus takes (``append``) and gathers, and of its queries."""
+        return element_dtype(self.storage)
+
     @classmethod
     def from_index(cls, path: str, device=None, rank: int = 0, world_size: int = 1,
-                   storage: str = "bf16") -> "FlatCorpus":
+                   storage: Optional[str] = None) -> "FlatCorpus":
         """Load a flat index (index_io.py) — or, with world_size > 1, only this rank's contiguous,
         token-balanced passage shard of it (SURVEY.md 8e) — into HBM.
 
@@ -151,12 +170,18 @@ class FlatCorpus:
         padded layout — no numpy copy of the shard, no pageable ``cudaMemcpy``.  ``load_stats`` records seconds
         and GB/s (replaces IndexLoader / ResidualEmbeddings.load_chunks, colbert/search/index_loader.py:24-62).
         ``storage="fp8"``: the staged rows fill the bf16 master in pinned host memory, HBM receives e4m3.
+        ``storage=None`` (default) keeps the index's own dtype: "fp16" for an fp16 index ("flmr-flat-f16"), "bf16"
+        otherwise.  A storage of another element type converts the shard once on its way in (read on the host,
+        ``.to()`` the storage's type) instead of streaming the files.
         The deletions an index records (``deleted.npy``, format v2) are applied to the passages of this shard."""
         import time
-        from .index_io import deleted_in_range, index_token_files, read_deleted
+        from .index_io import deleted_in_range, index_dtype, index_token_files, load_flat_index, read_deleted, \
+            read_metadata
         from .sharded import shard_ranges
         if not torch.cuda.is_available():
             raise RuntimeError("FlatCorpus needs a CUDA device: there is no CPU fallback for this path")
+        disk_storage = "fp16" if index_dtype(read_metadata(path)) == "float16" else "bf16"
+        storage = disk_storage if storage is None else storage
         flags = _storage_flag(storage)
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device())
@@ -168,6 +193,13 @@ class FlatCorpus:
         if p0 == p1:
             return None          # more ranks than passages: this rank holds nothing (Searcher copes)
         doclens = np.ascontiguousarray(all_doclens[p0:p1], dtype=np.int32)
+        if element_dtype(storage) != element_dtype(disk_storage):
+            tokens, _, _ = load_flat_index(path, (p0, p1))
+            self = cls(tokens, doclens, device=device, pid_base=p0, storage=storage)
+            dead = deleted_in_range(read_deleted(path), p0, p1)
+            if dead.size:
+                self.delete(dead)
+            return self
         L = _cabi.lib()
         t0 = time.perf_counter()
         b = C.c_void_p()
@@ -201,17 +233,18 @@ class FlatCorpus:
     def from_plaid(cls, path: str, device=None, rank: int = 0, world_size: int = 1,
                    storage: str = "bf16") -> "FlatCorpus":
         """Decode a reference PLAID index directory on the GPU (plaid.py) and keep it resident — with
-        world_size > 1 only this rank's contiguous, token-balanced passage shard (SURVEY.md 8e)."""
+        world_size > 1 only this rank's contiguous, token-balanced passage shard (SURVEY.md 8e).  ``storage="fp16"``
+        decodes straight to fp16 (``flmr_plaid_decode_fp16``), the type the reference's codec decodes to."""
         from .plaid import plaid_to_flat, read_plaid_doclens, read_plaid_metadata
         from .sharded import shard_ranges
         if world_size == 1:
-            tokens, doclens = plaid_to_flat(path, device)
+            tokens, doclens = plaid_to_flat(path, device, dtype=element_dtype(storage))
             return cls(tokens, doclens, device=tokens.device, storage=storage)
         all_doclens = np.concatenate(read_plaid_doclens(path, read_plaid_metadata(path)["num_chunks"]))
         p0, p1 = shard_ranges(all_doclens, world_size)[rank]
         if p0 == p1:
             return None
-        tokens, doclens = plaid_to_flat(path, device, passage_range=(p0, p1))
+        tokens, doclens = plaid_to_flat(path, device, passage_range=(p0, p1), dtype=element_dtype(storage))
         return cls(tokens, doclens, device=tokens.device, pid_base=p0, storage=storage)
 
     # -- properties ---------------------------------------------------------------------------
@@ -265,17 +298,17 @@ class FlatCorpus:
         return pids.to(self.device)
 
     def append(self, tokens: torch.Tensor, doclens) -> np.ndarray:
-        """Append passages (``tokens [sum(doclens), 128]``, on the CPU or on the corpus' GPU; ``doclens`` >= 1 each)
-        behind the stored ones, in place; returns their global ids (int64), which continue the shard's ids.  An
-        adopted token tensor is copied into library memory by the first append and released."""
+        """Append passages (``tokens [sum(doclens), 128]``, on the CPU or on the corpus' GPU, converted to ``dtype``;
+        ``doclens`` >= 1 each) behind the stored ones, in place; returns their global ids (int64), which continue the
+        shard's ids.  An adopted token tensor is copied into library memory by the first append and released."""
         doclens = _as_doclens(doclens)
         if tokens.dim() != 2 or tokens.size(1) != _cabi.DIM:
             raise ValueError("tokens must be [sum(doclens), %d], got %s" % (_cabi.DIM, tuple(tokens.shape)))
         if int(doclens.sum()) != tokens.size(0):
             raise ValueError("sum(doclens)=%d != tokens rows=%d" % (int(doclens.sum()), tokens.size(0)))
         tokens = tokens.detach()
-        if tokens.dtype != torch.bfloat16:
-            tokens = tokens.to(torch.bfloat16)
+        if tokens.dtype != self.dtype:
+            tokens = tokens.to(self.dtype)
         tokens = tokens.contiguous()
         if tokens.is_cuda and tokens.device != self.device:
             tokens = tokens.to(self.device)
@@ -317,7 +350,8 @@ class FlatCorpus:
     def gather_padded(self, pids: torch.Tensor, nd_max: Optional[int] = None):
         """Retrieved passages as a padded batch, straight out of HBM (an fp8 corpus: the exact bf16 rows of its
         pinned host master): ``pids`` (any shape, global ids) ->
-        (tokens bf16 ``[*pids.shape, nd_max, 128]``, mask bool ``[*pids.shape, nd_max, 1]``).  ``nd_max``
+        (tokens ``[*pids.shape, nd_max, 128]`` of ``dtype`` — bf16, fp16 on an fp16 corpus —, mask bool
+        ``[*pids.shape, nd_max, 1]``).  ``nd_max``
         defaults to the longest requested passage.  Ids outside this shard and deleted ids give an all-masked zero
         row.
         Replaces the host-dictionary lookup + stack + H2D of rag_model_blip.py:414-425."""
@@ -326,7 +360,7 @@ class FlatCorpus:
         if nd_max is None:
             local = (flat - self.pid_base).clamp(0, self.n_passages - 1).cpu().numpy()
             nd_max = int(self.doclens[local].max()) if flat.numel() else 1
-        out = torch.empty((flat.numel(), nd_max, _cabi.DIM), dtype=torch.bfloat16, device=self.device)
+        out = torch.empty((flat.numel(), nd_max, _cabi.DIM), dtype=self.dtype, device=self.device)
         mask = torch.empty((flat.numel(), nd_max), dtype=torch.uint8, device=self.device)
         with torch.cuda.device(self.device):
             _cabi.check(_cabi.lib().flmr_corpus_gather(

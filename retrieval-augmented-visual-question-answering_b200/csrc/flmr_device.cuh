@@ -226,6 +226,22 @@ __device__ __forceinline__ void wgmma_m64n96k16(float (&d)[48], uint64_t a_desc,
       : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
+// D (+)= A[smem] * B[smem]^T, m64n96k16, fp16 in / fp32 accumulate; operands, layout and fragment of the bf16 form.
+__device__ __forceinline__ void wgmma_m64n96k16_f16(float (&d)[48], uint64_t a_desc, uint64_t b_desc,
+                                                    uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47"
+      "}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+      : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16), FLMR_F8(24), FLMR_F8(32), FLMR_F8(40)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
 // D (+)= A[smem] * B[smem]^T, m64n96k32, e4m3 in / fp32 accumulate; d[48] per thread, the same fragment as
 // m64n96k16.  fp8 operands are K-major only and take no transpose immediates.
 __device__ __forceinline__ void wgmma_m64n96k32_e4m3(float (&d)[48], uint64_t a_desc, uint64_t b_desc,
@@ -250,6 +266,21 @@ __device__ __forceinline__ void wgmma_m64n48k16(float (&d)[24], uint64_t a_desc,
       "{\n\t.reg .pred p;\n\t"
       "setp.ne.b32 p, %26, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23"
+      "}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+      : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// D (+)= A[smem] * B[smem]^T, m64n48k16, fp16 in / fp32 accumulate; operands, layout and fragment of the bf16 form.
+__device__ __forceinline__ void wgmma_m64n48k16_f16(float (&d)[24], uint64_t a_desc, uint64_t b_desc,
+                                                    uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
       "{"
       "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
       "%16,%17,%18,%19,%20,%21,%22,%23"

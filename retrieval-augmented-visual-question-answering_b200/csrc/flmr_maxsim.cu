@@ -8,6 +8,7 @@
 // cudaGetDriverEntryPoint, so the library loads (and its symbols can be checked) without a GPU.
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -213,9 +214,10 @@ int gm_grow(GrowableMatrix* g, int device, size_t bytes) {
   return FLMR_OK;
 }
 
-// bf16 [rows, 128] row-major matrix, box = 64 columns (128 B, one swizzle span) x box_rows rows; fp8: an e4m3
+// bf16 (or fp16) [rows, 128] row-major matrix, box = 64 columns (128 B, one swizzle span) x box_rows rows; e4m3: a
 // [rows, 128] matrix (as bytes), box = 128 columns (128 B) x box_rows rows.
-int encode_rows_map(CUtensorMap* map, const void* base, uint64_t rows, uint32_t box_rows, bool fp8 = false) {
+int encode_rows_map(CUtensorMap* map, const void* base, uint64_t rows, uint32_t box_rows, Elem elem = Elem::kBF16) {
+  const bool fp8 = elem == Elem::kE4M3;
   EncodeTiledFn enc = nullptr;
   int rc = get_encode_fn(&enc);
   if (rc) return rc;
@@ -223,7 +225,11 @@ int encode_rows_map(CUtensorMap* map, const void* base, uint64_t rows, uint32_t 
   const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(kDim) * (fp8 ? 1 : 2)};
   const cuuint32_t box[2] = {fp8 ? 128u : 64u, box_rows};
   const cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = enc(map, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+  CUresult r = enc(map,
+                   fp8                   ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                   : elem == Elem::kF16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                         : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                   2,
                    const_cast<void*>(base), gdim, gstride,
                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -349,12 +355,19 @@ __global__ void flmr_round_e4m3_kernel(const uint4* __restrict__ src, uint4* __r
 
 // Independent plain-SIMT MaxSim (test infrastructure): one block per (passage, query), one thread
 // per query token (looping if nq > blockDim), fp32 FMA over bf16 inputs, fixed-order block sum.
-// kFp8: the corpus matrix is e4m3 (the queries come already rounded to e4m3, flmr_round_e4m3_kernel).  A deleted
-// passage (bit set in `dead`, which may be null) scores -inf.
-template <bool kFp8>
+// kE4M3: the corpus matrix is e4m3 (the queries come already rounded to e4m3 as bf16, flmr_round_e4m3_kernel).
+// kF16: corpus and queries are fp16.  A deleted passage (bit set in `dead`, which may be null) scores -inf.
+template <Elem kE>
+__device__ __forceinline__ float simt_query_elem(const void* q, int64_t i) {
+  if constexpr (kE == Elem::kF16)
+    return __half2float(static_cast<const __half*>(q)[i]);
+  else
+    return __bfloat162float(static_cast<const __nv_bfloat16*>(q)[i]);
+}
+template <Elem kE>
 __global__ void flmr_simt_maxsim_kernel(const void* __restrict__ d_any, const int64_t* poff,
                                         const int32_t* doclen, const uint32_t* __restrict__ dead,
-                                        const __nv_bfloat16* __restrict__ q,
+                                        const void* __restrict__ q,
                                         int nq, float init, float* __restrict__ out,
                                         int64_t n_passages) {
   __shared__ float drow[kDim];
@@ -371,14 +384,16 @@ __global__ void flmr_simt_maxsim_kernel(const void* __restrict__ d_any, const in
   for (int i0 = 0; i0 < nq; i0 += blockDim.x) {
     const int i = i0 + threadIdx.x;
     float m = init;
-    const __nv_bfloat16* qi = q + (static_cast<int64_t>(b) * nq + (i < nq ? i : 0)) * kDim;
+    const int64_t qi = (static_cast<int64_t>(b) * nq + (i < nq ? i : 0)) * kDim;
     for (int j = 0; j < len; ++j) {
       __syncthreads();
       if (threadIdx.x < kDim) {
         const int64_t e = d0 + j * kDim + threadIdx.x;
-        if constexpr (kFp8) {
+        if constexpr (kE == Elem::kE4M3) {
           const __half_raw h = __nv_cvt_fp8_to_halfraw(static_cast<const __nv_fp8_storage_t*>(d_any)[e], __NV_E4M3);
           drow[threadIdx.x] = __half2float(__half(h));
+        } else if constexpr (kE == Elem::kF16) {
+          drow[threadIdx.x] = __half2float(static_cast<const __half*>(d_any)[e]);
         } else {
           drow[threadIdx.x] = __bfloat162float(static_cast<const __nv_bfloat16*>(d_any)[e]);
         }
@@ -386,7 +401,7 @@ __global__ void flmr_simt_maxsim_kernel(const void* __restrict__ d_any, const in
       __syncthreads();
       float acc = 0.f;
 #pragma unroll 16
-      for (int c = 0; c < kDim; ++c) acc = fmaf(__bfloat162float(qi[c]), drow[c], acc);
+      for (int c = 0; c < kDim; ++c) acc = fmaf(simt_query_elem<kE>(q, qi + c), drow[c], acc);
       m = fmaxf(m, acc);
     }
     if (i < nq) total += m;
@@ -404,8 +419,10 @@ __global__ void flmr_simt_maxsim_kernel(const void* __restrict__ d_any, const in
 // idx = the nbits-wide field of dim i in the token's packed residual bytes, bit-reversed (the
 // reference packs each bucket index LSB-first into big-endian bytes: residual.py:188-204 binarize,
 // :51-73 reversed_bit_map, :77-93 lookup table; decode loop decompress_residuals.cpp:27-78), then the
-// row is L2-normalised (index_storage.py:173) and stored as bf16.  HBM-bound byte work: one warp per
-// token, lane = 4 dims, centroid rows come from L2, bucket weights from shared memory.
+// row is L2-normalised (index_storage.py:173) and stored as bf16 (kF16: fp16, the reference's own decode type,
+// residual.py:273), rounded once from fp32.  HBM-bound byte work: one warp per token, lane = 4 dims, centroid rows
+// come from L2, bucket weights from shared memory.
+template <bool kF16>
 __global__ void flmr_plaid_decode_kernel(const int32_t* __restrict__ codes,
                                          const uint8_t* __restrict__ residuals,
                                          const float* __restrict__ centroids,
@@ -448,11 +465,18 @@ __global__ void flmr_plaid_decode_kernel(const int32_t* __restrict__ codes,
 #pragma unroll
       for (int dd = 0; dd < 4; ++dd) v[dd] *= inv;
     }
-    __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]);
-    __nv_bfloat162 hi = __floats2bfloat162_rn(v[2], v[3]);
     uint2 w;
-    w.x = *reinterpret_cast<uint32_t*>(&lo);
-    w.y = *reinterpret_cast<uint32_t*>(&hi);
+    if constexpr (kF16) {
+      __half2 lo = __floats2half2_rn(v[0], v[1]);
+      __half2 hi = __floats2half2_rn(v[2], v[3]);
+      w.x = *reinterpret_cast<uint32_t*>(&lo);
+      w.y = *reinterpret_cast<uint32_t*>(&hi);
+    } else {
+      __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]);
+      __nv_bfloat162 hi = __floats2bfloat162_rn(v[2], v[3]);
+      w.x = *reinterpret_cast<uint32_t*>(&lo);
+      w.y = *reinterpret_cast<uint32_t*>(&hi);
+    }
     out[t * 32 + lane] = w;
   }
 }
@@ -694,13 +718,15 @@ struct flmr_corpus {
   int64_t n_tiles = 0;
   bool adopted = false;
   int64_t hbm_bytes = 0;
-  __nv_bfloat16* d_tokens = nullptr;   // [n_rows, 128] padded layout (e4m3 corpus: device alias of h_master)
-  GrowableMatrix vm_tokens;            // backs d_tokens of a library-owned bf16 corpus
+  __nv_bfloat16* d_tokens = nullptr;   // [n_rows, 128] padded layout (e4m3 corpus: device alias of h_master; fp16
+                                       // corpus: the fp16 rows, which every kernel but the scan only moves)
+  GrowableMatrix vm_tokens;            // backs d_tokens of a library-owned bf16 (or fp16) corpus
   // FLMR_CORPUS_FP8: the scan reads an e4m3 copy in HBM; the exact bf16 rows stay in pinned, mapped host memory
   bool fp8 = false;
   void* h_master = nullptr;            // bf16 [n_rows, 128] padded layout, pinned + mapped (e4m3 corpus only)
   uint8_t* d_fp8 = nullptr;            // e4m3 [n_rows, 128] padded layout (e4m3 corpus only), backed by vm_fp8
   GrowableMatrix vm_fp8;
+  bool f16 = false;                    // FLMR_CORPUS_FP16: d_tokens holds fp16 rows, and queries arrive as fp16
   int64_t* d_poff = nullptr;           // [n_passages + 1] stored-row offsets
   int32_t* d_doclen = nullptr;         // [n_passages] real lengths
   std::vector<int64_t> h_poff;         // host copies of the two above (an append extends them)
@@ -1018,6 +1044,11 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     FLMR_CUDA(cudaLaunchKernelEx(&cfg, flmr_scan_kernel<2, true>, c->tmap_half, p));
+  } else if (c->f16) {   // variants without an fp16 kernel are refused by run_search
+    if (split)
+      flmr_scan_split_f16_kernel<<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    else
+      flmr_scan_f16_kernel<<<c->n_ctas, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
   } else if (split) {
     if (c->fp8)
       flmr_scan_split_kernel<true><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
@@ -1100,6 +1131,8 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
                 code == kDevTimeoutProducer ? "TMA producer" : code == kDevTimeoutMma ? "MMA issuer" : "epilogue");
   if (c->fp8 && g_scan_variant == 4)
     return fail(FLMR_ERR_UNSUPPORTED, "the CTA-pair scan (variant 4) has no e4m3 kernel");
+  if (c->f16 && (g_scan_variant == 3 || g_scan_variant == 4))
+    return fail(FLMR_ERR_UNSUPPORTED, "scan variant %d has no fp16 kernel", g_scan_variant);
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
 
@@ -1235,13 +1268,14 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
     if ((rc = dev_upload(&c->d_tile_end_mask, end_mask, &c->hbm_bytes))) return bail(rc);
     if ((rc = dev_upload(&c->d_tile_first_pid, first_pid, &c->hbm_bytes))) return bail(rc);
   }
-  if ((rc = c->fp8 ? encode_rows_map(&c->tmap_d, c->d_fp8, static_cast<uint64_t>(n_rows), kTileN, true)
-                    : encode_rows_map(&c->tmap_d, c->d_tokens, static_cast<uint64_t>(n_rows), kTileN)))
+  if ((rc = c->fp8 ? encode_rows_map(&c->tmap_d, c->d_fp8, static_cast<uint64_t>(n_rows), kTileN, Elem::kE4M3)
+                    : encode_rows_map(&c->tmap_d, c->d_tokens, static_cast<uint64_t>(n_rows), kTileN,
+                                      c->f16 ? Elem::kF16 : Elem::kBF16)))
     return bail(rc);
   // CTA-pair passes: their own partition + half-tile tensor map.  The product never plans pair passes (see
   // run_search); these few KB per corpus are built so flmr_debug_set_scan_variant(4) can hold the cluster kernel
   // against the single-CTA kernels on any bf16 corpus.
-  if (!c->fp8 && n_ctas >= 2 && n_passages >= n_ctas / 2) {
+  if (!c->fp8 && !c->f16 && n_ctas >= 2 && n_passages >= n_ctas / 2) {
     std::vector<int32_t> row_begin, first_pid;
     std::vector<int64_t> tile_base;
     std::vector<uint32_t> end_mask;
@@ -1258,7 +1292,16 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
                                           ScanSmem::kBytes);
     if (e3 != cudaSuccess) return bail(fail(FLMR_ERR_CUDA, "pair kernel attribute: %s", cudaGetErrorString(e3)));
   }
-  {  // per-device function attribute, set here (idempotent) rather than at launch time
+  if (c->f16) {  // per-device function attributes of the two fp16 kernels
+    cudaError_t e1 = cudaFuncSetAttribute(flmr_scan_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          ScanSmem::kBytes);
+    if (e1 == cudaSuccess)
+      e1 = cudaFuncSetAttribute(flmr_scan_split_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                ScanSmem::kBytes);
+    if (e1 != cudaSuccess)
+      return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
+                       ScanSmem::kBytes, cudaGetErrorString(e1)));
+  } else {  // per-device function attribute, set here (idempotent) rather than at launch time
     cudaError_t e1 = c->fp8 ? cudaFuncSetAttribute(flmr_scan_kernel<2, false, true>,
                                                    cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes)
                             : cudaFuncSetAttribute(flmr_scan_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1393,6 +1436,8 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
     return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null tokens/doclens");
   if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_ADOPT))
     return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP8 keeps its own copies of the tokens and cannot adopt them");
+  if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_FP16))
+    return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP16 and FLMR_CORPUS_FP8 exclude each other");
   std::vector<int64_t> soff(n_passages + 1), poff(n_passages + 1);
   soff[0] = poff[0] = 0;
   bool aligned = true;
@@ -1437,6 +1482,7 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
   c->n_rows = n_rows;
   c->pid_base = pid_base;
   c->fp8 = (flags & FLMR_CORPUS_FP8) != 0;
+  c->f16 = (flags & FLMR_CORPUS_FP16) != 0;
   int rc = FLMR_OK;
   auto bail = [&](int code) {
     flmr_corpus_destroy(c);
@@ -1484,8 +1530,11 @@ int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, 
                                   int64_t pid_base, unsigned flags, flmr_corpus_builder_t** out) {
   if (!out) return fail(FLMR_ERR_INVALID_ARG, "out is null");
   *out = nullptr;
-  if (flags & ~FLMR_CORPUS_FP8)
-    return fail(FLMR_ERR_INVALID_ARG, "builder flags 0x%x: only FLMR_CORPUS_FP8 applies to a streamed load", flags);
+  if (flags & ~(FLMR_CORPUS_FP8 | FLMR_CORPUS_FP16))
+    return fail(FLMR_ERR_INVALID_ARG, "builder flags 0x%x: only FLMR_CORPUS_FP8 or FLMR_CORPUS_FP16 applies to a "
+                "streamed load", flags);
+  if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_FP16))
+    return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP16 and FLMR_CORPUS_FP8 exclude each other");
   if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
   if (n_passages <= 0 || !h_doclens) return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null doclens");
   flmr_corpus_builder* b = new (std::nothrow) flmr_corpus_builder();
@@ -1529,6 +1578,7 @@ int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, 
   c->n_rows = n_rows;
   c->pid_base = pid_base;
   c->fp8 = (flags & FLMR_CORPUS_FP8) != 0;
+  c->f16 = (flags & FLMR_CORPUS_FP16) != 0;
   if (int rc = alloc_token_matrix(c)) return bail(rc);
   // an e4m3 corpus always goes through the scatter kernel, which writes the master and the e4m3 copy
   const bool scatter = !b->aligned || c->fp8;
@@ -1687,7 +1737,7 @@ int flmr_corpus_info(const flmr_corpus_t* c, flmr_corpus_info_t* out) {
 
 int flmr_corpus_storage(const flmr_corpus_t* c, int* storage, int64_t* host_bytes) {
   if (!c) return fail(FLMR_ERR_INVALID_ARG, "null argument");
-  if (storage) *storage = c->fp8 ? 1 : 0;
+  if (storage) *storage = c->fp8 ? 1 : c->f16 ? 2 : 0;
   if (host_bytes) *host_bytes = c->fp8 ? c->n_rows * kDim * 2 : 0;
   return FLMR_OK;
 }
@@ -1969,9 +2019,12 @@ int flmr_topk_merge(const float* d_in_scores, const int64_t* d_in_pids, int n_li
   return FLMR_OK;
 }
 
-int flmr_plaid_decode(const int32_t* d_codes, const uint8_t* d_residuals, int64_t n_tokens,
-                      const float* d_centroids, int64_t n_centroids, const float* d_bucket_weights,
-                      int nbits, int dim, int normalize, void* d_out_bf16, int device, void* stream) {
+extern "C++" {
+namespace {
+template <bool kF16>
+int plaid_decode(const int32_t* d_codes, const uint8_t* d_residuals, int64_t n_tokens, const float* d_centroids,
+                 int64_t n_centroids, const float* d_bucket_weights, int nbits, int dim, int normalize,
+                 void* d_out_bf16, int device, void* stream) {
   if (!d_codes || !d_residuals || !d_centroids || !d_bucket_weights || !d_out_bf16)
     return fail(FLMR_ERR_INVALID_ARG, "null pointer");
   if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
@@ -1995,9 +2048,9 @@ int flmr_plaid_decode(const int32_t* d_codes, const uint8_t* d_residuals, int64_
   FLMR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
   const int blocks = static_cast<int>(std::min<int64_t>(want, static_cast<int64_t>(sms) * 16));
   if (e == cudaSuccess) {
-    flmr_plaid_decode_kernel<<<blocks, threads, 0, st>>>(d_codes, d_residuals, d_centroids,
-                                                       d_bucket_weights, nbits, normalize, n_tokens,
-                                                       n_centroids, static_cast<uint2*>(d_out_bf16), d_bad);
+    flmr_plaid_decode_kernel<kF16><<<blocks, threads, 0, st>>>(d_codes, d_residuals, d_centroids,
+                                                             d_bucket_weights, nbits, normalize, n_tokens,
+                                                             n_centroids, static_cast<uint2*>(d_out_bf16), d_bad);
     ++g_launches;
     e = cudaGetLastError();
   }
@@ -2006,6 +2059,22 @@ int flmr_plaid_decode(const int32_t* d_codes, const uint8_t* d_residuals, int64_
   if (e != cudaSuccess) return fail(FLMR_ERR_CUDA, "plaid decode failed: %s", cudaGetErrorString(e));
   if (bad) return fail(FLMR_ERR_INVALID_ARG, "a centroid code is outside [0, %lld)", (long long)n_centroids);
   return FLMR_OK;
+}
+}  // namespace
+}  // extern "C++"
+
+int flmr_plaid_decode(const int32_t* d_codes, const uint8_t* d_residuals, int64_t n_tokens,
+                      const float* d_centroids, int64_t n_centroids, const float* d_bucket_weights,
+                      int nbits, int dim, int normalize, void* d_out_bf16, int device, void* stream) {
+  return plaid_decode<false>(d_codes, d_residuals, n_tokens, d_centroids, n_centroids, d_bucket_weights, nbits, dim,
+                             normalize, d_out_bf16, device, stream);
+}
+
+int flmr_plaid_decode_fp16(const int32_t* d_codes, const uint8_t* d_residuals, int64_t n_tokens,
+                           const float* d_centroids, int64_t n_centroids, const float* d_bucket_weights,
+                           int nbits, int dim, int normalize, void* d_out_fp16, int device, void* stream) {
+  return plaid_decode<true>(d_codes, d_residuals, n_tokens, d_centroids, n_centroids, d_bucket_weights, nbits, dim,
+                            normalize, d_out_fp16, device, stream);
 }
 
 int flmr_topk_select(const float* d_scores, int n_queries, int64_t n, int k, int64_t pid_base,
@@ -2291,9 +2360,8 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const float init = (flags & FLMR_FLAG_RELU) ? 0.f : -INFINITY;
   if (!c->fp8) {
-    flmr_simt_maxsim_kernel<false><<<grid, threads, 0, st>>>(c->d_tokens, c->d_poff, c->d_doclen, c->d_dead,
-                                                             static_cast<const __nv_bfloat16*>(d_q), nq, init,
-                                                             d_out_scores, c->n_passages);
+    (c->f16 ? flmr_simt_maxsim_kernel<Elem::kF16> : flmr_simt_maxsim_kernel<Elem::kBF16>)<<<grid, threads, 0, st>>>(
+        c->d_tokens, c->d_poff, c->d_doclen, c->d_dead, d_q, nq, init, d_out_scores, c->n_passages);
     FLMR_CUDA(cudaGetLastError());
     ++g_launches;
     return FLMR_OK;
@@ -2306,7 +2374,7 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
   FLMR_CUDA(cudaMallocFromPoolAsync(reinterpret_cast<void**>(&q8), static_cast<size_t>(n_chunks) * 16, pool, st));
   flmr_round_e4m3_kernel<<<static_cast<unsigned>((n_chunks + 255) / 256), 256, 0, st>>>(
       static_cast<const uint4*>(d_q), reinterpret_cast<uint4*>(q8), n_chunks);
-  flmr_simt_maxsim_kernel<true><<<grid, threads, 0, st>>>(c->d_fp8, c->d_poff, c->d_doclen, c->d_dead, q8, nq, init,
+  flmr_simt_maxsim_kernel<Elem::kE4M3><<<grid, threads, 0, st>>>(c->d_fp8, c->d_poff, c->d_doclen, c->d_dead, q8, nq, init,
                                                           d_out_scores, c->n_passages);
   const cudaError_t e = cudaGetLastError();
   cudaFreeAsync(q8, st);

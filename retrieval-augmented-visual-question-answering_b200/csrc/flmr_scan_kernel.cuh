@@ -62,9 +62,12 @@ constexpr int kDStages = 4;
 constexpr int kDTileBytes = kTileN * kDim * 2;   // 24 KiB: [2 k-blocks][96 rows][64 bf16]; the D stage stride
 constexpr int kDKBlockBytes = kTileN * 128;      // 12 KiB; also a whole e4m3 tile: [1 k-block][96 rows][128 e4m3]
 constexpr int kQKBlockBytes = kMtMax * kTileM * 128;   // one 64-dim half of the resident bf16 queries (all of e4m3)
-// bytes one D tile brings into its stage: two 128-B k-blocks of bf16, or one of e4m3
-template <bool kFp8>
-__host__ __device__ constexpr int d_tile_bytes() { return kFp8 ? kDKBlockBytes : kDTileBytes; }
+// Element type of a corpus' tokens and staged queries.  bf16 and fp16 share everything but the MMA instruction (two
+// bytes per element, two 128-B k-blocks per row); e4m3 has one byte per element, one k-block per row.
+enum class Elem : int { kBF16 = 0, kF16 = 1, kE4M3 = 2 };
+// bytes one D tile brings into its stage: two 128-B k-blocks of a 16-bit type, or one of e4m3
+template <Elem kE>
+__host__ __device__ constexpr int d_tile_bytes() { return kE == Elem::kE4M3 ? kDKBlockBytes : kDTileBytes; }
 constexpr int kRedWarps = 1;
 
 static_assert(kTileN == 96, "the wgmma shape and accumulator fragment are written for 96-token tiles");
@@ -296,19 +299,19 @@ __device__ __forceinline__ int fold_accumulator(const float (&acc)[4 * kCb], uin
   return slot;
 }
 
-// acc = (64-row query block at q_block) . (D tile at d_stage)^T over K = 128, one commit group: bf16, 8 x
-// wgmma.m64n96k16 over two 128-byte k-blocks; e4m3 (kFp8), 4 x wgmma.m64n96k32 over one.  Either way a k-step is 32
+// acc = (64-row query block at q_block) . (D tile at d_stage)^T over K = 128, one commit group: bf16 or fp16, 8 x
+// wgmma.m64n96k16 over two 128-byte k-blocks; e4m3, 4 x wgmma.m64n96k32 over one.  Either way a k-step is 32
 // bytes along the row, and the accumulator fragment is the same.
 // A 24-register accumulator takes 48 tokens instead (m64n48, the split loop's tile halves): `d_stage` then points
 // 48 rows (6 KiB, whole swizzle atoms) into the stage for half 1, and the k-steps and their order are unchanged.
-template <bool kFp8, int kAcc>
+template <Elem kE, int kAcc>
 __device__ __forceinline__ void issue_block_mma(float (&acc)[kAcc], uint32_t q_block, uint32_t d_stage) {
   static_assert(kAcc == 4 * kNb || kAcc == 2 * kNb, "a whole 96-token tile or one 48-token half");
   // the query block's descriptors are loop-invariant: hidden from the compiler so that they are rebuilt here (a
   // few integer adds) rather than hoisted out of the tile loop into 16 registers per block
   asm volatile("" : "+r"(q_block));
   wgmma_fence();
-  if constexpr (kFp8) {
+  if constexpr (kE == Elem::kE4M3) {
 #pragma unroll
     for (int k = 0; k < kDim / 32; ++k) {
       const uint64_t a_desc = make_kmajor_sw128_desc(q_block + k * 32u);   // 32 elements along the 128-byte row
@@ -324,8 +327,12 @@ __device__ __forceinline__ void issue_block_mma(float (&acc)[kAcc], uint32_t q_b
       const uint32_t koff = (k & 3) * 32u;   // 16 elements along the 128-byte row
       const uint64_t a_desc = make_kmajor_sw128_desc(q_block + (k >> 2) * kQKBlockBytes + koff);
       const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + (k >> 2) * kDKBlockBytes + koff);
-      if constexpr (kAcc == 4 * kNb)
+      if constexpr (kAcc == 4 * kNb && kE == Elem::kF16)
+        wgmma_m64n96k16_f16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+      else if constexpr (kAcc == 4 * kNb)
         wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+      else if constexpr (kE == Elem::kF16)
+        wgmma_m64n48k16_f16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
       else
         wgmma_m64n48k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
     }
@@ -354,7 +361,7 @@ constexpr bool kScanSkeleton = true;
 constexpr bool kScanSkeleton = false;
 #endif
 
-template <int NB, int kWgs, bool kPair, bool kOverlap, bool kFp8>
+template <int NB, int kWgs, bool kPair, bool kOverlap, Elem kE>
 __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base, ScanBars bars,
                                               int n_tiles, int64_t tile_base, int wg, int wq, int lane) {
   using S = ScanSmem;
@@ -384,11 +391,11 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
       const bool last = u + 1 == NB;
       auto issue_next = [&](float (&acc_next)[4 * kNb]) {
         if (!last) {
-          issue_block_mma<kFp8>(acc_next, q_block(u + 1), d_stage(t));
+          issue_block_mma<kE>(acc_next, q_block(u + 1), d_stage(t));
         } else if (kNext) {
           mbar_wait_inline(bars.d_full((t + 1) % kDStages), ((t + 1) / kDStages) & 1u, p.status, kDevTimeoutMma);
           mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
-          issue_block_mma<kFp8>(acc_next, q_block(0), d_stage(t + 1));
+          issue_block_mma<kE>(acc_next, q_block(0), d_stage(t + 1));
         }
       };
       if (kOverlap && (!last || kNext)) {
@@ -432,7 +439,7 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
   if (n_tiles <= 0) return;
   mbar_wait(bars.d_full(0), 0u, p.status, kDevTimeoutMma);
   mask_next = __ldg(p.tile_end_mask + tile_base);
-  issue_block_mma<kFp8>(acc[0], q_block(0), d_stage(0));
+  issue_block_mma<kE>(acc[0], q_block(0), d_stage(0));
   int t = 0;
   for (; t + 2 < n_tiles; t += 2) {
     tile(t, H0{}, Next{});
@@ -456,7 +463,7 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
 // last tile is peeled.  The fold carries the open passage's maxima and the passage-end slot from half 0 to half 1 in
 // the same thread: a passage's row maxima and chunk sums are the values, in the order, of the whole-tile fold (max is
 // exact, whatever order it is taken in), and the scores bitwise those of flmr_scan_kernel.
-template <int NB, bool kFp8>
+template <int NB, Elem kE>
 __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base,
                                                     ScanBars bars, int n_tiles, int64_t tile_base, int wg, int wq,
                                                     int lane) {
@@ -488,7 +495,7 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
     for (int u = 0; u < NB; ++u) {
       const bool last = u + 1 == NB;
       const int j = wg + u * kWgs;
-      issue_block_mma<kFp8>(acc[1], q_block(u), d_half(t, 1));
+      issue_block_mma<kE>(acc[1], q_block(u), d_half(t, 1));
       wgmma_wait<1>();
       wgmma_fence_operands(acc[0]);
       // the reducer must have consumed the partial sums of tile t-2 before this buffer is reused
@@ -501,12 +508,12 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
         slot = fold_accumulator<kNb / 2, 1>(acc[0], mask & ((1u << kHalfGroups) - 1u), m[u], pend, init,
                                             lane_part_buf, partial_buf, j, wq, lane);
       if (!last) {
-        issue_block_mma<kFp8>(acc[0], q_block(u + 1), d_half(t, 0));
+        issue_block_mma<kE>(acc[0], q_block(u + 1), d_half(t, 0));
         wgmma_wait<1>();
       } else if (kNext) {
         mbar_wait_inline(bars.d_full((t + 1) % kDStages), ((t + 1) / kDStages) & 1u, p.status, kDevTimeoutMma);
         mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
-        issue_block_mma<kFp8>(acc[0], q_block(0), d_half(t + 1, 0));
+        issue_block_mma<kE>(acc[0], q_block(0), d_half(t + 1, 0));
         wgmma_wait<1>();
       } else {
         wgmma_wait<0>();
@@ -530,7 +537,7 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
   if (n_tiles <= 0) return;
   mbar_wait(bars.d_full(0), 0u, p.status, kDevTimeoutMma);
   mask_next = __ldg(p.tile_end_mask + tile_base);
-  issue_block_mma<kFp8>(acc[0], q_block(0), d_half(0, 0));
+  issue_block_mma<kE>(acc[0], q_block(0), d_half(0, 0));
   int t = 0;
   for (; t + 1 < n_tiles; ++t) tile(t, std::true_type{});
   tile(t, std::false_type{});
@@ -546,16 +553,18 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
 // from L2 / HBM once — CTA r loads rows [48 r, 48 r + 48) of the tile and TMA-multicasts them into both CTAs'
 // shared memory — and a D stage is recycled when the consumers of BOTH CTAs have released it (remote arrive).
 //
-// kFp8 = true is the e4m3 corpus (FLMR_CORPUS_FP8): the staged queries and the D tiles hold one 128-byte e4m3
+// kE = Elem::kE4M3 is the e4m3 corpus (FLMR_CORPUS_FP8): the staged queries and the D tiles hold one 128-byte e4m3
 // k-block per row (a D tile is one 96-row TMA box of 12 KiB) and the MMAs are wgmma.m64n96k32 e4m3.  Tiles, masks,
 // the shared-memory layout (each stage and the query area keep their bf16 size, half used), the fold, the reducer and
-// the top-k are those of the bf16 kernel.  There is no CTA-pair fp8 kernel.
+// the top-k are those of the bf16 kernel.  kE = Elem::kF16 (FLMR_CORPUS_FP16) differs from bf16 only in the MMA
+// instruction.  There is no CTA-pair kernel for either.
 //
 // kSplit = true (flmr_scan_split_kernel, three warpgroups) runs scan_split_consumer instead of scan_consumer; the
 // producer, the reducer, the barriers and the shared-memory layout are the same code.
-template <int kWgs, bool kPair, bool kFp8, bool kSplit>
+template <int kWgs, bool kPair, Elem kE, bool kSplit>
 __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, const ScanParams& p) {
-  static_assert(!(kPair && kFp8), "the CTA-pair kernel is bf16 only");
+  static_assert(!(kPair && kE != Elem::kBF16), "the CTA-pair kernel is bf16 only");
+  constexpr bool kFp8 = kE == Elem::kE4M3;
   static_assert(!kSplit || (kWgs == 3 && !kPair), "the split consumer loop is written for three single-CTA warpgroups");
   using S = ScanSmem;
   constexpr int kConsumerWarps = kWgs * 4;
@@ -636,7 +645,7 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
         const uint32_t ph = (t / kDStages) & 1;
         mbar_wait(bars.d_empty(s), ph ^ 1u, p.status, kDevTimeoutProducer);
         if (elect_one_sync()) {
-          mbar_arrive_expect_tx(bars.d_full(s), d_tile_bytes<kFp8>());   // (pair: 12 KB from this CTA's loads + 12 KB from the peer's)
+          mbar_arrive_expect_tx(bars.d_full(s), d_tile_bytes<kE>());   // (pair: 12 KB from this CTA's loads + 12 KB from the peer's)
           const uint32_t dst = smem_base + S::kOffD + s * kDTileBytes;
           const int32_t row = row_begin + t * kTileN;
           if constexpr (kPair) {   // tmap_d has a (kTileN / 2)-row box here
@@ -803,16 +812,16 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
     const int nb = wg < n_blocks ? (n_blocks - wg + kWgs - 1) / kWgs : 0;
     if constexpr (kSplit) {
       if (nb == 1) {
-        scan_split_consumer<1, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+        scan_split_consumer<1, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
       } else if (nb == 2) {
-        scan_split_consumer<2, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+        scan_split_consumer<2, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
       }
     } else if (nb == 1) {
-      scan_consumer<1, kWgs, kPair, kOverlap, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      scan_consumer<1, kWgs, kPair, kOverlap, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     } else if (nb == 2) {
-      scan_consumer<2, kWgs, kPair, kOverlap, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      scan_consumer<2, kWgs, kPair, kOverlap, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     } else if constexpr (kBlocksPerWg >= 3) {
-      if (nb == 3) scan_consumer<3, kWgs, kPair, kOverlap, kFp8>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      if (nb == 3) scan_consumer<3, kWgs, kPair, kOverlap, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     }
   }
 
@@ -823,7 +832,7 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
 template <int kWgs, bool kPair = false, bool kFp8 = false>
 __global__ void __launch_bounds__(scan_threads(kWgs), 1)
 flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<kWgs, kPair, kFp8, false>(tmap_d, p);
+  scan_kernel_body<kWgs, kPair, kFp8 ? Elem::kE4M3 : Elem::kBF16, false>(tmap_d, p);
 }
 
 // Three consumer warpgroups whose loop folds one half of each tile while the MMAs of the other half run
@@ -831,7 +840,20 @@ flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p)
 template <bool kFp8>
 __global__ void __launch_bounds__(scan_threads(3), 1)
 flmr_scan_split_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<3, false, kFp8, true>(tmap_d, p);
+  scan_kernel_body<3, false, kFp8 ? Elem::kE4M3 : Elem::kBF16, true>(tmap_d, p);
+}
+
+// The fp16 corpus (FLMR_CORPUS_FP16): the kernels above with wgmma .f16 in place of .bf16 — the same tiles, stages,
+// fold, reducer and top-k.  Their own names keep the bf16 and e4m3 kernels' symbols (and code) as they were.  There
+// is no CTA-pair fp16 kernel; launch_scan uses the two-warpgroup one below five occupied query blocks, the split one
+// from five up, and a forced variant without an fp16 instantiation is refused.
+__global__ void __launch_bounds__(scan_threads(2), 1)
+flmr_scan_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<2, false, Elem::kF16, false>(tmap_d, p);
+}
+__global__ void __launch_bounds__(scan_threads(3), 1)
+flmr_scan_split_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<3, false, Elem::kF16, true>(tmap_d, p);
 }
 
 }  // namespace flmr

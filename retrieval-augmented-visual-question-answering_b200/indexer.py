@@ -23,13 +23,14 @@ from typing import Callable, Optional, Sequence
 
 import torch
 
-from .index_io import chunk_exists, finalize_chunked_index, save_flat_chunk
+from .index_io import DTYPES, chunk_exists, finalize_chunked_index, save_flat_chunk
 from .infra import resolve_index_path, run_context_open
 
 
 class Indexer:
     def __init__(self, checkpoint=None, config=None, encode_fn: Optional[Callable] = None,
-                 index_root: Optional[str] = None, chunksize: int = 25_000, rank: int = 0, nranks: int = 1):
+                 index_root: Optional[str] = None, chunksize: int = 25_000, rank: int = 0, nranks: int = 1,
+                 storage: str = "bf16"):
         self.checkpoint = checkpoint
         self.config = config
         self.encode_fn = encode_fn
@@ -38,6 +39,11 @@ class Indexer:
         self.chunksize = int(chunksize)
         self.rank, self.nranks = int(rank), int(nranks)
         self.index_path = None
+        # token dtype of the index written: "bf16", or "fp16" (the encoder's own output type, ColBERT.doc's D.half(),
+        # written as an "flmr-flat-f16" index that Searcher loads as an fp16 corpus)
+        if storage not in ("bf16", "fp16"):
+            raise ValueError("Indexer storage must be 'bf16' or 'fp16', got %r" % (storage,))
+        self.dtype = "float16" if storage == "fp16" else "bfloat16"
 
     def get_index(self):
         return self.index_path
@@ -47,7 +53,7 @@ class Indexer:
         assert self.index_path is not None
         deleted = []
         for fn in sorted(os.listdir(self.index_path)):
-            if fn.endswith((".bf16", ".npy", ".json", ".tmp")):
+            if fn.endswith((".bf16", ".f16", ".npy", ".json", ".tmp")):
                 os.remove(os.path.join(self.index_path, fn))
                 deleted.append(fn)
         return deleted
@@ -154,7 +160,7 @@ class Indexer:
         def saver():
             for item in iter(q.get, None):
                 try:
-                    save_flat_chunk(self.index_path, *item)
+                    save_flat_chunk(self.index_path, *item, dtype=self.dtype)
                 except Exception as e:   # surfaced after join
                     errors.append(e)
 
@@ -164,7 +170,7 @@ class Indexer:
             for c in range(num_chunks):
                 if c % self.nranks != self.rank:                       # round-robin chunk ownership
                     continue
-                if resume and chunk_exists(self.index_path, c):
+                if resume and chunk_exists(self.index_path, c, self.dtype):
                     continue
                 p0, p1 = c * chunksize, min(n, (c + 1) * chunksize)
                 embs, doclens = self.encode_fn(list(collection[p0:p1]))
@@ -172,7 +178,7 @@ class Indexer:
                 if len(doclens) != p1 - p0 or int(sum(doclens)) != embs.size(0):
                     raise ValueError("encode_fn returned %d doclens / %d embeddings for %d passages"
                                      % (len(doclens), embs.size(0), p1 - p0))
-                q.put((c, p0, embs.detach().to("cpu", torch.bfloat16), list(doclens)))
+                q.put((c, p0, embs.detach().to("cpu", DTYPES[self.dtype][0]), list(doclens)))
         finally:
             q.put(None)
             th.join()
@@ -180,5 +186,5 @@ class Indexer:
             raise errors[0]
         self._barrier()                                   # every rank's chunks are on disk
         if self.rank == 0:
-            finalize_chunked_index(self.index_path, num_chunks)
+            finalize_chunked_index(self.index_path, num_chunks, DTYPES[self.dtype][2])
         self._barrier()                                   # nobody returns before metadata.json exists

@@ -21,7 +21,7 @@ def _prep_queries(corpus: FlatCorpus, Q: torch.Tensor) -> torch.Tensor:
     Q = Q.detach()
     if not Q.is_cuda or Q.device != corpus.device:
         Q = Q.to(corpus.device, non_blocking=True)   # H2D of the caller's dtype, cast on the device
-    return Q.to(torch.bfloat16).contiguous()
+    return Q.to(corpus.dtype).contiguous()           # the corpus' query type: fp16 on an fp16 corpus, else bf16
 
 
 def _stream(corpus: FlatCorpus) -> C.c_void_p:

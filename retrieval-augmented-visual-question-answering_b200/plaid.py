@@ -30,18 +30,21 @@ def read_plaid_metadata(path: str) -> dict:
 
 def decode_chunk(codes: torch.Tensor, residuals: torch.Tensor, centroids: torch.Tensor,
                  bucket_weights: torch.Tensor, nbits: int, out: torch.Tensor, normalize: bool = True) -> None:
-    """GPU decode of one chunk into ``out`` (bf16 ``[n, 128]`` CUDA, may be a slice of the corpus matrix)."""
+    """GPU decode of one chunk into ``out`` (bf16 or fp16 ``[n, 128]`` CUDA, may be a slice of the corpus matrix):
+    computed in fp32, normalised, rounded once to ``out``'s type."""
     dev = out.device
     codes = codes.to(dev, torch.int32).contiguous()
     residuals = residuals.to(dev, torch.uint8).contiguous()
     n = codes.numel()
-    if residuals.shape != (n, _cabi.DIM * nbits // 8) or out.shape != (n, _cabi.DIM) or out.dtype != torch.bfloat16:
+    if residuals.shape != (n, _cabi.DIM * nbits // 8) or out.shape != (n, _cabi.DIM) or \
+            out.dtype not in (torch.bfloat16, torch.float16):
         raise ValueError("shape mismatch: codes %s residuals %s out %s" % (tuple(codes.shape),
                          tuple(residuals.shape), tuple(out.shape)))
     if not out.is_contiguous():
         raise ValueError("out must be contiguous")
     with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().flmr_plaid_decode(
+        decode = _cabi.lib().flmr_plaid_decode_fp16 if out.dtype == torch.float16 else _cabi.lib().flmr_plaid_decode
+        _cabi.check(decode(
             C.c_void_p(codes.data_ptr()), C.c_void_p(residuals.data_ptr()), n,
             C.c_void_p(centroids.data_ptr()), centroids.size(0), C.c_void_p(bucket_weights.data_ptr()),
             nbits, _cabi.DIM, int(normalize), C.c_void_p(out.data_ptr()), int(dev.index),
@@ -57,10 +60,11 @@ def read_plaid_doclens(path: str, num_chunks: int):
     return out
 
 
-def plaid_to_flat(path: str, device=None, passage_range: Optional[Tuple[int, int]] = None
-                  ) -> Tuple[torch.Tensor, np.ndarray]:
+def plaid_to_flat(path: str, device=None, passage_range: Optional[Tuple[int, int]] = None,
+                  dtype: torch.dtype = torch.bfloat16) -> Tuple[torch.Tensor, np.ndarray]:
     """Decode a PLAID index — all of it, or the passages ``[p0, p1)`` only (one GPU's shard: only the chunks
-    that overlap are read) — into (tokens bf16 ``[n_tokens, 128]`` on the GPU, doclens int32)."""
+    that overlap are read) — into (tokens ``[n_tokens, 128]`` of ``dtype``, bf16 or fp16, on the GPU, doclens
+    int32)."""
     if not torch.cuda.is_available():
         raise RuntimeError("PLAID decode runs on the GPU; there is no CPU fallback")
     device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -84,7 +88,7 @@ def plaid_to_flat(path: str, device=None, passage_range: Optional[Tuple[int, int
             off = np.concatenate([[0], np.cumsum(dl)])
             pieces.append((c, int(off[a]), int(off[b]), dl[a:b], int(off[-1])))
         c0 += len(dl)
-    tokens = torch.empty((sum(p[2] - p[1] for p in pieces), _cabi.DIM), dtype=torch.bfloat16, device=device)
+    tokens = torch.empty((sum(p[2] - p[1] for p in pieces), _cabi.DIM), dtype=dtype, device=device)
     row = 0
     for c, r0, r1, _, n_chunk in pieces:
         codes = torch.load(os.path.join(path, "%d.codes.pt" % c), map_location="cpu")

@@ -232,7 +232,8 @@ class Searcher:
                     raise RuntimeError("shard_across_ranks needs an initialised torch.distributed process group")
                 rank, world = dist.get_rank(group), dist.get_world_size(group)
             load = FlatCorpus.from_index if self.index_kind == "flat" else FlatCorpus.from_plaid
-            extra = {"storage": storage} if storage not in (None, "bf16") else {}
+            # storage None: a flat index keeps its own dtype (fp16 for an "flmr-flat-f16" index), PLAID decodes to bf16
+            extra = {"storage": storage} if storage is not None else {}
             self.corpus = load(self.index, device=device, rank=rank, world_size=world, **extra)
         self.storage = getattr(self.corpus, "storage", None) or storage or "bf16"
         self._last_depth = None
@@ -567,7 +568,9 @@ class Searcher:
         ``Q [B, Nq, d]`` stays on the GPU; the retrieved embeddings are gathered out of the resident corpus
         (no host dictionary, no H2D copy).  Returns a dict with ``doc_scores [B, n_docs]`` (differentiable
         w.r.t. ``Q``), ``retrieved_doc_ids`` (int64 numpy ``[B, n_docs]``, as :441), ``search_scores``, and the
-        gathered ``item_embeddings [B, n_docs, Nd, d]`` / ``item_mask [B, n_docs, Nd, 1]``."""
+        gathered ``item_embeddings [B, n_docs, Nd, d]`` / ``item_mask [B, n_docs, Nd, 1]``.  On an fp16 corpus
+        ``item_embeddings`` are its fp16 rows; the re-score runs the bf16 training kernels, so ``doc_scores`` are
+        those of the rows (and the query) converted to bf16."""
         from .modeling import grouped_maxsim
         if Q.dim() != 3:
             raise ValueError("Q must be [B, Nq, d]")
