@@ -28,10 +28,11 @@
  *       APPROXIMATE; the exact bf16 rows stay in pinned host memory for flmr_corpus_gather.  The first stage of
  *       a two-stage search whose exact second stage re-scores a shortlist (the Python Searcher does both), as
  *       PLAID scores its ndocs/4 survivors exactly (CB/search/index_storage.py:160-177).
- *   FLMR_CORPUS_FP16, flmr_plaid_decode_fp16
+ *   FLMR_CORPUS_FP16, flmr_plaid_decode_fp16, flmr_maxsim_argmax_fp16 / _backward_fp16 (and _grouped_fp16)
  *       an fp16 corpus: the precision the reference keeps and scores its embeddings in (ColBERT.doc returns
  *       D.half(), colbert_score multiplies in D's dtype, CB/modeling/colbert.py:205-206, 284; the residual codec
- *       decodes to fp16, CB/indexing/codecs/residual.py:273), scanned with fp16 MMAs instead of being rounded to bf16.
+ *       decodes to fp16, CB/indexing/codecs/residual.py:273), scanned with fp16 MMAs instead of being rounded to bf16;
+ *       and the training / re-scoring calls on fp16 documents, with the query converted to fp16 as colbert_score does.
  *   flmr_corpus_append / _delete / _deleted
  *       the add / remove of ColBERT's later IndexUpdater (the vendored release has no update path): passages are
  *       appended to a resident shard in place and deleted ones are tombstoned, tested in the scan's reducer.
@@ -98,8 +99,10 @@ extern "C" {
  * INPUT ELEMENT TYPE (one rule for every call below): token rows and query rows arrive in the corpus' element
  * type.  An FLMR_CORPUS_FP16 corpus takes fp16 rows — the tokens of flmr_corpus_create, flmr_corpus_append,
  * flmr_corpus_builder_append(_file) and the d_q of every search call — and flmr_corpus_gather writes fp16 rows
- * from it.  A bf16 corpus and an FLMR_CORPUS_FP8 corpus take (and gather) bf16 rows.  Where a comment below says
- * "bf16" for such an operand, it means this type.
+ * from it.  A bf16 corpus and an FLMR_CORPUS_FP8 corpus take (and gather) bf16 rows.  The training calls
+ * (flmr_maxsim_argmax, flmr_maxsim_backward and their _grouped forms) take no corpus: their name gives the type.
+ * The plain names take bf16 d_q and d_docs, the _fp16 names fp16 ones; outputs are fp32 either way.  Where a comment
+ * below says "bf16" for such an operand, it means this type.
  */
 
 #define FLMR_DIM 128        /* embedding dim of FLMR / ColBERT (CB/infra/config/settings.py:101) */
@@ -375,6 +378,15 @@ int flmr_maxsim_argmax(const void* d_q, int n_queries, int nq, const void* d_doc
 int flmr_maxsim_backward(const void* d_q, int n_queries, int nq, const void* d_docs, int n_docs, int nd,
                          const int32_t* d_argmax, const float* d_grad, float* d_dq, float* d_dd,
                          int device, void* stream);
+/* The same two calls on fp16 d_q and d_docs (the reference's fp16 documents, CB/modeling/colbert.py:205-206, with the
+ * query converted to their type, :284): fp16 MMAs and loads, fp32 accumulation and outputs, the same kernels'
+ * structure, arguments and errors. */
+int flmr_maxsim_argmax_fp16(const void* d_q, int n_queries, int nq, const void* d_docs,
+                            const uint8_t* d_mask, int n_docs, int nd, int32_t* d_argmax, float* d_rowmax,
+                            int device, void* stream);
+int flmr_maxsim_backward_fp16(const void* d_q, int n_queries, int nq, const void* d_docs, int n_docs, int nd,
+                              const int32_t* d_argmax, const float* d_grad, float* d_dq, float* d_dd,
+                              int device, void* stream);
 
 /*
  * The loss head of ColBERT.compute_ib_loss_new (CB/modeling/colbert.py:82-113) on top of flmr_maxsim_argmax's
@@ -403,6 +415,13 @@ int flmr_maxsim_argmax_grouped(const void* d_q, int n_queries, int nq, const voi
 int flmr_maxsim_backward_grouped(const void* d_q, int n_queries, int nq, const void* d_docs,
                                  int docs_per_query, int nd, const int32_t* d_argmax, const float* d_grad,
                                  float* d_dq, float* d_dd, int device, void* stream);
+/* The grouped calls on fp16 d_q and d_docs (see flmr_maxsim_argmax_fp16). */
+int flmr_maxsim_argmax_grouped_fp16(const void* d_q, int n_queries, int nq, const void* d_docs,
+                                    const uint8_t* d_mask, int docs_per_query, int nd, int32_t* d_argmax,
+                                    float* d_rowmax, int device, void* stream);
+int flmr_maxsim_backward_grouped_fp16(const void* d_q, int n_queries, int nq, const void* d_docs,
+                                      int docs_per_query, int nd, const int32_t* d_argmax, const float* d_grad,
+                                      float* d_dq, float* d_dd, int device, void* stream);
 
 /* Test infrastructure: plain SIMT fp32 MaxSim of every passage (same contract as
  * flmr_maxsim_scores, e4m3 semantics on an e4m3 corpus, fp16 operands on an fp16 corpus), independent of the
@@ -420,9 +439,9 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* corpus, const void* d_q, 
  * fp16 forms of variants 2 and 6 only: a search on it under variant 3 or 4 returns FLMR_ERR_UNSUPPORTED. */
 int flmr_debug_set_scan_variant(int variant);
 
-/* Test infrastructure: which kernel flmr_maxsim_argmax(_grouped) runs on the calling thread — 0 = chosen by size
- * (the product behaviour), 1 = the warp-MMA kernel, 2 = the wgmma kernel — so tests can hold either against
- * the other and the oracle at any shape. */
+/* Test infrastructure: which kernel flmr_maxsim_argmax(_grouped)(_fp16) runs on the calling thread — 0 = chosen by
+ * size (the product behaviour), 1 = the warp-MMA kernel, 2 = the wgmma kernel, for bf16 and fp16 operands alike — so
+ * tests can hold either against the other and the oracle at any shape. */
 int flmr_debug_set_argmax_path(int path);
 
 /* Test infrastructure, host-only (no GPU needed): the token-balanced CTA partition + per-tile

@@ -36,8 +36,11 @@ TILE_TOKENS = _header_define("FLMR_TILE_TOKENS")
 UPDATE_SYMBOLS = ("flmr_corpus_append", "flmr_corpus_delete", "flmr_corpus_deleted")
 ALLOWED_SYMBOLS = ("flmr_maxsim_scores_allowed", "flmr_maxsim_topk_allowed", "flmr_maxsim_topk_sharded_allowed")
 FP16_SYMBOLS = ("flmr_plaid_decode_fp16",)
+# the training / re-scoring calls on fp16 operands
+FP16_TRAIN_SYMBOLS = ("flmr_maxsim_argmax_fp16", "flmr_maxsim_backward_fp16", "flmr_maxsim_argmax_grouped_fp16",
+                      "flmr_maxsim_backward_grouped_fp16")
 # symbols an earlier revision's library may lack (tools/scan_ab.py drives one through this binding)
-OPTIONAL_SYMBOLS = UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS
+OPTIONAL_SYMBOLS = UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS + FP16_TRAIN_SYMBOLS
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
@@ -47,7 +50,7 @@ SYMBOLS = [
     "flmr_maxsim_scores", "flmr_maxsim_topk", "flmr_topk_merge", "flmr_topk_select", "flmr_plaid_decode",
     *FP16_SYMBOLS,
     "flmr_maxsim_argmax", "flmr_maxsim_backward", "flmr_corpus_gather",
-    "flmr_maxsim_argmax_grouped", "flmr_maxsim_backward_grouped", "flmr_ib_loss",
+    "flmr_maxsim_argmax_grouped", "flmr_maxsim_backward_grouped", "flmr_ib_loss", *FP16_TRAIN_SYMBOLS,
     "flmr_corpus_builder_create", "flmr_corpus_builder_create_ex", "flmr_corpus_builder_append", "flmr_corpus_builder_append_file",
     "flmr_corpus_builder_finish", "flmr_corpus_builder_destroy",
     "flmr_comm_unique_id", "flmr_comm_create", "flmr_comm_adopt", "flmr_comm_destroy", "flmr_comm_info",
@@ -117,6 +120,11 @@ def lib() -> C.CDLL:
     L.flmr_ib_loss.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp]
     L.flmr_maxsim_argmax_grouped.argtypes = [vp, i32, i32, vp, vp, i32, i32, vp, vp, i32, vp]
     L.flmr_maxsim_backward_grouped.argtypes = [vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, i32, vp]
+    if hasattr(L, "flmr_maxsim_argmax_fp16"):
+        L.flmr_maxsim_argmax_fp16.argtypes = L.flmr_maxsim_argmax.argtypes
+        L.flmr_maxsim_backward_fp16.argtypes = L.flmr_maxsim_backward.argtypes
+        L.flmr_maxsim_argmax_grouped_fp16.argtypes = L.flmr_maxsim_argmax_grouped.argtypes
+        L.flmr_maxsim_backward_grouped_fp16.argtypes = L.flmr_maxsim_backward_grouped.argtypes
     L.flmr_corpus_builder_create.argtypes = [vp, i64, i32, i32, i64, C.POINTER(vp)]
     L.flmr_corpus_builder_create_ex.argtypes = [vp, i64, i32, i32, i64, u32, C.POINTER(vp)]
     L.flmr_corpus_builder_append.argtypes = [vp, vp, i64]

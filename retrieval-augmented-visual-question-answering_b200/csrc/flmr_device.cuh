@@ -8,6 +8,11 @@
 
 namespace flmr {
 
+// Element type of a corpus' tokens and staged queries, and of the training kernels' operands.  bf16 and fp16 share
+// everything but the MMA instruction (two bytes per element, two 128-B k-blocks per row); e4m3 has one byte per
+// element, one k-block per row.
+enum class Elem : int { kBF16 = 0, kF16 = 1, kE4M3 = 2 };
+
 // ---- error codes written to ScanParams::status by the device-side watchdog -------------------
 enum : int {
   kDevOk = 0,
@@ -318,6 +323,39 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc
       "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
       : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16), FLMR_F8(24), FLMR_F8(32), FLMR_F8(40), FLMR_F8(48), FLMR_F8(56)
       : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// D (+)= A[smem] * B[smem]^T, m64n128k16, fp16 in / fp32 accumulate; operands, layout and fragment of the bf16 form.
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t a_desc, uint64_t b_desc,
+                                                     uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{"
+      "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : FLMR_F8(0), FLMR_F8(8), FLMR_F8(16), FLMR_F8(24), FLMR_F8(32), FLMR_F8(40), FLMR_F8(48), FLMR_F8(56)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// ---- warp-level MMA (mma.sync m16n8k16, row.col, fp32 accumulate) ------------------------------------------------
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};\n"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// The same with fp16 operands: fragments, layout and accumulation of the bf16 form.
+__device__ __forceinline__ void mma_f16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};\n"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 __device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }

@@ -2140,7 +2140,7 @@ static int scratch_pool(cudaMemPool_t* out) {
 }
 
 static int argmax_tc(const void* d_q, int n_queries, int nq, const void* d_docs, const uint8_t* d_mask, int n_per,
-                     int stride_b, int nd, int32_t* d_argmax, float* d_rowmax, cudaStream_t st) {
+                     int stride_b, int nd, int32_t* d_argmax, float* d_rowmax, Elem elem, cudaStream_t st) {
   const int64_t n_total = stride_b ? static_cast<int64_t>(n_queries) * n_per : n_per;
   const int nd_c = (nd + kTcTile - 1) / kTcTile * kTcTile;
   if (n_total * nd_c + kTcTile >= (1ll << 31) || static_cast<int64_t>(n_queries) * nq + kTcTile >= (1ll << 31))
@@ -2165,14 +2165,16 @@ static int argmax_tc(const void* d_q, int n_queries, int nq, const void* d_docs,
   ++g_launches;
   CUtensorMap tmap_q, tmap_d;
   int rc;
-  if ((rc = encode_rows_map(&tmap_q, d_q, static_cast<uint64_t>(n_queries) * nq, kTcTile))) return done(rc);
-  if ((rc = encode_rows_map(&tmap_d, dc, static_cast<uint64_t>(n_total) * nd_c, kTcTile))) return done(rc);
-  static std::once_flag attr_once[64];
+  if ((rc = encode_rows_map(&tmap_q, d_q, static_cast<uint64_t>(n_queries) * nq, kTcTile, elem))) return done(rc);
+  if ((rc = encode_rows_map(&tmap_d, dc, static_cast<uint64_t>(n_total) * nd_c, kTcTile, elem))) return done(rc);
+  const bool f16 = elem == Elem::kF16;
+  auto* kernel = f16 ? flmr_argmax_tc_f16_kernel : flmr_argmax_tc_kernel;
+  static std::once_flag attr_once[2][64];
   int dev = 0;
   cudaGetDevice(&dev);
   cudaError_t attr_err = cudaSuccess;
-  std::call_once(attr_once[dev & 63], [&]() {
-    attr_err = cudaFuncSetAttribute(flmr_argmax_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes);
+  std::call_once(attr_once[f16][dev & 63], [&]() {
+    attr_err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes);
   });
   if (attr_err != cudaSuccess)
     return done(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit: %s", cudaGetErrorString(attr_err)));
@@ -2206,17 +2208,20 @@ static int argmax_tc(const void* d_q, int n_queries, int nq, const void* d_docs,
   prm.status = nullptr;
   dim3 grid(static_cast<unsigned>((n_per + dpc - 1) / dpc), static_cast<unsigned>(n_tiles),
             static_cast<unsigned>(n_queries));
-  flmr_argmax_tc_kernel<<<grid, kTcThreads, kTcSmemBytes, st>>>(tmap_q, tmap_d, prm);
+  kernel<<<grid, kTcThreads, kTcSmemBytes, st>>>(tmap_q, tmap_d, prm);
   cudaError_t e = cudaGetLastError();
   ++g_launches;
-  if (e != cudaSuccess) return done(fail(FLMR_ERR_CUDA, "flmr_argmax_tc_kernel launch failed: %s", cudaGetErrorString(e)));
+  if (e != cudaSuccess)
+    return done(fail(FLMR_ERR_CUDA, "%s launch failed: %s", f16 ? "flmr_argmax_tc_f16_kernel" : "flmr_argmax_tc_kernel",
+                     cudaGetErrorString(e)));
   return done(FLMR_OK);
 }
 
 // n_per documents per query; stride_b = 0: all queries meet documents [0, n_per) (all pairs),
-// stride_b = n_per: query b meets documents [b * n_per, (b + 1) * n_per) (block diagonal).
+// stride_b = n_per: query b meets documents [b * n_per, (b + 1) * n_per) (block diagonal).  elem: the element type of
+// both operands (Elem::kBF16 or Elem::kF16), which picks the kernels' bf16 or fp16 instantiations.
 static int argmax_impl(const void* d_q, int n_queries, int nq, const void* d_docs, const uint8_t* d_mask,
-                       int n_per, int stride_b, int nd, int32_t* d_argmax, float* d_rowmax, int device,
+                       int n_per, int stride_b, int nd, int32_t* d_argmax, float* d_rowmax, Elem elem, int device,
                        void* stream) {
   if (!d_q || !d_docs || !d_mask || !d_argmax) return fail(FLMR_ERR_INVALID_ARG, "null pointer");
   if (n_queries < 0 || n_per < 0 || nq <= 0 || nd <= 0)
@@ -2231,32 +2236,44 @@ static int argmax_impl(const void* d_q, int n_queries, int nq, const void* d_doc
   const double pairs = static_cast<double>(n_queries) * n_per * nq * nd;
   const bool tc_ok = n_queries <= 65535 && (nq + kTcTile - 1) / kTcTile <= 65535;
   if (tc_ok && (g_argmax_path == 2 || (g_argmax_path == 0 && nq >= 64 && nd >= 128 && pairs >= 16e6)))
-    return argmax_tc(d_q, n_queries, nq, d_docs, d_mask, n_per, stride_b, nd, d_argmax, d_rowmax,
+    return argmax_tc(d_q, n_queries, nq, d_docs, d_mask, n_per, stride_b, nd, d_argmax, d_rowmax, elem,
                      static_cast<cudaStream_t>(stream));
   dim3 grid(static_cast<unsigned>((nq + kArgTile - 1) / kArgTile), static_cast<unsigned>(n_per),
             static_cast<unsigned>(n_queries));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool f16 = elem == Elem::kF16;
 #ifdef FLMR_DEBUG
   // debug builds: FLMR_ARGMAX_SIMT=1 selects the plain-FMA twin (cross-check / A-B timing)
   const char* simt = getenv("FLMR_ARGMAX_SIMT");
   if (simt && atoi(simt)) {
-    flmr_argmax_kernel<<<grid, kArgThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const __nv_bfloat16*>(d_q), static_cast<const __nv_bfloat16*>(d_docs), d_mask, nq, nd,
-        n_per, stride_b, d_argmax, d_rowmax);
+    if (f16)
+      flmr_argmax_f16_kernel<<<grid, kArgThreads, 0, st>>>(static_cast<const __half*>(d_q),
+                                                           static_cast<const __half*>(d_docs), d_mask, nq, nd, n_per,
+                                                           stride_b, d_argmax, d_rowmax);
+    else
+      flmr_argmax_kernel<<<grid, kArgThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(d_q),
+                                                       static_cast<const __nv_bfloat16*>(d_docs), d_mask, nq, nd,
+                                                       n_per, stride_b, d_argmax, d_rowmax);
     FLMR_CUDA(cudaGetLastError());
     ++g_launches;
     return FLMR_OK;
   }
 #endif
-  flmr_argmax_mma_kernel<<<grid, kMmaThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __nv_bfloat16*>(d_q), static_cast<const __nv_bfloat16*>(d_docs), d_mask, nq, nd,
-      n_per, stride_b, d_argmax, d_rowmax);
+  if (f16)
+    flmr_argmax_mma_f16_kernel<<<grid, kMmaThreads, 0, st>>>(static_cast<const __half*>(d_q),
+                                                             static_cast<const __half*>(d_docs), d_mask, nq, nd,
+                                                             n_per, stride_b, d_argmax, d_rowmax);
+  else
+    flmr_argmax_mma_kernel<<<grid, kMmaThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(d_q),
+                                                         static_cast<const __nv_bfloat16*>(d_docs), d_mask, nq, nd,
+                                                         n_per, stride_b, d_argmax, d_rowmax);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;
 }
 
 static int backward_impl(const void* d_q, int n_queries, int nq, const void* d_docs, int n_per, int stride_b,
-                         int nd, const int32_t* d_argmax, const float* d_grad, float* d_dq, float* d_dd,
+                         int nd, const int32_t* d_argmax, const float* d_grad, float* d_dq, float* d_dd, Elem elem,
                          int device, void* stream) {
   if (n_queries < 0 || n_per < 0 || nq <= 0 || nd <= 0)
     return fail(FLMR_ERR_INVALID_ARG, "bad shape n_queries=%d nq=%d n_docs=%d nd=%d", n_queries, nq, n_per, nd);
@@ -2269,13 +2286,19 @@ static int backward_impl(const void* d_q, int n_queries, int nq, const void* d_d
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int threads = 256;
   const int64_t n_docs_total = stride_b ? static_cast<int64_t>(n_queries) * n_per : n_per;
+  const bool f16 = elem == Elem::kF16;
   if (d_dq && n_queries > 0) {
     const int64_t warps = static_cast<int64_t>(n_queries) * nq;
     if (n_per == 0) {
       FLMR_CUDA(cudaMemsetAsync(d_dq, 0, static_cast<size_t>(warps) * kDim * sizeof(float), st));
     } else {
-      flmr_bwd_dq_kernel<<<static_cast<unsigned>((warps * 32 + threads - 1) / threads), threads, 0, st>>>(
-          static_cast<const __nv_bfloat16*>(d_docs), d_argmax, d_grad, n_queries, nq, n_per, nd, stride_b, d_dq);
+      const unsigned blocks = static_cast<unsigned>((warps * 32 + threads - 1) / threads);
+      if (f16)
+        flmr_bwd_dq_f16_kernel<<<blocks, threads, 0, st>>>(static_cast<const __half*>(d_docs), d_argmax, d_grad,
+                                                           n_queries, nq, n_per, nd, stride_b, d_dq);
+      else
+        flmr_bwd_dq_kernel<<<blocks, threads, 0, st>>>(static_cast<const __nv_bfloat16*>(d_docs), d_argmax, d_grad,
+                                                       n_queries, nq, n_per, nd, stride_b, d_dq);
       FLMR_CUDA(cudaGetLastError());
       ++g_launches;
     }
@@ -2286,8 +2309,13 @@ static int backward_impl(const void* d_q, int n_queries, int nq, const void* d_d
     if (warps > 0) {
       if ((warps * 32 + threads - 1) / threads > 0x7fffffffll)
         return fail(FLMR_ERR_UNSUPPORTED, "backward grid too large (%lld warps)", (long long)warps);
-      flmr_bwd_dd_kernel<<<static_cast<unsigned>((warps * 32 + threads - 1) / threads), threads, 0, st>>>(
-          static_cast<const __nv_bfloat16*>(d_q), d_argmax, d_grad, n_queries, nq, n_per, nd, stride_b, d_dd);
+      const unsigned blocks = static_cast<unsigned>((warps * 32 + threads - 1) / threads);
+      if (f16)
+        flmr_bwd_dd_f16_kernel<<<blocks, threads, 0, st>>>(static_cast<const __half*>(d_q), d_argmax, d_grad,
+                                                           n_queries, nq, n_per, nd, stride_b, d_dd);
+      else
+        flmr_bwd_dd_kernel<<<blocks, threads, 0, st>>>(static_cast<const __nv_bfloat16*>(d_q), d_argmax, d_grad,
+                                                       n_queries, nq, n_per, nd, stride_b, d_dd);
       FLMR_CUDA(cudaGetLastError());
       ++g_launches;
     }
@@ -2298,13 +2326,29 @@ static int backward_impl(const void* d_q, int n_queries, int nq, const void* d_d
 int flmr_maxsim_argmax(const void* d_q, int n_queries, int nq, const void* d_docs,
                        const uint8_t* d_mask, int n_docs, int nd, int32_t* d_argmax, float* d_rowmax,
                        int device, void* stream) {
-  return argmax_impl(d_q, n_queries, nq, d_docs, d_mask, n_docs, 0, nd, d_argmax, d_rowmax, device, stream);
+  return argmax_impl(d_q, n_queries, nq, d_docs, d_mask, n_docs, 0, nd, d_argmax, d_rowmax, Elem::kBF16, device,
+                     stream);
+}
+
+int flmr_maxsim_argmax_fp16(const void* d_q, int n_queries, int nq, const void* d_docs,
+                            const uint8_t* d_mask, int n_docs, int nd, int32_t* d_argmax, float* d_rowmax,
+                            int device, void* stream) {
+  return argmax_impl(d_q, n_queries, nq, d_docs, d_mask, n_docs, 0, nd, d_argmax, d_rowmax, Elem::kF16, device,
+                     stream);
 }
 
 int flmr_maxsim_backward(const void* d_q, int n_queries, int nq, const void* d_docs, int n_docs, int nd,
                          const int32_t* d_argmax, const float* d_grad, float* d_dq, float* d_dd,
                          int device, void* stream) {
-  return backward_impl(d_q, n_queries, nq, d_docs, n_docs, 0, nd, d_argmax, d_grad, d_dq, d_dd, device, stream);
+  return backward_impl(d_q, n_queries, nq, d_docs, n_docs, 0, nd, d_argmax, d_grad, d_dq, d_dd, Elem::kBF16, device,
+                       stream);
+}
+
+int flmr_maxsim_backward_fp16(const void* d_q, int n_queries, int nq, const void* d_docs, int n_docs, int nd,
+                              const int32_t* d_argmax, const float* d_grad, float* d_dq, float* d_dd,
+                              int device, void* stream) {
+  return backward_impl(d_q, n_queries, nq, d_docs, n_docs, 0, nd, d_argmax, d_grad, d_dq, d_dd, Elem::kF16, device,
+                       stream);
 }
 
 int flmr_ib_loss(const float* d_rowmax, int n_queries, int n_docs, int nq, int nway, int label0,
@@ -2336,7 +2380,15 @@ int flmr_maxsim_argmax_grouped(const void* d_q, int n_queries, int nq, const voi
                                float* d_rowmax, int device, void* stream) {
   if (docs_per_query < 1) return fail(FLMR_ERR_INVALID_ARG, "docs_per_query=%d must be >= 1", docs_per_query);
   return argmax_impl(d_q, n_queries, nq, d_docs, d_mask, docs_per_query, docs_per_query, nd, d_argmax, d_rowmax,
-                     device, stream);
+                     Elem::kBF16, device, stream);
+}
+
+int flmr_maxsim_argmax_grouped_fp16(const void* d_q, int n_queries, int nq, const void* d_docs,
+                                    const uint8_t* d_mask, int docs_per_query, int nd, int32_t* d_argmax,
+                                    float* d_rowmax, int device, void* stream) {
+  if (docs_per_query < 1) return fail(FLMR_ERR_INVALID_ARG, "docs_per_query=%d must be >= 1", docs_per_query);
+  return argmax_impl(d_q, n_queries, nq, d_docs, d_mask, docs_per_query, docs_per_query, nd, d_argmax, d_rowmax,
+                     Elem::kF16, device, stream);
 }
 
 int flmr_maxsim_backward_grouped(const void* d_q, int n_queries, int nq, const void* d_docs,
@@ -2344,7 +2396,15 @@ int flmr_maxsim_backward_grouped(const void* d_q, int n_queries, int nq, const v
                                  float* d_dq, float* d_dd, int device, void* stream) {
   if (docs_per_query < 1) return fail(FLMR_ERR_INVALID_ARG, "docs_per_query=%d must be >= 1", docs_per_query);
   return backward_impl(d_q, n_queries, nq, d_docs, docs_per_query, docs_per_query, nd, d_argmax, d_grad, d_dq,
-                       d_dd, device, stream);
+                       d_dd, Elem::kBF16, device, stream);
+}
+
+int flmr_maxsim_backward_grouped_fp16(const void* d_q, int n_queries, int nq, const void* d_docs,
+                                      int docs_per_query, int nd, const int32_t* d_argmax, const float* d_grad,
+                                      float* d_dq, float* d_dd, int device, void* stream) {
+  if (docs_per_query < 1) return fail(FLMR_ERR_INVALID_ARG, "docs_per_query=%d must be >= 1", docs_per_query);
+  return backward_impl(d_q, n_queries, nq, d_docs, docs_per_query, docs_per_query, nd, d_argmax, d_grad, d_dq,
+                       d_dd, Elem::kF16, device, stream);
 }
 
 int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n_queries, int nq,

@@ -62,9 +62,6 @@ constexpr int kDStages = 4;
 constexpr int kDTileBytes = kTileN * kDim * 2;   // 24 KiB: [2 k-blocks][96 rows][64 bf16]; the D stage stride
 constexpr int kDKBlockBytes = kTileN * 128;      // 12 KiB; also a whole e4m3 tile: [1 k-block][96 rows][128 e4m3]
 constexpr int kQKBlockBytes = kMtMax * kTileM * 128;   // one 64-dim half of the resident bf16 queries (all of e4m3)
-// Element type of a corpus' tokens and staged queries.  bf16 and fp16 share everything but the MMA instruction (two
-// bytes per element, two 128-B k-blocks per row); e4m3 has one byte per element, one k-block per row.
-enum class Elem : int { kBF16 = 0, kF16 = 1, kE4M3 = 2 };
 // bytes one D tile brings into its stage: two 128-B k-blocks of a 16-bit type, or one of e4m3
 template <Elem kE>
 __host__ __device__ constexpr int d_tile_bytes() { return kE == Elem::kE4M3 ? kDKBlockBytes : kDTileBytes; }

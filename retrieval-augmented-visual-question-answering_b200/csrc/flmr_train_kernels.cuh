@@ -9,17 +9,36 @@
 // Shapes are training-sized (tens of documents, hundreds of tokens): a register-tiled SIMT fp32
 // contraction over bf16 operands is within a few percent of what these sizes allow, so the kernels
 // stay simple; the corpus-sized forward is the wgmma scan kernel.
+//
+// Every kernel has an fp16 twin under its own name (flmr_*_f16_kernel) for fp16 documents, the precision the
+// reference's ColBERT.doc returns on the GPU (colbert.py:205-206): the same body (a template on the element kind),
+// fp16 loads and fp16 MMAs, fp32 outputs.  The bf16 kernels keep their symbols and code.
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <cstdint>
+
+#include "flmr_device.cuh"
 
 namespace flmr {
 
 constexpr int kArgTile = 64;        // query rows and document tokens per shared-memory tile
 constexpr int kArgThreads = 256;    // 16 x 16 threads, 4 x 4 outputs each
 constexpr int kArgStride = 132;     // bf16 per staged row: 264 B = 66 words -> conflict-free column reads
+
+// Storage type of a training operand of element kind kE (bf16 or fp16).
+template <Elem kE>
+struct TrainElem {
+  using T = __nv_bfloat16;
+};
+template <>
+struct TrainElem<Elem::kF16> {
+  using T = __half;
+};
+template <Elem kE>
+using train_t = typename TrainElem<kE>::T;
 
 __device__ __forceinline__ void bf16x4_to_float(uint2 v, float* f) {
   const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162*>(&v.x);
@@ -31,6 +50,24 @@ __device__ __forceinline__ void bf16x4_to_float(uint2 v, float* f) {
   f[3] = fb.y;
 }
 
+__device__ __forceinline__ void f16x4_to_float(uint2 v, float* f) {
+  const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+  const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+  f[0] = fa.x;
+  f[1] = fa.y;
+  f[2] = fb.x;
+  f[3] = fb.y;
+}
+
+// Four consecutive elements of kind kE, widened (exactly) to fp32.
+template <Elem kE>
+__device__ __forceinline__ void x4_to_float(uint2 v, float* f) {
+  if constexpr (kE == Elem::kF16)
+    f16x4_to_float(v, f);
+  else
+    bf16x4_to_float(v, f);
+}
+
 // arg[b, p, i] = argmax_{j : mask[p, j]} <Q[b, i, :], D[p, j, :]>   (lowest j on ties; -1 if p has no
 // unmasked token); rowmax[b, p, i] = that maximum (optional: summed over i it is the MaxSim score, which
 // makes this kernel the whole forward of a training-sized batch).  grid = (ceil(Nq / 64), n, B), block = 256.
@@ -38,17 +75,18 @@ __device__ __forceinline__ void bf16x4_to_float(uint2 v, float* f) {
 // (every query against the same n documents), stride_b = n the block-diagonal one (query b against ITS n
 // documents: the aligned `score(Q.repeat_interleave(n), D)` of colbert.py:71 / rag_model_blip.py:433 /
 // FLMR_executor.py:828 without scoring the off-diagonal pairs).
-__global__ void __launch_bounds__(kArgThreads)
-flmr_argmax_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ d,
-                   const uint8_t* __restrict__ mask, int nq, int nd, int n, int stride_b,
-                   int32_t* __restrict__ arg, float* __restrict__ rowmax) {
-  __shared__ __align__(16) __nv_bfloat16 qs[kArgTile * kArgStride];
-  __shared__ __align__(16) __nv_bfloat16 ds[kArgTile * kArgStride];
+template <Elem kE>
+__device__ __forceinline__ void argmax_simt_body(const train_t<kE>* __restrict__ q, const train_t<kE>* __restrict__ d,
+                                                 const uint8_t* __restrict__ mask, int nq, int nd, int n,
+                                                 int stride_b, int32_t* __restrict__ arg, float* __restrict__ rowmax) {
+  using T = train_t<kE>;
+  __shared__ __align__(16) T qs[kArgTile * kArgStride];
+  __shared__ __align__(16) T ds[kArgTile * kArgStride];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int i0 = blockIdx.x * kArgTile, p = blockIdx.y, b = blockIdx.z;
   const int64_t pg = static_cast<int64_t>(b) * stride_b + p;   // document row (stride_b = 0: all pairs)
-  const __nv_bfloat16* qb = q + (static_cast<int64_t>(b) * nq + i0) * 128;
-  const __nv_bfloat16* db = d + pg * nd * 128;
+  const T* qb = q + (static_cast<int64_t>(b) * nq + i0) * 128;
+  const T* db = d + pg * nd * 128;
   const uint8_t* mp = mask + pg * nd;
 
   // stage the query tile once (rows past Nq read as zero; their results are never stored)
@@ -84,10 +122,10 @@ flmr_argmax_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __r
       float qf[4][4], df[4][4];
 #pragma unroll
       for (int r = 0; r < 4; ++r)
-        bf16x4_to_float(*reinterpret_cast<const uint2*>(qs + (ty * 4 + r) * kArgStride + k), qf[r]);
+        x4_to_float<kE>(*reinterpret_cast<const uint2*>(qs + (ty * 4 + r) * kArgStride + k), qf[r]);
 #pragma unroll
       for (int c = 0; c < 4; ++c)
-        bf16x4_to_float(*reinterpret_cast<const uint2*>(ds + (tx + 16 * c) * kArgStride + k), df[c]);
+        x4_to_float<kE>(*reinterpret_cast<const uint2*>(ds + (tx + 16 * c) * kArgStride + k), df[c]);
 #pragma unroll
       for (int r = 0; r < 4; ++r)
 #pragma unroll
@@ -130,7 +168,20 @@ flmr_argmax_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __r
   }
 }
 
-// ---- the same contract on the warp-level tensor-core path (mma.sync m16n8k16, bf16 -> fp32) -------------
+__global__ void __launch_bounds__(kArgThreads)
+flmr_argmax_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ d,
+                   const uint8_t* __restrict__ mask, int nq, int nd, int n, int stride_b,
+                   int32_t* __restrict__ arg, float* __restrict__ rowmax) {
+  argmax_simt_body<Elem::kBF16>(q, d, mask, nq, nd, n, stride_b, arg, rowmax);
+}
+__global__ void __launch_bounds__(kArgThreads)
+flmr_argmax_f16_kernel(const __half* __restrict__ q, const __half* __restrict__ d,
+                       const uint8_t* __restrict__ mask, int nq, int nd, int n, int stride_b,
+                       int32_t* __restrict__ arg, float* __restrict__ rowmax) {
+  argmax_simt_body<Elem::kF16>(q, d, mask, nq, nd, n, stride_b, arg, rowmax);
+}
+
+// ---- the same contract on the warp-level tensor-core path (mma.sync m16n8k16, bf16 or fp16 -> fp32) -----------
 // Training shapes are far too small to amortise the machinery of the scan kernel (mbarrier ring, TMA
 // descriptors, a persistent grid), but the legacy warp MMA is still several times the SIMT FMA rate.
 // CTA = 4 warps x 16 query rows; the query tile's A fragments are loaded once (ldmatrix) and stay in
@@ -145,25 +196,27 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* smem_p
                : "r"(addr));
 }
 
-__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-               "{%0, %1, %2, %3};\n"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+template <Elem kE>
+__device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  if constexpr (kE == Elem::kF16)
+    mma_f16_16816(c, a, b0, b1);
+  else
+    mma_bf16_16816(c, a, b0, b1);
 }
 
-__global__ void __launch_bounds__(kMmaThreads)
-flmr_argmax_mma_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ d,
-                       const uint8_t* __restrict__ mask, int nq, int nd, int n, int stride_b,
-                       int32_t* __restrict__ arg, float* __restrict__ rowmax) {
-  __shared__ __align__(16) __nv_bfloat16 qs[kArgTile * kMmaStride];
-  __shared__ __align__(16) __nv_bfloat16 ds[kArgTile * kMmaStride];
+template <Elem kE>
+__device__ __forceinline__ void argmax_mma_body(const train_t<kE>* __restrict__ q, const train_t<kE>* __restrict__ d,
+                                                const uint8_t* __restrict__ mask, int nq, int nd, int n,
+                                                int stride_b, int32_t* __restrict__ arg, float* __restrict__ rowmax) {
+  using T = train_t<kE>;
+  __shared__ __align__(16) T qs[kArgTile * kMmaStride];
+  __shared__ __align__(16) T ds[kArgTile * kMmaStride];
   __shared__ uint8_t ms[kArgTile];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int i0 = blockIdx.x * kArgTile, p = blockIdx.y, b = blockIdx.z;
   const int64_t pg = static_cast<int64_t>(b) * stride_b + p;   // document row (stride_b = 0: all pairs)
-  const __nv_bfloat16* qb = q + (static_cast<int64_t>(b) * nq + i0) * 128;
-  const __nv_bfloat16* db = d + pg * nd * 128;
+  const T* qb = q + (static_cast<int64_t>(b) * nq + i0) * 128;
+  const T* db = d + pg * nd * 128;
   const uint8_t* mp = mask + pg * nd;
 
   for (int t = tid; t < kArgTile * 16; t += kMmaThreads) {     // 16 uint4 (8 bf16) per row
@@ -205,8 +258,8 @@ flmr_argmax_mma_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16*
         const int tok = np * 16 + (lane & 7) + ((lane >> 4) & 1) * 8;
         const int kc = ks * 16 + ((lane >> 3) & 1) * 8;
         ldmatrix_x4(bf, ds + tok * kMmaStride + kc);
-        mma_bf16_16816(acc[2 * np], a[ks], bf[0], bf[1]);
-        mma_bf16_16816(acc[2 * np + 1], a[ks], bf[2], bf[3]);
+        mma_16816<kE>(acc[2 * np], a[ks], bf[0], bf[1]);
+        mma_16816<kE>(acc[2 * np + 1], a[ks], bf[2], bf[3]);
       }
     }
 #pragma unroll
@@ -247,10 +300,24 @@ flmr_argmax_mma_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16*
   }
 }
 
+__global__ void __launch_bounds__(kMmaThreads)
+flmr_argmax_mma_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ d,
+                       const uint8_t* __restrict__ mask, int nq, int nd, int n, int stride_b,
+                       int32_t* __restrict__ arg, float* __restrict__ rowmax) {
+  argmax_mma_body<Elem::kBF16>(q, d, mask, nq, nd, n, stride_b, arg, rowmax);
+}
+__global__ void __launch_bounds__(kMmaThreads)
+flmr_argmax_mma_f16_kernel(const __half* __restrict__ q, const __half* __restrict__ d,
+                           const uint8_t* __restrict__ mask, int nq, int nd, int n, int stride_b,
+                           int32_t* __restrict__ arg, float* __restrict__ rowmax) {
+  argmax_mma_body<Elem::kF16>(q, d, mask, nq, nd, n, stride_b, arg, rowmax);
+}
+
 // dQ[b, i, :] = sum_p g[b, p] * D[p, arg[b, p, i], :].  One warp per (b, i), 4 dims per lane.
-__global__ void flmr_bwd_dq_kernel(const __nv_bfloat16* __restrict__ d, const int32_t* __restrict__ arg,
-                                   const float* __restrict__ g, int B, int nq, int n, int nd,
-                                   int stride_b, float* __restrict__ dq) {
+template <Elem kE>
+__device__ __forceinline__ void bwd_dq_body(const train_t<kE>* __restrict__ d, const int32_t* __restrict__ arg,
+                                            const float* __restrict__ g, int B, int nq, int n, int nd,
+                                            int stride_b, float* __restrict__ dq) {
   const int64_t w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= static_cast<int64_t>(B) * nq) return;
@@ -261,19 +328,32 @@ __global__ void flmr_bwd_dq_kernel(const __nv_bfloat16* __restrict__ d, const in
     const float gp = g[static_cast<int64_t>(b) * n + p];
     if (j < 0) continue;
     float f[4];
-    bf16x4_to_float(*reinterpret_cast<const uint2*>(
+    x4_to_float<kE>(*reinterpret_cast<const uint2*>(
                         d + ((static_cast<int64_t>(b) * stride_b + p) * nd + j) * 128 + lane * 4), f);
 #pragma unroll
     for (int e = 0; e < 4; ++e) acc[e] = fmaf(gp, f[e], acc[e]);
   }
   *reinterpret_cast<float4*>(dq + w * 128 + lane * 4) = make_float4(acc[0], acc[1], acc[2], acc[3]);
 }
+__global__ void flmr_bwd_dq_kernel(const __nv_bfloat16* __restrict__ d, const int32_t* __restrict__ arg,
+                                   const float* __restrict__ g, int B, int nq, int n, int nd,
+                                   int stride_b, float* __restrict__ dq) {
+  bwd_dq_body<Elem::kBF16>(d, arg, g, B, nq, n, nd, stride_b, dq);
+}
+// launch bounds of 256 threads x 8 blocks: the register budget (32) of the bf16 kernel, which fp16 widening needs no
+// more than (without them ptxas takes 40)
+__global__ void __launch_bounds__(256, 8) flmr_bwd_dq_f16_kernel(const __half* __restrict__ d, const int32_t* __restrict__ arg,
+                                       const float* __restrict__ g, int B, int nq, int n, int nd,
+                                       int stride_b, float* __restrict__ dq) {
+  bwd_dq_body<Elem::kF16>(d, arg, g, B, nq, n, nd, stride_b, dq);
+}
 
 // dD[p, arg[b, p, i], :] += g[b, p] * Q[b, i, :].  One warp per (b, p, i); fp32 atomics (the order of
 // the additions, hence the last bits of dD, varies from run to run — as torch's index_add_ on CUDA).
-__global__ void flmr_bwd_dd_kernel(const __nv_bfloat16* __restrict__ q, const int32_t* __restrict__ arg,
-                                   const float* __restrict__ g, int B, int nq, int n, int nd,
-                                   int stride_b, float* __restrict__ dd) {
+template <Elem kE>
+__device__ __forceinline__ void bwd_dd_body(const train_t<kE>* __restrict__ q, const int32_t* __restrict__ arg,
+                                            const float* __restrict__ g, int B, int nq, int n, int nd,
+                                            int stride_b, float* __restrict__ dd) {
   const int64_t w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= static_cast<int64_t>(B) * n * nq) return;
@@ -284,10 +364,20 @@ __global__ void flmr_bwd_dd_kernel(const __nv_bfloat16* __restrict__ q, const in
   const float gp = g[bp];
   if (j < 0 || gp == 0.f) return;
   float f[4];
-  bf16x4_to_float(*reinterpret_cast<const uint2*>(q + (static_cast<int64_t>(b) * nq + i) * 128 + lane * 4), f);
+  x4_to_float<kE>(*reinterpret_cast<const uint2*>(q + (static_cast<int64_t>(b) * nq + i) * 128 + lane * 4), f);
   float* dst = dd + ((static_cast<int64_t>(b) * stride_b + p) * nd + j) * 128 + lane * 4;
 #pragma unroll
   for (int e = 0; e < 4; ++e) atomicAdd(dst + e, gp * f[e]);
+}
+__global__ void flmr_bwd_dd_kernel(const __nv_bfloat16* __restrict__ q, const int32_t* __restrict__ arg,
+                                   const float* __restrict__ g, int B, int nq, int n, int nd,
+                                   int stride_b, float* __restrict__ dd) {
+  bwd_dd_body<Elem::kBF16>(q, arg, g, B, nq, n, nd, stride_b, dd);
+}
+__global__ void flmr_bwd_dd_f16_kernel(const __half* __restrict__ q, const int32_t* __restrict__ arg,
+                                       const float* __restrict__ g, int B, int nq, int n, int nd,
+                                       int stride_b, float* __restrict__ dd) {
+  bwd_dd_body<Elem::kF16>(q, arg, g, B, nq, n, nd, stride_b, dd);
 }
 
 // In-batch-negatives loss head (compute_ib_loss_new, CB/modeling/colbert.py:82-113, after the MaxSim matrix):

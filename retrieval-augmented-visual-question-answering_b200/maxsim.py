@@ -138,11 +138,21 @@ def topk_select(scores: torch.Tensor, k: int, pid_base: int = 0) -> Tuple[torch.
 
 
 def _train_operands(Q: torch.Tensor, D_padded: torch.Tensor):
+    """The operands of the arg-max / backward kernels and their element type.  fp16 documents (what the reference's
+    ColBERT.doc returns on the GPU, colbert.py:205-206) keep their precision: both operands go to the fp16 kernels,
+    the query converted to fp16 as colbert_score converts it to the documents' dtype (:284).  Any other document dtype
+    takes the bf16 kernels, both operands rounded to bf16."""
     if not (Q.is_cuda and D_padded.is_cuda):
         raise RuntimeError("the scoring path is CUDA-only (no CPU fallback)")
     if Q.dim() != 3 or D_padded.dim() != 3 or Q.size(2) != _cabi.DIM or D_padded.size(2) != _cabi.DIM:
         raise ValueError("expected Q [B, Nq, %d] and D [n, Nd, %d]" % (_cabi.DIM, _cabi.DIM))
-    return (Q.detach().to(torch.bfloat16).contiguous(), D_padded.detach().to(torch.bfloat16).contiguous())
+    dtype = torch.float16 if D_padded.dtype == torch.float16 else torch.bfloat16
+    return Q.detach().to(dtype).contiguous(), D_padded.detach().to(dtype).contiguous()
+
+
+def _train_call(name: str, operand: torch.Tensor):
+    """The C entry point ``name`` for the element type of ``operand``: its ``_fp16`` form for fp16 operands."""
+    return getattr(_cabi.lib(), name + "_fp16" if operand.dtype == torch.float16 else name)
 
 
 def ib_loss_head(rowmax: torch.Tensor, nway: int, label0: int = 0):
@@ -177,7 +187,7 @@ def maxsim_argmax_grouped(Q: torch.Tensor, D_padded: torch.Tensor, D_mask: torch
     arg = torch.empty((B, r, nq), dtype=torch.int32, device=Qb.device)
     rowmax = torch.empty((B, r, nq), dtype=torch.float32, device=Qb.device) if return_rowmax else None
     with torch.cuda.device(Qb.device):
-        _cabi.check(_cabi.lib().flmr_maxsim_argmax_grouped(
+        _cabi.check(_train_call("flmr_maxsim_argmax_grouped", Db)(
             C.c_void_p(Qb.data_ptr()), B, nq, C.c_void_p(Db.data_ptr()), C.c_void_p(mask.data_ptr()), r, nd,
             C.c_void_p(arg.data_ptr()), C.c_void_p(rowmax.data_ptr() if return_rowmax else None),
             int(Qb.device.index), C.c_void_p(torch.cuda.current_stream(Qb.device).cuda_stream)))
@@ -198,7 +208,7 @@ def maxsim_backward_grouped(Q: torch.Tensor, D_padded: torch.Tensor, arg: torch.
     dq = torch.empty((B, nq, _cabi.DIM), dtype=torch.float32, device=Qb.device) if need_dq else None
     dd = torch.empty((n, nd, _cabi.DIM), dtype=torch.float32, device=Qb.device) if need_dd else None
     with torch.cuda.device(Qb.device):
-        _cabi.check(_cabi.lib().flmr_maxsim_backward_grouped(
+        _cabi.check(_train_call("flmr_maxsim_backward_grouped", Db)(
             C.c_void_p(Qb.data_ptr()), B, nq, C.c_void_p(Db.data_ptr()), r, nd, C.c_void_p(a.data_ptr()),
             C.c_void_p(g.data_ptr()), C.c_void_p(dq.data_ptr() if need_dq else None),
             C.c_void_p(dd.data_ptr() if need_dd else None), int(Qb.device.index),
@@ -218,7 +228,7 @@ def maxsim_argmax(Q: torch.Tensor, D_padded: torch.Tensor, D_mask: torch.Tensor,
     arg = torch.empty((B, n, nq), dtype=torch.int32, device=Qb.device)
     rowmax = torch.empty((B, n, nq), dtype=torch.float32, device=Qb.device) if return_rowmax else None
     with torch.cuda.device(Qb.device):
-        _cabi.check(_cabi.lib().flmr_maxsim_argmax(
+        _cabi.check(_train_call("flmr_maxsim_argmax", Db)(
             C.c_void_p(Qb.data_ptr()), B, nq, C.c_void_p(Db.data_ptr()), C.c_void_p(mask.data_ptr()), n, nd,
             C.c_void_p(arg.data_ptr()), C.c_void_p(rowmax.data_ptr() if return_rowmax else None),
             int(Qb.device.index), C.c_void_p(torch.cuda.current_stream(Qb.device).cuda_stream)))
@@ -238,7 +248,7 @@ def maxsim_backward(Q: torch.Tensor, D_padded: torch.Tensor, arg: torch.Tensor, 
     dq = torch.empty((B, nq, _cabi.DIM), dtype=torch.float32, device=Qb.device) if need_dq else None
     dd = torch.empty((n, nd, _cabi.DIM), dtype=torch.float32, device=Qb.device) if need_dd else None
     with torch.cuda.device(Qb.device):
-        _cabi.check(_cabi.lib().flmr_maxsim_backward(
+        _cabi.check(_train_call("flmr_maxsim_backward", Db)(
             C.c_void_p(Qb.data_ptr()), B, nq, C.c_void_p(Db.data_ptr()), n, nd, C.c_void_p(a.data_ptr()),
             C.c_void_p(g.data_ptr()), C.c_void_p(dq.data_ptr() if need_dq else None),
             C.c_void_p(dd.data_ptr() if need_dd else None), int(Qb.device.index),

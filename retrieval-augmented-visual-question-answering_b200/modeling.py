@@ -17,8 +17,10 @@ scored by one launch of the wgmma scan kernel; the backward then recomputes the 
 
 Backward: ``flmr_maxsim_backward`` routes the gradient through the winners (``dQ_i += g * D_argmax``
 gathered, ``dD_argmax += g * Q_i`` scattered with fp32 atomics).  Both are CUDA kernels behind the C ABI
-(csrc/flmr_train_kernels.cuh).  Inputs are rounded to bf16 for forward and backward, like the reference's
-fp16 GPU path (colbert.py:205-206).
+(csrc/flmr_train_kernels.cuh).  fp16 documents, what the reference's ColBERT.doc returns on the GPU
+(colbert.py:205-206), are scored in fp16 forward and backward, the query converted to fp16 as colbert_score does
+(:284); documents of any other dtype are rounded to bf16 with the query.  Accumulation is fp32 either way, and the
+gradients come back in the inputs' dtypes.
 """
 from __future__ import annotations
 
@@ -27,7 +29,7 @@ from typing import Optional
 import torch
 
 from .corpus import FlatCorpus
-from .maxsim import (ib_loss_head, maxsim_argmax, maxsim_argmax_grouped, maxsim_backward,
+from .maxsim import (_train_operands, ib_loss_head, maxsim_argmax, maxsim_argmax_grouped, maxsim_backward,
                      maxsim_backward_grouped, maxsim_scores)
 
 
@@ -53,7 +55,9 @@ def _forward_scores(Q: torch.Tensor, D_padded: torch.Tensor, D_mask: torch.Tenso
         raise ValueError("a document has no unmasked token: its MaxSim score is undefined "
                          "(-9999 * Nq on the reference's padded path)")
     packed = D_padded.detach()[mask]
-    corpus = FlatCorpus(packed.to(torch.bfloat16), mask.sum(dim=1).cpu(), device=Q.device, adopt=True)
+    fp16 = D_padded.dtype == torch.float16                  # the arg-max kernels' rule (_train_operands)
+    corpus = FlatCorpus(packed.to(torch.float16 if fp16 else torch.bfloat16), mask.sum(dim=1).cpu(), device=Q.device,
+                        adopt=True, storage="fp16" if fp16 else "bf16")
     try:
         scores = maxsim_scores(corpus, Q.detach())
         torch.cuda.current_stream(Q.device).synchronize()   # corpus buffers die with this scope
@@ -194,10 +198,10 @@ class _FusedIBLoss(torch.autograd.Function):
     def forward(ctx, Q: torch.Tensor, D_padded: torch.Tensor, D_mask: torch.Tensor, nway: int, label0: int):
         n, nd = D_padded.size(0), D_padded.size(1)
         mask = D_mask.reshape(n, nd).bool()
-        Qb, Db = Q.detach().to(torch.bfloat16).contiguous(), D_padded.detach().to(torch.bfloat16).contiguous()
+        Qb, Db = _train_operands(Q, D_padded)
         arg, rowmax = maxsim_argmax(Qb, Db, mask, return_rowmax=True)
         scores, loss_q, dscores = ib_loss_head(rowmax, nway, label0)
-        ctx.save_for_backward(Qb, Db, arg, dscores)       # bf16 operands: no second cast in backward
+        ctx.save_for_backward(Qb, Db, arg, dscores)       # converted operands: no second cast in backward
         ctx.dtypes = (Q.dtype, D_padded.dtype)
         ctx.mark_non_differentiable(scores)
         return loss_q.mean(), scores

@@ -569,8 +569,8 @@ class Searcher:
         (no host dictionary, no H2D copy).  Returns a dict with ``doc_scores [B, n_docs]`` (differentiable
         w.r.t. ``Q``), ``retrieved_doc_ids`` (int64 numpy ``[B, n_docs]``, as :441), ``search_scores``, and the
         gathered ``item_embeddings [B, n_docs, Nd, d]`` / ``item_mask [B, n_docs, Nd, 1]``.  On an fp16 corpus
-        ``item_embeddings`` are its fp16 rows; the re-score runs the bf16 training kernels, so ``doc_scores`` are
-        those of the rows (and the query) converted to bf16."""
+        ``item_embeddings`` are its fp16 rows and the re-score runs the fp16 training kernels on them, with the query
+        converted to fp16 as the search converts it: ``doc_scores`` and ``search_scores`` score the same operands."""
         from .modeling import grouped_maxsim
         if Q.dim() != 3:
             raise ValueError("Q must be [B, Nq, d]")
