@@ -36,6 +36,9 @@
  *   flmr_corpus_append / _delete / _deleted
  *       the add / remove of ColBERT's later IndexUpdater (the vendored release has no update path): passages are
  *       appended to a resident shard in place and deleted ones are tombstoned, tested in the scan's reducer.
+ *   flmr_corpus_compact / _stored
+ *       drops the rows of deleted passages from HBM and from every later scan, keeping every id (a fresh index
+ *       build is the reference's only way to shrink an index, and it renumbers the passages).
  *   flmr_maxsim_scores_allowed / flmr_maxsim_topk_allowed / flmr_maxsim_topk_sharded_allowed
  *       the pids= / qid_to_pids= restriction of later ColBERT Searchers: a per-query allow bitmap tested in the
  *       scan's reducer (the vendored release filters scores with filter_fn, CB/searcher.py:61-132).
@@ -51,14 +54,21 @@
  *     corpus' device, "h_" parameters are HOST pointers;
  *   - compute entry points are asynchronous on the supplied CUDA stream (passed as void* so the
  *     header needs no CUDA include; NULL = default stream);
- *   - a corpus changes only through flmr_corpus_append and flmr_corpus_delete.  Between those calls a handle
- *     may be shared by threads; concurrent searches on one handle must use distinct flmr_workspace handles.
- *     The two mutating calls must not run concurrently with any other call on the handle or on its workspaces;
- *     they wait for the device themselves, so work already enqueued on any stream sees the corpus as it was.
- *   - a DELETED passage keeps its id (ids are never reused) and its rows (they are still scanned); it yields
- *     -inf from flmr_maxsim_scores and flmr_debug_maxsim_scores_simt, never appears in the lists of
- *     flmr_maxsim_topk / flmr_maxsim_topk_sharded (short lists are filled with -1 / -inf), and
- *     flmr_corpus_gather returns an all-masked zero row for it, as for an id outside the shard.
+ *   - a corpus changes only through flmr_corpus_append, flmr_corpus_delete and flmr_corpus_compact.  Between
+ *     those calls a handle may be shared by threads; concurrent searches on one handle must use distinct
+ *     flmr_workspace handles.  The three mutating calls must not run concurrently with any other call on the
+ *     handle or on its workspaces; they wait for the device themselves, so work already enqueued on any stream
+ *     sees the corpus as it was.
+ *   - ID EXTENT and SLOTS: a shard's ids are pid_base .. pid_base + n_passages, and n_passages (the id extent)
+ *     never shrinks.  Every id-indexed argument and output (allow bitmaps and their stride, the score rows of
+ *     flmr_maxsim_scores, deleted lists) is sized by the id extent.  The slots are the passages that still have
+ *     rows: all of them until the first flmr_corpus_compact, afterwards the ones that were live when it ran plus
+ *     those appended since.  The scan, its partition and the token matrices are indexed by slot.
+ *   - a DELETED passage keeps its id (ids are never reused) and, until the next flmr_corpus_compact, its rows
+ *     (they are still scanned); it yields -inf from flmr_maxsim_scores and flmr_debug_maxsim_scores_simt, never
+ *     appears in the lists of flmr_maxsim_topk / flmr_maxsim_topk_sharded (short lists are filled with -1 / -inf),
+ *     and flmr_corpus_gather returns an all-masked zero row for it, as for an id outside the shard.  A
+ *     compacted-away id is a deleted id in every one of these respects.
  */
 #ifndef FLMR_MAXSIM_H_
 #define FLMR_MAXSIM_H_
@@ -115,14 +125,16 @@ typedef struct flmr_workspace flmr_workspace_t; /* per-caller scratch (candidate
 typedef struct flmr_comm flmr_comm_t;           /* this rank's end of the shard exchange   */
 typedef struct flmr_corpus_builder flmr_corpus_builder_t; /* streaming index load          */
 
+/* After flmr_corpus_compact n_passages and pid_base are unchanged (the id extent); n_tokens, n_rows, n_tiles and
+ * hbm_bytes describe the stored corpus (the slots), and n_ctas = min(SMs, slots). */
 typedef struct flmr_corpus_info {
-  int64_t n_passages;     /* passages stored in this shard, deleted ones included             */
-  int64_t n_tokens;       /* real tokens (sum of doclens)                                     */
+  int64_t n_passages;     /* id extent: passages of this shard, deleted and compacted ones included */
+  int64_t n_tokens;       /* real tokens (sum of doclens) of the stored passages              */
   int64_t n_rows;         /* stored rows (tokens incl. group padding)                         */
   int64_t pid_base;       /* global id of passage 0 of this shard                             */
   int32_t dim;            /* = FLMR_DIM                                                       */
   int32_t device;         /* CUDA device ordinal                                              */
-  int32_t n_ctas;         /* persistent CTAs the scan kernel launches (= SMs of the device)   */
+  int32_t n_ctas;         /* persistent CTAs the scan kernel launches (= min(SMs, stored passages)) */
   int32_t adopted;        /* 1 if the token matrix is the caller's buffer (zero-copy)         */
   int64_t n_tiles;        /* passage-token tiles streamed per corpus pass                     */
   int64_t hbm_bytes;      /* bytes of HBM held by the handle (excluding an adopted matrix)    */
@@ -179,11 +191,32 @@ int flmr_corpus_storage(const flmr_corpus_t* corpus, int* storage, int64_t* host
  *                      The first delete allocates the shard's bitmap (1 bit per passage, counted in hbm_bytes).
  * flmr_corpus_deleted  *n_deleted = how many ids are deleted; if h_pids is not NULL it receives them (global,
  *                      ascending), capacity >= *n_deleted entries.
+ * flmr_corpus_compact  removes the rows of every deleted passage from HBM and from every later scan.  No id changes
+ *                      and no result changes: every call on the corpus returns bitwise what it returned before
+ *                      (a passage's score does not depend on where it is stored, and the kept passages keep their
+ *                      order, so ties still go to the lower id); only memory, time and the storage figures of
+ *                      flmr_corpus_info change.  Each run of kept passages moves down by the rows removed before
+ *                      it, in chunks of at most 256 MiB of rows, through a staging buffer of at most 256 MiB where a
+ *                      chunk overlaps its own source: HBM never holds a second matrix.  Every whole piece of
+ *                      physical memory (a matrix is mapped in pieces of at most 1 GiB) behind the new end is
+ *                      unmapped and released; *bytes_released (may be NULL) counts those bytes, *n_removed (may be
+ *                      NULL) the passages removed.  An adopted matrix is never written: its live rows are copied
+ *                      into a library-owned matrix, and the caller's buffer is no longer referenced.  The pinned
+ *                      bf16 master of an FLMR_CORPUS_FP8 corpus is compacted in place and keeps its allocation until
+ *                      the next append reallocates it.  A later append continues the ids from the id extent; a later
+ *                      delete of a compacted-away id does nothing.  With no deleted rows stored the call does
+ *                      nothing; when every stored passage is deleted it returns FLMR_ERR_INVALID_ARG and changes
+ *                      nothing.  Synchronous, like append and delete.
+ * flmr_corpus_stored   *n_stored_passages = the slots (passages with rows); *mapped_device_bytes = physical device
+ *                      memory mapped behind the library-owned token matrices (0 for an adopted one).  Either output
+ *                      may be NULL.
  */
 int flmr_corpus_append(flmr_corpus_t* corpus, const void* tokens, const int32_t* h_doclens, int64_t n_passages,
                        int64_t* first_pid);
 int flmr_corpus_delete(flmr_corpus_t* corpus, const int64_t* h_pids, int64_t n);
 int flmr_corpus_deleted(const flmr_corpus_t* corpus, int64_t* n_deleted, int64_t* h_pids, int64_t capacity);
+int flmr_corpus_compact(flmr_corpus_t* corpus, int64_t* n_removed, int64_t* bytes_released);
+int flmr_corpus_stored(const flmr_corpus_t* corpus, int64_t* n_stored_passages, int64_t* mapped_device_bytes);
 
 /*
  * Streaming construction of a corpus shard — the index LOAD path (replaces IndexLoader / ResidualEmbeddings.load_chunks,
@@ -463,6 +496,14 @@ int flmr_debug_build_partition(const int32_t* h_doclens, int64_t n_passages, int
  * CTA, flags (1 = adds earlier partial scores, 2 = stores partial scores, 4 = final: scores complete, top-k taken,
  * 8 = pair pass), row of the pass's first query in the partial-score buffer. */
 int flmr_debug_plan_passes(int n_queries, int nq, int allow_pair, int32_t* out_plan, int capacity, int* n_passes_out);
+
+/* Test infrastructure, host-only: the row moves flmr_corpus_compact makes on a corpus of these doclens when the LOCAL
+ * passages h_deleted[0..n_deleted) are removed, in execution order.  out_moves (may be NULL to query *n_moves_out)
+ * receives 5 int64 per move: source row, destination row, rows, 1 if the move goes through the staging buffer, chunk.
+ * The moves of one chunk run together: a staged chunk reads all of its source rows before it writes any.
+ * chunk_rows bounds the rows of a chunk (0: the library's bound, 256 MiB of bf16 rows). */
+int flmr_debug_compact_plan(const int32_t* h_doclens, int64_t n_passages, const int64_t* h_deleted, int64_t n_deleted,
+                            int64_t chunk_rows, int64_t* out_moves, int64_t capacity, int64_t* n_moves_out);
 
 /* Kernels launched by this library on the calling thread since the last reset (bench evidence). */
 int64_t flmr_launch_count(int reset);

@@ -36,16 +36,17 @@ TILE_TOKENS = _header_define("FLMR_TILE_TOKENS")
 UPDATE_SYMBOLS = ("flmr_corpus_append", "flmr_corpus_delete", "flmr_corpus_deleted")
 ALLOWED_SYMBOLS = ("flmr_maxsim_scores_allowed", "flmr_maxsim_topk_allowed", "flmr_maxsim_topk_sharded_allowed")
 FP16_SYMBOLS = ("flmr_plaid_decode_fp16",)
+COMPACT_SYMBOLS = ("flmr_corpus_compact", "flmr_corpus_stored", "flmr_debug_compact_plan")
 # the training / re-scoring calls on fp16 operands
 FP16_TRAIN_SYMBOLS = ("flmr_maxsim_argmax_fp16", "flmr_maxsim_backward_fp16", "flmr_maxsim_argmax_grouped_fp16",
                       "flmr_maxsim_backward_grouped_fp16")
 # symbols an earlier revision's library may lack (tools/scan_ab.py drives one through this binding)
-OPTIONAL_SYMBOLS = UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS + FP16_TRAIN_SYMBOLS
+OPTIONAL_SYMBOLS = UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS + FP16_TRAIN_SYMBOLS + COMPACT_SYMBOLS
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
     "flmr_corpus_create", "flmr_corpus_destroy", "flmr_corpus_info", "flmr_corpus_storage",
-    *UPDATE_SYMBOLS,
+    *UPDATE_SYMBOLS, *COMPACT_SYMBOLS,
     "flmr_workspace_create", "flmr_workspace_destroy", "flmr_workspace_status",
     "flmr_maxsim_scores", "flmr_maxsim_topk", "flmr_topk_merge", "flmr_topk_select", "flmr_plaid_decode",
     *FP16_SYMBOLS,
@@ -100,6 +101,10 @@ def lib() -> C.CDLL:
         L.flmr_corpus_append.argtypes = [vp, vp, vp, i64, C.POINTER(i64)]
         L.flmr_corpus_delete.argtypes = [vp, vp, i64]
         L.flmr_corpus_deleted.argtypes = [vp, C.POINTER(i64), vp, i64]
+    if hasattr(L, "flmr_corpus_compact"):
+        L.flmr_corpus_compact.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
+        L.flmr_corpus_stored.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
+        L.flmr_debug_compact_plan.argtypes = [vp, i64, vp, i64, i64, vp, i64, C.POINTER(i64)]
     if hasattr(L, "flmr_maxsim_topk_allowed"):
         L.flmr_maxsim_scores_allowed.argtypes = [vp, vp, vp, i32, i32, u32, vp, i64, vp, vp]
         L.flmr_maxsim_topk_allowed.argtypes = [vp, vp, vp, i32, i32, i32, u32, vp, i64, vp, vp, vp]

@@ -270,8 +270,16 @@ class FlatCorpus:
 
     @property
     def n_live(self) -> int:
-        """Passages a search can return: every stored passage but the deleted ones."""
+        """Passages a search can return: every passage but the deleted ones."""
         return self.n_passages - self.n_deleted
+
+    @property
+    def n_stored(self) -> int:
+        """Passages whose rows are held in HBM and scanned: all ``n_passages`` until ``compact`` removes the deleted
+        ones.  ``n_passages`` is the id extent and never shrinks."""
+        n = C.c_int64(0)
+        _cabi.check(_cabi.lib().flmr_corpus_stored(self.handle, C.byref(n), None))
+        return int(n.value)
 
     def deleted_pids(self) -> np.ndarray:
         """Global ids of the deleted passages, ascending (int64)."""
@@ -331,6 +339,23 @@ class FlatCorpus:
         arr = np.ascontiguousarray(np.asarray(pids, dtype=np.int64).reshape(-1))
         _cabi.check(_cabi.lib().flmr_corpus_delete(self.handle, arr.ctypes.data_as(C.c_void_p), int(arr.size)))
         self._refresh()
+
+    def compact(self) -> dict:
+        """Remove the rows of the deleted passages from HBM and from every later search, keeping every id: every call
+        on the corpus returns bitwise what it returned before, in less memory and time.  Physical memory behind the
+        new end of the token matrix is returned to the device; an adopted token tensor is copied once and released.
+        Waits for the device first, so searches already enqueued see the corpus as it was.  Returns ``{"removed",
+        "rows_before", "rows_after", "bytes_released", "seconds"}``; nothing happens when no stored passage is deleted,
+        and ``FlmrError`` is raised (nothing changes) when every one is."""
+        import time
+        rows_before = int(self.info.n_rows)
+        removed, released = C.c_int64(0), C.c_int64(0)
+        t0 = time.perf_counter()
+        _cabi.check(_cabi.lib().flmr_corpus_compact(self.handle, C.byref(removed), C.byref(released)))
+        seconds = time.perf_counter() - t0
+        self._refresh()
+        return {"removed": int(removed.value), "rows_before": rows_before, "rows_after": int(self.info.n_rows),
+                "bytes_released": int(released.value), "seconds": seconds}
 
     def _refresh(self) -> None:
         info = _cabi.CorpusInfo()

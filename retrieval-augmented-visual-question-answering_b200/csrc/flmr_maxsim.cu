@@ -172,8 +172,14 @@ void gm_free(GrowableMatrix* g) {
   *g = GrowableMatrix();
 }
 
+// Largest physical allocation behind a growable matrix.  A growth is mapped as pieces of at most this size, so that a
+// compaction (flmr_corpus_compact) can release every piece that lies wholly behind the matrix's new end; at most one
+// piece per matrix then stays partly used.
+constexpr size_t kGmPieceBytes = 1ull << 30;
+
 // Back at least `bytes` of g with physical memory on `device` (reserving the range first if g has none).  Only the
-// new tail is mapped: rows already there stay where they are.
+// new tail is mapped, in pieces of at most kGmPieceBytes (the last one rounded up to the granularity): rows already
+// there stay where they are.  On failure the pieces this call mapped are released again.
 int gm_grow(GrowableMatrix* g, int device, size_t bytes) {
   const VmmApi* api = nullptr;
   if (int rc = get_vmm_api(&api)) return rc;
@@ -194,24 +200,58 @@ int gm_grow(GrowableMatrix* g, int device, size_t bytes) {
   const size_t add = (bytes - g->mapped + g->gran - 1) / g->gran * g->gran;
   if (g->mapped + add > g->reserved)
     return fail(FLMR_ERR_OOM, "a token matrix of %zu bytes exceeds the device's %zu bytes", bytes, g->reserved);
-  CUmemGenericAllocationHandle h;
-  FLMR_CU(api->Create(&h, add, &prop, 0));
-  CUresult r = api->Map(g->base + g->mapped, add, 0, h, 0);
-  if (r == CUDA_SUCCESS) {
-    CUmemAccessDesc acc{};
-    acc.location = prop.location;
-    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-    r = api->SetAccess(g->base + g->mapped, add, &acc, 1);
-    if (r != CUDA_SUCCESS) api->Unmap(g->base + g->mapped, add);
+  const size_t piece_max = std::max(g->gran, kGmPieceBytes / g->gran * g->gran);
+  const size_t mapped0 = g->mapped, chunks0 = g->chunks.size();
+  CUmemAccessDesc acc{};
+  acc.location = prop.location;
+  acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+  CUresult r = CUDA_SUCCESS;
+  while (g->mapped < mapped0 + add) {
+    const size_t piece = std::min(piece_max, mapped0 + add - g->mapped);
+    CUmemGenericAllocationHandle h;
+    r = api->Create(&h, piece, &prop, 0);
+    if (r != CUDA_SUCCESS) break;
+    r = api->Map(g->base + g->mapped, piece, 0, h, 0);
+    if (r == CUDA_SUCCESS) {
+      r = api->SetAccess(g->base + g->mapped, piece, &acc, 1);
+      if (r != CUDA_SUCCESS) api->Unmap(g->base + g->mapped, piece);
+    }
+    if (r != CUDA_SUCCESS) {
+      api->Release(h);
+      break;
+    }
+    g->chunks.emplace_back(h, piece);
+    g->mapped += piece;
   }
   if (r != CUDA_SUCCESS) {
-    api->Release(h);
+    while (g->chunks.size() > chunks0) {   // give back what this call mapped: the matrix is as it was
+      const auto ch = g->chunks.back();
+      g->mapped -= ch.second;
+      api->Unmap(g->base + g->mapped, ch.second);
+      api->Release(ch.first);
+      g->chunks.pop_back();
+    }
     return fail(r == CUDA_ERROR_OUT_OF_MEMORY ? FLMR_ERR_OOM : FLMR_ERR_CUDA,
                 "mapping %zu bytes behind the token matrix failed (CUresult %d)", add, (int)r);
   }
-  g->chunks.emplace_back(h, add);
-  g->mapped += add;
   return FLMR_OK;
+}
+
+// Unmap and release every piece of g that lies wholly at or behind byte `bytes`; returns the bytes released.  The
+// rows in front stay mapped where they are, and a later gm_grow maps behind the new end.
+size_t gm_shrink(GrowableMatrix* g, size_t bytes) {
+  const VmmApi* api = nullptr;
+  if (!g->base || get_vmm_api(&api)) return 0;
+  size_t released = 0;
+  while (!g->chunks.empty() && g->mapped - g->chunks.back().second >= bytes) {
+    const auto ch = g->chunks.back();
+    g->mapped -= ch.second;
+    api->Unmap(g->base + g->mapped, ch.second);
+    api->Release(ch.first);
+    g->chunks.pop_back();
+    released += ch.second;
+  }
+  return released;
 }
 
 // bf16 (or fp16) [rows, 128] row-major matrix, box = 64 columns (128 B, one swizzle span) x box_rows rows; e4m3: a
@@ -353,6 +393,81 @@ __global__ void flmr_round_e4m3_kernel(const uint4* __restrict__ src, uint4* __r
   dst[i] = make_uint4(out[0], out[1], out[2], out[3]);
 }
 
+// ---- compacted corpora: rows stored by slot, ids through the slot -> id map -------------------------------------
+// slot_pid[0 .. n_slots) holds the global id of each slot, strictly increasing.  The slot of global id `gid`, or -1
+// if it has none.
+__device__ __forceinline__ int64_t slot_of(const int64_t* __restrict__ slot_pid, int64_t n_slots, int64_t gid) {
+  int64_t lo = 0, hi = n_slots;   // first slot whose id is >= gid
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (__ldg(slot_pid + mid) < gid) lo = mid + 1; else hi = mid;
+  }
+  return lo < n_slots && __ldg(slot_pid + lo) == gid ? lo : -1;
+}
+
+// Compaction row move: destination rows [d0, d0 + rows) of one chunk, each read from the source row its piece gives.
+// The chunk's pieces k0 .. k1 - 1 are sorted by destination (piece k starts at destination row pdst[k] and reads from
+// source row psrc[k] on); their destinations are contiguous.  Row r is written at dst + (r - dst_row0) rows: in place
+// (dst_row0 = 0) when the chunk's destinations overlap none of its sources, else into the staging buffer
+// (dst_row0 = d0).  One thread per 16 bytes, row_vecs of them per row.  src and dst may be the same matrix, so they
+// are not declared __restrict__.
+__global__ void flmr_move_rows_kernel(const uint4* src, uint4* dst, const int64_t* __restrict__ pdst,
+                                      const int64_t* __restrict__ psrc, int64_t k0, int64_t k1, int64_t d0,
+                                      int64_t rows, int64_t dst_row0, int row_vecs) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= rows * row_vecs) return;
+  const int64_t r = d0 + i / row_vecs;
+  const int c = static_cast<int>(i % row_vecs);
+  int64_t lo = k0, hi = k1;   // last piece starting at or before r
+  while (hi - lo > 1) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (__ldg(pdst + mid) <= r) lo = mid; else hi = mid;
+  }
+  const int64_t s = __ldg(psrc + lo) + (r - __ldg(pdst + lo));
+  dst[(r - dst_row0) * row_vecs + c] = src[s * row_vecs + c];
+}
+
+// Id-indexed allow bitmaps (the caller's, `stride` words apart; 0: one shared bitmap) -> the slot-indexed bitmaps the
+// scan of a compacted corpus tests, `words` words apart.  One thread per output word.
+__global__ void flmr_slot_allow_kernel(const uint32_t* __restrict__ allow, int64_t stride,
+                                       const int64_t* __restrict__ slot_pid, int64_t pid_base, int64_t n_slots,
+                                       int64_t words, int64_t n_bitmaps, uint32_t* __restrict__ out) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n_bitmaps * words) return;
+  const int64_t b = i / words, w = i % words;
+  const uint32_t* row = allow + b * stride;
+  uint32_t bits = 0u;
+  for (int j = 0; j < 32; ++j) {
+    const int64_t s = w * 32 + j;
+    if (s >= n_slots) break;
+    const int64_t p = __ldg(slot_pid + s) - pid_base;
+    bits |= ((__ldg(row + (p >> 5)) >> (p & 31)) & 1u) << j;
+  }
+  out[i] = bits;
+}
+
+// Global ids -> the ids the slot-indexed gather reads: pid_base + slot, or pid_base - 1 (outside the shard) for an id
+// without a slot (compacted away, or not in this shard).
+__global__ void flmr_slot_ids_kernel(const int64_t* __restrict__ pids, int64_t n, const int64_t* __restrict__ slot_pid,
+                                     int64_t n_slots, int64_t pid_base, int64_t* __restrict__ out) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t s = slot_of(slot_pid, n_slots, pids[i]);
+  out[i] = pid_base + (s >= 0 ? s : -1);
+}
+
+// Slot-indexed score rows [n_rows, n_slots] -> id-indexed rows [n_rows, n_ids]: an id without a slot scores -inf,
+// as a deleted passage does.  One thread per output score.
+__global__ void flmr_expand_slot_scores_kernel(const float* __restrict__ src, int64_t n_slots,
+                                               const int64_t* __restrict__ slot_pid, int64_t pid_base, int64_t n_ids,
+                                               int64_t n_rows, float* __restrict__ dst) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n_rows * n_ids) return;
+  const int64_t b = i / n_ids, p = i % n_ids;
+  const int64_t s = slot_of(slot_pid, n_slots, pid_base + p);
+  dst[i] = s >= 0 ? src[b * n_slots + s] : -INFINITY;
+}
+
 // Independent plain-SIMT MaxSim (test infrastructure): one block per (passage, query), one thread
 // per query token (looping if nq > blockDim), fp32 FMA over bf16 inputs, fixed-order block sum.
 // kE4M3: the corpus matrix is e4m3 (the queries come already rounded to e4m3 as bf16, flmr_round_e4m3_kernel).
@@ -482,8 +597,8 @@ __global__ void flmr_plaid_decode_kernel(const int32_t* __restrict__ codes,
 }
 
 // Candidate merge: per query, select the k_out best of n candidates by (score desc, pid asc).
-// Candidates come either as packed keys written by the scan kernel (keys != null; pid = pid_base +
-// ~low32) or as (score, pid) arrays laid out [list][query][k_in].  One 1024-thread block per query,
+// Candidates come either as packed keys written by the scan kernel (keys != null; slot = ~low32, pid = pid_base +
+// slot, or slot_pid[slot] on a compacted corpus) or as (score, pid) arrays laid out [list][query][k_in].  One 1024-thread block per query,
 // up to kMergePer candidates per thread in registers, k_out selection rounds.
 constexpr int kMergeThreads = 1024;
 constexpr int kMergePer = 20;
@@ -500,7 +615,7 @@ __device__ __forceinline__ bool cand_better(const Cand& a, const Cand& b) {
 __global__ void __launch_bounds__(kMergeThreads)
 flmr_merge_kernel(const uint64_t* __restrict__ keys, const float* __restrict__ in_scores,
                   const int64_t* __restrict__ in_pids, int n_lists, int n_queries, int k_in,
-                  int k_out, int64_t pid_base, float* __restrict__ out_scores,
+                  int k_out, int64_t pid_base, const int64_t* __restrict__ slot_pid, float* __restrict__ out_scores,
                   int64_t* __restrict__ out_pids, int q_offset) {
   __shared__ uint32_t s_ord[32];
   __shared__ int64_t s_pid[32];
@@ -522,7 +637,8 @@ flmr_merge_kernel(const uint64_t* __restrict__ keys, const float* __restrict__ i
         const uint64_t key = keys[g];
         if (key != 0ull) {
           c[i].ord = static_cast<uint32_t>(key >> 32);
-          c[i].pid = pid_base + (0xFFFFFFFFu - static_cast<uint32_t>(key));
+          const uint32_t slot = 0xFFFFFFFFu - static_cast<uint32_t>(key);
+          c[i].pid = slot_pid ? __ldg(slot_pid + slot) : pid_base + slot;   // slots keep the order of their ids
         }
       } else {
         const int64_t pid = in_pids[g];
@@ -727,16 +843,24 @@ struct flmr_corpus {
   uint8_t* d_fp8 = nullptr;            // e4m3 [n_rows, 128] padded layout (e4m3 corpus only), backed by vm_fp8
   GrowableMatrix vm_fp8;
   bool f16 = false;                    // FLMR_CORPUS_FP16: d_tokens holds fp16 rows, and queries arrive as fp16
-  int64_t* d_poff = nullptr;           // [n_passages + 1] stored-row offsets
-  int32_t* d_doclen = nullptr;         // [n_passages] real lengths
+  // Ids and slots.  n_passages is the id extent: ids pid_base .. pid_base + n_passages, never shrinking.  A slot is a
+  // passage that has rows.  Until the first flmr_corpus_compact every id has the slot of the same index and
+  // h_slot_pid / d_slot_pid stay empty / null; after it, slot s holds global id h_slot_pid[s] (strictly increasing).
+  // Everything the scan reads (offsets, lengths, partition, d_dead) is indexed by slot.
+  std::vector<int64_t> h_slot_pid;
+  int64_t* d_slot_pid = nullptr;
+  int64_t* d_poff = nullptr;           // [slots + 1] stored-row offsets
+  int32_t* d_doclen = nullptr;         // [slots] real lengths
   std::vector<int64_t> h_poff;         // host copies of the two above (an append extends them)
   std::vector<int32_t> h_doclen;
-  // tombstones: bit p & 31 of word p >> 5 set <=> local passage p is deleted; d_dead stays null until the first
-  // delete, so a corpus without deletions runs the scan exactly as before
+  // tombstones: h_dead is indexed by LOCAL ID (bit p & 31 of word p >> 5 set <=> local passage p is deleted, a
+  // compacted-away id included); d_dead by SLOT, for the scan's reducer, the gather and the SIMT kernel.  d_dead stays
+  // null while no slot is deleted (until the first delete, and again right after a compaction), so a corpus without
+  // deletions runs the scan exactly as before
   uint32_t* d_dead = nullptr;
   std::vector<uint32_t> h_dead;
   int64_t n_deleted = 0;
-  int sm_total = 0;                    // SMs of the device (n_ctas = min(sm_total, n_passages))
+  int sm_total = 0;                    // SMs of the device (n_ctas = min(sm_total, slots))
   int32_t* d_cta_row_begin = nullptr;  // [n_ctas + 1]
   int64_t* d_cta_tile_base = nullptr;  // [n_ctas + 1]
   uint32_t* d_tile_end_mask = nullptr; // [n_tiles]
@@ -868,6 +992,27 @@ struct EventPair {
 };
 thread_local std::vector<EventPair> g_scan_events;
 
+int64_t slots(const flmr_corpus* c) {
+  return c->h_slot_pid.empty() ? c->n_passages : static_cast<int64_t>(c->h_slot_pid.size());
+}
+
+// The tombstones by slot (d_dead's words) of a compacted corpus, from its tombstones by id (`dead`, as h_dead).
+std::vector<uint32_t> dead_by_slot(const std::vector<int64_t>& slot_pid, int64_t pid_base,
+                                   const std::vector<uint32_t>& dead, bool* any) {
+  const int64_t ns = static_cast<int64_t>(slot_pid.size());
+  std::vector<uint32_t> out((ns + 31) / 32, 0u);
+  *any = false;
+  for (int64_t s = 0; s < ns; ++s) {
+    const int64_t p = slot_pid[s] - pid_base;
+    if (static_cast<size_t>(p >> 5) < dead.size() && ((dead[p >> 5] >> (p & 31)) & 1u)) {
+      out[s >> 5] |= 1u << (s & 31);
+      *any = true;
+    }
+  }
+  return out;
+}
+
+
 template <typename T>
 int dev_upload(T** dptr, const std::vector<T>& h, int64_t* bytes_acc) {
   const size_t bytes = std::max<size_t>(h.size(), 1) * sizeof(T);
@@ -876,6 +1021,53 @@ int dev_upload(T** dptr, const std::vector<T>& h, int64_t* bytes_acc) {
   if (bytes_acc) *bytes_acc += static_cast<int64_t>(bytes);
   return FLMR_OK;
 }
+
+// The library's own stream-ordered memory pool (one per device) for per-call scratch: it keeps what it has
+// been given (release threshold = max), so after the first call an allocation is a pointer bump in stream order —
+// the default pool hands memory back to the driver at every synchronisation and re-maps it on the next call.
+static int scratch_pool(cudaMemPool_t* out) {
+  static cudaMemPool_t pools[64] = {};
+  static std::mutex mu;
+  int dev = 0;
+  FLMR_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  if (!pools[dev & 63]) {
+    cudaMemPoolProps props{};
+    props.allocType = cudaMemAllocationTypePinned;
+    props.handleTypes = cudaMemHandleTypeNone;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = dev;
+    cudaMemPool_t p = nullptr;
+    FLMR_CUDA(cudaMemPoolCreate(&p, &props));
+    uint64_t keep = ~0ull;
+    FLMR_CUDA(cudaMemPoolSetAttribute(p, cudaMemPoolAttrReleaseThreshold, &keep));
+    pools[dev & 63] = p;
+  }
+  *out = pools[dev & 63];
+  return FLMR_OK;
+}
+
+// Per-call device scratch from the library's pool, handed back in stream order when the call has enqueued its work.
+struct StreamScratch {
+  cudaStream_t st;
+  std::vector<void*> ptrs;
+  explicit StreamScratch(cudaStream_t s) : st(s) {}
+  StreamScratch(const StreamScratch&) = delete;
+  StreamScratch& operator=(const StreamScratch&) = delete;
+  ~StreamScratch() {
+    for (void* q : ptrs) cudaFreeAsync(q, st);
+  }
+  template <typename T>
+  int alloc(T** out, size_t bytes) {
+    cudaMemPool_t pool = nullptr;
+    if (int rc = scratch_pool(&pool)) return rc;
+    void* q = nullptr;
+    FLMR_CUDA(cudaMallocFromPoolAsync(&q, std::max<size_t>(bytes, 16), pool, st));
+    ptrs.push_back(q);
+    *out = static_cast<T*>(q);
+    return FLMR_OK;
+  }
+};
 
 // Token-balanced split of the passages into n_ctas contiguous ranges + per-tile metadata.
 void build_partition(const std::vector<int64_t>& poff, int n_ctas, int tile_n,
@@ -1094,7 +1286,7 @@ int launch_merge_keys(const flmr_corpus* c, flmr_workspace* ws, int n_lists, int
     return fail(FLMR_ERR_UNSUPPORTED, "n_lists*k = %lld exceeds merge capacity %d",
                 (long long)n_lists * k, kMergeThreads * kMergePer);
   flmr_merge_kernel<<<nq, kMergeThreads, 0, st>>>(ws->d_cand_keys, nullptr, nullptr, n_lists, stride, k, k,
-                                                  c->pid_base, d_out_scores, d_out_pids, q0);
+                                                  c->pid_base, c->d_slot_pid, d_out_scores, d_out_pids, q0);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;
@@ -1135,6 +1327,30 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
     return fail(FLMR_ERR_UNSUPPORTED, "scan variant %d has no fp16 kernel", g_scan_variant);
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
+  int rc;
+  // The scan works in slot space: it scans the stored passages and writes score rows of `ns` entries.  On a compacted
+  // corpus the id-indexed allow bitmaps are translated to slots first, and score rows go through stream-ordered
+  // scratch that flmr_expand_slot_scores_kernel spreads over the ids (-inf where an id has no slot).
+  const int64_t ns = slots(c);
+  const bool compacted = c->d_slot_pid != nullptr;
+  StreamScratch scratch(st);
+  float* d_slot_scores = nullptr;   // [min(n_queries, max_queries), ns]
+  if (compacted && allow) {
+    const int64_t words = (ns + 31) / 32, n_bitmaps = allow_stride ? n_queries : 1;
+    uint32_t* slot_allow = nullptr;
+    if ((rc = scratch.alloc(&slot_allow, static_cast<size_t>(n_bitmaps * words) * sizeof(uint32_t)))) return rc;
+    const int64_t n = n_bitmaps * words;
+    flmr_slot_allow_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
+        allow, allow_stride, c->d_slot_pid, c->pid_base, ns, words, n_bitmaps, slot_allow);
+    FLMR_CUDA(cudaGetLastError());
+    ++g_launches;
+    allow = slot_allow;
+    allow_stride = allow_stride ? words : 0;
+  }
+  if (compacted && d_all_scores &&
+      (rc = scratch.alloc(&d_slot_scores,
+                          static_cast<size_t>(std::min(ws->max_queries, n_queries)) * ns * sizeof(float))))
+    return rc;
 
   ScanParams p{};
   p.cta_row_begin = c->d_cta_row_begin;
@@ -1142,8 +1358,8 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   p.tile_end_mask = c->d_tile_end_mask;
   p.tile_first_pid = c->d_tile_first_pid;
   p.init_val = (flags & FLMR_FLAG_RELU) ? 0.f : -INFINITY;
-  p.n_passages = c->n_passages;
-  p.dead = c->d_dead;   // null until the first delete: the reducer then makes no extra load
+  p.n_passages = ns;
+  p.dead = c->d_dead;   // null while no slot is deleted: the reducer then makes no extra load
   if (ws->cand_lists < c->n_ctas) {
     // the corpus grew past the CTA count this workspace was sized for (a corpus of fewer passages than SMs launches
     // one CTA per passage); cudaFree waits for the searches still using the old buffer
@@ -1173,14 +1389,14 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   // within a chunk: every pass's scan, then the merge over the chunk's queries (one launch per kind of pass)
   std::vector<PassPlan> plan;
   std::vector<int> slot;
-  int rc;
   for (int c0 = 0; c0 < n_queries; c0 += ws->max_queries) {
     const int nqc = std::min(ws->max_queries, n_queries - c0);
     const __nv_bfloat16* d_qc = static_cast<const __nv_bfloat16*>(d_q) + static_cast<int64_t>(c0) * nq * kDim;
-    float* d_all_c = d_all_scores ? d_all_scores + static_cast<int64_t>(c0) * c->n_passages : nullptr;
+    float* d_all_c = d_slot_scores ? d_slot_scores
+                                   : d_all_scores ? d_all_scores + static_cast<int64_t>(c0) * c->n_passages : nullptr;
     int group = 1, n_pair_q = 0;
     plan_passes(nqc, nq, allow_pair, &plan, &group, &n_pair_q);
-    if (!d_all_c && nq > kRbMax * 32 && (rc = ensure_acc(ws, static_cast<int64_t>(group) * c->n_passages)))
+    if (!d_all_c && nq > kRbMax * 32 && (rc = ensure_acc(ws, static_cast<int64_t>(group) * ns)))
       return rc;
     p.cand_q_stride = nqc;
     slot.assign(plan.size(), 0);
@@ -1205,8 +1421,8 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
       const PassPlan& pp = plan[pi];
       // partial / final scores of query (group_first + acc_slot + i) live in row i of `acc`
       float* acc = d_all_c
-                       ? d_all_c + static_cast<int64_t>(pp.group_first + pp.acc_slot) * c->n_passages
-                       : (ws->d_acc ? ws->d_acc + static_cast<int64_t>(pp.acc_slot) * c->n_passages : nullptr);
+                       ? d_all_c + static_cast<int64_t>(pp.group_first + pp.acc_slot) * ns
+                       : (ws->d_acc ? ws->d_acc + static_cast<int64_t>(pp.acc_slot) * ns : nullptr);
       p.q_pad = reinterpret_cast<const uint4*>(ws->d_qpad) + static_cast<int64_t>(slot[pi]) * (kMtMax * kTileM * 16);
       p.n_mtiles = pp.n_mtiles;
       p.nq_pass = pp.n_q;
@@ -1218,6 +1434,14 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
       p.allow = allow ? allow + static_cast<int64_t>(c0 + pp.q_first) * allow_stride : nullptr;
       p.allow_stride = allow_stride;
       if ((rc = launch_scan(c, ws, p, (pp.flags & kPassPair) != 0, st))) return rc;
+    }
+    if (d_slot_scores) {
+      const int64_t n = static_cast<int64_t>(nqc) * c->n_passages;
+      flmr_expand_slot_scores_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
+          d_slot_scores, ns, c->d_slot_pid, c->pid_base, c->n_passages, nqc,
+          d_all_scores + static_cast<int64_t>(c0) * c->n_passages);
+      FLMR_CUDA(cudaGetLastError());
+      ++g_launches;
     }
     if (k > 0) {
       float* os = d_topk_scores + static_cast<int64_t>(c0) * k;
@@ -1232,8 +1456,9 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
 
 // Everything a corpus needs besides its token matrix: offsets / lengths, the CTA partition + per-tile metadata,
 // the TMA descriptor, the kernel's shared-memory attribute.  Shared by flmr_corpus_create and the streaming builder.
+// poff / h_doclens describe the stored passages (the slots): all of them until a compaction.
 int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_t* h_doclens, int sm_count) {
-  const int64_t n_passages = c->n_passages;
+  const int64_t n_passages = static_cast<int64_t>(poff.size()) - 1;
   const int64_t n_rows = c->n_rows;
   int rc = FLMR_OK;
   auto bail = [](int code) { return code; };
@@ -1419,6 +1644,101 @@ void free_metadata(flmr_corpus* c) {
   c->n_tiles_pair = 0;
 }
 
+// ---- compaction schedule (pure host logic; exported for tests as flmr_debug_compact_plan) ----------------------
+// The kept passages keep their padded row blocks and their order: each run of kept rows moves down by the rows removed
+// before it, so no destination lies above its source.  The moves are cut into chunks of at most `chunk_rows`
+// destination rows, executed in destination order.  A chunk whose destination rows overlap its own source rows goes
+// through a staging buffer (all of its rows read, then all written); any other chunk is copied directly.  Writing
+// chunk i never touches a source row of a later chunk: those lie at or above chunk i's source rows, which lie at or
+// above its destinations.  The staging buffer therefore never holds more than chunk_rows rows.
+constexpr int64_t kCompactStageBytes = 256ll << 20;
+constexpr int64_t kCompactChunkRows = kCompactStageBytes / (kDim * 2);   // a chunk of bf16 rows fills the stage
+
+struct MovePiece {
+  int64_t src, dst, rows;
+  bool staged;
+  int64_t chunk;
+};
+
+// runs: (first source row, rows) of each run of kept rows, ascending; their destinations are packed from row 0.
+// in_place = false: the destination is another matrix (an adopted one is copied out), so every run moves, directly.
+void plan_compaction(const std::vector<std::pair<int64_t, int64_t>>& runs, int64_t chunk_rows, bool in_place,
+                     std::vector<MovePiece>* out) {
+  out->clear();
+  int64_t d = 0, chunk = 0, chunk_rows_used = 0;
+  size_t chunk_first = 0;
+  auto close_chunk = [&]() {
+    if (chunk_rows_used == 0) return;
+    // the chunk's destinations are [d - used, d); its lowest source row is its first piece's
+    const bool staged = in_place && d > (*out)[chunk_first].src;
+    for (size_t i = chunk_first; i < out->size(); ++i) (*out)[i].staged = staged;
+    ++chunk;
+    chunk_rows_used = 0;
+    chunk_first = out->size();
+  };
+  for (const auto& run : runs) {
+    int64_t src = run.first, n = run.second;
+    if (in_place && src == d) {   // rows already in place (in front of the first removed passage)
+      d += n;
+      continue;
+    }
+    while (n > 0) {
+      const int64_t take = std::min(n, chunk_rows - chunk_rows_used);
+      out->push_back({src, d, take, false, chunk});
+      src += take;
+      d += take;
+      n -= take;
+      chunk_rows_used += take;
+      if (chunk_rows_used == chunk_rows) close_chunk();
+    }
+  }
+  close_chunk();
+}
+
+// Runs of kept rows of a corpus whose passages have padded row offsets poff, keep[s] = the passage stays.
+std::vector<std::pair<int64_t, int64_t>> kept_runs(const std::vector<int64_t>& poff, const std::vector<char>& keep) {
+  std::vector<std::pair<int64_t, int64_t>> runs;
+  const int64_t n = static_cast<int64_t>(keep.size());
+  for (int64_t s = 0; s < n;) {
+    if (!keep[s]) {
+      ++s;
+      continue;
+    }
+    int64_t e = s;
+    while (e < n && keep[e]) ++e;
+    runs.emplace_back(poff[s], poff[e] - poff[s]);
+    s = e;
+  }
+  return runs;
+}
+
+// Execute a compaction schedule on one matrix of `row_vecs` 16-byte vectors per row (16: bf16 / fp16, 8: e4m3):
+// src and dst are the same matrix in place, or (an adopted matrix) two.  Stream-ordered on the legacy stream.
+cudaError_t run_moves(const std::vector<MovePiece>& plan, const int64_t* d_pdst, const int64_t* d_psrc,
+                      const uint4* src, uint4* dst, uint4* stage, int row_vecs) {
+  const int threads = 256;
+  for (size_t k0 = 0; k0 < plan.size();) {
+    size_t k1 = k0;
+    while (k1 < plan.size() && plan[k1].chunk == plan[k0].chunk) ++k1;
+    const int64_t d0 = plan[k0].dst, rows = plan[k1 - 1].dst + plan[k1 - 1].rows - d0;
+    const int64_t n = rows * row_vecs;
+    const unsigned blocks = static_cast<unsigned>((n + threads - 1) / threads);
+    if (plan[k0].staged) {   // every source row of the chunk is read before any of its destinations is written
+      flmr_move_rows_kernel<<<blocks, threads>>>(src, stage, d_pdst, d_psrc, k0, k1, d0, rows, d0, row_vecs);
+      ++g_launches;
+      const cudaError_t e = cudaMemcpyAsync(dst + d0 * row_vecs, stage, static_cast<size_t>(n) * 16,
+                                            cudaMemcpyDeviceToDevice, 0);
+      if (e != cudaSuccess) return e;
+    } else {
+      flmr_move_rows_kernel<<<blocks, threads>>>(src, dst, d_pdst, d_psrc, k0, k1, d0, rows, 0, row_vecs);
+      ++g_launches;
+    }
+    if (const cudaError_t e = cudaGetLastError(); e != cudaSuccess) return e;
+    k0 = k1;
+  }
+  return cudaSuccess;
+}
+
 }  // namespace
 
 // =================================== C ABI =============================================================
@@ -1517,6 +1837,7 @@ int flmr_corpus_destroy(flmr_corpus_t* c) {
   gm_free(&c->vm_fp8);
   free_metadata(c);
   cudaFree(c->d_dead);
+  cudaFree(c->d_slot_pid);
   delete c;
   return FLMR_OK;
 }
@@ -1836,6 +2157,7 @@ int flmr_corpus_append(flmr_corpus_t* c, const void* tokens, const int32_t* h_do
   nc.n_pairs = 0;
   nc.n_tiles_pair = 0;
   nc.d_dead = nullptr;
+  nc.d_slot_pid = nullptr;
   nc.n_passages = new_n;
   nc.n_tokens = c->n_tokens + soff[n_passages];
   nc.n_rows = new_rows;
@@ -1846,18 +2168,31 @@ int flmr_corpus_append(flmr_corpus_t* c, const void* tokens, const int32_t* h_do
   std::vector<int32_t> all_len(c->h_doclen);
   all_len.insert(all_len.end(), h_doclens, h_doclens + n_passages);
   int rc = FLMR_OK;
-  if (!c->h_dead.empty()) {
+  if (c->h_slot_pid.empty()) {
+    if (!c->h_dead.empty()) {
+      nc.h_dead.resize((new_n + 31) / 32, 0u);
+      rc = dev_upload(&nc.d_dead, nc.h_dead, &nc.hbm_bytes);
+    }
+  } else {
+    // compacted: the new passages take the next slots and the next ids
+    for (int64_t p = 0; p < n_passages; ++p) nc.h_slot_pid.push_back(c->pid_base + old_n + p);
     nc.h_dead.resize((new_n + 31) / 32, 0u);
-    rc = dev_upload(&nc.d_dead, nc.h_dead, &nc.hbm_bytes);
+    rc = dev_upload(&nc.d_slot_pid, nc.h_slot_pid, &nc.hbm_bytes);
+    if (!rc && c->d_dead) {
+      bool any = false;
+      rc = dev_upload(&nc.d_dead, dead_by_slot(nc.h_slot_pid, nc.pid_base, nc.h_dead, &any), &nc.hbm_bytes);
+    }
   }
   if (!rc) rc = finish_corpus(&nc, all_poff, all_len.data(), c->sm_total);
   if (rc) {
     free_metadata(&nc);
     cudaFree(nc.d_dead);
+    cudaFree(nc.d_slot_pid);
     return rc;
   }
   free_metadata(c);
   cudaFree(c->d_dead);
+  cudaFree(c->d_slot_pid);
   *c = std::move(nc);
   if (first_pid) *first_pid = c->pid_base + old_n;
   return FLMR_OK;
@@ -1883,14 +2218,20 @@ int flmr_corpus_delete(flmr_corpus_t* c, const int64_t* h_pids, int64_t n) {
   if (added == 0) return FLMR_OK;   // already deleted (or nothing to do): no change, no bitmap allocated
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
+  // a compacted corpus: the device bitmap is indexed by slot (a newly deleted id always has one: a compacted-away id
+  // was deleted already)
+  bool any = false;
+  const std::vector<uint32_t> by_slot =
+      c->h_slot_pid.empty() ? std::vector<uint32_t>() : dead_by_slot(c->h_slot_pid, c->pid_base, dead, &any);
+  const std::vector<uint32_t>& words = c->h_slot_pid.empty() ? dead : by_slot;
   // searches enqueued before this call (any stream) finish with the old bitmap
   FLMR_CUDA(cudaDeviceSynchronize());
-  const size_t bytes = dead.size() * sizeof(uint32_t);
+  const size_t bytes = words.size() * sizeof(uint32_t);
   if (!c->d_dead) {
     FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&c->d_dead), bytes));
     c->hbm_bytes += static_cast<int64_t>(bytes);
   }
-  FLMR_CUDA(cudaMemcpy(c->d_dead, dead.data(), bytes, cudaMemcpyHostToDevice));
+  FLMR_CUDA(cudaMemcpy(c->d_dead, words.data(), bytes, cudaMemcpyHostToDevice));
   c->h_dead.swap(dead);
   c->n_deleted += added;
   return FLMR_OK;
@@ -1907,6 +2248,157 @@ int flmr_corpus_deleted(const flmr_corpus_t* c, int64_t* n_deleted, int64_t* h_p
   for (size_t w = 0; w < c->h_dead.size(); ++w)
     for (uint32_t bits = c->h_dead[w]; bits; bits &= bits - 1)
       h_pids[j++] = c->pid_base + static_cast<int64_t>(w) * 32 + __builtin_ctz(bits);
+  return FLMR_OK;
+}
+
+int flmr_corpus_compact(flmr_corpus_t* c, int64_t* n_removed, int64_t* bytes_released) {
+  if (n_removed) *n_removed = 0;
+  if (bytes_released) *bytes_released = 0;
+  if (!c) return fail(FLMR_ERR_INVALID_ARG, "null corpus");
+  const int64_t ns = slots(c);
+  // --- 1. which slots stay: their ids, offsets and lengths in the compacted corpus ---
+  std::vector<char> keep(ns, 1);
+  int64_t removed = 0;
+  for (int64_t s = 0; s < ns; ++s) {
+    const int64_t p = c->h_slot_pid.empty() ? s : c->h_slot_pid[s] - c->pid_base;
+    if (static_cast<size_t>(p >> 5) < c->h_dead.size() && ((c->h_dead[p >> 5] >> (p & 31)) & 1u)) {
+      keep[s] = 0;
+      ++removed;
+    }
+  }
+  if (removed == 0) return FLMR_OK;   // nothing deleted since the last compaction: the corpus is already compact
+  if (removed == ns)
+    return fail(FLMR_ERR_INVALID_ARG, "every passage of the shard is deleted; a corpus keeps at least one passage");
+  std::vector<int64_t> slot_pid, poff(1, 0);
+  std::vector<int32_t> lens;
+  slot_pid.reserve(ns - removed);
+  lens.reserve(ns - removed);
+  poff.reserve(ns - removed + 1);
+  for (int64_t s = 0; s < ns; ++s) {
+    if (!keep[s]) continue;
+    slot_pid.push_back(c->h_slot_pid.empty() ? c->pid_base + s : c->h_slot_pid[s]);
+    lens.push_back(c->h_doclen[s]);
+    poff.push_back(poff.back() + (c->h_poff[s + 1] - c->h_poff[s]));
+  }
+  int64_t n_tokens = 0;
+  for (int32_t l : lens) n_tokens += l;
+  const int64_t new_rows = poff.back();
+  std::vector<MovePiece> plan;
+  plan_compaction(kept_runs(c->h_poff, keep), kCompactChunkRows, !c->adopted, &plan);
+
+  DeviceGuard guard(c->device);
+  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
+  // searches enqueued before this call (any stream) finish on the corpus as it was
+  FLMR_CUDA(cudaDeviceSynchronize());
+
+  // --- 2. everything that can fail on allocation, before a row moves: the matrix an adopted corpus is copied into,
+  // the schedule on the device, the staging buffer, and the metadata of the compacted corpus ---
+  const size_t row_bytes = c->fp8 ? kDim : kDim * 2;   // of the matrix in HBM
+  flmr_corpus nc = *c;
+  nc.d_poff = nullptr;
+  nc.d_doclen = nullptr;
+  nc.d_cta_row_begin = nullptr;
+  nc.d_cta_tile_base = nullptr;
+  nc.d_tile_end_mask = nullptr;
+  nc.d_tile_first_pid = nullptr;
+  nc.d_pair_row_begin = nullptr;
+  nc.d_pair_tile_base = nullptr;
+  nc.d_pair_end_mask = nullptr;
+  nc.d_pair_first_pid = nullptr;
+  nc.n_pairs = 0;
+  nc.n_tiles_pair = 0;
+  nc.d_dead = nullptr;          // every deleted slot is removed
+  nc.d_slot_pid = nullptr;
+  nc.n_tokens = n_tokens;
+  nc.n_rows = new_rows;
+  nc.hbm_bytes = new_rows * static_cast<int64_t>(row_bytes);
+  GrowableMatrix copy;          // an adopted corpus: the library-owned matrix its live rows go to
+  int64_t *d_pdst = nullptr, *d_psrc = nullptr;
+  uint4* stage = nullptr;
+  auto release = [&](int code) {
+    free_metadata(&nc);
+    cudaFree(nc.d_slot_pid);
+    gm_free(&copy);
+    cudaFree(d_pdst);
+    cudaFree(d_psrc);
+    cudaFree(stage);
+    return code;
+  };
+  int rc = FLMR_OK;
+  if (c->adopted) {
+    if ((rc = gm_grow(&copy, c->device, static_cast<size_t>(new_rows) * row_bytes))) return release(rc);
+    nc.d_tokens = reinterpret_cast<__nv_bfloat16*>(copy.base);
+  }
+  {
+    std::vector<int64_t> pdst(plan.size()), psrc(plan.size());
+    int64_t stage_rows = 0;
+    for (size_t i = 0; i < plan.size(); ++i) {
+      pdst[i] = plan[i].dst;
+      psrc[i] = plan[i].src;
+    }
+    for (size_t k0 = 0; k0 < plan.size();) {
+      size_t k1 = k0;
+      while (k1 < plan.size() && plan[k1].chunk == plan[k0].chunk) ++k1;
+      if (plan[k0].staged) stage_rows = std::max(stage_rows, plan[k1 - 1].dst + plan[k1 - 1].rows - plan[k0].dst);
+      k0 = k1;
+    }
+    if (!plan.empty() && ((rc = dev_upload(&d_pdst, pdst, nullptr)) || (rc = dev_upload(&d_psrc, psrc, nullptr))))
+      return release(rc);
+    if (stage_rows > 0) {
+      const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&stage), static_cast<size_t>(stage_rows) * row_bytes);
+      if (e != cudaSuccess)
+        return release(fail(FLMR_ERR_OOM, "compaction staging buffer (%lld rows): %s", (long long)stage_rows,
+                            cudaGetErrorString(e)));
+    }
+  }
+  nc.h_slot_pid = slot_pid;
+  if ((rc = dev_upload(&nc.d_slot_pid, nc.h_slot_pid, &nc.hbm_bytes))) return release(rc);
+  if ((rc = finish_corpus(&nc, poff, lens.data(), c->sm_total))) return release(rc);
+
+  // --- 3. the rows move: the HBM matrix on the device, the pinned bf16 master of an e4m3 corpus on the host ---
+  cudaError_t e = cudaSuccess;
+  if (!plan.empty()) {
+    if (c->fp8) {
+      e = run_moves(plan, d_pdst, d_psrc, reinterpret_cast<const uint4*>(c->d_fp8), reinterpret_cast<uint4*>(c->d_fp8),
+                    stage, static_cast<int>(kDim / 16));
+      // ordered memmove in place: every destination lies at or below its source, and earlier pieces come first
+      char* m = static_cast<char*>(c->h_master);
+      for (const MovePiece& mp : plan)
+        memmove(m + mp.dst * kDim * 2, m + mp.src * kDim * 2, static_cast<size_t>(mp.rows) * kDim * 2);
+    } else {
+      e = run_moves(plan, d_pdst, d_psrc, reinterpret_cast<const uint4*>(c->d_tokens),
+                    reinterpret_cast<uint4*>(nc.d_tokens), stage, static_cast<int>(kDim * 2 / 16));
+    }
+  }
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) return release(fail(FLMR_ERR_CUDA, "compaction row move failed: %s", cudaGetErrorString(e)));
+  cudaFree(d_pdst);
+  cudaFree(d_psrc);
+  cudaFree(stage);
+
+  // --- 4. physical memory wholly behind the new end goes back to the device; the handle takes the new state ---
+  size_t released = 0;
+  if (c->adopted) {
+    nc.vm_tokens = copy;          // the caller's buffer is no longer referenced
+    nc.adopted = false;
+  } else if (c->fp8) {
+    released = gm_shrink(&nc.vm_fp8, static_cast<size_t>(new_rows) * kDim);
+  } else {
+    released = gm_shrink(&nc.vm_tokens, static_cast<size_t>(new_rows) * kDim * 2);
+  }
+  free_metadata(c);
+  cudaFree(c->d_dead);
+  cudaFree(c->d_slot_pid);
+  *c = std::move(nc);
+  if (n_removed) *n_removed = removed;
+  if (bytes_released) *bytes_released = static_cast<int64_t>(released);
+  return FLMR_OK;
+}
+
+int flmr_corpus_stored(const flmr_corpus_t* c, int64_t* n_stored_passages, int64_t* mapped_device_bytes) {
+  if (!c) return fail(FLMR_ERR_INVALID_ARG, "null corpus");
+  if (n_stored_passages) *n_stored_passages = slots(c);
+  if (mapped_device_bytes) *mapped_device_bytes = static_cast<int64_t>(c->vm_tokens.mapped + c->vm_fp8.mapped);
   return FLMR_OK;
 }
 
@@ -2013,7 +2505,7 @@ int flmr_topk_merge(const float* d_in_scores, const int64_t* d_in_pids, int n_li
   DeviceGuard guard(device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
   flmr_merge_kernel<<<n_queries, kMergeThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      nullptr, d_in_scores, d_in_pids, n_lists, n_queries, k_in, k_out, 0, d_out_scores, d_out_pids, 0);
+      nullptr, d_in_scores, d_in_pids, n_lists, n_queries, k_in, k_out, 0, nullptr, d_out_scores, d_out_pids, 0);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;
@@ -2103,9 +2595,20 @@ int flmr_corpus_gather(const flmr_corpus_t* c, const int64_t* d_pids, int64_t n_
   const int threads = 256;
   const int64_t blocks = (n_pids * nd_max * 32 + threads - 1) / threads;
   if (blocks > 0x7fffffffll) return fail(FLMR_ERR_UNSUPPORTED, "gather of %lld x %d rows is too large", (long long)n_pids, nd_max);
-  flmr_gather_kernel<<<static_cast<unsigned>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  StreamScratch scratch(st);
+  if (c->d_slot_pid) {   // compacted: the gather reads slots, each id's found by binary search in the slot map
+    int64_t* slot_ids = nullptr;
+    if (int rc = scratch.alloc(&slot_ids, static_cast<size_t>(n_pids) * sizeof(int64_t))) return rc;
+    flmr_slot_ids_kernel<<<static_cast<unsigned>((n_pids + threads - 1) / threads), threads, 0, st>>>(
+        d_pids, n_pids, c->d_slot_pid, slots(c), c->pid_base, slot_ids);
+    FLMR_CUDA(cudaGetLastError());
+    ++g_launches;
+    d_pids = slot_ids;
+  }
+  flmr_gather_kernel<<<static_cast<unsigned>(blocks), threads, 0, st>>>(
       reinterpret_cast<const uint2*>(c->d_tokens), c->d_poff, c->d_doclen, c->d_dead, d_pids, n_pids, nd_max,
-      c->n_passages, c->pid_base, static_cast<uint2*>(d_out_bf16), d_mask);
+      slots(c), c->pid_base, static_cast<uint2*>(d_out_bf16), d_mask);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;
@@ -2113,31 +2616,6 @@ int flmr_corpus_gather(const flmr_corpus_t* c, const int64_t* d_pids, int64_t n_
 
 // ---- the wgmma route of the arg-max forward (flmr_train_tc_kernel.cuh) ----------------------------------------
 thread_local int g_argmax_path = 0;   // 0 = by size, 1 = warp-MMA kernel, 2 = wgmma kernel (flmr_debug_set_argmax_path)
-
-// The library's own stream-ordered memory pool (one per device) for per-call scratch: it keeps what it has
-// been given (release threshold = max), so after the first call an allocation is a pointer bump in stream order —
-// the default pool hands memory back to the driver at every synchronisation and re-maps it on the next call.
-static int scratch_pool(cudaMemPool_t* out) {
-  static cudaMemPool_t pools[64] = {};
-  static std::mutex mu;
-  int dev = 0;
-  FLMR_CUDA(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> lock(mu);
-  if (!pools[dev & 63]) {
-    cudaMemPoolProps props{};
-    props.allocType = cudaMemAllocationTypePinned;
-    props.handleTypes = cudaMemHandleTypeNone;
-    props.location.type = cudaMemLocationTypeDevice;
-    props.location.id = dev;
-    cudaMemPool_t p = nullptr;
-    FLMR_CUDA(cudaMemPoolCreate(&p, &props));
-    uint64_t keep = ~0ull;
-    FLMR_CUDA(cudaMemPoolSetAttribute(p, cudaMemPoolAttrReleaseThreshold, &keep));
-    pools[dev & 63] = p;
-  }
-  *out = pools[dev & 63];
-  return FLMR_OK;
-}
 
 static int argmax_tc(const void* d_q, int n_queries, int nq, const void* d_docs, const uint8_t* d_mask, int n_per,
                      int stride_b, int nd, int32_t* d_argmax, float* d_rowmax, Elem elem, cudaStream_t st) {
@@ -2416,30 +2894,41 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
   const int threads = nq >= 256 ? 256 : (nq > 128 ? 256 : 128);
-  dim3 grid(static_cast<unsigned>(c->n_passages), static_cast<unsigned>(n_queries));
+  const int64_t ns = slots(c);
+  dim3 grid(static_cast<unsigned>(ns), static_cast<unsigned>(n_queries));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const float init = (flags & FLMR_FLAG_RELU) ? 0.f : -INFINITY;
+  StreamScratch scratch(st);
+  // a compacted corpus: slot-indexed rows into scratch, then spread over the ids as flmr_maxsim_scores does
+  float* out = d_out_scores;
+  if (c->d_slot_pid) {
+    if (int rc = scratch.alloc(&out, static_cast<size_t>(n_queries) * ns * sizeof(float))) return rc;
+  }
   if (!c->fp8) {
     (c->f16 ? flmr_simt_maxsim_kernel<Elem::kF16> : flmr_simt_maxsim_kernel<Elem::kBF16>)<<<grid, threads, 0, st>>>(
-        c->d_tokens, c->d_poff, c->d_doclen, c->d_dead, d_q, nq, init, d_out_scores, c->n_passages);
+        c->d_tokens, c->d_poff, c->d_doclen, c->d_dead, d_q, nq, init, out, ns);
     FLMR_CUDA(cudaGetLastError());
     ++g_launches;
-    return FLMR_OK;
+  } else {
+    // e4m3 corpus: MaxSim of e4m3(Q) against the e4m3 matrix, the queries rounded into stream-ordered scratch
+    const int64_t n_chunks = static_cast<int64_t>(n_queries) * nq * (kDim / 8);
+    __nv_bfloat16* q8 = nullptr;
+    if (int rc = scratch.alloc(&q8, static_cast<size_t>(n_chunks) * 16)) return rc;
+    flmr_round_e4m3_kernel<<<static_cast<unsigned>((n_chunks + 255) / 256), 256, 0, st>>>(
+        static_cast<const uint4*>(d_q), reinterpret_cast<uint4*>(q8), n_chunks);
+    flmr_simt_maxsim_kernel<Elem::kE4M3><<<grid, threads, 0, st>>>(c->d_fp8, c->d_poff, c->d_doclen, c->d_dead, q8, nq,
+                                                                   init, out, ns);
+    const cudaError_t e = cudaGetLastError();
+    g_launches += 2;
+    if (e != cudaSuccess) return fail(FLMR_ERR_CUDA, "SIMT cross-check launch failed: %s", cudaGetErrorString(e));
   }
-  // e4m3 corpus: MaxSim of e4m3(Q) against the e4m3 matrix, the queries rounded into stream-ordered scratch
-  const int64_t n_chunks = static_cast<int64_t>(n_queries) * nq * (kDim / 8);
-  cudaMemPool_t pool = nullptr;
-  if (int rc = scratch_pool(&pool)) return rc;
-  __nv_bfloat16* q8 = nullptr;
-  FLMR_CUDA(cudaMallocFromPoolAsync(reinterpret_cast<void**>(&q8), static_cast<size_t>(n_chunks) * 16, pool, st));
-  flmr_round_e4m3_kernel<<<static_cast<unsigned>((n_chunks + 255) / 256), 256, 0, st>>>(
-      static_cast<const uint4*>(d_q), reinterpret_cast<uint4*>(q8), n_chunks);
-  flmr_simt_maxsim_kernel<Elem::kE4M3><<<grid, threads, 0, st>>>(c->d_fp8, c->d_poff, c->d_doclen, c->d_dead, q8, nq, init,
-                                                          d_out_scores, c->n_passages);
-  const cudaError_t e = cudaGetLastError();
-  cudaFreeAsync(q8, st);
-  g_launches += 2;
-  if (e != cudaSuccess) return fail(FLMR_ERR_CUDA, "SIMT cross-check launch failed: %s", cudaGetErrorString(e));
+  if (c->d_slot_pid) {
+    const int64_t n = static_cast<int64_t>(n_queries) * c->n_passages;
+    flmr_expand_slot_scores_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
+        out, ns, c->d_slot_pid, c->pid_base, c->n_passages, n_queries, d_out_scores);
+    FLMR_CUDA(cudaGetLastError());
+    ++g_launches;
+  }
   return FLMR_OK;
 }
 
@@ -2499,6 +2988,37 @@ int flmr_debug_plan_passes(int n_queries, int nq, int allow_pair, int32_t* out_p
       const PassPlan& q = plan[i];
       const int32_t row[8] = {q.q_first, q.n_q, q.row0, q.rows, q.rbq, q.n_mtiles, q.flags, q.group_first + q.acc_slot};
       std::copy(row, row + 8, out_plan + i * 8);
+    }
+  }
+  return FLMR_OK;
+}
+
+int flmr_debug_compact_plan(const int32_t* h_doclens, int64_t n_passages, const int64_t* h_deleted, int64_t n_deleted,
+                            int64_t chunk_rows, int64_t* out_moves, int64_t capacity, int64_t* n_moves_out) {
+  if (!h_doclens || n_passages <= 0 || n_deleted < 0 || (n_deleted > 0 && !h_deleted) || chunk_rows < 0 ||
+      !n_moves_out)
+    return fail(FLMR_ERR_INVALID_ARG, "bad argument");
+  std::vector<int64_t> poff(n_passages + 1, 0);
+  for (int64_t p = 0; p < n_passages; ++p) {
+    if (h_doclens[p] < 1) return fail(FLMR_ERR_INVALID_ARG, "passage %lld has length %d", (long long)p, h_doclens[p]);
+    poff[p + 1] = poff[p] + (h_doclens[p] + kGroup - 1) / kGroup * kGroup;
+  }
+  std::vector<char> keep(n_passages, 1);
+  for (int64_t i = 0; i < n_deleted; ++i) {
+    if (h_deleted[i] < 0 || h_deleted[i] >= n_passages)
+      return fail(FLMR_ERR_INVALID_ARG, "deleted passage %lld outside [0, %lld)", (long long)h_deleted[i],
+                  (long long)n_passages);
+    keep[h_deleted[i]] = 0;
+  }
+  std::vector<MovePiece> plan;
+  plan_compaction(kept_runs(poff, keep), chunk_rows ? chunk_rows : kCompactChunkRows, true, &plan);
+  *n_moves_out = static_cast<int64_t>(plan.size());
+  if (out_moves) {
+    if (static_cast<int64_t>(plan.size()) > capacity)
+      return fail(FLMR_ERR_INVALID_ARG, "capacity %lld < %zu moves", (long long)capacity, plan.size());
+    for (size_t i = 0; i < plan.size(); ++i) {
+      const int64_t row[5] = {plan[i].src, plan[i].dst, plan[i].rows, plan[i].staged ? 1 : 0, plan[i].chunk};
+      std::copy(row, row + 5, out_moves + i * 5);
     }
   }
   return FLMR_OK;
@@ -2612,7 +3132,7 @@ int flmr_topk_exchange(flmr_comm_t* c, const float* d_scores, const int64_t* d_p
   if (r1 != 0 || r2 != 0)
     return fail(FLMR_ERR_CUDA, "ncclAllGather failed: %s", api->GetErrorString(r1 ? r1 : r2));
   flmr_merge_kernel<<<n_queries, kMergeThreads, 0, st>>>(nullptr, c->d_recv_s, c->d_recv_p, c->world, n_queries,
-                                                        k_in, k_out, 0, d_out_scores, d_out_pids, 0);
+                                                        k_in, k_out, 0, nullptr, d_out_scores, d_out_pids, 0);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;

@@ -8,8 +8,9 @@ the updater later ColBERT releases ship (``IndexUpdater(config, searcher, checkp
     updater.persist_to_disk()                            # the flat index on disk catches up
 
 The resident corpus grows in place (``FlatCorpus.append``) and deletions are tombstones tested inside the scan
-(``FlatCorpus.delete``): no rebuild, no reload.  Ids are stable: an added passage gets the next id, a removed one keeps
-its id and is never reused; only a fresh ``Indexer`` build renumbers.
+(``FlatCorpus.delete``): no rebuild, no reload.  ``compact`` drops the deleted passages' rows from HBM and from the
+scan.  Ids are stable: an added passage gets the next id, a removed one keeps its id and is never reused, compaction
+moves rows but renumbers nothing; only a fresh ``Indexer`` build renumbers.
 """
 from __future__ import annotations
 
@@ -79,6 +80,12 @@ class IndexUpdater:
     def remove(self, pids) -> None:
         """Delete passages by id: no search returns them again.  Every id must exist."""
         self.corpus.delete(pids)
+
+    def compact(self) -> dict:
+        """Remove the removed passages' rows from the resident corpus (``FlatCorpus.compact``): memory and scan time
+        shrink, ids and search results stay as they are.  The index on disk is not rewritten: ``persist_to_disk``
+        writes what it would have written without compaction."""
+        return self.corpus.compact()
 
     def persist_to_disk(self) -> dict:
         """Write the updates to the flat index the searcher was opened on: appended passages as new chunks, the
