@@ -30,6 +30,7 @@ import numpy as np
 import torch
 
 import fp8_oracle as F8
+from oracle import maxsim_oracle as O
 from train_fp64 import U, bf16_rows, pairwise_cases
 
 ALIGN_BITS = {"bf16": 25, "fp8": 13}   # bits a k-step keeps below its leading bit (measured, see above)
@@ -105,6 +106,39 @@ def scan_bound(amax: torch.Tensor, rabs: torch.Tensor, nq: int, storage: str = "
 def simt_bound(amax: torch.Tensor, rabs: torch.Tensor, nq: int) -> torch.Tensor:
     """Rigorous bound of the SIMT kernel: gamma(128) per row maximum, gamma(Nq) for their sum (of computed maxima)."""
     return gamma(128) * amax * (1 + gamma(nq)) + gamma(nq) * rabs
+
+
+# ---- checks: error / bound ratios and the fused top-k certified by float64 -------------------------------------------
+def check_ratio(ratios: dict, name, err, bound):
+    """err <= bound elementwise (a zero bound demands an exact zero); records the largest err / bound of `name` in
+    `ratios`."""
+    err, bound = err.double().reshape(-1), bound.double().reshape(-1)
+    assert not torch.isnan(err).any(), name
+    if err.numel() == 0:
+        return
+    ratio = torch.where(bound > 0, err / bound.clamp_min(1e-300), torch.where(err > 0, torch.inf, 0.0))
+    worst = int(ratio.argmax())
+    r = float(ratio[worst])
+    ratios[name] = max(ratios.get(name, 0.0), r)
+    assert r <= 1.0, "%s: error %.3e > bound %.3e (ratio %.3g)" % (name, err[worst], bound[worst], r)
+
+
+def check_topk(scores, ts, tp, s64, bound, k, tag):
+    """The fused top-k: a stable sort of the kernel's own scores, and certified by the float64 scores: no passage left
+    out is surely better than a returned one, consecutive returned ones are ordered up to their bounds."""
+    rs, rp = O.topk(scores.cpu().numpy(), k)
+    assert np.array_equal(tp.cpu().numpy(), rp) and np.array_equal(ts.cpu().numpy(), rs), tag
+    lo, hi = s64 - bound, s64 + bound
+    n = s64.size(1)
+    for b in range(s64.size(0)):
+        ids = tp[b][tp[b] >= 0]
+        assert ids.numel() == min(k, n), tag
+        out = torch.ones(n, dtype=torch.bool, device=s64.device)
+        out[ids] = False
+        if out.any():
+            assert lo[b][out].max() <= hi[b][ids].min(), "%s: query %d, a passage left out beats a returned one" % (
+                tag, b)
+        assert (hi[b][ids[:-1]] >= lo[b][ids[1:]]).all(), "%s: query %d returned out of order" % (tag, b)
 
 
 # ---- the scan's pass plan, as the host builds it (the partition: helpers.scan_partition) ---------------------------

@@ -19,7 +19,6 @@ import torch
 
 import scan_fp64 as S
 from helpers import scan_partition
-from oracle import maxsim_oracle as O
 
 pytestmark = pytest.mark.gpu
 
@@ -28,16 +27,7 @@ REPORT = []
 
 
 def _check(name, err, bound):
-    """err <= bound elementwise (a zero bound demands an exact zero); records the largest err / bound of `name`."""
-    err, bound = err.double().reshape(-1), bound.double().reshape(-1)
-    assert not torch.isnan(err).any(), name
-    if err.numel() == 0:
-        return
-    ratio = torch.where(bound > 0, err / bound.clamp_min(1e-300), torch.where(err > 0, torch.inf, 0.0))
-    worst = int(ratio.argmax())
-    r = float(ratio[worst])
-    RATIOS[name] = max(RATIOS.get(name, 0.0), r)
-    assert r <= 1.0, "%s: error %.3e > bound %.3e (ratio %.3g)" % (name, err[worst], bound[worst], r)
+    S.check_ratio(RATIOS, name, err, bound)
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -216,24 +206,6 @@ def test_accumulator_probes(R, storage):
 GRID = S.scan_grid()
 
 
-def _check_topk(scores, ts, tp, s64, bound, k, tag):
-    """The fused top-k: a stable sort of the kernel's own scores, and certified by the float64 scores: no passage left
-    out is surely better than a returned one, consecutive returned ones are ordered up to their bounds."""
-    rs, rp = O.topk(scores.cpu().numpy(), k)
-    assert np.array_equal(tp.cpu().numpy(), rp) and np.array_equal(ts.cpu().numpy(), rs), tag
-    lo, hi = s64 - bound, s64 + bound
-    n = s64.size(1)
-    for b in range(s64.size(0)):
-        ids = tp[b][tp[b] >= 0]
-        assert ids.numel() == min(k, n), tag
-        out = torch.ones(n, dtype=torch.bool, device=s64.device)
-        out[ids] = False
-        if out.any():
-            assert lo[b][out].max() <= hi[b][ids].min(), "%s: query %d, a passage left out beats a returned one" % (
-                tag, b)
-        assert (hi[b][ids[:-1]] >= lo[b][ids[1:]]).all(), "%s: query %d returned out of order" % (tag, b)
-
-
 @pytest.mark.parametrize("ci", range(len(GRID)), ids=lambda i: "c%03d" % i)
 def test_scan_grid(R, scan_variant, ci):
     c = GRID[ci]
@@ -257,4 +229,4 @@ def test_scan_grid(R, scan_variant, ci):
     if c["zeros"] == "query":
         assert (got[0] == 0).all() and (simt[0] == 0).all(), tag
     for k, (ts, tp) in tops.items():
-        _check_topk(got, ts, tp, s64, bound, k, "%s k=%d" % (tag, k))
+        S.check_topk(got, ts, tp, s64, bound, k, "%s k=%d" % (tag, k))
