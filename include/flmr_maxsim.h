@@ -42,6 +42,9 @@
  *   flmr_maxsim_scores_allowed / flmr_maxsim_topk_allowed / flmr_maxsim_topk_sharded_allowed
  *       the pids= / qid_to_pids= restriction of later ColBERT Searchers: a per-query allow bitmap tested in the
  *       scan's reducer (the vendored release filters scores with filter_fn, CB/searcher.py:61-132).
+ *   flmr_maxsim_topk_listed / flmr_maxsim_scores_listed
+ *       the same restriction given as id lists, at the cost of the listed passages: the scan runs over a per-call
+ *       plan of their rows (the reference's pipeline likewise scores only its candidates, CB/search/index_storage.py).
  *   flmr_debug_maxsim_scores_simt
  *       test infrastructure: an independent plain-SIMT fp32 device kernel used by tests to
  *       cross-check the tensor-core kernel at sizes where the CPU oracle is too slow.
@@ -275,8 +278,9 @@ int flmr_maxsim_topk(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const vo
 /*
  * Restricted search: each query is scored against its own set of passages (the pids= / qid_to_pids= of later
  * ColBERT Searchers: re-ranking a first stage's candidates, one entity's or tenant's passages, a training query
- * without its positives).  The restriction is tested inside the scan's reducer, so no score matrix is written; the
- * scan still streams the whole shard, so a restricted search costs what an unrestricted one does.
+ * without its positives).  The restriction is tested inside the scan's reducer, so no score matrix is written.  The
+ * _allowed calls take bitmaps and stream the whole shard: they cost what an unrestricted search does.  The _listed
+ * calls (below) take id lists and stream only the listed passages' rows.
  *   d_allow             uint32 device bitmaps, one per query: bit p & 31 of word p >> 5 set <=> query b may return
  *                       LOCAL passage p (global id pid_base + p).  Query b's bitmap starts at
  *                       d_allow + b * allow_stride_words.  Bits at or beyond n_passages are ignored.
@@ -294,6 +298,30 @@ int flmr_maxsim_scores_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws
 int flmr_maxsim_topk_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries,
                              int nq, int k, unsigned flags, const uint32_t* d_allow, int64_t allow_stride_words,
                              float* d_out_scores, int64_t* d_out_pids, void* stream);
+
+/*
+ * Restricted search over id lists, at the cost of the listed passages: the same scan kernel runs over a per-call plan
+ * of the listed passages' rows only, re-balanced over the persistent CTAs (the planner runs on the device, in stream
+ * order, without a host synchronisation).  The fold and the reducer are those of every other scan, so results are
+ * bitwise those of the _allowed calls for bitmaps of the same sets.
+ *   h_list_offsets  HOST int64 [n_queries + 1], non-decreasing: query b's list is
+ *                   d_list_pids[h_list_offsets[b] .. h_list_offsets[b + 1])
+ *   d_list_pids     DEVICE int64 GLOBAL ids (pid_base + local id), in any order, duplicates allowed.  Ids outside this
+ *                   shard are ignored (every rank of a sharded search may pass the same lists); deleted and
+ *                   compacted-away ids are never returned.
+ * flmr_maxsim_topk_listed    = flmr_maxsim_topk_allowed for bitmaps of the same sets: the same (score, id) lists, ties
+ *                              to the lower id, (-inf, -1) fill when fewer than k listed passages are live.
+ * flmr_maxsim_scores_listed  d_out_scores fp32 [h_list_offsets[n_queries]], aligned with d_list_pids (entry i at
+ *                              index i): the flmr_maxsim_scores_allowed score of the pair; -inf for an id outside the
+ *                              shard, deleted or compacted away.
+ * Scan variants 3 and 4 have no plan-mode kernel (FLMR_ERR_UNSUPPORTED).
+ */
+int flmr_maxsim_topk_listed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries, int nq,
+                            int k, unsigned flags, const int64_t* h_list_offsets, const int64_t* d_list_pids,
+                            float* d_out_scores, int64_t* d_out_pids, void* stream);
+int flmr_maxsim_scores_listed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries,
+                              int nq, unsigned flags, const int64_t* h_list_offsets, const int64_t* d_list_pids,
+                              float* d_out_scores, void* stream);
 
 /*
  * Merge n_lists candidate lists per query into one top-k (the post-all-gather step of the
@@ -504,6 +532,17 @@ int flmr_debug_plan_passes(int n_queries, int nq, int allow_pair, int32_t* out_p
  * chunk_rows bounds the rows of a chunk (0: the library's bound, 256 MiB of bf16 rows). */
 int flmr_debug_compact_plan(const int32_t* h_doclens, int64_t n_passages, const int64_t* h_deleted, int64_t n_deleted,
                             int64_t chunk_rows, int64_t* out_moves, int64_t capacity, int64_t* n_moves_out);
+
+/* Test infrastructure: the plans a listed search of these lists (n_queries <= the workspace's max_queries) would scan,
+ * computed on the device as flmr_maxsim_topk_listed computes them and copied back (synchronous, default stream).
+ * h_out (may be NULL to query *n_out) receives int64: the number of passes, then per pass q_first, n_q, n_ctas, the
+ * union size U, the tile count T and the tile bound the buffers hold, the union's slots (U, sorted), cta_tile_base
+ * (n_ctas + 1: CTA c scans tiles [base[c], base[c + 1])), each tile's first stored row (T), end mask (T: bit g = a
+ * listed passage ends with 4-token group g, bit 31 = the tile starts a run of consecutive slots or a CTA's share of
+ * one) and first slot ending in it (T; 0x7fffffff when none does). */
+int flmr_debug_listed_plan(const flmr_corpus_t* corpus, flmr_workspace_t* ws, int n_queries, int nq,
+                           const int64_t* h_list_offsets, const int64_t* d_list_pids, int64_t* h_out,
+                           int64_t capacity, int64_t* n_out);
 
 /* Kernels launched by this library on the calling thread since the last reset (bench evidence). */
 int64_t flmr_launch_count(int reset);

@@ -2,9 +2,9 @@
 repository accelerates).  Import name: ``ravqa_b200`` (the directory name carries hyphens)."""
 from . import _cabi  # noqa: F401
 from .corpus import FlatCorpus, allow_bitmaps  # noqa: F401
-from .maxsim import maxsim_scores, maxsim_topk, topk_merge, topk_select, debug_scores_simt  # noqa: F401
+from .maxsim import maxsim_scores, maxsim_scores_listed, maxsim_topk, topk_merge, topk_select, debug_scores_simt  # noqa: F401
 
-__all__ = ["FlatCorpus", "allow_bitmaps", "maxsim_scores", "maxsim_topk", "topk_merge", "topk_select",
+__all__ = ["FlatCorpus", "allow_bitmaps", "maxsim_scores", "maxsim_scores_listed", "maxsim_topk", "topk_merge", "topk_select",
            "debug_scores_simt"]
 from .searcher import Searcher, Ranking  # noqa: F401,E402
 from .sharded import ShardedSearcher, shard_ranges  # noqa: F401,E402

@@ -40,8 +40,11 @@ COMPACT_SYMBOLS = ("flmr_corpus_compact", "flmr_corpus_stored", "flmr_debug_comp
 # the training / re-scoring calls on fp16 operands
 FP16_TRAIN_SYMBOLS = ("flmr_maxsim_argmax_fp16", "flmr_maxsim_backward_fp16", "flmr_maxsim_argmax_grouped_fp16",
                       "flmr_maxsim_backward_grouped_fp16")
+# restricted search over id lists at the cost of the listed passages (the scan's plan mode)
+LISTED_SYMBOLS = ("flmr_maxsim_topk_listed", "flmr_maxsim_scores_listed", "flmr_debug_listed_plan")
 # symbols an earlier revision's library may lack (tools/scan_ab.py drives one through this binding)
-OPTIONAL_SYMBOLS = UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS + FP16_TRAIN_SYMBOLS + COMPACT_SYMBOLS
+OPTIONAL_SYMBOLS = (UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS + FP16_TRAIN_SYMBOLS + COMPACT_SYMBOLS
+                    + LISTED_SYMBOLS)
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
@@ -55,7 +58,7 @@ SYMBOLS = [
     "flmr_corpus_builder_create", "flmr_corpus_builder_create_ex", "flmr_corpus_builder_append", "flmr_corpus_builder_append_file",
     "flmr_corpus_builder_finish", "flmr_corpus_builder_destroy",
     "flmr_comm_unique_id", "flmr_comm_create", "flmr_comm_adopt", "flmr_comm_destroy", "flmr_comm_info",
-    "flmr_topk_exchange", "flmr_maxsim_topk_sharded", *ALLOWED_SYMBOLS,
+    "flmr_topk_exchange", "flmr_maxsim_topk_sharded", *ALLOWED_SYMBOLS, *LISTED_SYMBOLS,
     "flmr_debug_maxsim_scores_simt", "flmr_debug_set_argmax_path", "flmr_debug_set_scan_variant", "flmr_debug_build_partition", "flmr_debug_plan_passes",
     "flmr_launch_count", "flmr_set_profiling", "flmr_scan_kernel_stats",
 ]
@@ -109,6 +112,10 @@ def lib() -> C.CDLL:
         L.flmr_maxsim_scores_allowed.argtypes = [vp, vp, vp, i32, i32, u32, vp, i64, vp, vp]
         L.flmr_maxsim_topk_allowed.argtypes = [vp, vp, vp, i32, i32, i32, u32, vp, i64, vp, vp, vp]
         L.flmr_maxsim_topk_sharded_allowed.argtypes = [vp, vp, vp, vp, i32, i32, i32, u32, vp, i64, vp, vp, vp]
+    if hasattr(L, "flmr_maxsim_topk_listed"):
+        L.flmr_maxsim_topk_listed.argtypes = [vp, vp, vp, i32, i32, i32, u32, vp, vp, vp, vp, vp]
+        L.flmr_maxsim_scores_listed.argtypes = [vp, vp, vp, i32, i32, u32, vp, vp, vp, vp]
+        L.flmr_debug_listed_plan.argtypes = [vp, vp, i32, i32, vp, vp, vp, i64, C.POINTER(i64)]
     L.flmr_workspace_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
     L.flmr_workspace_destroy.argtypes = [vp]
     L.flmr_workspace_status.argtypes = [vp, C.POINTER(i32)]

@@ -468,6 +468,206 @@ __global__ void flmr_expand_slot_scores_kernel(const float* __restrict__ src, in
   dst[i] = s >= 0 ? src[b * n_slots + s] : -INFINITY;
 }
 
+// ---- listed search: the per-call scan plan over the listed passages' rows (flmr_maxsim_*_listed) ----------------
+// Slot of global id `gid`, or -1: outside the shard, or compacted away (slot_pid null: slot = local id).
+__device__ __forceinline__ int64_t listed_slot(int64_t gid, const int64_t* __restrict__ slot_pid, int64_t n_slots,
+                                               int64_t pid_base, int64_t n_ids) {
+  const int64_t local = gid - pid_base;
+  if (local < 0 || local >= n_ids) return -1;
+  return slot_pid ? slot_of(slot_pid, n_slots, gid) : local;
+}
+
+// Query of list entry i: the last b < n_q with off[b] <= i (off: the chunk's CSR offsets, off[0] <= i < off[n_q]).
+__device__ __forceinline__ int listed_query(const int64_t* __restrict__ off, int n_q, int64_t i) {
+  int lo = 0, hi = n_q;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(off + mid) <= i) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// Entries [off[0], off[n_q]) of the lists -> the queries' slot bitmaps (`words` words apart, zeroed by the caller): the
+// allow test of the plan-mode reducer, and the planner's input.  One thread per entry.
+__global__ void flmr_listed_mark_kernel(const int64_t* __restrict__ pids, const int64_t* __restrict__ off, int n_q,
+                                        const int64_t* __restrict__ slot_pid, int64_t n_slots, int64_t pid_base,
+                                        int64_t n_ids, int64_t words, uint32_t* __restrict__ allow) {
+  const int64_t i = __ldg(off) + static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= __ldg(off + n_q)) return;
+  const int64_t s = listed_slot(__ldg(pids + i), slot_pid, n_slots, pid_base, n_ids);
+  if (s < 0) return;
+  atomicOr(allow + listed_query(off, n_q, i) * words + (s >> 5), 1u << (s & 31));
+}
+
+// Slot-indexed score rows [n_q, n_slots] -> the scores of entries [off[0], off[n_q]), aligned with the lists: -inf for
+// an id without a slot.  One thread per entry.
+__global__ void flmr_listed_scores_kernel(const int64_t* __restrict__ pids, const int64_t* __restrict__ off, int n_q,
+                                          const int64_t* __restrict__ slot_pid, int64_t n_slots, int64_t pid_base,
+                                          int64_t n_ids, const float* __restrict__ src, float* __restrict__ out) {
+  const int64_t i = __ldg(off) + static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= __ldg(off + n_q)) return;
+  const int64_t s = listed_slot(__ldg(pids + i), slot_pid, n_slots, pid_base, n_ids);
+  out[i] = s >= 0 ? src[listed_query(off, n_q, i) * n_slots + s] : -INFINITY;
+}
+
+constexpr int kPlanThreads = 1024;
+
+// Exclusive scan of x over the kPlanThreads threads of the block under `op` (identity `id`); *total = the reduction
+// of every thread's x.  `s` is 32 elements of shared memory; every thread must call it.
+template <typename T, typename Op>
+__device__ __forceinline__ T block_exclusive_scan(T x, T id, Op op, T* s, T* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T incl = x;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const T y = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl = op(y, incl);
+  }
+  if (lane == 31) s[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    T w = s[lane];
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const T y = __shfl_up_sync(0xffffffffu, w, d);
+      if (lane >= d) w = op(y, w);
+    }
+    s[lane] = w;
+  }
+  __syncthreads();
+  T excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane == 0) excl = id;
+  if (warp > 0) excl = op(s[warp - 1], excl);
+  *total = s[31];
+  __syncthreads();   // s is reused by the next call
+  return excl;
+}
+
+// One pass of a listed search, as the planner sees it.  Offsets are in elements of the plan's arrays.
+struct ListedPass {
+  int32_t q_first, n_q;   // queries of the pass (bitmaps allow + (q_first .. q_first + n_q - 1) * words)
+  int64_t u_off;          // its union entries: u_slot / u_cum / u_tile [u_off, u_off + union bound)
+  int64_t c_off;          // its cta_tile_base [c_off, c_off + n_ctas + 1)
+  int64_t t_off;          // its tiles: tile_row / tile_mask / tile_first [t_off, t_off + tile bound)
+};
+
+// The planner: one block per pass.
+//   1. the union of the pass's queries' slot bitmaps -> its slots, sorted and unique (u_slot);
+//   2. their stored rows -> each one's first row inside the union (u_cum) and the union's rows R;
+//   3. the union is cut into CTA shares at passage boundaries, as build_partition cuts the corpus (CTA c starts at the
+//      first passage at or past row R c / n_ctas), and into runs of consecutive slots inside a share; each run is
+//      tiled from its first row in steps of 96 rows (u_tile: the run's first tile).  A tile's end mask marks the ends
+//      of the run's passages that fall in it (bit g: 4-token group g, as tile_end_mask), plus kTileRunStart on a
+//      run's first tile; tile_first is the first slot ending in the tile;
+//   4. cta_tile_base: CTA c's tiles, in the scan kernel's layout.
+// meta[2 pass] = union size, meta[2 pass + 1] = tiles.
+__global__ void __launch_bounds__(kPlanThreads)
+flmr_listed_plan_kernel(const ListedPass* __restrict__ passes, const uint32_t* __restrict__ allow, int64_t words,
+                        const int64_t* __restrict__ poff, int n_ctas, int32_t* u_slot_all, int64_t* u_cum_all,
+                        int64_t* u_tile_all, int64_t* cta_tile_base_all, int32_t* tile_row_all,
+                        uint32_t* tile_mask_all, int32_t* tile_first_all, int64_t* meta) {
+  __shared__ long long s_scan[32];
+  const ListedPass ps = passes[blockIdx.x];
+  int32_t* const u_slot = u_slot_all + ps.u_off;
+  int64_t* const u_cum = u_cum_all + ps.u_off;
+  int64_t* const u_tile = u_tile_all + ps.u_off;
+  int32_t* const tile_row = tile_row_all + ps.t_off;
+  uint32_t* const tile_mask = tile_mask_all + ps.t_off;
+  int32_t* const tile_first = tile_first_all + ps.t_off;
+  const int tid = threadIdx.x;
+  auto add = [](long long a, long long b) { return a + b; };
+  auto mx = [](long long a, long long b) { return a > b ? a : b; };
+  long long tot;
+  // 1. union slots, in slot order
+  long long n = 0;
+  for (int64_t w0 = 0; w0 < words; w0 += kPlanThreads) {
+    const int64_t w = w0 + tid;
+    uint32_t bits = 0u;
+    if (w < words)
+      for (int q = 0; q < ps.n_q; ++q) bits |= __ldg(allow + (ps.q_first + q) * words + w);
+    long long pos = n + block_exclusive_scan<long long>(__popc(bits), 0ll, add, s_scan, &tot);
+    while (bits) {
+      u_slot[pos++] = static_cast<int32_t>(w * 32 + __ffs(bits) - 1);
+      bits &= bits - 1u;
+    }
+    n += tot;
+  }
+  __syncthreads();
+  // 2. first row of each inside the union
+  long long R = 0;
+  for (int64_t i0 = 0; i0 < n; i0 += kPlanThreads) {
+    const int64_t i = i0 + tid;
+    long long rows = 0;
+    if (i < n) rows = __ldg(poff + u_slot[i] + 1) - __ldg(poff + u_slot[i]);
+    const long long excl = block_exclusive_scan<long long>(rows, 0ll, add, s_scan, &tot);
+    if (i < n) u_cum[i] = R + excl;
+    R += tot;
+  }
+  __syncthreads();
+  // 3. shares, runs, tiles
+  auto cta_of = [&](long long x) {   // the last c with R c / n_ctas <= x
+    return static_cast<int>(min(static_cast<long long>(n_ctas) - 1, (static_cast<long long>(n_ctas) * (x + 1) + R - 1) / R - 1));
+  };
+  long long run_carry = -1, tile_carry = 0;
+  for (int64_t i0 = 0; i0 < n; i0 += kPlanThreads) {
+    const int64_t i = i0 + tid;
+    const bool ok = i < n;
+    long long x = 0, rows = 0;
+    int32_t s = 0;
+    bool start = false;
+    if (ok) {
+      s = u_slot[i];
+      x = u_cum[i];
+      rows = __ldg(poff + s + 1) - __ldg(poff + s);
+      start = i == 0 || u_slot[i - 1] != s - 1 || cta_of(u_cum[i - 1]) != cta_of(x);
+    }
+    // first row of the run holding i: the last run start at or before it (a running max: u_cum increases)
+    const long long mine = start ? x : -1ll;
+    const long long rs = mx(mx(run_carry, block_exclusive_scan<long long>(mine, -1ll, mx, s_scan, &tot)), mine);
+    run_carry = mx(run_carry, tot);
+    const long long b = x - rs, e = b + rows;               // the passage's rows inside its run
+    const long long t0 = (b + kTileN - 1) / kTileN, t1 = (e + kTileN - 1) / kTileN;   // tiles starting in it
+    const long long T = tile_carry + block_exclusive_scan<long long>(ok ? t1 - t0 : 0ll, 0ll, add, s_scan, &tot);
+    tile_carry += tot;
+    const long long run_tile = T - t0;                      // the run's first tile
+    if (ok) {
+      u_tile[i] = run_tile;
+      for (long long t = t0; t < t1; ++t) {
+        tile_row[run_tile + t] = static_cast<int32_t>(__ldg(poff + s) - b + t * kTileN);
+        tile_mask[run_tile + t] = t == 0 ? kTileRunStart : 0u;
+        tile_first[run_tile + t] = 0x7fffffff;
+      }
+    }
+    __syncthreads();   // a tile is initialised (above, by the passage it starts in) before anyone marks an end in it
+    if (ok) {
+      const long long g = run_tile + (e - 1) / kTileN;
+      atomicOr(tile_mask + g, 1u << (((e - 1) % kTileN) / kGroup));
+      atomicMin(tile_first + g, s);
+    }
+    __syncthreads();
+  }
+  // 4. CTA c's tiles start at the run of its first passage (the first one at or past row R c / n_ctas)
+  for (int c = tid; c <= n_ctas; c += kPlanThreads) {
+    int64_t first = n;
+    if (c == 0) {
+      first = 0;
+    } else if (c < n_ctas && R > 0) {
+      const long long target = R * c / n_ctas;
+      int64_t lo = 0, hi = n;
+      while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (u_cum[mid] < target) lo = mid + 1; else hi = mid;
+      }
+      first = lo;
+    }
+    cta_tile_base_all[ps.c_off + c] = first < n ? u_tile[first] : tile_carry;
+  }
+  if (tid == 0) {
+    meta[2 * blockIdx.x] = n;
+    meta[2 * blockIdx.x + 1] = tile_carry;
+  }
+}
+
 // Independent plain-SIMT MaxSim (test infrastructure): one block per (passage, query), one thread
 // per query token (looping if nq > blockDim), fp32 FMA over bf16 inputs, fixed-order block sum.
 // kE4M3: the corpus matrix is e4m3 (the queries come already rounded to e4m3 as bf16, flmr_round_e4m3_kernel).
@@ -853,6 +1053,7 @@ struct flmr_corpus {
   int32_t* d_doclen = nullptr;         // [slots] real lengths
   std::vector<int64_t> h_poff;         // host copies of the two above (an append extends them)
   std::vector<int32_t> h_doclen;
+  int64_t max_rows = 0;                // stored rows of the longest slot (bounds a listed search's plan)
   // tombstones: h_dead is indexed by LOCAL ID (bit p & 31 of word p >> 5 set <=> local passage p is deleted, a
   // compacted-away id included); d_dead by SLOT, for the scan's reducer, the gather and the SIMT kernel.  d_dead stays
   // null while no slot is deleted (until the first delete, and again right after a compaction), so a corpus without
@@ -907,6 +1108,8 @@ struct flmr_workspace {
   int cand_lists = 0;                  // CTAs d_cand_keys is sized for (grown when an append raises n_ctas)
   float* d_acc = nullptr;              // [group][n_passages] lazily allocated (row-sliced queries)
   int64_t acc_capacity = 0;            // floats allocated at d_acc
+  void* d_plan = nullptr;              // a listed search's slot bitmaps and scan plans (one call chunk), grown on demand
+  size_t plan_capacity = 0;            // bytes allocated at d_plan
   int* h_status = nullptr;             // pinned + mapped: readable by the host even after a device trap
   int* d_status = nullptr;             // device alias of h_status
   int dbg_lane_rbq = 4;  // -DFLMR_DEBUG builds: FLMR_LANE_RBQ, read once at creation
@@ -1199,7 +1402,11 @@ void plan_passes(int n_queries, int nq, bool allow_pair, std::vector<PassPlan>* 
   if (n_pair_queries_out) *n_pair_queries_out = n_pair_q;
 }
 
-int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pair, cudaStream_t st) {
+//
+// listed: p holds a listed search's plan (run_search's ListedArgs); the plan-mode twins of the two product kernels run
+// it, chosen by the same rule (variant 2 forces the two-warpgroup one, 6 the split one).
+int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pair, cudaStream_t st,
+                bool listed = false) {
   // by the pass's occupied 64-row blocks: from five up (Nq = 320: five, a full row slice: six) three warpgroups with
   // the split-tile loop (2 / 2 / 1 or 2 / 2 / 2 blocks, each warpgroup folding one half of a tile under the MMAs of
   // the other), below that two (each with two accumulators, its own MMAs overlapping its fold).  On an H100 80GB HBM3
@@ -1217,7 +1424,23 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
     FLMR_CUDA(cudaEventRecord(ev.a, st));
   }
   (void)ws;
-  if (pair) {
+  if (listed) {
+    const dim3 grid(c->n_ctas);
+    if (split) {
+      if (c->f16)
+        flmr_scan_listed_split_f16_kernel<<<grid, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+      else if (c->fp8)
+        flmr_scan_listed_split_kernel<true><<<grid, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+      else
+        flmr_scan_listed_split_kernel<false><<<grid, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    } else if (c->f16) {
+      flmr_scan_listed_f16_kernel<<<grid, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    } else if (c->fp8) {
+      flmr_scan_listed_kernel<true><<<grid, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    } else {
+      flmr_scan_listed_kernel<false><<<grid, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
+    }
+  } else if (pair) {
     // clusters of two CTAs share one of the n_pairs token ranges; the tensor map has a half-tile box
     p.cta_row_begin = c->d_pair_row_begin;
     p.cta_tile_base = c->d_pair_tile_base;
@@ -1303,11 +1526,104 @@ int ensure_acc(flmr_workspace* ws, int64_t floats) {
   return FLMR_OK;
 }
 
+// A listed search (flmr_maxsim_topk_listed / flmr_maxsim_scores_listed): query b's passages are the global ids
+// d_pids[h_off[b] .. h_off[b + 1]).
+struct ListedArgs {
+  const int64_t* h_off;   // [n_queries + 1] host CSR offsets
+  const int64_t* d_off;   // the same on the device
+  const int64_t* d_pids;
+  float* d_scores;        // scores_listed: [h_off[n_queries]] scores aligned with d_pids; null for topk_listed
+};
+
+// The plan of one call chunk's passes, in the workspace's plan buffer (flmr_listed_plan_kernel's arrays).
+struct ListedChunkPlan {
+  std::vector<ListedPass> passes;
+  std::vector<int64_t> u_bound, t_bound;   // per pass: union entries and tiles the buffers hold at most
+  int64_t words = 0;                       // of a slot bitmap
+  uint32_t* allow = nullptr;               // [n_q of the chunk][words] slot bitmaps
+  ListedPass* d_passes = nullptr;
+  int64_t* meta = nullptr;                 // [passes][2]: union size, tiles
+  int64_t *u_cum = nullptr, *u_tile = nullptr, *cta_tile_base = nullptr;
+  int32_t *u_slot = nullptr, *tile_row = nullptr, *tile_first = nullptr;
+  uint32_t* tile_mask = nullptr;
+};
+
+// Plans a listed search's passes `plan` over the chunk of queries [c0, c0 + nqc): the chunk's slot bitmaps (ids outside
+// the shard and ids without a slot dropped), then one planner block per pass.  Stream-ordered; no host synchronisation.
+// A pass of L listed ids holds at most min(L, slots) union entries and min(L, slots) (ceil(max rows / 96) + 1) + n_ctas
+// tiles (a passage starts at most ceil(its rows / 96) tiles of its run).
+int plan_listed_chunk(const flmr_corpus* c, flmr_workspace* ws, const std::vector<PassPlan>& plan, int c0, int nqc,
+                      const ListedArgs& la, cudaStream_t st, ListedChunkPlan* out) {
+  const int64_t ns = slots(c);
+  const int n_p = static_cast<int>(plan.size());
+  out->words = (ns + 31) / 32;
+  out->passes.resize(n_p);
+  out->u_bound.resize(n_p);
+  out->t_bound.resize(n_p);
+  const int64_t tiles_per = (c->max_rows + kTileN - 1) / kTileN + 1;
+  int64_t u_total = 0, t_total = 0;
+  for (int i = 0; i < n_p; ++i) {
+    const PassPlan& pp = plan[i];
+    const int64_t listed = la.h_off[c0 + pp.q_first + pp.n_q] - la.h_off[c0 + pp.q_first];
+    out->u_bound[i] = std::min(listed, ns);
+    out->t_bound[i] = out->u_bound[i] * tiles_per + c->n_ctas;
+    out->passes[i] = {pp.q_first, pp.n_q, u_total, static_cast<int64_t>(i) * (c->n_ctas + 1), t_total};
+    u_total += out->u_bound[i];
+    t_total += out->t_bound[i];
+  }
+  size_t bytes = 0;
+  auto take = [&](size_t n) {
+    const size_t at = bytes;
+    bytes += (n + 15) / 16 * 16;
+    return at;
+  };
+  const size_t o_allow = take(static_cast<size_t>(nqc) * out->words * 4);
+  const size_t o_passes = take(n_p * sizeof(ListedPass));
+  const size_t o_meta = take(2 * n_p * 8);
+  const size_t o_cum = take(u_total * 8), o_tile = take(u_total * 8), o_slot = take(u_total * 4);
+  const size_t o_base = take(static_cast<size_t>(n_p) * (c->n_ctas + 1) * 8);
+  const size_t o_row = take(t_total * 4), o_mask = take(t_total * 4), o_first = take(t_total * 4);
+  if (ws->plan_capacity < bytes) {
+    cudaFree(ws->d_plan);   // waits for the searches still using it
+    ws->d_plan = nullptr;
+    ws->plan_capacity = 0;
+    FLMR_CUDA(cudaMalloc(&ws->d_plan, bytes));
+    ws->plan_capacity = bytes;
+  }
+  uint8_t* base = static_cast<uint8_t*>(ws->d_plan);
+  out->allow = reinterpret_cast<uint32_t*>(base + o_allow);
+  out->d_passes = reinterpret_cast<ListedPass*>(base + o_passes);
+  out->meta = reinterpret_cast<int64_t*>(base + o_meta);
+  out->u_cum = reinterpret_cast<int64_t*>(base + o_cum);
+  out->u_tile = reinterpret_cast<int64_t*>(base + o_tile);
+  out->u_slot = reinterpret_cast<int32_t*>(base + o_slot);
+  out->cta_tile_base = reinterpret_cast<int64_t*>(base + o_base);
+  out->tile_row = reinterpret_cast<int32_t*>(base + o_row);
+  out->tile_mask = reinterpret_cast<uint32_t*>(base + o_mask);
+  out->tile_first = reinterpret_cast<int32_t*>(base + o_first);
+  FLMR_CUDA(cudaMemsetAsync(out->allow, 0, static_cast<size_t>(nqc) * out->words * 4, st));
+  // pageable source: staged by the call, so the vector may go before the copy runs
+  FLMR_CUDA(cudaMemcpyAsync(out->d_passes, out->passes.data(), n_p * sizeof(ListedPass), cudaMemcpyHostToDevice, st));
+  const int64_t n_entries = la.h_off[c0 + nqc] - la.h_off[c0];
+  if (n_entries > 0) {
+    flmr_listed_mark_kernel<<<static_cast<unsigned>((n_entries + 255) / 256), 256, 0, st>>>(
+        la.d_pids, la.d_off + c0, nqc, c->d_slot_pid, ns, c->pid_base, c->n_passages, out->words, out->allow);
+    FLMR_CUDA(cudaGetLastError());
+    ++g_launches;
+  }
+  flmr_listed_plan_kernel<<<n_p, kPlanThreads, 0, st>>>(out->d_passes, out->allow, out->words, c->d_poff, c->n_ctas,
+                                                         out->u_slot, out->u_cum, out->u_tile, out->cta_tile_base,
+                                                         out->tile_row, out->tile_mask, out->tile_first, out->meta);
+  FLMR_CUDA(cudaGetLastError());
+  ++g_launches;
+  return FLMR_OK;
+}
+
 // Shared driver of flmr_maxsim_scores / flmr_maxsim_topk (and their _allowed forms: `allow` null = unrestricted,
-// else query b's bitmap starts at allow + b * allow_stride).
+// else query b's bitmap starts at allow + b * allow_stride; and their _listed forms: `listed` non-null, `allow` null).
 int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_queries, int nq,
                unsigned flags, int k, const uint32_t* allow, int64_t allow_stride, float* d_all_scores,
-               float* d_topk_scores, int64_t* d_topk_pids, cudaStream_t st) {
+               float* d_topk_scores, int64_t* d_topk_pids, cudaStream_t st, const ListedArgs* listed = nullptr) {
   if (!c || !ws || !d_q) return fail(FLMR_ERR_INVALID_ARG, "null corpus / workspace / query pointer");
   if (ws->corpus != c) return fail(FLMR_ERR_INVALID_ARG, "workspace belongs to a different corpus");
   if (n_queries < 0 || nq <= 0) return fail(FLMR_ERR_INVALID_ARG, "bad n_queries=%d nq=%d", n_queries, nq);
@@ -1347,7 +1663,7 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
     allow = slot_allow;
     allow_stride = allow_stride ? words : 0;
   }
-  if (compacted && d_all_scores &&
+  if ((compacted || listed) && d_all_scores &&
       (rc = scratch.alloc(&d_slot_scores,
                           static_cast<size_t>(std::min(ws->max_queries, n_queries)) * ns * sizeof(float))))
     return rc;
@@ -1399,6 +1715,8 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
     if (!d_all_c && nq > kRbMax * 32 && (rc = ensure_acc(ws, static_cast<int64_t>(group) * ns)))
       return rc;
     p.cand_q_stride = nqc;
+    ListedChunkPlan lp;
+    if (listed && (rc = plan_listed_chunk(c, ws, plan, c0, nqc, *listed, st, &lp))) return rc;
     slot.assign(plan.size(), 0);
     size_t staged_until = 0;                    // passes [0, staged_until) have their queries staged
     for (size_t pi = 0; pi < plan.size(); ++pi) {
@@ -1433,9 +1751,28 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
       p.cand_q_first = pp.q_first;
       p.allow = allow ? allow + static_cast<int64_t>(c0 + pp.q_first) * allow_stride : nullptr;
       p.allow_stride = allow_stride;
-      if ((rc = launch_scan(c, ws, p, (pp.flags & kPassPair) != 0, st))) return rc;
+      if (listed) {   // the pass's plan, and its queries' slot bitmaps
+        const ListedPass& lpp = lp.passes[pi];
+        p.cta_row_begin = nullptr;
+        p.cta_tile_base = lp.cta_tile_base + lpp.c_off;
+        p.tile_end_mask = lp.tile_mask + lpp.t_off;
+        p.tile_first_pid = lp.tile_first + lpp.t_off;
+        p.tile_row = lp.tile_row + lpp.t_off;
+        p.allow = lp.allow + static_cast<int64_t>(pp.q_first) * lp.words;
+        p.allow_stride = lp.words;
+      }
+      if ((rc = launch_scan(c, ws, p, (pp.flags & kPassPair) != 0, st, listed != nullptr))) return rc;
     }
-    if (d_slot_scores) {
+    if (listed && d_slot_scores) {
+      const int64_t n = listed->h_off[c0 + nqc] - listed->h_off[c0];
+      if (n > 0) {
+        flmr_listed_scores_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
+            listed->d_pids, listed->d_off + c0, nqc, c->d_slot_pid, ns, c->pid_base, c->n_passages, d_slot_scores,
+            listed->d_scores);
+        FLMR_CUDA(cudaGetLastError());
+        ++g_launches;
+      }
+    } else if (d_slot_scores) {
       const int64_t n = static_cast<int64_t>(nqc) * c->n_passages;
       flmr_expand_slot_scores_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
           d_slot_scores, ns, c->d_slot_pid, c->pid_base, c->n_passages, nqc,
@@ -1472,6 +1809,8 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
     if ((rc = dev_upload(&c->d_doclen, lens, &c->hbm_bytes))) return bail(rc);
     c->h_poff = poff;
     c->h_doclen.swap(lens);
+    c->max_rows = 0;
+    for (int64_t s = 0; s < n_passages; ++s) c->max_rows = std::max(c->max_rows, poff[s + 1] - poff[s]);
     c->sm_total = sm_count;
   }
 
@@ -1541,6 +1880,25 @@ int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_
                                          ScanSmem::kBytes)
                   : cudaFuncSetAttribute(flmr_scan_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          ScanSmem::kBytes);
+    if (e1 != cudaSuccess)
+      return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
+                       ScanSmem::kBytes, cudaGetErrorString(e1)));
+  }
+  {  // the plan-mode kernels of this storage (listed searches)
+    cudaError_t e1 = cudaSuccess;
+    auto set = [&](const void* fn) {
+      if (e1 == cudaSuccess) e1 = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes);
+    };
+    if (c->f16) {
+      set(reinterpret_cast<const void*>(flmr_scan_listed_f16_kernel));
+      set(reinterpret_cast<const void*>(flmr_scan_listed_split_f16_kernel));
+    } else if (c->fp8) {
+      set(reinterpret_cast<const void*>(flmr_scan_listed_kernel<true>));
+      set(reinterpret_cast<const void*>(flmr_scan_listed_split_kernel<true>));
+    } else {
+      set(reinterpret_cast<const void*>(flmr_scan_listed_kernel<false>));
+      set(reinterpret_cast<const void*>(flmr_scan_listed_split_kernel<false>));
+    }
     if (e1 != cudaSuccess)
       return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
                        ScanSmem::kBytes, cudaGetErrorString(e1)));
@@ -2450,6 +2808,7 @@ int flmr_workspace_destroy(flmr_workspace_t* ws) {
   cudaFree(ws->d_qpad);
   cudaFree(ws->d_cand_keys);
   cudaFree(ws->d_acc);
+  cudaFree(ws->d_plan);
   if (ws->h_status) cudaFreeHost(ws->h_status);
   delete ws;
   return FLMR_OK;
@@ -2488,6 +2847,113 @@ int flmr_maxsim_topk_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, 
   if (k < 1) return fail(FLMR_ERR_INVALID_ARG, "k=%d must be >= 1", k);
   return run_search(corpus, ws, d_q, n_queries, nq, flags, k, d_allow, allow_stride_words, nullptr, d_out_scores,
                     d_out_pids, static_cast<cudaStream_t>(stream));
+}
+
+extern "C++" {
+namespace {
+// Checks a listed call's lists and runs it: the offsets go to the device (stream-ordered scratch), then run_search.
+int run_listed(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_queries, int nq, unsigned flags,
+               int k, const int64_t* h_off, const int64_t* d_pids, float* d_scores, float* d_topk_scores,
+               int64_t* d_topk_pids, cudaStream_t st) {
+  if (!c || !ws) return fail(FLMR_ERR_INVALID_ARG, "null corpus / workspace");
+  if (n_queries < 0) return fail(FLMR_ERR_INVALID_ARG, "bad n_queries=%d", n_queries);
+  if (!h_off) return fail(FLMR_ERR_INVALID_ARG, "h_list_offsets is null");
+  if (h_off[0] < 0) return fail(FLMR_ERR_INVALID_ARG, "h_list_offsets[0] = %lld < 0", (long long)h_off[0]);
+  for (int b = 0; b < n_queries; ++b)
+    if (h_off[b + 1] < h_off[b])
+      return fail(FLMR_ERR_INVALID_ARG, "h_list_offsets decreases at query %d", b);
+  if (h_off[n_queries] > h_off[0] && !d_pids) return fail(FLMR_ERR_INVALID_ARG, "d_list_pids is null");
+  if (g_scan_variant == 3 || g_scan_variant == 4)
+    return fail(FLMR_ERR_UNSUPPORTED, "scan variant %d has no plan-mode (listed) kernel", g_scan_variant);
+  if (n_queries == 0) return FLMR_OK;
+  DeviceGuard guard(c->device);
+  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
+  StreamScratch scratch(st);
+  int64_t* d_off = nullptr;
+  if (int rc = scratch.alloc(&d_off, (n_queries + 1) * sizeof(int64_t))) return rc;
+  FLMR_CUDA(cudaMemcpyAsync(d_off, h_off, (n_queries + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  const ListedArgs la{h_off, d_off, d_pids, d_scores};
+  return run_search(c, ws, d_q, n_queries, nq, flags, k, nullptr, 0, d_scores, d_topk_scores, d_topk_pids, st, &la);
+}
+}  // namespace
+}
+
+int flmr_maxsim_topk_listed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries, int nq,
+                            int k, unsigned flags, const int64_t* h_list_offsets, const int64_t* d_list_pids,
+                            float* d_out_scores, int64_t* d_out_pids, void* stream) {
+  if (!d_out_scores || !d_out_pids) return fail(FLMR_ERR_INVALID_ARG, "output pointer is null");
+  if (k < 1) return fail(FLMR_ERR_INVALID_ARG, "k=%d must be >= 1", k);
+  return run_listed(corpus, ws, d_q, n_queries, nq, flags, k, h_list_offsets, d_list_pids, nullptr, d_out_scores,
+                    d_out_pids, static_cast<cudaStream_t>(stream));
+}
+
+int flmr_maxsim_scores_listed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, const void* d_q, int n_queries,
+                              int nq, unsigned flags, const int64_t* h_list_offsets, const int64_t* d_list_pids,
+                              float* d_out_scores, void* stream) {
+  if (!d_out_scores) return fail(FLMR_ERR_INVALID_ARG, "d_out_scores is null");
+  return run_listed(corpus, ws, d_q, n_queries, nq, flags, 0, h_list_offsets, d_list_pids, d_out_scores, nullptr,
+                    nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int flmr_debug_listed_plan(const flmr_corpus_t* c, flmr_workspace_t* ws, int n_queries, int nq,
+                           const int64_t* h_list_offsets, const int64_t* d_list_pids, int64_t* h_out,
+                           int64_t capacity, int64_t* n_out) {
+  if (!c || !ws || !h_list_offsets || !n_out || n_queries < 1 || nq < 1)
+    return fail(FLMR_ERR_INVALID_ARG, "bad argument");
+  if (ws->corpus != c) return fail(FLMR_ERR_INVALID_ARG, "workspace belongs to a different corpus");
+  if (n_queries > ws->max_queries)
+    return fail(FLMR_ERR_INVALID_ARG, "n_queries=%d > the workspace's max_queries=%d", n_queries, ws->max_queries);
+  for (int b = 0; b < n_queries; ++b)
+    if (h_list_offsets[b + 1] < h_list_offsets[b] || h_list_offsets[b] < 0)
+      return fail(FLMR_ERR_INVALID_ARG, "bad h_list_offsets at query %d", b);
+  DeviceGuard guard(c->device);
+  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
+  cudaStream_t st = nullptr;
+  std::vector<PassPlan> plan;
+  int group = 1;
+  plan_passes(n_queries, nq, false, &plan, &group, nullptr);
+  int64_t* d_off = nullptr;
+  FLMR_CUDA(cudaMalloc(&d_off, (n_queries + 1) * sizeof(int64_t)));
+  FLMR_CUDA(cudaMemcpy(d_off, h_list_offsets, (n_queries + 1) * sizeof(int64_t), cudaMemcpyHostToDevice));
+  const ListedArgs la{h_list_offsets, d_off, d_list_pids, nullptr};
+  ListedChunkPlan lp;
+  int rc = plan_listed_chunk(c, ws, plan, 0, n_queries, la, st, &lp);
+  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = fail(FLMR_ERR_CUDA, "planner failed");
+  cudaFree(d_off);
+  if (rc) return rc;
+  // per pass: q_first, n_q, n_ctas, union size, tiles, tile bound, the union's slots, cta_tile_base [n_ctas + 1],
+  // then per tile its start row, end mask and first slot
+  const int n_p = static_cast<int>(plan.size());
+  std::vector<int64_t> meta(2 * n_p), out{n_p};
+  FLMR_CUDA(cudaMemcpy(meta.data(), lp.meta, meta.size() * 8, cudaMemcpyDeviceToHost));
+  for (int i = 0; i < n_p; ++i) {
+    const ListedPass& q = lp.passes[i];
+    const int64_t nu = meta[2 * i], nt = meta[2 * i + 1];
+    if (nt > lp.t_bound[i] || nu > lp.u_bound[i])
+      return fail(FLMR_ERR_KERNEL, "pass %d: plan of %lld tiles exceeds its bound %lld", i, (long long)nt,
+                  (long long)lp.t_bound[i]);
+    out.insert(out.end(), {q.q_first, q.n_q, c->n_ctas, nu, nt, lp.t_bound[i]});
+    std::vector<int32_t> slots_(nu), row(nt), first(nt);
+    std::vector<int64_t> base(c->n_ctas + 1);
+    std::vector<uint32_t> mask(nt);
+    FLMR_CUDA(cudaMemcpy(slots_.data(), lp.u_slot + q.u_off, nu * 4, cudaMemcpyDeviceToHost));
+    FLMR_CUDA(cudaMemcpy(base.data(), lp.cta_tile_base + q.c_off, base.size() * 8, cudaMemcpyDeviceToHost));
+    FLMR_CUDA(cudaMemcpy(row.data(), lp.tile_row + q.t_off, nt * 4, cudaMemcpyDeviceToHost));
+    FLMR_CUDA(cudaMemcpy(mask.data(), lp.tile_mask + q.t_off, nt * 4, cudaMemcpyDeviceToHost));
+    FLMR_CUDA(cudaMemcpy(first.data(), lp.tile_first + q.t_off, nt * 4, cudaMemcpyDeviceToHost));
+    out.insert(out.end(), slots_.begin(), slots_.end());
+    out.insert(out.end(), base.begin(), base.end());
+    out.insert(out.end(), row.begin(), row.end());
+    out.insert(out.end(), mask.begin(), mask.end());
+    out.insert(out.end(), first.begin(), first.end());
+  }
+  *n_out = static_cast<int64_t>(out.size());
+  if (h_out) {
+    if (static_cast<int64_t>(out.size()) > capacity)
+      return fail(FLMR_ERR_INVALID_ARG, "capacity %lld < %zu", (long long)capacity, out.size());
+    std::copy(out.begin(), out.end(), h_out);
+  }
+  return FLMR_OK;
 }
 
 int flmr_topk_merge(const float* d_in_scores, const int64_t* d_in_pids, int n_lists, int n_queries,

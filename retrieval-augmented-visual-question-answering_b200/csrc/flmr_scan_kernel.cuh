@@ -103,7 +103,15 @@ struct ScanParams {
   int32_t cand_q_stride;           // queries of the whole call chunk (one merge launch serves them all)
   int32_t cand_q_first;            // index of this pass's first query inside the chunk
   int* status;                     // mapped pinned host word: watchdog code of a trapped launch
+  // plan mode (the listed kernels): the tile arrays above are a per-call plan over the listed passages' rows only, and
+  // tile i starts at stored row tile_row[i] instead of cta_row_begin + 96 t (null for the partition kernels)
+  const int32_t* tile_row;
 };
+
+// Plan mode: bit 31 of a tile's end mask marks a tile that starts a run of listed passages or a CTA's share of one.
+// The passage open at such a tile's start is a new one, whatever the CTA's previous tile folded, so the consumers
+// reset their running maxima there; the end groups proper stay in bits 0 .. kSlots - 1.
+constexpr uint32_t kTileRunStart = 1u << 31;
 
 struct ScanSmem {
   static constexpr int kOffQ = 0;                                     // [2 k-blocks][kMtMax * 128 rows][128 B]
@@ -358,7 +366,9 @@ constexpr bool kScanSkeleton = true;
 constexpr bool kScanSkeleton = false;
 #endif
 
-template <int NB, int kWgs, bool kPair, bool kOverlap, Elem kE>
+//
+// kPlan (the listed kernels): a tile whose mask has kTileRunStart set starts from init maxima (see kTileRunStart).
+template <int NB, int kWgs, bool kPair, bool kOverlap, Elem kE, bool kPlan = false>
 __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base, ScanBars bars,
                                               int n_tiles, int64_t tile_base, int wg, int wq, int lane) {
   using S = ScanSmem;
@@ -378,7 +388,14 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
   auto tile = [&](int t, auto kh, auto knext) {
     constexpr int kH = decltype(kh)::value;
     constexpr bool kNext = decltype(knext)::value;
-    const uint32_t mask = mask_next;
+    uint32_t mask = mask_next;
+    if constexpr (kPlan) {
+      if (mask & kTileRunStart) {
+#pragma unroll
+        for (int u = 0; u < NB; ++u) m[u][0] = m[u][1] = init;
+      }
+      mask &= ~kTileRunStart;
+    }
     const int buf = t & 1;
     float* lane_part_buf = lane_part + buf * (kFastSlots * kRbMax * kLaneStride);
     float* partial_buf = partial + buf * (kHbMax * kSlots);
@@ -460,7 +477,8 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
 // last tile is peeled.  The fold carries the open passage's maxima and the passage-end slot from half 0 to half 1 in
 // the same thread: a passage's row maxima and chunk sums are the values, in the order, of the whole-tile fold (max is
 // exact, whatever order it is taken in), and the scores bitwise those of flmr_scan_kernel.
-template <int NB, Elem kE>
+// kPlan: as scan_consumer's (the reset happens before half 0 of the tile is folded).
+template <int NB, Elem kE, bool kPlan = false>
 __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base,
                                                     ScanBars bars, int n_tiles, int64_t tile_base, int wg, int wq,
                                                     int lane) {
@@ -484,7 +502,14 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
   // tile t, entered with the MMAs of (t, 0, half 0) in flight in acc[0]; kNext: a tile t + 1 follows
   auto tile = [&](int t, auto knext) {
     constexpr bool kNext = decltype(knext)::value;
-    const uint32_t mask = mask_next;
+    uint32_t mask = mask_next;
+    if constexpr (kPlan) {
+      if (mask & kTileRunStart) {
+#pragma unroll
+        for (int u = 0; u < NB; ++u) m[u][0] = m[u][1] = init;
+      }
+      mask &= ~kTileRunStart;
+    }
     const int buf = t & 1;
     float* lane_part_buf = lane_part + buf * (kFastSlots * kRbMax * kLaneStride);
     float* partial_buf = partial + buf * (kHbMax * kSlots);
@@ -558,9 +583,17 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
 //
 // kSplit = true (flmr_scan_split_kernel, three warpgroups) runs scan_split_consumer instead of scan_consumer; the
 // producer, the reducer, the barriers and the shared-memory layout are the same code.
-template <int kWgs, bool kPair, Elem kE, bool kSplit>
+//
+// kPlan = true (the listed kernels) scans a per-call plan instead of the corpus partition: CTA c's tiles are
+// cta_tile_base[c] .. cta_tile_base[c + 1] of the plan's arrays, tile i is loaded from stored row tile_row[i], and a
+// tile with kTileRunStart set resets the consumers' running maxima.  The fold, the reducer (its tombstone and allow
+// tests drop whatever the plan's tiles cover besides the listed passages) and the top-k are the same code, so every
+// score is bitwise the one the partition kernels compute.  A CTA without tiles publishes its empty top-k lists and
+// waits on no barrier.
+template <int kWgs, bool kPair, Elem kE, bool kSplit, bool kPlan = false>
 __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, const ScanParams& p) {
   static_assert(!(kPair && kE != Elem::kBF16), "the CTA-pair kernel is bf16 only");
+  static_assert(!(kPair && kPlan), "plan mode has no CTA-pair kernel");
   constexpr bool kFp8 = kE == Elem::kE4M3;
   static_assert(!kSplit || (kWgs == 3 && !kPair), "the split consumer loop is written for three single-CTA warpgroups");
   using S = ScanSmem;
@@ -586,7 +619,7 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
 
   const ScanBars bars{smem_base + S::kOffBars};
 
-  const int32_t row_begin = p.cta_row_begin[cta];
+  const int32_t row_begin = kPlan ? 0 : p.cta_row_begin[cta];
   const int64_t tile_base = p.cta_tile_base[cta];
   const int n_tiles = static_cast<int>(p.cta_tile_base[cta + 1] - tile_base);
   const int n_mtiles = p.n_mtiles;
@@ -644,7 +677,7 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
         if (elect_one_sync()) {
           mbar_arrive_expect_tx(bars.d_full(s), d_tile_bytes<kE>());   // (pair: 12 KB from this CTA's loads + 12 KB from the peer's)
           const uint32_t dst = smem_base + S::kOffD + s * kDTileBytes;
-          const int32_t row = row_begin + t * kTileN;
+          const int32_t row = kPlan ? __ldg(p.tile_row + tile_base + t) : row_begin + t * kTileN;
           if constexpr (kPair) {   // tmap_d has a (kTileN / 2)-row box here
             const uint32_t half = pair_rank * (kTileN / 2);
             tma_load_2d_multicast(dst + half * 128, &tmap_d, bars.d_full(s), 0, row + half, 3, kPolicyEvictFirst);
@@ -677,7 +710,7 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
         fpid_next = __ldg(p.tile_first_pid + tile_base);
       }
       for (int t = 0; t < n_tiles_red; ++t) {
-        const uint32_t mask = mask_next;
+        const uint32_t mask = kPlan ? mask_next & ~kTileRunStart : mask_next;
         const int32_t first_pid = fpid_next;
         if (t + 1 < n_tiles_red) {
           mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
@@ -809,16 +842,17 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
     const int nb = wg < n_blocks ? (n_blocks - wg + kWgs - 1) / kWgs : 0;
     if constexpr (kSplit) {
       if (nb == 1) {
-        scan_split_consumer<1, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+        scan_split_consumer<1, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
       } else if (nb == 2) {
-        scan_split_consumer<2, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+        scan_split_consumer<2, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
       }
     } else if (nb == 1) {
-      scan_consumer<1, kWgs, kPair, kOverlap, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      scan_consumer<1, kWgs, kPair, kOverlap, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     } else if (nb == 2) {
-      scan_consumer<2, kWgs, kPair, kOverlap, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      scan_consumer<2, kWgs, kPair, kOverlap, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     } else if constexpr (kBlocksPerWg >= 3) {
-      if (nb == 3) scan_consumer<3, kWgs, kPair, kOverlap, kE>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+      if (nb == 3)
+        scan_consumer<3, kWgs, kPair, kOverlap, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
     }
   }
 
@@ -851,6 +885,28 @@ flmr_scan_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParam
 __global__ void __launch_bounds__(scan_threads(3), 1)
 flmr_scan_split_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
   scan_kernel_body<3, false, Elem::kF16, true>(tmap_d, p);
+}
+
+// Plan mode (flmr_maxsim_topk_listed / flmr_maxsim_scores_listed): the two kernels the product launches, over a plan
+// of the listed passages' rows (see scan_kernel_body's kPlan).  Their own names keep the partition kernels' symbols
+// and code as they were.
+template <bool kFp8>
+__global__ void __launch_bounds__(scan_threads(2), 1)
+flmr_scan_listed_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<2, false, kFp8 ? Elem::kE4M3 : Elem::kBF16, false, true>(tmap_d, p);
+}
+template <bool kFp8>
+__global__ void __launch_bounds__(scan_threads(3), 1)
+flmr_scan_listed_split_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<3, false, kFp8 ? Elem::kE4M3 : Elem::kBF16, true, true>(tmap_d, p);
+}
+__global__ void __launch_bounds__(scan_threads(2), 1)
+flmr_scan_listed_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<2, false, Elem::kF16, false, true>(tmap_d, p);
+}
+__global__ void __launch_bounds__(scan_threads(3), 1)
+flmr_scan_listed_split_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<3, false, Elem::kF16, true, true>(tmap_d, p);
 }
 
 }  // namespace flmr

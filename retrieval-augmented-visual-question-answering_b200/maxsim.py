@@ -7,6 +7,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Optional, Tuple
 
+import numpy as np
 import torch
 
 from . import _cabi
@@ -41,6 +42,42 @@ def _prep_allow(corpus: FlatCorpus, allow: Optional[torch.Tensor], B: int) -> Tu
     return allow, (words if allow.dim() == 2 else 0)
 
 
+def _prep_lists(corpus: FlatCorpus, pids, B: int) -> Tuple[np.ndarray, torch.Tensor]:
+    """(host CSR offsets int64 ``[B + 1]``, the concatenated ids on the corpus' device) of ``pids``: one sequence or
+    tensor of GLOBAL ids per query."""
+    if len(pids) != B:
+        raise ValueError("pids holds %d lists for %d queries" % (len(pids), B))
+    lists = []
+    for ids in pids:
+        if ids is None:
+            raise ValueError("pids= takes one list of ids per query (None: use maxsim_topk without pids)")
+        lists.append(torch.as_tensor(ids, dtype=torch.int64).reshape(-1))
+    off = np.zeros(B + 1, dtype=np.int64)
+    off[1:] = np.cumsum([x.numel() for x in lists])
+    flat = (torch.cat([x.to(corpus.device) for x in lists]) if off[-1] else
+            torch.empty(0, dtype=torch.int64, device=corpus.device))
+    return off, flat.contiguous()
+
+
+def maxsim_scores_listed(corpus: FlatCorpus, Q: torch.Tensor, pids, relu: bool = False) -> torch.Tensor:
+    """Scores of query b against each global id of ``pids[b]``: fp32 ``[sum of the list lengths]``, the lists'
+    entries in order (query 0's first).  The scan streams only the listed passages' rows; each score is bitwise the
+    ``maxsim_scores(..., allow=...)`` entry of the pair.  An id outside the shard, deleted or compacted away scores -inf;
+    duplicates score alike."""
+    Qd = _prep_queries(corpus, Q)
+    B, nq = Qd.size(0), Qd.size(1)
+    off, flat = _prep_lists(corpus, pids, B)
+    out = torch.empty(int(off[-1]), dtype=torch.float32, device=corpus.device)
+    if B == 0 or out.numel() == 0:
+        return out
+    with torch.cuda.device(corpus.device):
+        _cabi.check(_cabi.lib().flmr_maxsim_scores_listed(
+            corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq, _cabi.FLAG_RELU if relu else 0,
+            off.ctypes.data_as(C.c_void_p), C.c_void_p(flat.data_ptr()), C.c_void_p(out.data_ptr()),
+            _stream(corpus)))
+    return out
+
+
 def maxsim_scores(corpus: FlatCorpus, Q: torch.Tensor, relu: bool = False,
                   out: Optional[torch.Tensor] = None, allow: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``out[b, p] = sum_i max_j <Q[b,i], D_p[j]>`` for every passage of the shard (fp32, on GPU).
@@ -70,23 +107,34 @@ def maxsim_scores(corpus: FlatCorpus, Q: torch.Tensor, relu: bool = False,
 
 
 def maxsim_topk(corpus: FlatCorpus, Q: torch.Tensor, k: int, relu: bool = False,
-                allow: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                allow: Optional[torch.Tensor] = None, pids=None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Fused scan + top-k: ``(scores fp32 [B,k], pids int64 [B,k])`` sorted by descending score.
 
     ``allow`` (see ``maxsim_scores``): query b ranks only its allowed live passages; a list with fewer than k of them
-    is filled with (-inf, -1)."""
+    is filled with (-inf, -1).  ``pids`` (one sequence or tensor of GLOBAL ids per query, in any order, duplicates and
+    ids outside the shard allowed) restricts query b to the ids ``pids[b]`` at the cost of those passages: the scan
+    streams only their rows.  The result is bitwise that of ``allow=allow_bitmaps(pids, ...)``."""
     if not 1 <= k <= _cabi.MAX_K:
         raise ValueError("k=%d outside [1, %d]" % (k, _cabi.MAX_K))
+    if allow is not None and pids is not None:
+        raise ValueError("pass allow= or pids=, not both")
     Qd = _prep_queries(corpus, Q)
     B, nq = Qd.size(0), Qd.size(1)
     allow, stride = _prep_allow(corpus, allow, B)
+    lists = _prep_lists(corpus, pids, B) if pids is not None else None
     scores = torch.empty((B, k), dtype=torch.float32, device=corpus.device)
     pids = torch.empty((B, k), dtype=torch.int64, device=corpus.device)
     if B == 0:
         return scores, pids
     with torch.cuda.device(corpus.device):
         flags = _cabi.FLAG_RELU if relu else 0
-        if allow is None:
+        if lists is not None:
+            off, flat = lists
+            _cabi.check(_cabi.lib().flmr_maxsim_topk_listed(
+                corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq, k, flags,
+                off.ctypes.data_as(C.c_void_p), C.c_void_p(flat.data_ptr()), C.c_void_p(scores.data_ptr()),
+                C.c_void_p(pids.data_ptr()), _stream(corpus)))
+        elif allow is None:
             _cabi.check(_cabi.lib().flmr_maxsim_topk(
                 corpus.handle, corpus.workspace(), C.c_void_p(Qd.data_ptr()), B, nq, k, flags,
                 C.c_void_p(scores.data_ptr()), C.c_void_p(pids.data_ptr()), _stream(corpus)))
@@ -254,6 +302,31 @@ def maxsim_backward(Q: torch.Tensor, D_padded: torch.Tensor, arg: torch.Tensor, 
             C.c_void_p(dd.data_ptr() if need_dd else None), int(Qb.device.index),
             C.c_void_p(torch.cuda.current_stream(Qb.device).cuda_stream)))
     return dq, dd
+
+
+def debug_listed_plan(corpus: FlatCorpus, n_queries: int, nq: int, pids) -> list:
+    """Test infrastructure: the plans ``maxsim_topk(..., pids=pids)`` scans for ``n_queries`` queries of ``nq`` tokens
+    (``flmr_debug_listed_plan``), one dict per pass: ``q_first``, ``n_q``, ``n_ctas``, ``tile_bound``, ``slots`` (the
+    union of the pass's listed slots), ``cta_tile_base``, ``tile_row``, ``tile_mask``, ``tile_first`` (numpy)."""
+    off, flat = _prep_lists(corpus, pids, n_queries)
+    n = C.c_int64(0)
+    L = _cabi.lib()
+    args = (corpus.handle, corpus.workspace(), n_queries, nq, off.ctypes.data_as(C.c_void_p), C.c_void_p(flat.data_ptr()))
+    with torch.cuda.device(corpus.device):
+        _cabi.check(L.flmr_debug_listed_plan(*args, None, 0, C.byref(n)))
+        buf = np.zeros(n.value, dtype=np.int64)
+        _cabi.check(L.flmr_debug_listed_plan(*args, buf.ctypes.data_as(C.c_void_p), n.value, C.byref(n)))
+    out, at = [], 1
+    for _ in range(int(buf[0])):
+        q_first, n_q, n_ctas, nu, nt, bound = (int(x) for x in buf[at:at + 6])
+        at += 6
+        d = {"q_first": q_first, "n_q": n_q, "n_ctas": n_ctas, "tile_bound": bound}
+        for name, size in (("slots", nu), ("cta_tile_base", n_ctas + 1), ("tile_row", nt), ("tile_mask", nt),
+                           ("tile_first", nt)):
+            d[name] = buf[at:at + size].copy()
+            at += size
+        out.append(d)
+    return out
 
 
 def debug_scores_simt(corpus: FlatCorpus, Q: torch.Tensor, relu: bool = False) -> torch.Tensor:

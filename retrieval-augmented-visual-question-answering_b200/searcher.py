@@ -35,16 +35,23 @@ import json
 import os
 from typing import Callable, Dict, List, Optional, Tuple, Union
 
+import numpy as np
 import torch
 
 from . import _cabi
 from .corpus import FlatCorpus, allow_bitmaps
 from .index_io import FORMATS as FLAT_FORMATS
 from .infra import ColBERTConfig, active_run_config, resolve_index_path
-from .maxsim import maxsim_argmax_grouped, maxsim_scores, maxsim_topk, topk_select
+from .maxsim import maxsim_argmax_grouped, maxsim_scores, maxsim_scores_listed, maxsim_topk, topk_select
 
 # bytes of gathered bf16 candidate tokens one re-rank launch may hold: larger batches are split by queries
 RERANK_GATHER_BYTES = 1 << 30
+
+# A restricted search scans a plan of its listed passages' rows (maxsim_topk(pids=)) while those rows are at most this
+# fraction of the rows its bitmap scan streams (the shard's rows once per scan pass), and tests bitmaps in a full scan
+# above it.  tools/listed_scan_probe.py brackets the crossover between 0.12 and 1.2 of this measure on an H100
+# (profiles/r09_listed_scan_probe.md).
+LISTED_SCAN_MAX_ROW_FRACTION = 0.5
 
 
 def _default_knobs(k: int) -> Tuple[int, float, int]:
@@ -458,7 +465,18 @@ class Searcher:
         if corpus is not None:
             for b0 in range(0, B, self.query_batch):
                 Qb = Q[b0:b0 + self.query_batch]
-                allow = corpus.allow_bitmaps(lists[b0:b0 + self.query_batch])     # built on the device
+                lb = lists[b0:b0 + self.query_batch]
+                if self._listed_is_cheaper(Qb, lb):
+                    # the scan streams the listed passages' rows only; on the C-level sharded path the exchange that
+                    # flmr_maxsim_topk_sharded_allowed would make follows, so every rank makes the same collectives
+                    s_, p_ = self._listed_topk(Qb, k, lb)
+                    if c_level:
+                        s_ = torch.cat([s_, s_.new_full((s_.size(0), k - s_.size(1)), float("-inf"))], dim=1)
+                        p_ = torch.cat([p_, p_.new_full((p_.size(0), k - p_.size(1)), -1)], dim=1)
+                        s_, p_ = self._nccl.exchange(s_, p_, k)
+                    parts.append((s_, p_))
+                    continue
+                allow = corpus.allow_bitmaps(lb)     # built on the device
                 if c_level:
                     parts.append(self._nccl.search(corpus, Qb, k, relu=self._relu, allow=allow))
                 else:
@@ -480,6 +498,86 @@ class Searcher:
             s, p = torch.cat([m[0] for m in merged]), torch.cat([m[1] for m in merged])
         n_valid = int((p >= 0).sum(dim=1).max()) if p.numel() else 0
         return s[:, :n_valid], p[:, :n_valid]
+
+    def _listed_is_cheaper(self, Q: torch.Tensor, lists: List) -> bool:
+        """Whether a batch's restricted search takes the listed scan: every query has a list, and the rows of the
+        listed passages of this shard are at most LISTED_SCAN_MAX_ROW_FRACTION of what the bitmap scan streams (the
+        shard's rows once per scan pass; a pass holds up to 12 queries of at most 32 tokens, fewer of longer ones)."""
+        corpus = self.corpus
+        if corpus is None or any(ids is None for ids in lists):
+            return False
+        rbq = (Q.size(1) + 31) // 32
+        per_pass = max(1, min(12, 12 // rbq)) if rbq <= 12 else 1
+        n_passes = (len(lists) + per_pass - 1) // per_pass
+        rows = 0
+        for ids in lists:
+            local = ids.cpu().numpy() - corpus.pid_base
+            local = local[(local >= 0) & (local < corpus.n_passages)]
+            rows += int(((corpus.doclens[local].astype(np.int64) + 3) // 4 * 4).sum())
+        return rows <= LISTED_SCAN_MAX_ROW_FRACTION * n_passes * int(corpus.info.n_rows)
+
+    def _listed_scores(self, Q: torch.Tensor, lists: List) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(scores fp32 ``[B, w]``, global ids ``[B, w]``) of each query against its listed passages of this shard,
+        each list made sorted and unique and padded with (-inf, -1) to the longest (``maxsim_scores_listed``)."""
+        corpus = self.corpus
+        uniq = []
+        for ids in lists:
+            ids = torch.unique(ids.cpu())
+            uniq.append(ids[(ids >= corpus.pid_base) & (ids < corpus.pid_base + corpus.n_passages)])
+        lens = torch.tensor([len(x) for x in uniq], dtype=torch.int64)
+        B, w = len(uniq), int(lens.max()) if len(uniq) else 0
+        flat = torch.cat(uniq).to(corpus.device) if w else torch.empty(0, dtype=torch.int64, device=corpus.device)
+        sc = maxsim_scores_listed(corpus, Q, uniq, relu=self._relu)
+        rows = torch.repeat_interleave(torch.arange(B), lens).to(corpus.device)
+        cols = (torch.arange(int(lens.sum())) - torch.repeat_interleave(torch.cumsum(lens, 0) - lens, lens))
+        cols = cols.to(corpus.device)
+        s = torch.full((B, w), float("-inf"), dtype=torch.float32, device=corpus.device)
+        p = torch.full((B, w), -1, dtype=torch.int64, device=corpus.device)
+        s[rows, cols] = sc
+        p[rows, cols] = flat
+        return s, p
+
+    def _listed_topk(self, Q: torch.Tensor, k: int, lists: List) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``_allowed_topk`` for queries restricted to id lists, on the listed scan: the same (scores, global pids)."""
+        corpus = self.corpus
+        kq = min(k, _n_live(corpus))
+        n_allowed = None
+        if self.storage == "fp8" and kq > 0:
+            dead = set(corpus.deleted_pids().tolist()) if hasattr(corpus, "deleted_pids") else set()
+            lo, hi = corpus.pid_base, corpus.pid_base + corpus.n_passages
+            n_allowed = max([len([i for i in set(ids.cpu().tolist()) if lo <= i < hi and i not in dead])
+                             for ids in lists], default=0)
+            kq = min(kq, n_allowed)
+        if kq == 0:
+            return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=corpus.device),
+                    torch.empty((Q.size(0), 0), dtype=torch.int64, device=corpus.device))
+        if self.storage != "fp8" and kq <= _cabi.MAX_K:
+            return maxsim_topk(corpus, Q, kq, relu=self._relu, pids=lists)
+        if self.storage == "fp8":
+            depth = shortlist_depth(kq, getattr(self.config, "ndocs", None), n_allowed)
+            self._last_depth = depth
+            Qb = Q.to(corpus.device).to(torch.bfloat16)
+            s, ids = self._listed_scores(Qb, lists)
+            vals, col = topk_select(s, depth)
+            # a -inf e4m3 score is a deleted passage or padding: it never reaches the exact re-rank
+            cand = torch.where(vals == float("-inf"), -1, ids.gather(1, col.clamp_min(0)))
+            cand = torch.sort(cand, dim=1).values        # pid order: the select below breaks exact ties by lower pid
+            exact = self._exact_scores(Qb, cand).masked_fill(cand < 0, float("-inf"))
+            vals, col = topk_select(exact, kq)
+            pids = cand.gather(1, col)
+        else:
+            s, ids = self._listed_scores(Q, lists)
+            if s.size(1) < kq:                           # fewer listed passages than kq in every row
+                pad = kq - s.size(1)
+                s = torch.cat([s, s.new_full((s.size(0), pad), float("-inf"))], dim=1)
+                ids = torch.cat([ids, ids.new_full((ids.size(0), pad), -1)], dim=1)
+            if kq <= _cabi.SELECT_MAX_K:
+                vals, col = topk_select(s, kq)           # ids ascend along a row: ties go to the lower id
+            else:
+                vals, col = torch.sort(s, dim=1, descending=True, stable=True)
+                vals, col = vals[:, :kq], col[:, :kq]
+            pids = ids.gather(1, col.clamp_min(0))
+        return vals, pids.masked_fill(vals == float("-inf"), -1)
 
     def _allowed_topk(self, Q: torch.Tensor, k: int, allow: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         """Top-k of this shard for queries restricted by ``allow`` (``[B, words]``): (scores, global pids)
