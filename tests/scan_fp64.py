@@ -141,6 +141,25 @@ def check_topk(scores, ts, tp, s64, bound, k, tag):
         assert (hi[b][ids[:-1]] >= lo[b][ids[1:]]).all(), "%s: query %d returned out of order" % (tag, b)
 
 
+def positions(tp, P, pid_base):
+    """Global ids ``tp`` (-1: empty) -> their positions in the sorted local ids ``P``; every id must be one of P."""
+    local = tp - pid_base
+    if P.numel() == 0:
+        assert (tp < 0).all(), "an id returned where none may be"
+        return torch.full_like(tp, -1)
+    pos = torch.searchsorted(P, local.clamp_min(0).contiguous())
+    hit = P[pos.clamp_max(P.numel() - 1)] == local
+    assert ((tp < 0) | hit).all(), "a returned id is deleted or not allowed"
+    return torch.where(tp >= 0, pos, -1)
+
+
+def check_topk_subset(scores, ts, tp, s64, bound, P, pid_base, k, tag):
+    """check_topk of one query whose candidates are the sorted local ids ``P`` (its allowed or listed live passages):
+    ``scores``, ``s64`` and ``bound`` are ``[len(P)]``, the kernel's scores and float64's of those candidates; ``ts`` /
+    ``tp`` the query's ``[k]`` top-k (global ids)."""
+    check_topk(scores[None], ts[None], positions(tp[None], P, pid_base), s64[None], bound[None], k, tag)
+
+
 # ---- the scan's pass plan, as the host builds it (the partition: helpers.scan_partition) ---------------------------
 def scan_plan(n_queries: int, nq: int, allow_pair: bool = False) -> np.ndarray:
     """``flmr_debug_plan_passes`` of one call chunk: rows of (q_first, n_q, row0, rows, rbq, n_mtiles, flags, slot)."""

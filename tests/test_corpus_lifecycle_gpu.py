@@ -14,6 +14,10 @@ every operation:
 7. ``Searcher`` at k 200 (select kernel) and 3000 (sort) certified by float64; on fp8 the exact re-rank's scores within
    the arg-max bound of their bf16 float64 scores, and no passage surely better than the k-th and surely inside the
    shortlist left out;
+   the listed scan (``maxsim_scores_listed``, ``maxsim_topk(pids=)`` at k 10 / 128) on the lists of 4, at Nq 32 and,
+   every fourth state, 320: -inf wherever the model has no live passage, within the scan bound elsewhere, bitwise the
+   allow observations, top-k certified over each query's listed live ids; and a restricted ``Searcher`` (k 200) on
+   its listed and on its bitmap path: bitwise alike, certified (fp8: the re-rank held as above) per query;
 8. every call repeated gives bitwise the same answer, and every observation right after a compaction (effective, no-op
    or refused) is bitwise what it was just before.
 
@@ -71,16 +75,26 @@ def _same(a: dict, b: dict, tag):
             assert _eq(u, w), "%s: %s differs" % (tag, key)
 
 
-def _positions(tp, P, pid_base):
-    """Global ids ``tp`` (-1: empty) -> their positions in the sorted local ids ``P``; every id must be one of P."""
-    local = tp - pid_base
-    if P.numel() == 0:
-        assert (tp < 0).all(), "an id returned where none may be"
-        return torch.full_like(tp, -1)
-    pos = torch.searchsorted(P, local.clamp_min(0).contiguous())
-    hit = P[pos.clamp_max(P.numel() - 1)] == local
-    assert ((tp < 0) | hit).all(), "a returned id is deleted or not allowed"
-    return torch.where(tp >= 0, pos, -1)
+_positions = S.positions
+
+
+SEARCHER_LISTED_K = 200     # a restricted Searcher's k: past the fused top-k, through the select kernel
+
+
+def _ranking_tensors(rk, B, k):
+    """A Ranking's dict (qid -> [(pid, rank, score)]) as (scores, pids) ``[B, k]``, padded with (-inf, -1)."""
+    s = torch.full((B, k), -torch.inf, device="cuda")
+    p = torch.full((B, k), -1, dtype=torch.int64, device="cuda")
+    for b in range(B):
+        hits = rk.get(b, [])
+        if hits:
+            p[b, :len(hits)] = torch.tensor([h[0] for h in hits])
+            s[b, :len(hits)] = torch.tensor([h[2] for h in hits], dtype=torch.float32)
+    return s, p
+
+
+def _same_pair(a, b):
+    return _eq(a[0], b[0]) and _eq(a[1], b[1])
 
 
 def _pad(s, p, k):
@@ -230,6 +244,23 @@ class Sequence:
         return {"lists": lists, "heavy": self.state % HEAVY_EVERY == 0, "gather": ids,
                 "nd_max": int(m.lens[local].max())}
 
+    def _searcher_lists(self):
+        """inp["lists"] without the ids a Searcher refuses (below 0, or past the index)."""
+        end = self.m.pid_base + self.m.n_passages
+        return [ids[(ids >= 0) & (ids < end)] for ids in self.inp["lists"]]
+
+    def _listed_sets(self, lists):
+        """(query of each entry, local id of each entry clipped into the shard, live mask of the entries, the sorted
+        live local ids of each query) of per-query id lists."""
+        m = self.m
+        q = np.repeat(np.arange(len(lists)), [len(x) for x in lists])
+        local = np.concatenate(lists).astype(np.int64) - m.pid_base
+        live = (local >= 0) & (local < m.n_passages)
+        live[live] = ~m.deleted[local[live]]
+        sets = [torch.from_numpy(np.unique(local[(q == b) & live])).cuda() for b in range(len(lists))]
+        return (torch.from_numpy(q).cuda(), torch.from_numpy(np.clip(local, 0, m.n_passages - 1)).cuda(),
+                torch.from_numpy(live).cuda(), sets)
+
     def _searcher(self):
         return self.searcher if self.updater is not None else self.R.Searcher(index=self.A)
 
@@ -249,6 +280,11 @@ class Sequence:
             out["allow", name] = R.maxsim_scores(A, Q[32], allow=bm)
             for k in (10, 128):
                 out["allow topk", name, k] = R.maxsim_topk(A, Q[32], k, allow=bm)
+        for nq in ((32, 320) if inp["heavy"] else (32,)):     # the listed scan on the same lists
+            lists = inp["lists"][:Q[nq].size(0)]
+            out["listed", nq] = R.maxsim_scores_listed(A, Q[nq], lists)
+            for k in (10, 128):
+                out["listed topk", nq, k] = R.maxsim_topk(A, Q[nq], k, pids=lists)
         out["gather"] = A.gather_padded(torch.from_numpy(inp["gather"]), inp["nd_max"])
         out["simt"] = R.debug_scores_simt(A, Q[32])
         sr = self._searcher()
@@ -256,6 +292,20 @@ class Sequence:
             out["searcher", k] = sr._search_tensors(Q[32], k)
         if self.storage == "fp8":      # the shortlist depth (none when no passage is live)
             out["depth"] = torch.tensor([sr._last_depth if self.A.n_live else 0])
+        # a restricted Searcher on the listed scan and on the bitmap scan
+        import ravqa_b200.searcher as SR
+        q2p = dict(enumerate(self._searcher_lists()))
+        keep = SR.LISTED_SCAN_MAX_ROW_FRACTION
+        try:
+            for path, frac in (("listed", float("inf")), ("bitmap", -1.0)):
+                SR.LISTED_SCAN_MAX_ROW_FRACTION = frac
+                sr._last_depth = 0
+                rk = sr._search_all_Q(list(q2p), Q[32], SEARCHER_LISTED_K, qid_to_pids=q2p).todict()
+                out["searcher listed", path] = _ranking_tensors(rk, len(q2p), SEARCHER_LISTED_K)
+                if self.storage == "fp8":
+                    out["depth listed", path] = torch.tensor([sr._last_depth])
+        finally:
+            SR.LISTED_SCAN_MAX_ROW_FRACTION = keep
         # the same calls again: bitwise the same answers
         assert _eq(R.maxsim_scores(A, Q[32]), out["scores", 32]), "scores differ on a second call"
         again = R.maxsim_topk(A, Q[32], 10)
@@ -317,6 +367,44 @@ class Sequence:
                     ts, tp = obs["allow topk", name, k]
                     S.check_topk(got[b:b + 1, Pb], ts[b:b + 1], _positions(tp[b:b + 1], Pb, m.pid_base),
                                  s64[b:b + 1, Pb], bound[b:b + 1, Pb], k, "allow %s k=%d" % (name, k))
+        # 4b. the listed scan: within the bound where the model has a live passage, -inf elsewhere, bitwise the allow
+        # observations (allowed scores are bitwise the unrestricted ones); top-k certified over the listed live ids
+        for nq in [key[1] for key in obs if key[0] == "listed"]:
+            lists = inp["lists"][:self.Q[nq].size(0)]
+            q, local, lv, sets = self._listed_sets(lists)
+            s64, bound = model[nq][:2]
+            got = obs["listed", nq]
+            assert torch.isneginf(got[~lv]).all(), "listed: an id without a live passage scores"
+            S.check_ratio(RATIOS, "listed %s" % st, (got[lv].double() - s64[q[lv], local[lv]]).abs(),
+                          bound[q[lv], local[lv]])
+            ref = obs["allow", "per query"] if nq == 32 else obs["scores", nq]
+            assert _eq(got[lv], ref[q[lv], local[lv]]), "listed scores differ from the allow observations"
+            dense = torch.full_like(ref, -torch.inf)
+            dense[q[lv], local[lv]] = got[lv]
+            for k in (10, 128):
+                ts, tp = obs["listed topk", nq, k]
+                if nq == 32:
+                    ws, wp = obs["allow topk", "per query", k]
+                    assert _eq(ts, ws) and _eq(tp, wp), "listed top-k differs from the allow observation"
+                for b, Pb in enumerate(sets):
+                    S.check_topk_subset(dense[b, Pb], ts[b], tp[b], s64[b, Pb], bound[b, Pb], Pb, m.pid_base, k,
+                                        "listed nq=%d k=%d" % (nq, k))
+        # the restricted Searcher: both paths alike, certified over each query's listed live ids
+        s64, bound = model[32][:2]
+        assert _same_pair(obs["searcher listed", "listed"], obs["searcher listed", "bitmap"]), \
+            "the Searcher's listed and bitmap paths differ"
+        _, _, _, sets = self._listed_sets(self._searcher_lists())
+        s, p = obs["searcher listed", "listed"]
+        k = SEARCHER_LISTED_K
+        for b, Pb in enumerate(sets):
+            n_b = int((p[b] >= 0).sum())
+            assert n_b == min(k, Pb.numel()), "restricted Searcher: %d hits of %d" % (n_b, Pb.numel())
+            if st != "fp8":
+                S.check_topk_subset(plain[b, Pb], s[b], p[b], s64[b, Pb], bound[b, Pb], Pb, m.pid_base, k,
+                                    "restricted searcher")
+            else:
+                self._check_fp8_searcher((s[b:b + 1, :n_b], p[b:b + 1, :n_b]), int(obs["depth listed", "listed"][0]),
+                                         k, s64, bound, Pb, row=b)
         # 5. gather, bitwise
         D, mask = obs["gather"]
         Dm, mm = m.gather(inp["gather"], inp["nd_max"])
@@ -338,22 +426,27 @@ class Sequence:
         else:
             self._check_fp8_searcher(obs["searcher", 200], int(obs["depth"][0]), 200, s64, bound, P)
 
-    def _check_fp8_searcher(self, result, depth, k, s8, b8, P):
+    def _check_fp8_searcher(self, result, depth, k, s8, b8, P, row=None):
         """The exact re-rank: scores within the arg-max bound of float64 over the bf16 rows, in order, and no passage
-        that surely beats the k-th returned one while surely inside the shortlist left out."""
+        that surely beats the k-th returned one while surely inside the shortlist left out.  ``row``: the result is
+        query ``row``'s alone, over its candidates P (a restricted search), at the depth the search reported."""
         m = self.m
         s, p = result
-        kq = min(k, m.n_live)
+        Q = self.Q[32]
+        if row is not None:
+            Q, s8, b8 = Q[row:row + 1], s8[row:row + 1], b8[row:row + 1]
+        kq = min(k, m.n_live if row is None else P.numel())
         assert s.size(1) == kq and (p >= 0).all()
         if kq == 0:
             return
-        e64, eamax, erabs = m.exact_scores(self.Q[32])
-        ebound = C_BOUND * U * eamax + self.Q[32].size(1) * U * erabs
+        e64, eamax, erabs = m.exact_scores(Q)
+        ebound = C_BOUND * U * eamax + Q.size(1) * U * erabs
         local = p - m.pid_base
         assert torch.from_numpy(~m.deleted).cuda()[local].all(), "fp8 searcher returned a deleted id"
         S.check_ratio(RATIOS, "searcher fp8 exact", (s.double() - e64.gather(1, local)).abs(), ebound.gather(1, local))
         assert (s[:, :-1] >= s[:, 1:]).all(), "fp8 searcher out of order"
-        assert depth == min(max(k, 1024), 2048, m.n_live)
+        if row is None:
+            assert depth == min(max(k, 1024), 2048, m.n_live)
         lo8, hi8 = (s8 - b8)[:, P], (s8 + b8)[:, P]
         thr = hi8.sort(dim=1, descending=True).values[:, depth - 1] if depth < P.numel() else \
             torch.full((s.size(0),), -torch.inf, dtype=torch.float64, device="cuda")

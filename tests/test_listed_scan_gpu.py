@@ -7,8 +7,8 @@
     outside the shard, on the placement fixture (many passage ends per tile) and on 1000-5000-token passages (longer
     than a CTA's share);
 (b) pid_base != 0, deleted, compacted-away and appended ids; (c) no stale candidates after a full search;
-(d) the planner's invariants (flmr_debug_listed_plan); (e) the Searcher's pids= / qid_to_pids= on both paths, bf16
-    and fp8, k up to 3000, and a two-rank gloo Searcher.
+(d) the planner's invariants (flmr_debug_listed_plan); (e) the Searcher's pids= / qid_to_pids= on both paths, bf16,
+    fp16 and fp8, k up to 3000, and two-rank Searchers (gloo; NCCL with two GPUs) with one rank on each path.
 """
 import os
 
@@ -252,7 +252,7 @@ def _both_paths(R, sr, fn):
 
 
 @pytest.mark.parametrize("k", [10, 128, 300, 3000])
-@pytest.mark.parametrize("storage", ["bf16", "fp8"])
+@pytest.mark.parametrize("storage", ["bf16", "fp16", "fp8"])
 def test_searcher_listed_and_bitmap_paths_agree(R, corpora, storage, k):
     if storage == "fp8" and k > 2048:
         pytest.skip("fp8 storage re-ranks at most 2048 candidates")
@@ -277,14 +277,16 @@ def _free_port():
     return port
 
 
-def _gloo_worker(rank, world, port, root, storage, ret):
+def _sharded_worker(rank, world, port, root, backend, storage, ret):
     import torch.distributed as dist
     import ravqa_b200 as R
     import ravqa_b200.searcher as S
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+    dev = rank if backend == "nccl" else 0
+    torch.cuda.set_device(dev)
+    kw = {"device_id": torch.device("cuda", dev)} if backend == "nccl" else {}
+    dist.init_process_group(backend, rank=rank, world_size=world, **kw)
     z = np.load(os.path.join(root, "case.npz"))
     lists = {b: z["l%d" % b] for b in range(int(z["B"]))}
     with R.Run().context(R.RunConfig(root=root, experiment="e")):
@@ -301,9 +303,8 @@ def _gloo_worker(rank, world, port, root, storage, ret):
     dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("storage", ["bf16", "fp8"])
-def test_sharded_gloo_listed_matches_unsharded(R, tmp_path, storage):
-    import torch.multiprocessing as mp
+def _sharded_case(R, tmp_path, storage):
+    """Writes the index and the queries; returns the unsharded Searcher's results {k: {row: [(pid, _, score)]}}."""
     dl = placement_doclens(4000, seed=9)
     D = _unit_rows(int(dl.sum()), 10)
     Q = _unit_rows(5 * 32, 11).view(5, 32, 128)
@@ -313,13 +314,14 @@ def test_sharded_gloo_listed_matches_unsharded(R, tmp_path, storage):
     np.savez(tmp_path / "case.npz", Q=Q.float().numpy().astype(np.float32), B=5, **lists)
     c = R.FlatCorpus(D, dl, storage=storage)
     try:
-        want = {k: R.Searcher(index=c)._search_all_Q(list(range(5)), Q, k=k,
+        return {k: R.Searcher(index=c)._search_all_Q(list(range(5)), Q, k=k,
                                                      qid_to_pids={b: lists["l%d" % b] for b in range(5)}).todict()
                 for k in (10, 128)}
     finally:
         c.close()
-    ret = mp.Manager().dict()
-    mp.spawn(_gloo_worker, args=(2, _free_port(), str(tmp_path), storage, ret), nprocs=2, join=True)
+
+
+def _check_sharded(ret, want, storage):
     for rank in range(2):
         for mode in (0, 1):
             for k in (10, 128):
@@ -331,3 +333,25 @@ def test_sharded_gloo_listed_matches_unsharded(R, tmp_path, storage):
                     else:
                         assert len(got[b]) == len(w), (rank, mode, k, b)
                 assert got == ret[(1 - rank, mode, k)]
+
+
+@pytest.mark.parametrize("storage", ["bf16", "fp8"])
+def test_sharded_gloo_listed_matches_unsharded(R, tmp_path, storage):
+    import torch.multiprocessing as mp
+    want = _sharded_case(R, tmp_path, storage)
+    ret = mp.Manager().dict()
+    mp.spawn(_sharded_worker, args=(2, _free_port(), str(tmp_path), "gloo", storage, ret), nprocs=2, join=True)
+    _check_sharded(ret, want, storage)
+
+
+def test_sharded_nccl_listed_matches_unsharded(R, tmp_path):
+    """The Searcher's C-level NCCL path, one rank per GPU: a rank on the listed scan (_listed_topk, then
+    flmr_topk_exchange) next to a rank on the bitmap scan (flmr_maxsim_topk_sharded_allowed) makes the same
+    collectives, and both answer bitwise as the unsharded bf16 Searcher."""
+    import torch.multiprocessing as mp
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs >= 2 GPUs")
+    want = _sharded_case(R, tmp_path, "bf16")
+    ret = mp.Manager().dict()
+    mp.spawn(_sharded_worker, args=(2, _free_port(), str(tmp_path), "nccl", "bf16", ret), nprocs=2, join=True)
+    _check_sharded(ret, want, "bf16")
