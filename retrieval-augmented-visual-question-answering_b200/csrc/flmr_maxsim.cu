@@ -1024,36 +1024,58 @@ flmr_select_kernel(const float* __restrict__ scores, int64_t n, int k, int64_t p
   }
 }
 
+// A token-balanced split of the slots into contiguous ranges (one per CTA, or per pair of CTAs) and the per-tile
+// metadata the scan reads, on the device.
+struct Partition {
+  int64_t n_tiles = 0;
+  int32_t* row_begin = nullptr;   // [ranges + 1]
+  int64_t* tile_base = nullptr;   // [ranges + 1]
+  uint32_t* end_mask = nullptr;   // [n_tiles]
+  int32_t* first_pid = nullptr;   // [n_tiles]
+};
+
+// Everything build_layout derives from the stored passages' (the slots') offsets: what the scan, the SIMT kernel and
+// the gather read.  An append or a compaction builds a new one and swaps it in whole (free_layout frees one).
+struct SlotLayout {
+  std::vector<int64_t> h_poff;         // [slots + 1] stored-row offsets
+  std::vector<int32_t> h_doclen;       // [slots] real lengths
+  int64_t* d_poff = nullptr;           // device copies of the two above
+  int32_t* d_doclen = nullptr;
+  int64_t max_rows = 0;                // stored rows of the longest slot (bounds a listed search's plan)
+  int n_ctas = 0;                      // min(sm_total, slots)
+  Partition cta;
+  CUtensorMap tmap_d;
+  // CTA-pair experiment (flmr_debug_set_scan_variant(4), bf16 only): n_pairs ranges, and a tensor map with a
+  // half-tile box
+  int n_pairs = 0;
+  Partition pair;
+  CUtensorMap tmap_half;
+  int64_t bytes = 0;                   // HBM the device arrays above take
+};
+
 }  // namespace
 
 // ---- handles -----------------------------------------------------------------------------------------
 struct flmr_corpus {
   int device = 0;
   int64_t n_passages = 0, n_tokens = 0, n_rows = 0, pid_base = 0;
-  int n_ctas = 0;
-  int64_t n_tiles = 0;
   bool adopted = false;
-  int64_t hbm_bytes = 0;
+  // FLMR_CORPUS_FP16 (kF16): d_tokens holds fp16 rows, and queries arrive as fp16.  FLMR_CORPUS_FP8 (kE4M3): the scan
+  // reads an e4m3 copy in HBM; the exact bf16 rows stay in pinned, mapped host memory
+  Elem elem = Elem::kBF16;
   __nv_bfloat16* d_tokens = nullptr;   // [n_rows, 128] padded layout (e4m3 corpus: device alias of h_master; fp16
                                        // corpus: the fp16 rows, which every kernel but the scan only moves)
   GrowableMatrix vm_tokens;            // backs d_tokens of a library-owned bf16 (or fp16) corpus
-  // FLMR_CORPUS_FP8: the scan reads an e4m3 copy in HBM; the exact bf16 rows stay in pinned, mapped host memory
-  bool fp8 = false;
   void* h_master = nullptr;            // bf16 [n_rows, 128] padded layout, pinned + mapped (e4m3 corpus only)
   uint8_t* d_fp8 = nullptr;            // e4m3 [n_rows, 128] padded layout (e4m3 corpus only), backed by vm_fp8
   GrowableMatrix vm_fp8;
-  bool f16 = false;                    // FLMR_CORPUS_FP16: d_tokens holds fp16 rows, and queries arrive as fp16
   // Ids and slots.  n_passages is the id extent: ids pid_base .. pid_base + n_passages, never shrinking.  A slot is a
   // passage that has rows.  Until the first flmr_corpus_compact every id has the slot of the same index and
   // h_slot_pid / d_slot_pid stay empty / null; after it, slot s holds global id h_slot_pid[s] (strictly increasing).
-  // Everything the scan reads (offsets, lengths, partition, d_dead) is indexed by slot.
+  // Everything the scan reads (layout, d_dead) is indexed by slot.
   std::vector<int64_t> h_slot_pid;
   int64_t* d_slot_pid = nullptr;
-  int64_t* d_poff = nullptr;           // [slots + 1] stored-row offsets
-  int32_t* d_doclen = nullptr;         // [slots] real lengths
-  std::vector<int64_t> h_poff;         // host copies of the two above (an append extends them)
-  std::vector<int32_t> h_doclen;
-  int64_t max_rows = 0;                // stored rows of the longest slot (bounds a listed search's plan)
+  SlotLayout layout;
   // tombstones: h_dead is indexed by LOCAL ID (bit p & 31 of word p >> 5 set <=> local passage p is deleted, a
   // compacted-away id included); d_dead by SLOT, for the scan's reducer, the gather and the SIMT kernel.  d_dead stays
   // null while no slot is deleted (until the first delete, and again right after a compaction), so a corpus without
@@ -1061,22 +1083,7 @@ struct flmr_corpus {
   uint32_t* d_dead = nullptr;
   std::vector<uint32_t> h_dead;
   int64_t n_deleted = 0;
-  int sm_total = 0;                    // SMs of the device (n_ctas = min(sm_total, slots))
-  int32_t* d_cta_row_begin = nullptr;  // [n_ctas + 1]
-  int64_t* d_cta_tile_base = nullptr;  // [n_ctas + 1]
-  uint32_t* d_tile_end_mask = nullptr; // [n_tiles]
-  int32_t* d_tile_first_pid = nullptr; // [n_tiles]
-  CUtensorMap tmap_d;
-  // CTA-pair experiment (flmr_debug_set_scan_variant(4)): n_pairs contiguous ranges, one per pair of CTAs, and a
-  // tensor map with a half-tile box
-  int n_pairs = 0;
-  int sm_count = 0;
-  int64_t n_tiles_pair = 0;
-  int32_t* d_pair_row_begin = nullptr;
-  int64_t* d_pair_tile_base = nullptr;
-  uint32_t* d_pair_end_mask = nullptr;
-  int32_t* d_pair_first_pid = nullptr;
-  CUtensorMap tmap_half;
+  int sm_total = 0;                    // SMs of the device
 };
 
 // Streaming corpus construction (index load): the padded token matrix is allocated once, packed rows arrive in
@@ -1087,7 +1094,6 @@ struct flmr_corpus_builder {
   std::vector<int32_t> doclens;
   bool aligned = true;                  // every doclen a multiple of kGroup: rows land in place, no scatter
   int64_t rows_done = 0;
-  int sm_count = 0;
   cudaStream_t stream = nullptr;
   static constexpr int kBufs = 2;
   static constexpr int64_t kBufRows = (64ll << 20) / (kDim * 2);   // 64 MB of rows per staging buffer
@@ -1186,7 +1192,7 @@ int load_nccl(const NcclApi** out) {
 constexpr int kNcclInt64 = 4, kNcclFloat32 = 7;   // ncclDataType_t values (nccl.h: ncclInt64 = 4, ncclFloat32 = 7)
 
 thread_local bool g_profiling = false;
-// which scan kernel a search on this thread launches: 0 = chosen per pass (launch_scan), 2 = flmr_scan_kernel<2> (two
+// which scan kernel a search on this thread launches: 0 = chosen per pass (pick_scan), 2 = flmr_scan_kernel<2> (two
 // consumer warpgroups), 3 = flmr_scan_kernel<3> (three), 4 = CTA-pair passes forced, 6 = flmr_scan_split_kernel
 // (three, split-tile loop; 5 stays unassigned); flmr_debug_set_scan_variant
 thread_local int g_scan_variant = 0;
@@ -1199,18 +1205,80 @@ int64_t slots(const flmr_corpus* c) {
   return c->h_slot_pid.empty() ? c->n_passages : static_cast<int64_t>(c->h_slot_pid.size());
 }
 
+// Bytes per row of the matrix the scan reads (an e4m3 corpus's bf16 master is host memory).
+int64_t hbm_row_bytes(Elem elem) { return elem == Elem::kE4M3 ? kDim : kDim * 2; }
+
+const char* elem_name(Elem elem) { return elem == Elem::kE4M3 ? "e4m3" : elem == Elem::kF16 ? "fp16" : "bf16"; }
+
+// HBM a corpus holds: its matrix (an adopted one is the caller's), its layout, its tombstones by slot and its
+// slot -> id map.
+int64_t hbm_bytes(const flmr_corpus* c) {
+  const int64_t ns = slots(c);
+  return (c->adopted ? 0 : c->n_rows * hbm_row_bytes(c->elem)) + c->layout.bytes +
+         (c->d_dead ? (ns + 31) / 32 * 4 : 0) + (c->d_slot_pid ? ns * 8 : 0);
+}
+
+// The storage a corpus's flags select (FLMR_CORPUS_ADOPT reaches here only from flmr_corpus_create).
+int storage_from_flags(unsigned flags, Elem* elem) {
+  if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_ADOPT))
+    return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP8 keeps its own copies of the tokens and cannot adopt them");
+  if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_FP16))
+    return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP16 and FLMR_CORPUS_FP8 exclude each other");
+  *elem = (flags & FLMR_CORPUS_FP8) ? Elem::kE4M3 : (flags & FLMR_CORPUS_FP16) ? Elem::kF16 : Elem::kBF16;
+  return FLMR_OK;
+}
+
+// Packed (*soff, may be null) and padded (*poff) row offsets of n passages, relative to the first; *aligned (may be
+// null): every length is a multiple of kGroup, so packed rows are stored rows.
+int passage_offsets(const int32_t* h_doclens, int64_t n, std::vector<int64_t>* soff, std::vector<int64_t>* poff,
+                    bool* aligned) {
+  std::vector<int64_t> s(n + 1, 0), p(n + 1, 0);
+  bool al = true;
+  for (int64_t i = 0; i < n; ++i) {
+    const int32_t len = h_doclens[i];
+    if (len < 1)
+      return fail(FLMR_ERR_INVALID_ARG, "passage %lld has length %d; zero-length passages have no defined MaxSim score",
+                  (long long)i, len);
+    s[i + 1] = s[i] + len;
+    p[i + 1] = p[i] + (len + kGroup - 1) / kGroup * kGroup;
+    al &= (len % kGroup == 0);
+  }
+  if (soff) soff->swap(s);
+  poff->swap(p);
+  if (aligned) *aligned = al;
+  return FLMR_OK;
+}
+
+// The SM count of the device a corpus is built on, which must be an sm_90 one.
+int sm90_count(int device, int* sm_count) {
+  cudaDeviceProp prop;
+  FLMR_CUDA(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(FLMR_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is sm_90a only", device, prop.major,
+                prop.minor);
+  *sm_count = prop.multiProcessorCount;
+  return FLMR_OK;
+}
+
+// Whether a token matrix to copy from is device (or managed) memory; device memory must be on the corpus's device.
+int token_source(const void* tokens, int device, bool* is_device_ptr) {
+  cudaPointerAttributes attr{};
+  *is_device_ptr = (cudaPointerGetAttributes(&attr, tokens) == cudaSuccess) &&
+                   (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+  cudaGetLastError();
+  if (*is_device_ptr && attr.type == cudaMemoryTypeDevice && attr.device != device)
+    return fail(FLMR_ERR_INVALID_ARG, "token matrix lives on device %d, corpus on %d", attr.device, device);
+  return FLMR_OK;
+}
+
 // The tombstones by slot (d_dead's words) of a compacted corpus, from its tombstones by id (`dead`, as h_dead).
 std::vector<uint32_t> dead_by_slot(const std::vector<int64_t>& slot_pid, int64_t pid_base,
-                                   const std::vector<uint32_t>& dead, bool* any) {
+                                   const std::vector<uint32_t>& dead) {
   const int64_t ns = static_cast<int64_t>(slot_pid.size());
   std::vector<uint32_t> out((ns + 31) / 32, 0u);
-  *any = false;
   for (int64_t s = 0; s < ns; ++s) {
     const int64_t p = slot_pid[s] - pid_base;
-    if (static_cast<size_t>(p >> 5) < dead.size() && ((dead[p >> 5] >> (p & 31)) & 1u)) {
-      out[s >> 5] |= 1u << (s & 31);
-      *any = true;
-    }
+    if (static_cast<size_t>(p >> 5) < dead.size() && ((dead[p >> 5] >> (p & 31)) & 1u)) out[s >> 5] |= 1u << (s & 31);
   }
   return out;
 }
@@ -1402,84 +1470,82 @@ void plan_passes(int n_queries, int nq, bool allow_pair, std::vector<PassPlan>* 
   if (n_pair_queries_out) *n_pair_queries_out = n_pair_q;
 }
 
-//
-// listed: p holds a listed search's plan (run_search's ListedArgs); the plan-mode twins of the two product kernels run
-// it, chosen by the same rule (variant 2 forces the two-warpgroup one, 6 the split one).
-int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pair, cudaStream_t st,
-                bool listed = false) {
-  // by the pass's occupied 64-row blocks: from five up (Nq = 320: five, a full row slice: six) three warpgroups with
-  // the split-tile loop (2 / 2 / 1 or 2 / 2 / 2 blocks, each warpgroup folding one half of a tile under the MMAs of
-  // the other), below that two (each with two accumulators, its own MMAs overlapping its fold).  On an H100 80GB HBM3
-  // (700 W, 200k x 180-token passages, median of 5, DESIGN.md 4.1) 16 x Nq = 320 took 6.27 ms split, 6.72 ms with
-  // the serial three-warpgroup loop and 7.98 ms with two warpgroups; 3 x Nq = 832 row slices 6.63 / 6.73 / 7.19 ms;
-  // a 4-block pass (4 x Nq = 256) 5.55 / 5.91 / 5.46 ms.  e4m3 follows the same threshold (5 blocks: 3.95 ms split,
-  // 5.00 ms serial).  Every instantiation computes bit-identical results
-  const bool split = !pair && ((g_scan_variant == 6) ||
-                               (g_scan_variant == 0 && scan_blocks(p.nq_pass, p.rbq) >= 5));
-  const bool use3 = !pair && g_scan_variant == 3;
+// The scan kernels of one storage and mode (partition or listed plan): null where the storage has no such kernel.
+// Every one runs ScanSmem::kBytes of dynamic shared memory; pick_scan gives its warpgroup count.
+using ScanFn = void (*)(CUtensorMap, ScanParams);
+struct ScanKernels {
+  ScanFn two;     // two consumer warpgroups, each overlapping its own MMAs with its fold
+  ScanFn three;   // three, serial loop (variant 3)
+  ScanFn split;   // three, split-tile loop
+  ScanFn pair;    // clusters of two CTAs (variant 4)
+};
+constexpr ScanKernels kScanKernels[3][2] = {   // [Elem][listed]
+    {{flmr_scan_kernel<2>, flmr_scan_kernel<3>, flmr_scan_split_kernel<false>, flmr_scan_kernel<2, true>},
+     {flmr_scan_listed_kernel<false>, nullptr, flmr_scan_listed_split_kernel<false>, nullptr}},
+    {{flmr_scan_f16_kernel, nullptr, flmr_scan_split_f16_kernel, nullptr},
+     {flmr_scan_listed_f16_kernel, nullptr, flmr_scan_listed_split_f16_kernel, nullptr}},
+    {{flmr_scan_kernel<2, false, true>, flmr_scan_kernel<3, false, true>, flmr_scan_split_kernel<true>, nullptr},
+     {flmr_scan_listed_kernel<true>, nullptr, flmr_scan_listed_split_kernel<true>, nullptr}},
+};
+
+struct ScanKernel {
+  ScanFn fn;   // null: no kernel (run_search and run_listed refuse the variant)
+  int wgs;
+};
+
+// The kernel a pass of `blocks` occupied 64-row query blocks runs under scan variant `variant`.  Variant 0 picks by
+// the blocks: from five up (Nq = 320: five, a full row slice: six) three warpgroups with the split-tile loop (2 / 2 / 1
+// or 2 / 2 / 2 blocks, each warpgroup folding one half of a tile under the MMAs of the other), below that two (each
+// with two accumulators, its own MMAs overlapping its fold).  On an H100 80GB HBM3 (700 W, 200k x 180-token passages,
+// median of 5, DESIGN.md 4.1) 16 x Nq = 320 took 6.27 ms split, 6.72 ms with the serial three-warpgroup loop and
+// 7.98 ms with two warpgroups; 3 x Nq = 832 row slices 6.63 / 6.73 / 7.19 ms; a 4-block pass (4 x Nq = 256) 5.55 /
+// 5.91 / 5.46 ms.  e4m3 follows the same threshold (5 blocks: 3.95 ms split, 5.00 ms serial).  Variants 2, 3, 4 and 6
+// force a kernel.  Every kernel computes bit-identical results.
+ScanKernel pick_scan(Elem elem, bool listed, int variant, int blocks) {
+  const ScanKernels& t = kScanKernels[static_cast<int>(elem)][listed];
+  if (variant == 3) return {t.three, 3};
+  if (variant == 4) return {t.pair, 2};
+  if (variant == 6 || (variant == 0 && blocks >= 5)) return {t.split, 3};
+  return {t.two, 2};
+}
+
+// One scan pass.  pair: a CTA-pair pass (planned only under variant 4).  listed: p holds a listed search's plan
+// (run_search's ListedArgs).
+int launch_scan(const flmr_corpus* c, ScanParams p, bool pair, bool listed, cudaStream_t st) {
+  const SlotLayout& l = c->layout;
+  // the passes variant 4 leaves to single CTAs run the two-warpgroup kernel
+  const int variant = g_scan_variant == 4 && !pair ? 2 : g_scan_variant;
+  const ScanKernel k = pick_scan(c->elem, listed, variant, scan_blocks(p.nq_pass, p.rbq));
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(static_cast<unsigned>(pair ? 2 * l.n_pairs : l.n_ctas));
+  cfg.blockDim = dim3(scan_threads(k.wgs));
+  cfg.dynamicSmemBytes = ScanSmem::kBytes;
+  cfg.stream = st;
+  if (!listed) {   // a listed pass brings its plan's tiles
+    const Partition& part = pair ? l.pair : l.cta;
+    p.cta_row_begin = part.row_begin;
+    p.cta_tile_base = part.tile_base;
+    p.tile_end_mask = part.end_mask;
+    p.tile_first_pid = part.first_pid;
+  }
+  cudaLaunchAttribute cluster{};
+  if (pair) {
+    // clusters of two CTAs share one of the n_pairs token ranges; the tensor map has a half-tile box
+    cluster.id = cudaLaunchAttributeClusterDimension;
+    cluster.val.clusterDim = {2, 1, 1};
+    cfg.attrs = &cluster;
+    cfg.numAttrs = 1;
+  }
+  void* args[] = {const_cast<CUtensorMap*>(pair ? &l.tmap_half : &l.tmap_d), &p};
   EventPair ev{};
   if (g_profiling) {
     FLMR_CUDA(cudaEventCreate(&ev.a));
     FLMR_CUDA(cudaEventCreate(&ev.b));
     FLMR_CUDA(cudaEventRecord(ev.a, st));
   }
-  (void)ws;
-  if (listed) {
-    const dim3 grid(c->n_ctas);
-    if (split) {
-      if (c->f16)
-        flmr_scan_listed_split_f16_kernel<<<grid, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-      else if (c->fp8)
-        flmr_scan_listed_split_kernel<true><<<grid, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-      else
-        flmr_scan_listed_split_kernel<false><<<grid, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-    } else if (c->f16) {
-      flmr_scan_listed_f16_kernel<<<grid, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-    } else if (c->fp8) {
-      flmr_scan_listed_kernel<true><<<grid, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-    } else {
-      flmr_scan_listed_kernel<false><<<grid, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-    }
-  } else if (pair) {
-    // clusters of two CTAs share one of the n_pairs token ranges; the tensor map has a half-tile box
-    p.cta_row_begin = c->d_pair_row_begin;
-    p.cta_tile_base = c->d_pair_tile_base;
-    p.tile_end_mask = c->d_pair_end_mask;
-    p.tile_first_pid = c->d_pair_first_pid;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(2 * c->n_pairs));
-    cfg.blockDim = dim3(scan_threads(2));
-    cfg.dynamicSmemBytes = ScanSmem::kBytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    FLMR_CUDA(cudaLaunchKernelEx(&cfg, flmr_scan_kernel<2, true>, c->tmap_half, p));
-  } else if (c->f16) {   // variants without an fp16 kernel are refused by run_search
-    if (split)
-      flmr_scan_split_f16_kernel<<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-    else
-      flmr_scan_f16_kernel<<<c->n_ctas, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-  } else if (split) {
-    if (c->fp8)
-      flmr_scan_split_kernel<true><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-    else
-      flmr_scan_split_kernel<false><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-  } else if (c->fp8) {
-    if (use3)
-      flmr_scan_kernel<3, false, true><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-    else
-      flmr_scan_kernel<2, false, true><<<c->n_ctas, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-  } else if (use3) {
-    flmr_scan_kernel<3><<<c->n_ctas, scan_threads(3), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-  } else {
-    flmr_scan_kernel<2><<<c->n_ctas, scan_threads(2), ScanSmem::kBytes, st>>>(c->tmap_d, p);
-  }
-  FLMR_CUDA(cudaGetLastError());
+  cudaError_t e = cudaLaunchKernelExC(&cfg, reinterpret_cast<const void*>(k.fn), args);
+  if (const cudaError_t last = cudaGetLastError(); e == cudaSuccess) e = last;   // also clears a failed launch's error
+  if (e != cudaSuccess) return fail(FLMR_ERR_CUDA, "scan launch failed: %s", cudaGetErrorString(e));
   ++g_launches;
   if (g_profiling) {
     FLMR_CUDA(cudaEventRecord(ev.b, st));
@@ -1491,7 +1557,7 @@ int launch_scan(const flmr_corpus* c, flmr_workspace* ws, ScanParams p, bool pai
 // One launch stages `count` zero-padded query blocks (slot i of the workspace's staging buffer <- sp.pass[i]).
 int stage_queries(flmr_workspace* ws, const void* d_q, int nq, const StageParams& sp, int count, cudaStream_t st) {
   const int threads = 256;
-  const bool fp8 = ws->corpus->fp8;
+  const bool fp8 = ws->corpus->elem == Elem::kE4M3;
   dim3 grid((kMtMax * kTileM * (fp8 ? 8 : 16) + threads - 1) / threads, static_cast<unsigned>(count));
   (fp8 ? flmr_stage_queries_kernel<true> : flmr_stage_queries_kernel<false>)<<<grid, threads, 0, st>>>(
       reinterpret_cast<const uint4*>(d_q), reinterpret_cast<uint4*>(ws->d_qpad), nq, sp);
@@ -1560,14 +1626,15 @@ int plan_listed_chunk(const flmr_corpus* c, flmr_workspace* ws, const std::vecto
   out->passes.resize(n_p);
   out->u_bound.resize(n_p);
   out->t_bound.resize(n_p);
-  const int64_t tiles_per = (c->max_rows + kTileN - 1) / kTileN + 1;
+  const int n_ctas = c->layout.n_ctas;
+  const int64_t tiles_per = (c->layout.max_rows + kTileN - 1) / kTileN + 1;
   int64_t u_total = 0, t_total = 0;
   for (int i = 0; i < n_p; ++i) {
     const PassPlan& pp = plan[i];
     const int64_t listed = la.h_off[c0 + pp.q_first + pp.n_q] - la.h_off[c0 + pp.q_first];
     out->u_bound[i] = std::min(listed, ns);
-    out->t_bound[i] = out->u_bound[i] * tiles_per + c->n_ctas;
-    out->passes[i] = {pp.q_first, pp.n_q, u_total, static_cast<int64_t>(i) * (c->n_ctas + 1), t_total};
+    out->t_bound[i] = out->u_bound[i] * tiles_per + n_ctas;
+    out->passes[i] = {pp.q_first, pp.n_q, u_total, static_cast<int64_t>(i) * (n_ctas + 1), t_total};
     u_total += out->u_bound[i];
     t_total += out->t_bound[i];
   }
@@ -1581,7 +1648,7 @@ int plan_listed_chunk(const flmr_corpus* c, flmr_workspace* ws, const std::vecto
   const size_t o_passes = take(n_p * sizeof(ListedPass));
   const size_t o_meta = take(2 * n_p * 8);
   const size_t o_cum = take(u_total * 8), o_tile = take(u_total * 8), o_slot = take(u_total * 4);
-  const size_t o_base = take(static_cast<size_t>(n_p) * (c->n_ctas + 1) * 8);
+  const size_t o_base = take(static_cast<size_t>(n_p) * (n_ctas + 1) * 8);
   const size_t o_row = take(t_total * 4), o_mask = take(t_total * 4), o_first = take(t_total * 4);
   if (ws->plan_capacity < bytes) {
     cudaFree(ws->d_plan);   // waits for the searches still using it
@@ -1611,9 +1678,9 @@ int plan_listed_chunk(const flmr_corpus* c, flmr_workspace* ws, const std::vecto
     FLMR_CUDA(cudaGetLastError());
     ++g_launches;
   }
-  flmr_listed_plan_kernel<<<n_p, kPlanThreads, 0, st>>>(out->d_passes, out->allow, out->words, c->d_poff, c->n_ctas,
-                                                         out->u_slot, out->u_cum, out->u_tile, out->cta_tile_base,
-                                                         out->tile_row, out->tile_mask, out->tile_first, out->meta);
+  flmr_listed_plan_kernel<<<n_p, kPlanThreads, 0, st>>>(
+      out->d_passes, out->allow, out->words, c->layout.d_poff, n_ctas, out->u_slot, out->u_cum, out->u_tile,
+      out->cta_tile_base, out->tile_row, out->tile_mask, out->tile_first, out->meta);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;
@@ -1637,10 +1704,9 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
                 "an earlier scan on this workspace tripped the device watchdog (code %d: %s starved); "
                 "the CUDA context is poisoned", code,
                 code == kDevTimeoutProducer ? "TMA producer" : code == kDevTimeoutMma ? "MMA issuer" : "epilogue");
-  if (c->fp8 && g_scan_variant == 4)
-    return fail(FLMR_ERR_UNSUPPORTED, "the CTA-pair scan (variant 4) has no e4m3 kernel");
-  if (c->f16 && (g_scan_variant == 3 || g_scan_variant == 4))
-    return fail(FLMR_ERR_UNSUPPORTED, "scan variant %d has no fp16 kernel", g_scan_variant);
+  // under variant 0 every storage has both kernels a pass may pick
+  if (!pick_scan(c->elem, listed != nullptr, g_scan_variant, 0).fn)
+    return fail(FLMR_ERR_UNSUPPORTED, "scan variant %d has no %s kernel", g_scan_variant, elem_name(c->elem));
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
   int rc;
@@ -1669,22 +1735,19 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
     return rc;
 
   ScanParams p{};
-  p.cta_row_begin = c->d_cta_row_begin;
-  p.cta_tile_base = c->d_cta_tile_base;
-  p.tile_end_mask = c->d_tile_end_mask;
-  p.tile_first_pid = c->d_tile_first_pid;
+  const SlotLayout& l = c->layout;
   p.init_val = (flags & FLMR_FLAG_RELU) ? 0.f : -INFINITY;
   p.n_passages = ns;
   p.dead = c->d_dead;   // null while no slot is deleted: the reducer then makes no extra load
-  if (ws->cand_lists < c->n_ctas) {
+  if (ws->cand_lists < l.n_ctas) {
     // the corpus grew past the CTA count this workspace was sized for (a corpus of fewer passages than SMs launches
     // one CTA per passage); cudaFree waits for the searches still using the old buffer
     cudaFree(ws->d_cand_keys);
     ws->d_cand_keys = nullptr;
     ws->cand_lists = 0;
     FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&ws->d_cand_keys),
-                         static_cast<size_t>(c->n_ctas) * ws->max_queries * kMaxK * 8));
-    ws->cand_lists = c->n_ctas;
+                         static_cast<size_t>(l.n_ctas) * ws->max_queries * kMaxK * 8));
+    ws->cand_lists = l.n_ctas;
   }
   p.cand_keys = ws->d_cand_keys;
   p.q_pad = reinterpret_cast<const uint4*>(ws->d_qpad);
@@ -1700,7 +1763,7 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   // D tile fetched once and TMA-multicast into both: half the HBM / L2 traffic per query) are planned only when forced
   // (variant 4): on an H100 a pair pass of two Nq = 320 queries over 1M passages took 105.9 ms against 39.4 ms for a
   // single-CTA pass of one, so the product (variant 0) runs single-CTA passes.
-  const bool allow_pair = c->n_pairs > 0 && g_scan_variant == 4;
+  const bool allow_pair = l.n_pairs > 0 && g_scan_variant == 4;
   // a call is processed in chunks of at most ws->max_queries queries (the candidate buffer's capacity);
   // within a chunk: every pass's scan, then the merge over the chunk's queries (one launch per kind of pass)
   std::vector<PassPlan> plan;
@@ -1761,7 +1824,7 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
         p.allow = lp.allow + static_cast<int64_t>(pp.q_first) * lp.words;
         p.allow_stride = lp.words;
       }
-      if ((rc = launch_scan(c, ws, p, (pp.flags & kPassPair) != 0, st, listed != nullptr))) return rc;
+      if ((rc = launch_scan(c, p, (pp.flags & kPassPair) != 0, listed != nullptr, st))) return rc;
     }
     if (listed && d_slot_scores) {
       const int64_t n = listed->h_off[c0 + nqc] - listed->h_off[c0];
@@ -1784,134 +1847,81 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
       float* os = d_topk_scores + static_cast<int64_t>(c0) * k;
       int64_t* op = d_topk_pids + static_cast<int64_t>(c0) * k;
       // queries of pair passes have one candidate list per CTA PAIR, the others one per CTA
-      if ((rc = launch_merge_keys(c, ws, c->n_pairs, nqc, 0, n_pair_q, k, os, op, st))) return rc;
-      if ((rc = launch_merge_keys(c, ws, c->n_ctas, nqc, n_pair_q, nqc - n_pair_q, k, os, op, st))) return rc;
+      if ((rc = launch_merge_keys(c, ws, l.n_pairs, nqc, 0, n_pair_q, k, os, op, st))) return rc;
+      if ((rc = launch_merge_keys(c, ws, l.n_ctas, nqc, n_pair_q, nqc - n_pair_q, k, os, op, st))) return rc;
     }
   }
   return FLMR_OK;
 }
 
-// Everything a corpus needs besides its token matrix: offsets / lengths, the CTA partition + per-tile metadata,
-// the TMA descriptor, the kernel's shared-memory attribute.  Shared by flmr_corpus_create and the streaming builder.
-// poff / h_doclens describe the stored passages (the slots): all of them until a compaction.
-int finish_corpus(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_t* h_doclens, int sm_count) {
-  const int64_t n_passages = static_cast<int64_t>(poff.size()) - 1;
-  const int64_t n_rows = c->n_rows;
-  int rc = FLMR_OK;
-  auto bail = [](int code) { return code; };
-  struct {
-    int multiProcessorCount;
-  } prop{sm_count};
-  // --- offsets / lengths (SIMT cross-check kernel, info) ---
-  {
-    std::vector<int32_t> lens(h_doclens, h_doclens + n_passages);
-    if ((rc = dev_upload(&c->d_poff, poff, &c->hbm_bytes))) return bail(rc);
-    if ((rc = dev_upload(&c->d_doclen, lens, &c->hbm_bytes))) return bail(rc);
-    c->h_poff = poff;
-    c->h_doclen.swap(lens);
-    c->max_rows = 0;
-    for (int64_t s = 0; s < n_passages; ++s) c->max_rows = std::max(c->max_rows, poff[s + 1] - poff[s]);
-    c->sm_total = sm_count;
-  }
+void free_layout(SlotLayout* l) {
+  cudaFree(l->d_poff);
+  cudaFree(l->d_doclen);
+  for (const Partition& q : {l->cta, l->pair})
+    for (void* p : {static_cast<void*>(q.row_begin), static_cast<void*>(q.tile_base), static_cast<void*>(q.end_mask),
+                    static_cast<void*>(q.first_pid)})
+      cudaFree(p);
+  *l = SlotLayout();
+}
 
-  // --- partition + tile metadata ---
-  int n_ctas = prop.multiProcessorCount;
+// The layout of a corpus of storage `elem` whose stored passages (the slots: all of them until a compaction) have row
+// offsets poff and lengths lens, over the token matrix d_tokens (and the e4m3 copy d_fp8 of an e4m3 corpus) of n_rows
+// rows, into the empty layout *l.  On failure nothing stays allocated.
+int build_layout(Elem elem, const __nv_bfloat16* d_tokens, const uint8_t* d_fp8, int64_t n_rows,
+                 const std::vector<int64_t>& poff, const int32_t* lens, int sm_total, SlotLayout* l) {
+  // per-device function attributes of the storage's scan kernels (idempotent), set here rather than at launch time
+  for (const ScanKernels& t : kScanKernels[static_cast<int>(elem)])
+    for (ScanFn fn : {t.two, t.three, t.split, t.pair}) {
+      const cudaError_t e =
+          fn ? cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes) : cudaSuccess;
+      if (e != cudaSuccess)
+        return fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s", ScanSmem::kBytes,
+                    cudaGetErrorString(e));
+    }
+  const int64_t ns = static_cast<int64_t>(poff.size()) - 1;
+  l->h_poff = poff;
+  l->h_doclen.assign(lens, lens + ns);
+  for (int64_t s = 0; s < ns; ++s) l->max_rows = std::max(l->max_rows, poff[s + 1] - poff[s]);
+  int n_ctas = sm_total;
 #ifdef FLMR_DEBUG
   if (const char* e = getenv("FLMR_NUM_CTAS")) n_ctas = std::max(1, atoi(e));
 #endif
-  n_ctas = static_cast<int>(std::min<int64_t>(n_ctas, n_passages));
-  c->n_ctas = n_ctas;
-  {
-    std::vector<int32_t> row_begin, first_pid;
-    std::vector<int64_t> tile_base;
-    std::vector<uint32_t> end_mask;
-    build_partition(poff, n_ctas, kTileN, &row_begin, &tile_base, &end_mask, &first_pid);
-    c->n_tiles = static_cast<int64_t>(end_mask.size());
-    if ((rc = dev_upload(&c->d_cta_row_begin, row_begin, &c->hbm_bytes))) return bail(rc);
-    if ((rc = dev_upload(&c->d_cta_tile_base, tile_base, &c->hbm_bytes))) return bail(rc);
-    if ((rc = dev_upload(&c->d_tile_end_mask, end_mask, &c->hbm_bytes))) return bail(rc);
-    if ((rc = dev_upload(&c->d_tile_first_pid, first_pid, &c->hbm_bytes))) return bail(rc);
-  }
-  if ((rc = c->fp8 ? encode_rows_map(&c->tmap_d, c->d_fp8, static_cast<uint64_t>(n_rows), kTileN, Elem::kE4M3)
-                    : encode_rows_map(&c->tmap_d, c->d_tokens, static_cast<uint64_t>(n_rows), kTileN,
-                                      c->f16 ? Elem::kF16 : Elem::kBF16)))
-    return bail(rc);
+  l->n_ctas = static_cast<int>(std::min<int64_t>(n_ctas, ns));
+  auto partition = [&](int n, Partition* q) {   // the slots split into n ranges, uploaded
+    std::vector<int32_t> rb, fp;
+    std::vector<int64_t> tb;
+    std::vector<uint32_t> em;
+    build_partition(poff, n, kTileN, &rb, &tb, &em, &fp);
+    q->n_tiles = static_cast<int64_t>(em.size());
+    int rc = dev_upload(&q->row_begin, rb, &l->bytes);
+    if (!rc) rc = dev_upload(&q->tile_base, tb, &l->bytes);
+    if (!rc) rc = dev_upload(&q->end_mask, em, &l->bytes);
+    return rc ? rc : dev_upload(&q->first_pid, fp, &l->bytes);
+  };
+  int rc = dev_upload(&l->d_poff, l->h_poff, &l->bytes);
+  if (!rc) rc = dev_upload(&l->d_doclen, l->h_doclen, &l->bytes);
+  if (!rc) rc = partition(l->n_ctas, &l->cta);
+  if (!rc)
+    rc = encode_rows_map(&l->tmap_d, elem == Elem::kE4M3 ? static_cast<const void*>(d_fp8) : d_tokens,
+                         static_cast<uint64_t>(n_rows), kTileN, elem);
   // CTA-pair passes: their own partition + half-tile tensor map.  The product never plans pair passes (see
   // run_search); these few KB per corpus are built so flmr_debug_set_scan_variant(4) can hold the cluster kernel
   // against the single-CTA kernels on any bf16 corpus.
-  if (!c->fp8 && !c->f16 && n_ctas >= 2 && n_passages >= n_ctas / 2) {
-    std::vector<int32_t> row_begin, first_pid;
-    std::vector<int64_t> tile_base;
-    std::vector<uint32_t> end_mask;
-    c->n_pairs = n_ctas / 2;
-    c->sm_count = sm_count;
-    build_partition(poff, c->n_pairs, kTileN, &row_begin, &tile_base, &end_mask, &first_pid);
-    c->n_tiles_pair = static_cast<int64_t>(end_mask.size());
-    if ((rc = dev_upload(&c->d_pair_row_begin, row_begin, &c->hbm_bytes))) return bail(rc);
-    if ((rc = dev_upload(&c->d_pair_tile_base, tile_base, &c->hbm_bytes))) return bail(rc);
-    if ((rc = dev_upload(&c->d_pair_end_mask, end_mask, &c->hbm_bytes))) return bail(rc);
-    if ((rc = dev_upload(&c->d_pair_first_pid, first_pid, &c->hbm_bytes))) return bail(rc);
-    if ((rc = encode_rows_map(&c->tmap_half, c->d_tokens, static_cast<uint64_t>(n_rows), kTileN / 2))) return bail(rc);
-    cudaError_t e3 = cudaFuncSetAttribute(flmr_scan_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          ScanSmem::kBytes);
-    if (e3 != cudaSuccess) return bail(fail(FLMR_ERR_CUDA, "pair kernel attribute: %s", cudaGetErrorString(e3)));
+  if (!rc && elem == Elem::kBF16 && l->n_ctas >= 2) {
+    l->n_pairs = l->n_ctas / 2;
+    rc = partition(l->n_pairs, &l->pair);
+    if (!rc) rc = encode_rows_map(&l->tmap_half, d_tokens, static_cast<uint64_t>(n_rows), kTileN / 2);
   }
-  if (c->f16) {  // per-device function attributes of the two fp16 kernels
-    cudaError_t e1 = cudaFuncSetAttribute(flmr_scan_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          ScanSmem::kBytes);
-    if (e1 == cudaSuccess)
-      e1 = cudaFuncSetAttribute(flmr_scan_split_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                ScanSmem::kBytes);
-    if (e1 != cudaSuccess)
-      return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
-                       ScanSmem::kBytes, cudaGetErrorString(e1)));
-  } else {  // per-device function attribute, set here (idempotent) rather than at launch time
-    cudaError_t e1 = c->fp8 ? cudaFuncSetAttribute(flmr_scan_kernel<2, false, true>,
-                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes)
-                            : cudaFuncSetAttribute(flmr_scan_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                   ScanSmem::kBytes);
-    if (e1 == cudaSuccess)
-      e1 = c->fp8 ? cudaFuncSetAttribute(flmr_scan_kernel<3, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         ScanSmem::kBytes)
-                  : cudaFuncSetAttribute(flmr_scan_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         ScanSmem::kBytes);
-    if (e1 == cudaSuccess)
-      e1 = c->fp8 ? cudaFuncSetAttribute(flmr_scan_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         ScanSmem::kBytes)
-                  : cudaFuncSetAttribute(flmr_scan_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         ScanSmem::kBytes);
-    if (e1 != cudaSuccess)
-      return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
-                       ScanSmem::kBytes, cudaGetErrorString(e1)));
-  }
-  {  // the plan-mode kernels of this storage (listed searches)
-    cudaError_t e1 = cudaSuccess;
-    auto set = [&](const void* fn) {
-      if (e1 == cudaSuccess) e1 = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes);
-    };
-    if (c->f16) {
-      set(reinterpret_cast<const void*>(flmr_scan_listed_f16_kernel));
-      set(reinterpret_cast<const void*>(flmr_scan_listed_split_f16_kernel));
-    } else if (c->fp8) {
-      set(reinterpret_cast<const void*>(flmr_scan_listed_kernel<true>));
-      set(reinterpret_cast<const void*>(flmr_scan_listed_split_kernel<true>));
-    } else {
-      set(reinterpret_cast<const void*>(flmr_scan_listed_kernel<false>));
-      set(reinterpret_cast<const void*>(flmr_scan_listed_split_kernel<false>));
-    }
-    if (e1 != cudaSuccess)
-      return bail(fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s",
-                       ScanSmem::kBytes, cudaGetErrorString(e1)));
-  }
-  return FLMR_OK;
+  if (rc) free_layout(l);
+  return rc;
 }
 
-// The token matrix of a new corpus (n_rows set): bf16 in HBM, or (c->fp8) the e4m3 copy in HBM plus the bf16 master
+// The token matrix of a new corpus (n_rows set): bf16 in HBM, or (e4m3) the e4m3 copy in HBM plus the bf16 master
 // in pinned, mapped host memory, whose device alias becomes d_tokens (the repack / scatter kernels write both).
 int alloc_token_matrix(flmr_corpus* c) {
   const size_t rows = static_cast<size_t>(c->n_rows);
   cudaError_t e;
-  if (c->fp8) {
+  if (c->elem == Elem::kE4M3) {
     if ((e = cudaHostAlloc(&c->h_master, rows * kDim * 2, cudaHostAllocMapped | cudaHostAllocPortable)) != cudaSuccess) {
       c->h_master = nullptr;
       return fail(FLMR_ERR_OOM, "cudaHostAlloc(%zu B) for the bf16 master failed: %s", rows * kDim * 2,
@@ -1920,12 +1930,10 @@ int alloc_token_matrix(flmr_corpus* c) {
     FLMR_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&c->d_tokens), c->h_master, 0));
     if (int rc = gm_grow(&c->vm_fp8, c->device, rows * kDim)) return rc;
     c->d_fp8 = reinterpret_cast<uint8_t*>(c->vm_fp8.base);
-    c->hbm_bytes += static_cast<int64_t>(rows * kDim);
     return FLMR_OK;
   }
   if (int rc = gm_grow(&c->vm_tokens, c->device, rows * kDim * 2)) return rc;
   c->d_tokens = reinterpret_cast<__nv_bfloat16*>(c->vm_tokens.base);
-  c->hbm_bytes += static_cast<int64_t>(rows * kDim * 2);
   return FLMR_OK;
 }
 
@@ -1978,28 +1986,6 @@ cudaError_t pack_passages(const void* tokens, bool is_device_ptr, const std::vec
   cudaFree(d_soff);
   cudaFree(d_poff);
   return e;
-}
-
-// The per-passage arrays, partition and tensor maps finish_corpus builds (the token matrices are not touched).
-void free_metadata(flmr_corpus* c) {
-  for (void* p : {static_cast<void*>(c->d_poff), static_cast<void*>(c->d_doclen),
-                  static_cast<void*>(c->d_cta_row_begin), static_cast<void*>(c->d_cta_tile_base),
-                  static_cast<void*>(c->d_tile_end_mask), static_cast<void*>(c->d_tile_first_pid),
-                  static_cast<void*>(c->d_pair_row_begin), static_cast<void*>(c->d_pair_tile_base),
-                  static_cast<void*>(c->d_pair_end_mask), static_cast<void*>(c->d_pair_first_pid)})
-    cudaFree(p);
-  c->d_poff = nullptr;
-  c->d_doclen = nullptr;
-  c->d_cta_row_begin = nullptr;
-  c->d_cta_tile_base = nullptr;
-  c->d_tile_end_mask = nullptr;
-  c->d_tile_first_pid = nullptr;
-  c->d_pair_row_begin = nullptr;
-  c->d_pair_tile_base = nullptr;
-  c->d_pair_end_mask = nullptr;
-  c->d_pair_first_pid = nullptr;
-  c->n_pairs = 0;
-  c->n_tiles_pair = 0;
 }
 
 // ---- compaction schedule (pure host logic; exported for tests as flmr_debug_compact_plan) ----------------------
@@ -2112,23 +2098,12 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
   if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
   if (n_passages <= 0 || !tokens || !h_doclens)
     return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null tokens/doclens");
-  if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_ADOPT))
-    return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP8 keeps its own copies of the tokens and cannot adopt them");
-  if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_FP16))
-    return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP16 and FLMR_CORPUS_FP8 exclude each other");
-  std::vector<int64_t> soff(n_passages + 1), poff(n_passages + 1);
-  soff[0] = poff[0] = 0;
-  bool aligned = true;
-  for (int64_t p = 0; p < n_passages; ++p) {
-    const int32_t len = h_doclens[p];
-    if (len < 1)
-      return fail(FLMR_ERR_INVALID_ARG,
-                  "passage %lld has length %d; zero-length passages have no defined MaxSim score",
-                  (long long)p, len);
-    soff[p + 1] = soff[p] + len;
-    poff[p + 1] = poff[p] + (len + kGroup - 1) / kGroup * kGroup;
-    aligned &= (len % kGroup == 0);
-  }
+  Elem elem;
+  std::vector<int64_t> soff, poff;
+  bool aligned;
+  int rc;
+  if ((rc = storage_from_flags(flags, &elem)) || (rc = passage_offsets(h_doclens, n_passages, &soff, &poff, &aligned)))
+    return rc;
   const int64_t n_rows = poff[n_passages];
   if (n_rows + kTileN >= (1ll << 31))
     return fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
@@ -2136,21 +2111,11 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
 
   DeviceGuard guard(device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
-  cudaDeviceProp prop;
-  FLMR_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0)
-    return fail(FLMR_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is sm_90a only", device,
-                prop.major, prop.minor);
-
-  cudaPointerAttributes attr{};
-  const bool is_device_ptr = (cudaPointerGetAttributes(&attr, tokens) == cudaSuccess) &&
-                             (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
-  cudaGetLastError();
+  int sm_count;
+  bool is_device_ptr;
+  if ((rc = sm90_count(device, &sm_count)) || (rc = token_source(tokens, device, &is_device_ptr))) return rc;
   if ((flags & FLMR_CORPUS_ADOPT) && !is_device_ptr)
     return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_ADOPT requires a device pointer");
-  if (is_device_ptr && attr.type == cudaMemoryTypeDevice && attr.device != device)
-    return fail(FLMR_ERR_INVALID_ARG, "token matrix lives on device %d, corpus requested on %d",
-                attr.device, device);
 
   flmr_corpus* c = new (std::nothrow) flmr_corpus();
   if (!c) return fail(FLMR_ERR_OOM, "host allocation failed");
@@ -2159,9 +2124,8 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
   c->n_tokens = soff[n_passages];
   c->n_rows = n_rows;
   c->pid_base = pid_base;
-  c->fp8 = (flags & FLMR_CORPUS_FP8) != 0;
-  c->f16 = (flags & FLMR_CORPUS_FP16) != 0;
-  int rc = FLMR_OK;
+  c->elem = elem;
+  c->sm_total = sm_count;
   auto bail = [&](int code) {
     flmr_corpus_destroy(c);
     return code;
@@ -2181,7 +2145,8 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
       return bail(fail(FLMR_ERR_CUDA, "corpus repack failed: %s", cudaGetErrorString(e)));
   }
 
-  if ((rc = finish_corpus(c, poff, h_doclens, prop.multiProcessorCount))) return bail(rc);
+  if ((rc = build_layout(elem, c->d_tokens, c->d_fp8, n_rows, poff, h_doclens, sm_count, &c->layout)))
+    return bail(rc);
   *out = c;
   return FLMR_OK;
 }
@@ -2193,7 +2158,7 @@ int flmr_corpus_destroy(flmr_corpus_t* c) {
   if (c->h_master) cudaFreeHost(c->h_master);   // d_tokens is its device alias
   gm_free(&c->vm_tokens);                       // (an adopted matrix is the caller's and has no mapping here)
   gm_free(&c->vm_fp8);
-  free_metadata(c);
+  free_layout(&c->layout);
   cudaFree(c->d_dead);
   cudaFree(c->d_slot_pid);
   delete c;
@@ -2212,8 +2177,8 @@ int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, 
   if (flags & ~(FLMR_CORPUS_FP8 | FLMR_CORPUS_FP16))
     return fail(FLMR_ERR_INVALID_ARG, "builder flags 0x%x: only FLMR_CORPUS_FP8 or FLMR_CORPUS_FP16 applies to a "
                 "streamed load", flags);
-  if ((flags & FLMR_CORPUS_FP8) && (flags & FLMR_CORPUS_FP16))
-    return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_FP16 and FLMR_CORPUS_FP8 exclude each other");
+  Elem elem;
+  if (int rc = storage_from_flags(flags, &elem)) return rc;
   if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
   if (n_passages <= 0 || !h_doclens) return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null doclens");
   flmr_corpus_builder* b = new (std::nothrow) flmr_corpus_builder();
@@ -2222,32 +2187,16 @@ int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, 
     flmr_corpus_builder_destroy(b);
     return code;
   };
-  b->soff.resize(n_passages + 1);
-  b->poff.resize(n_passages + 1);
   b->doclens.assign(h_doclens, h_doclens + n_passages);
-  b->soff[0] = b->poff[0] = 0;
-  for (int64_t p = 0; p < n_passages; ++p) {
-    const int32_t len = h_doclens[p];
-    if (len < 1)
-      return bail(fail(FLMR_ERR_INVALID_ARG, "passage %lld has length %d; zero-length passages have no defined MaxSim score",
-                       (long long)p, len));
-    b->soff[p + 1] = b->soff[p] + len;
-    b->poff[p + 1] = b->poff[p] + (len + kGroup - 1) / kGroup * kGroup;
-    b->aligned &= (len % kGroup == 0);
-  }
+  if (int rc = passage_offsets(h_doclens, n_passages, &b->soff, &b->poff, &b->aligned)) return bail(rc);
   const int64_t n_rows = b->poff[n_passages];
   if (n_rows + kTileN >= (1ll << 31))
     return bail(fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
                      (long long)n_rows));
   DeviceGuard guard(device);
   if (!guard.ok) return bail(fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device));
-  cudaDeviceProp prop;
-  cudaError_t e = cudaGetDeviceProperties(&prop, device);
-  if (e != cudaSuccess) return bail(fail(FLMR_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e)));
-  if (prop.major != 9 || prop.minor != 0)
-    return bail(fail(FLMR_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is sm_90a only", device, prop.major,
-                     prop.minor));
-  b->sm_count = prop.multiProcessorCount;
+  int sm_count;
+  if (int rc = sm90_count(device, &sm_count)) return bail(rc);
   flmr_corpus* c = new (std::nothrow) flmr_corpus();
   if (!c) return bail(fail(FLMR_ERR_OOM, "host allocation failed"));
   b->corpus = c;
@@ -2256,12 +2205,13 @@ int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, 
   c->n_tokens = b->soff[n_passages];
   c->n_rows = n_rows;
   c->pid_base = pid_base;
-  c->fp8 = (flags & FLMR_CORPUS_FP8) != 0;
-  c->f16 = (flags & FLMR_CORPUS_FP16) != 0;
+  c->elem = elem;
+  c->sm_total = sm_count;
   if (int rc = alloc_token_matrix(c)) return bail(rc);
   // an e4m3 corpus always goes through the scatter kernel, which writes the master and the e4m3 copy
-  const bool scatter = !b->aligned || c->fp8;
+  const bool scatter = !b->aligned || elem == Elem::kE4M3;
   const size_t buf_bytes = static_cast<size_t>(flmr_corpus_builder::kBufRows) * kDim * 2;
+  cudaError_t e;
   if ((e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking)) != cudaSuccess)
     return bail(fail(FLMR_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e)));
   for (int i = 0; i < flmr_corpus_builder::kBufs; ++i) {
@@ -2303,7 +2253,7 @@ int builder_feed(flmr_corpus_builder* b, int64_t n_rows, Fill fill) {
     b->fill_s += (t1.tv_sec - t0.tv_sec) + 1e-9 * (t1.tv_nsec - t0.tv_nsec);
     const size_t bytes = static_cast<size_t>(rows) * kDim * 2;
     const int64_t s0 = b->rows_done;
-    if (b->aligned && !c->fp8) {                             // packed order == stored order: straight into place
+    if (b->aligned && c->elem != Elem::kE4M3) {   // packed order == stored order: straight into place
       FLMR_CUDA(cudaMemcpyAsync(c->d_tokens + s0 * kDim, b->h_pin[i], bytes, cudaMemcpyHostToDevice, b->stream));
     } else {
       FLMR_CUDA(cudaMemcpyAsync(b->d_stage[i], b->h_pin[i], bytes, cudaMemcpyHostToDevice, b->stream));
@@ -2373,7 +2323,9 @@ int flmr_corpus_builder_finish(flmr_corpus_builder_t* b, flmr_corpus_t** out, do
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
   FLMR_CUDA(cudaStreamSynchronize(b->stream));
-  if (int rc = finish_corpus(c, b->poff, b->doclens.data(), b->sm_count)) return rc;
+  if (int rc = build_layout(c->elem, c->d_tokens, c->d_fp8, c->n_rows, b->poff, b->doclens.data(), c->sm_total,
+                            &c->layout))
+    return rc;
   if (host_fill_seconds) *host_fill_seconds = b->fill_s;
   b->corpus = nullptr;     // ownership passes to the caller
   flmr_corpus_builder_destroy(b);
@@ -2383,7 +2335,6 @@ int flmr_corpus_builder_finish(flmr_corpus_builder_t* b, flmr_corpus_t** out, do
 
 int flmr_corpus_builder_destroy(flmr_corpus_builder_t* b) {
   if (!b) return FLMR_OK;
-  const int device = b->corpus ? b->corpus->device : -1;
   if (b->stream) cudaStreamSynchronize(b->stream);
   for (int i = 0; i < flmr_corpus_builder::kBufs; ++i) {
     if (b->h_pin[i]) cudaFreeHost(b->h_pin[i]);
@@ -2394,7 +2345,6 @@ int flmr_corpus_builder_destroy(flmr_corpus_builder_t* b) {
   cudaFree(b->d_poff);
   if (b->stream) cudaStreamDestroy(b->stream);
   if (b->corpus) flmr_corpus_destroy(b->corpus);
-  (void)device;
   delete b;
   return FLMR_OK;
 }
@@ -2407,17 +2357,18 @@ int flmr_corpus_info(const flmr_corpus_t* c, flmr_corpus_info_t* out) {
   out->pid_base = c->pid_base;
   out->dim = kDim;
   out->device = c->device;
-  out->n_ctas = c->n_ctas;
+  out->n_ctas = c->layout.n_ctas;
   out->adopted = c->adopted ? 1 : 0;
-  out->n_tiles = c->n_tiles;
-  out->hbm_bytes = c->hbm_bytes;
+  out->n_tiles = c->layout.cta.n_tiles;
+  out->hbm_bytes = hbm_bytes(c);
   return FLMR_OK;
 }
 
 int flmr_corpus_storage(const flmr_corpus_t* c, int* storage, int64_t* host_bytes) {
   if (!c) return fail(FLMR_ERR_INVALID_ARG, "null argument");
-  if (storage) *storage = c->fp8 ? 1 : c->f16 ? 2 : 0;
-  if (host_bytes) *host_bytes = c->fp8 ? c->n_rows * kDim * 2 : 0;
+  const bool e4m3 = c->elem == Elem::kE4M3;
+  if (storage) *storage = e4m3 ? 1 : c->elem == Elem::kF16 ? 2 : 0;   // the ABI's codes, not the Elem values
+  if (host_bytes) *host_bytes = e4m3 ? c->n_rows * kDim * 2 : 0;
   return FLMR_OK;
 }
 
@@ -2427,16 +2378,8 @@ int flmr_corpus_append(flmr_corpus_t* c, const void* tokens, const int32_t* h_do
   if (n_passages <= 0) return fail(FLMR_ERR_INVALID_ARG, "n_passages=%lld must be >= 1", (long long)n_passages);
   const int64_t old_n = c->n_passages, old_rows = c->n_rows;
   // the new passages, relative to their first: packed (soff) and padded (poff) row offsets
-  std::vector<int64_t> soff(n_passages + 1), poff(n_passages + 1);
-  soff[0] = poff[0] = 0;
-  for (int64_t p = 0; p < n_passages; ++p) {
-    const int32_t len = h_doclens[p];
-    if (len < 1)
-      return fail(FLMR_ERR_INVALID_ARG, "passage %lld has length %d; zero-length passages have no defined MaxSim score",
-                  (long long)p, len);
-    soff[p + 1] = soff[p] + len;
-    poff[p + 1] = poff[p] + (len + kGroup - 1) / kGroup * kGroup;
-  }
+  std::vector<int64_t> soff, poff;
+  if (int rc = passage_offsets(h_doclens, n_passages, &soff, &poff, nullptr)) return rc;
   const int64_t new_n = old_n + n_passages, new_rows = old_rows + poff[n_passages];
   // the partition stores first passage ids and CTA row starts as int32, the scan's top-k key a 32-bit ~local id
   if (new_n > 0x7fffffffll)
@@ -2446,18 +2389,15 @@ int flmr_corpus_append(flmr_corpus_t* c, const void* tokens, const int32_t* h_do
                 (long long)new_rows);
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
-  cudaPointerAttributes attr{};
-  const bool is_device_ptr = (cudaPointerGetAttributes(&attr, tokens) == cudaSuccess) &&
-                             (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
-  cudaGetLastError();
-  if (is_device_ptr && attr.type == cudaMemoryTypeDevice && attr.device != c->device)
-    return fail(FLMR_ERR_INVALID_ARG, "token matrix lives on device %d, corpus on %d", attr.device, c->device);
+  bool is_device_ptr;
+  if (int rc = token_source(tokens, c->device, &is_device_ptr)) return rc;
   // searches enqueued before this call (any stream) finish on the corpus as it was
   FLMR_CUDA(cudaDeviceSynchronize());
 
   // --- 1. room for the new rows: mapped behind the library-owned matrices, which stay where they are ---
   const size_t row_bytes = static_cast<size_t>(kDim) * 2;
-  if (c->fp8) {
+  const bool e4m3 = c->elem == Elem::kE4M3;
+  if (e4m3) {
     if (int rc = gm_grow(&c->vm_fp8, c->device, static_cast<size_t>(new_rows) * kDim)) return rc;
     // the bf16 master is pinned host memory: reallocated and copied (old + new size are held for the copy)
     void* h = nullptr;
@@ -2497,61 +2437,44 @@ int flmr_corpus_append(flmr_corpus_t* c, const void* tokens, const int32_t* h_do
   // --- 2. the new rows into place (bf16, and e4m3 for an fp8 corpus), behind the old ones ---
   cudaError_t e = pack_passages(tokens, is_device_ptr, soff, poff, h_doclens, n_passages,
                                 reinterpret_cast<uint4*>(c->d_tokens + old_rows * kDim),
-                                c->fp8 ? reinterpret_cast<uint2*>(c->d_fp8 + old_rows * kDim) : nullptr);
+                                e4m3 ? reinterpret_cast<uint2*>(c->d_fp8 + old_rows * kDim) : nullptr);
   if (e != cudaSuccess) return fail(FLMR_ERR_CUDA, "packing the appended passages failed: %s", cudaGetErrorString(e));
 
-  // --- 3. offsets, lengths, partition, tensor maps and tombstones for the grown corpus, then swapped in ---
-  flmr_corpus nc = *c;
-  nc.d_poff = nullptr;
-  nc.d_doclen = nullptr;
-  nc.d_cta_row_begin = nullptr;
-  nc.d_cta_tile_base = nullptr;
-  nc.d_tile_end_mask = nullptr;
-  nc.d_tile_first_pid = nullptr;
-  nc.d_pair_row_begin = nullptr;
-  nc.d_pair_tile_base = nullptr;
-  nc.d_pair_end_mask = nullptr;
-  nc.d_pair_first_pid = nullptr;
-  nc.n_pairs = 0;
-  nc.n_tiles_pair = 0;
-  nc.d_dead = nullptr;
-  nc.d_slot_pid = nullptr;
-  nc.n_passages = new_n;
-  nc.n_tokens = c->n_tokens + soff[n_passages];
-  nc.n_rows = new_rows;
-  nc.hbm_bytes = new_rows * (c->fp8 ? kDim : kDim * 2);
-  std::vector<int64_t> all_poff(c->h_poff);
-  all_poff.reserve(new_n + 1);
+  // --- 3. layout and tombstones for the grown corpus, then swapped in ---
+  std::vector<int64_t> all_poff(c->layout.h_poff);
   for (int64_t p = 1; p <= n_passages; ++p) all_poff.push_back(old_rows + poff[p]);
-  std::vector<int32_t> all_len(c->h_doclen);
+  std::vector<int32_t> all_len(c->layout.h_doclen);
   all_len.insert(all_len.end(), h_doclens, h_doclens + n_passages);
-  int rc = FLMR_OK;
-  if (c->h_slot_pid.empty()) {
-    if (!c->h_dead.empty()) {
-      nc.h_dead.resize((new_n + 31) / 32, 0u);
-      rc = dev_upload(&nc.d_dead, nc.h_dead, &nc.hbm_bytes);
-    }
-  } else {
-    // compacted: the new passages take the next slots and the next ids
-    for (int64_t p = 0; p < n_passages; ++p) nc.h_slot_pid.push_back(c->pid_base + old_n + p);
-    nc.h_dead.resize((new_n + 31) / 32, 0u);
-    rc = dev_upload(&nc.d_slot_pid, nc.h_slot_pid, &nc.hbm_bytes);
-    if (!rc && c->d_dead) {
-      bool any = false;
-      rc = dev_upload(&nc.d_dead, dead_by_slot(nc.h_slot_pid, nc.pid_base, nc.h_dead, &any), &nc.hbm_bytes);
-    }
-  }
-  if (!rc) rc = finish_corpus(&nc, all_poff, all_len.data(), c->sm_total);
+  std::vector<int64_t> slot_pid(c->h_slot_pid);
+  std::vector<uint32_t> dead(c->h_dead);
+  uint32_t* d_dead = nullptr;
+  int64_t* d_slot_pid = nullptr;
+  // compacted: the new passages take the next slots and the next ids (h_dead is never empty after a compaction)
+  const bool compacted = !slot_pid.empty();
+  if (compacted)
+    for (int64_t p = 0; p < n_passages; ++p) slot_pid.push_back(c->pid_base + old_n + p);
+  if (!dead.empty()) dead.resize((new_n + 31) / 32, 0u);
+  int rc = compacted ? dev_upload(&d_slot_pid, slot_pid, nullptr) : FLMR_OK;
+  if (!rc && c->d_dead)   // d_dead exists once anything is deleted, except right after a compaction
+    rc = dev_upload(&d_dead, compacted ? dead_by_slot(slot_pid, c->pid_base, dead) : dead, nullptr);
+  SlotLayout layout;
+  if (!rc) rc = build_layout(c->elem, c->d_tokens, c->d_fp8, new_rows, all_poff, all_len.data(), c->sm_total, &layout);
   if (rc) {
-    free_metadata(&nc);
-    cudaFree(nc.d_dead);
-    cudaFree(nc.d_slot_pid);
+    cudaFree(d_dead);
+    cudaFree(d_slot_pid);
     return rc;
   }
-  free_metadata(c);
+  free_layout(&c->layout);
   cudaFree(c->d_dead);
   cudaFree(c->d_slot_pid);
-  *c = std::move(nc);
+  c->layout = std::move(layout);
+  c->d_dead = d_dead;
+  c->d_slot_pid = d_slot_pid;
+  c->h_slot_pid.swap(slot_pid);
+  c->h_dead.swap(dead);
+  c->n_passages = new_n;
+  c->n_tokens += soff[n_passages];
+  c->n_rows = new_rows;
   if (first_pid) *first_pid = c->pid_base + old_n;
   return FLMR_OK;
 }
@@ -2578,17 +2501,11 @@ int flmr_corpus_delete(flmr_corpus_t* c, const int64_t* h_pids, int64_t n) {
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
   // a compacted corpus: the device bitmap is indexed by slot (a newly deleted id always has one: a compacted-away id
   // was deleted already)
-  bool any = false;
-  const std::vector<uint32_t> by_slot =
-      c->h_slot_pid.empty() ? std::vector<uint32_t>() : dead_by_slot(c->h_slot_pid, c->pid_base, dead, &any);
-  const std::vector<uint32_t>& words = c->h_slot_pid.empty() ? dead : by_slot;
+  const std::vector<uint32_t> words = c->h_slot_pid.empty() ? dead : dead_by_slot(c->h_slot_pid, c->pid_base, dead);
   // searches enqueued before this call (any stream) finish with the old bitmap
   FLMR_CUDA(cudaDeviceSynchronize());
   const size_t bytes = words.size() * sizeof(uint32_t);
-  if (!c->d_dead) {
-    FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&c->d_dead), bytes));
-    c->hbm_bytes += static_cast<int64_t>(bytes);
-  }
+  if (!c->d_dead) FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&c->d_dead), bytes));
   FLMR_CUDA(cudaMemcpy(c->d_dead, words.data(), bytes, cudaMemcpyHostToDevice));
   c->h_dead.swap(dead);
   c->n_deleted += added;
@@ -2635,14 +2552,14 @@ int flmr_corpus_compact(flmr_corpus_t* c, int64_t* n_removed, int64_t* bytes_rel
   for (int64_t s = 0; s < ns; ++s) {
     if (!keep[s]) continue;
     slot_pid.push_back(c->h_slot_pid.empty() ? c->pid_base + s : c->h_slot_pid[s]);
-    lens.push_back(c->h_doclen[s]);
-    poff.push_back(poff.back() + (c->h_poff[s + 1] - c->h_poff[s]));
+    lens.push_back(c->layout.h_doclen[s]);
+    poff.push_back(poff.back() + (c->layout.h_poff[s + 1] - c->layout.h_poff[s]));
   }
   int64_t n_tokens = 0;
   for (int32_t l : lens) n_tokens += l;
   const int64_t new_rows = poff.back();
   std::vector<MovePiece> plan;
-  plan_compaction(kept_runs(c->h_poff, keep), kCompactChunkRows, !c->adopted, &plan);
+  plan_compaction(kept_runs(c->layout.h_poff, keep), kCompactChunkRows, !c->adopted, &plan);
 
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
@@ -2650,32 +2567,17 @@ int flmr_corpus_compact(flmr_corpus_t* c, int64_t* n_removed, int64_t* bytes_rel
   FLMR_CUDA(cudaDeviceSynchronize());
 
   // --- 2. everything that can fail on allocation, before a row moves: the matrix an adopted corpus is copied into,
-  // the schedule on the device, the staging buffer, and the metadata of the compacted corpus ---
-  const size_t row_bytes = c->fp8 ? kDim : kDim * 2;   // of the matrix in HBM
-  flmr_corpus nc = *c;
-  nc.d_poff = nullptr;
-  nc.d_doclen = nullptr;
-  nc.d_cta_row_begin = nullptr;
-  nc.d_cta_tile_base = nullptr;
-  nc.d_tile_end_mask = nullptr;
-  nc.d_tile_first_pid = nullptr;
-  nc.d_pair_row_begin = nullptr;
-  nc.d_pair_tile_base = nullptr;
-  nc.d_pair_end_mask = nullptr;
-  nc.d_pair_first_pid = nullptr;
-  nc.n_pairs = 0;
-  nc.n_tiles_pair = 0;
-  nc.d_dead = nullptr;          // every deleted slot is removed
-  nc.d_slot_pid = nullptr;
-  nc.n_tokens = n_tokens;
-  nc.n_rows = new_rows;
-  nc.hbm_bytes = new_rows * static_cast<int64_t>(row_bytes);
+  // the schedule on the device, the staging buffer, and the slot -> id map and layout of the compacted corpus ---
+  const bool e4m3 = c->elem == Elem::kE4M3;
+  const size_t row_bytes = hbm_row_bytes(c->elem);   // of the matrix in HBM
   GrowableMatrix copy;          // an adopted corpus: the library-owned matrix its live rows go to
-  int64_t *d_pdst = nullptr, *d_psrc = nullptr;
+  __nv_bfloat16* d_tokens = c->d_tokens;   // where the rows end up
+  int64_t *d_slot_pid = nullptr, *d_pdst = nullptr, *d_psrc = nullptr;
   uint4* stage = nullptr;
+  SlotLayout layout;
   auto release = [&](int code) {
-    free_metadata(&nc);
-    cudaFree(nc.d_slot_pid);
+    free_layout(&layout);
+    cudaFree(d_slot_pid);
     gm_free(&copy);
     cudaFree(d_pdst);
     cudaFree(d_psrc);
@@ -2685,7 +2587,7 @@ int flmr_corpus_compact(flmr_corpus_t* c, int64_t* n_removed, int64_t* bytes_rel
   int rc = FLMR_OK;
   if (c->adopted) {
     if ((rc = gm_grow(&copy, c->device, static_cast<size_t>(new_rows) * row_bytes))) return release(rc);
-    nc.d_tokens = reinterpret_cast<__nv_bfloat16*>(copy.base);
+    d_tokens = reinterpret_cast<__nv_bfloat16*>(copy.base);
   }
   {
     std::vector<int64_t> pdst(plan.size()), psrc(plan.size());
@@ -2709,23 +2611,20 @@ int flmr_corpus_compact(flmr_corpus_t* c, int64_t* n_removed, int64_t* bytes_rel
                             cudaGetErrorString(e)));
     }
   }
-  nc.h_slot_pid = slot_pid;
-  if ((rc = dev_upload(&nc.d_slot_pid, nc.h_slot_pid, &nc.hbm_bytes))) return release(rc);
-  if ((rc = finish_corpus(&nc, poff, lens.data(), c->sm_total))) return release(rc);
+  if ((rc = dev_upload(&d_slot_pid, slot_pid, nullptr)) ||
+      (rc = build_layout(c->elem, d_tokens, c->d_fp8, new_rows, poff, lens.data(), c->sm_total, &layout)))
+    return release(rc);
 
   // --- 3. the rows move: the HBM matrix on the device, the pinned bf16 master of an e4m3 corpus on the host ---
   cudaError_t e = cudaSuccess;
   if (!plan.empty()) {
-    if (c->fp8) {
-      e = run_moves(plan, d_pdst, d_psrc, reinterpret_cast<const uint4*>(c->d_fp8), reinterpret_cast<uint4*>(c->d_fp8),
-                    stage, static_cast<int>(kDim / 16));
-      // ordered memmove in place: every destination lies at or below its source, and earlier pieces come first
+    uint4* rows = reinterpret_cast<uint4*>(e4m3 ? static_cast<void*>(c->d_fp8) : c->d_tokens);   // in HBM
+    e = run_moves(plan, d_pdst, d_psrc, rows, e4m3 ? rows : reinterpret_cast<uint4*>(d_tokens), stage,
+                  static_cast<int>(row_bytes / 16));
+    if (e4m3) {   // ordered memmove in place: every destination lies at or below its source, earlier pieces first
       char* m = static_cast<char*>(c->h_master);
       for (const MovePiece& mp : plan)
         memmove(m + mp.dst * kDim * 2, m + mp.src * kDim * 2, static_cast<size_t>(mp.rows) * kDim * 2);
-    } else {
-      e = run_moves(plan, d_pdst, d_psrc, reinterpret_cast<const uint4*>(c->d_tokens),
-                    reinterpret_cast<uint4*>(nc.d_tokens), stage, static_cast<int>(kDim * 2 / 16));
     }
   }
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
@@ -2737,17 +2636,21 @@ int flmr_corpus_compact(flmr_corpus_t* c, int64_t* n_removed, int64_t* bytes_rel
   // --- 4. physical memory wholly behind the new end goes back to the device; the handle takes the new state ---
   size_t released = 0;
   if (c->adopted) {
-    nc.vm_tokens = copy;          // the caller's buffer is no longer referenced
-    nc.adopted = false;
-  } else if (c->fp8) {
-    released = gm_shrink(&nc.vm_fp8, static_cast<size_t>(new_rows) * kDim);
+    c->vm_tokens = copy;          // the caller's buffer is no longer referenced
+    c->d_tokens = d_tokens;
+    c->adopted = false;
   } else {
-    released = gm_shrink(&nc.vm_tokens, static_cast<size_t>(new_rows) * kDim * 2);
+    released = gm_shrink(e4m3 ? &c->vm_fp8 : &c->vm_tokens, static_cast<size_t>(new_rows) * row_bytes);
   }
-  free_metadata(c);
+  free_layout(&c->layout);
   cudaFree(c->d_dead);
   cudaFree(c->d_slot_pid);
-  *c = std::move(nc);
+  c->layout = std::move(layout);
+  c->d_dead = nullptr;          // every deleted slot is removed
+  c->d_slot_pid = d_slot_pid;
+  c->h_slot_pid.swap(slot_pid);
+  c->n_tokens = n_tokens;
+  c->n_rows = new_rows;
   if (n_removed) *n_removed = removed;
   if (bytes_released) *bytes_released = static_cast<int64_t>(released);
   return FLMR_OK;
@@ -2783,16 +2686,16 @@ int flmr_workspace_create(const flmr_corpus_t* c, int max_queries, int max_nq,
   if ((e = cudaMalloc(reinterpret_cast<void**>(&ws->d_qpad), qbytes)) != cudaSuccess ||
       (e = cudaMemset(ws->d_qpad, 0, qbytes)) != cudaSuccess ||
       (e = cudaMalloc(reinterpret_cast<void**>(&ws->d_cand_keys),
-                      static_cast<size_t>(c->n_ctas) * max_queries * kMaxK * 8)) != cudaSuccess ||
+                      static_cast<size_t>(c->layout.n_ctas) * max_queries * kMaxK * 8)) != cudaSuccess ||
       (e = cudaHostAlloc(reinterpret_cast<void**>(&ws->h_status), sizeof(int), cudaHostAllocMapped)) != cudaSuccess ||
       (e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&ws->d_status), ws->h_status, 0)) != cudaSuccess)
     return bail(fail(FLMR_ERR_CUDA, "workspace allocation failed: %s", cudaGetErrorString(e)));
-  ws->cand_lists = c->n_ctas;
+  ws->cand_lists = c->layout.n_ctas;
   *ws->h_status = 0;
   if (max_nq > kRbMax * 32) {   // row-sliced queries expected: size their partial-score rows now
     std::vector<PassPlan> plan;
     int group = 1;
-    plan_passes(max_queries, max_nq, c->n_pairs > 0, &plan, &group, nullptr);
+    plan_passes(max_queries, max_nq, c->layout.n_pairs > 0, &plan, &group, nullptr);
     if (int rc = ensure_acc(ws, static_cast<int64_t>(group) * c->n_passages)) return bail(rc);
   }
 #ifdef FLMR_DEBUG
@@ -2863,7 +2766,7 @@ int run_listed(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
     if (h_off[b + 1] < h_off[b])
       return fail(FLMR_ERR_INVALID_ARG, "h_list_offsets decreases at query %d", b);
   if (h_off[n_queries] > h_off[0] && !d_pids) return fail(FLMR_ERR_INVALID_ARG, "d_list_pids is null");
-  if (g_scan_variant == 3 || g_scan_variant == 4)
+  if (!pick_scan(c->elem, true, g_scan_variant, 0).fn)   // as in run_search
     return fail(FLMR_ERR_UNSUPPORTED, "scan variant %d has no plan-mode (listed) kernel", g_scan_variant);
   if (n_queries == 0) return FLMR_OK;
   DeviceGuard guard(c->device);
@@ -2932,9 +2835,9 @@ int flmr_debug_listed_plan(const flmr_corpus_t* c, flmr_workspace_t* ws, int n_q
     if (nt > lp.t_bound[i] || nu > lp.u_bound[i])
       return fail(FLMR_ERR_KERNEL, "pass %d: plan of %lld tiles exceeds its bound %lld", i, (long long)nt,
                   (long long)lp.t_bound[i]);
-    out.insert(out.end(), {q.q_first, q.n_q, c->n_ctas, nu, nt, lp.t_bound[i]});
+    out.insert(out.end(), {q.q_first, q.n_q, c->layout.n_ctas, nu, nt, lp.t_bound[i]});
     std::vector<int32_t> slots_(nu), row(nt), first(nt);
-    std::vector<int64_t> base(c->n_ctas + 1);
+    std::vector<int64_t> base(c->layout.n_ctas + 1);
     std::vector<uint32_t> mask(nt);
     FLMR_CUDA(cudaMemcpy(slots_.data(), lp.u_slot + q.u_off, nu * 4, cudaMemcpyDeviceToHost));
     FLMR_CUDA(cudaMemcpy(base.data(), lp.cta_tile_base + q.c_off, base.size() * 8, cudaMemcpyDeviceToHost));
@@ -3073,8 +2976,8 @@ int flmr_corpus_gather(const flmr_corpus_t* c, const int64_t* d_pids, int64_t n_
     d_pids = slot_ids;
   }
   flmr_gather_kernel<<<static_cast<unsigned>(blocks), threads, 0, st>>>(
-      reinterpret_cast<const uint2*>(c->d_tokens), c->d_poff, c->d_doclen, c->d_dead, d_pids, n_pids, nd_max,
-      slots(c), c->pid_base, static_cast<uint2*>(d_out_bf16), d_mask);
+      reinterpret_cast<const uint2*>(c->d_tokens), c->layout.d_poff, c->layout.d_doclen, c->d_dead, d_pids, n_pids,
+      nd_max, slots(c), c->pid_base, static_cast<uint2*>(d_out_bf16), d_mask);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;
@@ -3370,9 +3273,10 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
   if (c->d_slot_pid) {
     if (int rc = scratch.alloc(&out, static_cast<size_t>(n_queries) * ns * sizeof(float))) return rc;
   }
-  if (!c->fp8) {
-    (c->f16 ? flmr_simt_maxsim_kernel<Elem::kF16> : flmr_simt_maxsim_kernel<Elem::kBF16>)<<<grid, threads, 0, st>>>(
-        c->d_tokens, c->d_poff, c->d_doclen, c->d_dead, d_q, nq, init, out, ns);
+  const SlotLayout& l = c->layout;
+  if (c->elem != Elem::kE4M3) {
+    auto* kernel = c->elem == Elem::kF16 ? flmr_simt_maxsim_kernel<Elem::kF16> : flmr_simt_maxsim_kernel<Elem::kBF16>;
+    kernel<<<grid, threads, 0, st>>>(c->d_tokens, l.d_poff, l.d_doclen, c->d_dead, d_q, nq, init, out, ns);
     FLMR_CUDA(cudaGetLastError());
     ++g_launches;
   } else {
@@ -3382,7 +3286,7 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
     if (int rc = scratch.alloc(&q8, static_cast<size_t>(n_chunks) * 16)) return rc;
     flmr_round_e4m3_kernel<<<static_cast<unsigned>((n_chunks + 255) / 256), 256, 0, st>>>(
         static_cast<const uint4*>(d_q), reinterpret_cast<uint4*>(q8), n_chunks);
-    flmr_simt_maxsim_kernel<Elem::kE4M3><<<grid, threads, 0, st>>>(c->d_fp8, c->d_poff, c->d_doclen, c->d_dead, q8, nq,
+    flmr_simt_maxsim_kernel<Elem::kE4M3><<<grid, threads, 0, st>>>(c->d_fp8, l.d_poff, l.d_doclen, c->d_dead, q8, nq,
                                                                    init, out, ns);
     const cudaError_t e = cudaGetLastError();
     g_launches += 2;
@@ -3418,12 +3322,8 @@ int flmr_debug_build_partition(const int32_t* h_doclens, int64_t n_passages, int
                                int64_t tile_capacity, int64_t* n_tiles_out) {
   if (!h_doclens || n_passages <= 0 || n_ctas < 1 || !cta_row_begin || !cta_tile_base || !n_tiles_out)
     return fail(FLMR_ERR_INVALID_ARG, "bad argument");
-  std::vector<int64_t> poff(n_passages + 1);
-  poff[0] = 0;
-  for (int64_t p = 0; p < n_passages; ++p) {
-    if (h_doclens[p] < 1) return fail(FLMR_ERR_INVALID_ARG, "passage %lld has length %d", (long long)p, h_doclens[p]);
-    poff[p + 1] = poff[p] + (h_doclens[p] + kGroup - 1) / kGroup * kGroup;
-  }
+  std::vector<int64_t> poff;
+  if (int rc = passage_offsets(h_doclens, n_passages, nullptr, &poff, nullptr)) return rc;
   n_ctas = static_cast<int>(std::min<int64_t>(n_ctas, n_passages));
   std::vector<int32_t> rb, fp;
   std::vector<int64_t> tb;
@@ -3464,11 +3364,8 @@ int flmr_debug_compact_plan(const int32_t* h_doclens, int64_t n_passages, const 
   if (!h_doclens || n_passages <= 0 || n_deleted < 0 || (n_deleted > 0 && !h_deleted) || chunk_rows < 0 ||
       !n_moves_out)
     return fail(FLMR_ERR_INVALID_ARG, "bad argument");
-  std::vector<int64_t> poff(n_passages + 1, 0);
-  for (int64_t p = 0; p < n_passages; ++p) {
-    if (h_doclens[p] < 1) return fail(FLMR_ERR_INVALID_ARG, "passage %lld has length %d", (long long)p, h_doclens[p]);
-    poff[p + 1] = poff[p] + (h_doclens[p] + kGroup - 1) / kGroup * kGroup;
-  }
+  std::vector<int64_t> poff;
+  if (int rc = passage_offsets(h_doclens, n_passages, nullptr, &poff, nullptr)) return rc;
   std::vector<char> keep(n_passages, 1);
   for (int64_t i = 0; i < n_deleted; ++i) {
     if (h_deleted[i] < 0 || h_deleted[i] >= n_passages)
