@@ -57,6 +57,13 @@
  *     corpus' device, "h_" parameters are HOST pointers;
  *   - compute entry points are asynchronous on the supplied CUDA stream (passed as void* so the
  *     header needs no CUDA include; NULL = default stream);
+ *   - CUDA graph capture: flmr_maxsim_scores, flmr_maxsim_topk and their _allowed forms (every storage, compacted
+ *     corpora included), flmr_topk_select, flmr_topk_merge, flmr_corpus_gather, flmr_maxsim_argmax /
+ *     flmr_maxsim_backward with their _grouped and _fp16 forms (either arg-max kernel) and flmr_ib_loss may be captured
+ *     on the stream they are given and replayed with new contents in the same buffers, once a call of the same shape
+ *     has run outside the capture on the same workspace (it sizes the workspace's buffers), and while the corpus does
+ *     not change.  The _listed calls are not capturable: their host offsets size the plan when the call is made, and
+ *     their host tables are copied then.  flmr_plaid_decode synchronises its stream and is not capturable either;
  *   - a corpus changes only through flmr_corpus_append, flmr_corpus_delete and flmr_corpus_compact.  Between
  *     those calls a handle may be shared by threads; concurrent searches on one handle must use distinct
  *     flmr_workspace handles.  The three mutating calls must not run concurrently with any other call on the
@@ -303,7 +310,10 @@ int flmr_maxsim_topk_allowed(const flmr_corpus_t* corpus, flmr_workspace_t* ws, 
  * Restricted search over id lists, at the cost of the listed passages: the same scan kernel runs over a per-call plan
  * of the listed passages' rows only, re-balanced over the persistent CTAs (the planner runs on the device, in stream
  * order, without a host synchronisation).  The fold and the reducer are those of every other scan, so results are
- * bitwise those of the _allowed calls for bitmaps of the same sets.
+ * bitwise those of the _allowed calls for bitmaps of the same sets.  The host tables of a call (h_list_offsets and the
+ * pass plan of each call chunk) are copied when the call is made, so h_list_offsets may be reused as soon as the call
+ * returns.  The first call whose plan outgrows the workspace's plan buffer waits for the device (the buffer is
+ * reallocated).  These calls cannot be captured in a CUDA graph.
  *   h_list_offsets  HOST int64 [n_queries + 1], non-decreasing: query b's list is
  *                   d_list_pids[h_list_offsets[b] .. h_list_offsets[b + 1])
  *   d_list_pids     DEVICE int64 GLOBAL ids (pid_base + local id), in any order, duplicates allowed.  Ids outside this

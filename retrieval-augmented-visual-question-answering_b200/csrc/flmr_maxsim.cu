@@ -1148,7 +1148,8 @@ struct flmr_comm {
   int64_t* d_send_p = nullptr;
   float* d_recv_s = nullptr;
   int64_t* d_recv_p = nullptr;
-  int64_t capacity = 0;   // entries (B * k) the send buffers hold
+  int64_t capacity = 0;        // entries (B * k) per rank the receive buffers hold
+  int64_t send_capacity = 0;   // entries (B * k) the send buffers hold
 };
 
 namespace {
@@ -3522,13 +3523,15 @@ int flmr_maxsim_topk_sharded_allowed(const flmr_corpus_t* corpus, flmr_workspace
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", comm->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t n = static_cast<int64_t>(n_queries) * k;
-  if (comm->capacity < n || !comm->d_send_s) {
+  if (comm->send_capacity < n) {   // sized apart from the receive buffers, which flmr_topk_exchange alone may grow
     cudaFree(comm->d_send_s);
     cudaFree(comm->d_send_p);
     comm->d_send_s = nullptr;
     comm->d_send_p = nullptr;
+    comm->send_capacity = 0;
     FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&comm->d_send_s), static_cast<size_t>(n) * sizeof(float)));
     FLMR_CUDA(cudaMalloc(reinterpret_cast<void**>(&comm->d_send_p), static_cast<size_t>(n) * sizeof(int64_t)));
+    comm->send_capacity = n;
   }
   // this rank's shard (the fused scan fills short lists with (-inf, -1), which the merge ignores)
   if (int rc = run_search(corpus, ws, d_q, n_queries, nq, flags, k, d_allow, allow_stride_words, nullptr,

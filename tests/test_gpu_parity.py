@@ -384,33 +384,51 @@ def test_big_cta_pair_passes_properties(R, big):
 def test_search_call_is_cuda_graph_capturable(R):
     """flmr_maxsim_topk / flmr_maxsim_scores enqueue their launches (query staging, single-CTA and cluster scan
     passes, merges) on the caller's stream and synchronise nothing: a call captured into a CUDA graph and replayed
-    on NEW query contents gives exactly what the eager call gives — whole queries, CTA-pair passes forced, and
-    row-sliced queries whose partial scores live in the workspace."""
+    on NEW query contents gives exactly what the eager call gives — whole queries, CTA-pair passes forced, the product's
+    split kernel and row-sliced queries (variant 0), fp16 and e4m3 corpora, allow bitmaps (replayed with new contents
+    too), and a compacted corpus with deletions, whose score rows and bitmaps go through stream-ordered scratch."""
     from ravqa_b200 import _cabi
     L = _cabi.lib()
-    for (n, nd, B, nq, k, variant) in [(3000, 60, 5, 97, 7, 0), (2000, 120, 6, 320, 10, 4), (900, 50, 7, 832, 5, 4)]:
+    cases = [  # n, nd, B, nq, k, variant, storage, allow, compact
+        (3000, 60, 5, 97, 7, 0, "bf16", False, False), (2000, 120, 6, 320, 10, 4, "bf16", False, False),
+        (900, 50, 7, 832, 5, 4, "bf16", False, False), (2000, 120, 6, 320, 10, 0, "bf16", False, False),
+        (900, 50, 3, 832, 128, 0, "bf16", False, False), (1500, 80, 12, 32, 128, 0, "fp16", False, False),
+        (1500, 80, 4, 320, 16, 0, "fp8", False, False), (2500, 60, 5, 97, 128, 0, "bf16", True, False),
+        (2500, 60, 3, 320, 20, 0, "fp8", True, True), (2500, 60, 6, 32, 50, 0, "fp16", False, True),
+        (1200, 40, 2, 832, 9, 0, "bf16", True, True)]
+    for (n, nd, B, nq, k, variant, storage, with_allow, compact) in cases:
         Q0, D, dl = O.synth(n, nd, B, nq, seed=17 + nq, ragged=True)
-        corpus = R.FlatCorpus(torch.from_numpy(D).to(torch.bfloat16), dl, device=0)
+        dt = torch.float16 if storage == "fp16" else torch.bfloat16
+        corpus = R.FlatCorpus(torch.from_numpy(D).to(dt), dl, device=0, storage=storage)
         try:
+            if compact:
+                corpus.delete(np.arange(0, n, 3))
+                corpus.compact()
             _cabi.check(L.flmr_debug_set_scan_variant(variant))
-            Qs = torch.from_numpy(Q0).cuda().bfloat16()
-            R.maxsim_topk(corpus, Qs, k)                      # first call outside capture (sizes the workspace)
-            R.maxsim_scores(corpus, Qs)
+            Qs = torch.from_numpy(Q0).cuda().to(dt)
+            rng = np.random.default_rng(nq)
+            allow = (corpus.allow_bitmaps([rng.choice(n, 60, replace=False) for _ in range(B)])
+                     if with_allow else None)
+            R.maxsim_topk(corpus, Qs, k, allow=allow)         # first call outside capture (sizes the workspace)
+            R.maxsim_scores(corpus, Qs, allow=allow)
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                gs, gp = R.maxsim_topk(corpus, Qs, k)
-                ga = R.maxsim_scores(corpus, Qs)
+                gs, gp = R.maxsim_topk(corpus, Qs, k, allow=allow)
+                ga = R.maxsim_scores(corpus, Qs, allow=allow)
             for seed in (1, 2):
                 Q1, _, _ = O.synth(4, 4, B, nq, seed=seed)
-                Qs.copy_(torch.from_numpy(Q1).cuda().bfloat16())
+                Qs.copy_(torch.from_numpy(Q1).cuda().to(dt))
+                if with_allow:
+                    allow.copy_(corpus.allow_bitmaps([rng.choice(n, 60, replace=False) for _ in range(B)]))
                 graph.replay()
                 torch.cuda.synchronize()
-                es, ep = R.maxsim_topk(corpus, Qs, k)
-                ea = R.maxsim_scores(corpus, Qs)
-                assert torch.equal(gs, es) and torch.equal(gp, ep) and torch.equal(ga, ea)
-                ref = O.maxsim_scores(Q1, D, dl)
-                np.testing.assert_allclose(ga.cpu().numpy(), ref, rtol=2e-5)
+                es, ep = R.maxsim_topk(corpus, Qs, k, allow=allow)
+                ea = R.maxsim_scores(corpus, Qs, allow=allow)
+                assert torch.equal(gs, es) and torch.equal(gp, ep) and torch.equal(ga, ea), (nq, variant, storage)
+                if storage == "bf16" and not with_allow and not compact:
+                    ref = O.maxsim_scores(Q1, D, dl)
+                    np.testing.assert_allclose(ga.cpu().numpy(), ref, rtol=2e-5)
         finally:
             L.flmr_debug_set_scan_variant(0)
             corpus.close()
