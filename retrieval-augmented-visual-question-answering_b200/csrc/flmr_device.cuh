@@ -195,6 +195,10 @@ __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1) << 62;             // SWIZZLE_128B
   return d;
 }
+// The two 32-bit words of make_kmajor_sw128_desc(smem_addr): the low word (start address and LBO) and the high word
+// (SBO and layout type), which is the same for every address.
+__device__ __forceinline__ uint32_t sw128_desc_lo(uint32_t smem_addr) { return ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16); }
+constexpr uint32_t kSw128DescHi = (1024 >> 4) | (1u << 30);
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

@@ -345,6 +345,34 @@ __device__ __forceinline__ void issue_block_mma(float (&acc)[kAcc], uint32_t q_b
   wgmma_commit();
 }
 
+// The m64n48 MMAs of one half tile (issue_block_mma's k-steps, in its order) from the low words of its two descriptors,
+// `a_lo` for the 64-row query block and `b_lo` for the half tile (sw128_desc_lo).  A k-step moves a start address by 32
+// bytes, 2 in the descriptor's address field, and a k-block by a constant; the field never carries into the word's
+// LBO bits (shared addresses are below 2^18), so each k-step is one 32-bit add per operand and the high word is the
+// constant kSw128DescHi.  With warp-uniform bases the adds run on the uniform datapath and every descriptor stays in
+// uniform registers, where the HGMMA reads it, instead of being rebuilt from regular registers for each MMA.
+template <Elem kE>
+__device__ __forceinline__ void issue_half_mma_udesc(float (&acc)[2 * kNb], uint32_t a_lo, uint32_t b_lo) {
+  auto desc = [](uint32_t lo) { return (static_cast<uint64_t>(kSw128DescHi) << 32) | lo; };
+  wgmma_fence();
+  if constexpr (kE == Elem::kE4M3) {
+#pragma unroll
+    for (int k = 0; k < kDim / 32; ++k)
+      wgmma_m64n48k32_e4m3(acc, desc(a_lo + 2u * k), desc(b_lo + 2u * k), k > 0 ? 1u : 0u);
+  } else {
+#pragma unroll
+    for (int k = 0; k < kDim / 16; ++k) {
+      const uint32_t a = a_lo + (k >> 2) * (kQKBlockBytes >> 4) + 2u * (k & 3);
+      const uint32_t b = b_lo + (k >> 2) * (kDKBlockBytes >> 4) + 2u * (k & 3);
+      if constexpr (kE == Elem::kF16)
+        wgmma_m64n48k16_f16(acc, desc(a), desc(b), k > 0 ? 1u : 0u);
+      else
+        wgmma_m64n48k16(acc, desc(a), desc(b), k > 0 ? 1u : 0u);
+    }
+  }
+  wgmma_commit();
+}
+
 // One consumer warpgroup that owns NB of the pass's 64-row query blocks (j = wg + u kWgs, u < NB), over all tiles.
 // Software-pipelined over the sequence of (tile, block) pairs with two accumulators: the MMAs of the next pair are
 // issued before the accumulator of the current one is folded (wait_group 1), so the tensor pipe works while the
@@ -478,7 +506,9 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
 // the same thread: a passage's row maxima and chunk sums are the values, in the order, of the whole-tile fold (max is
 // exact, whatever order it is taken in), and the scores bitwise those of flmr_scan_kernel.
 // kPlan: as scan_consumer's (the reset happens before half 0 of the tile is folded).
-template <int NB, Elem kE, bool kPlan = false>
+// kUDesc (flmr_scan_udesc_kernel): the same loop, whose MMAs take their descriptors from warp-uniform bases
+// (issue_half_mma_udesc): the query blocks' once per warpgroup, the half tile's once per tile.
+template <int NB, Elem kE, bool kPlan = false, bool kUDesc = false>
 __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base,
                                                     ScanBars bars, int n_tiles, int64_t tile_base, int wg, int wq,
                                                     int lane) {
@@ -496,6 +526,25 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
   const uint32_t q_smem = smem_base + S::kOffQ;
   auto q_block = [&](int u) { return q_smem + (wg + u * kWgs) * 64 * 128; };
   auto d_half = [&](int t, int hf) { return smem_base + S::kOffD + (t % kDStages) * kDTileBytes + hf * kHalfBytes; };
+  // kUDesc: descriptor low words.  The shuffles from lane 0 tell ptxas that the warpgroup, the shared-memory base and
+  // the tile count (hence every base below, and the tile index the D stage follows) are the same in all lanes, so it
+  // can keep them in uniform registers.
+  uint32_t q_lo[NB], d_lo = 0;
+  if constexpr (kUDesc) {
+    n_tiles = __shfl_sync(0xffffffffu, n_tiles, 0);
+    const int wg_u = __shfl_sync(0xffffffffu, wg, 0);
+    const uint32_t base_u = __shfl_sync(0xffffffffu, smem_base, 0);
+#pragma unroll
+    for (int u = 0; u < NB; ++u) q_lo[u] = sw128_desc_lo(base_u + S::kOffQ + (wg_u + u * kWgs) * 64 * 128);
+    d_lo = sw128_desc_lo(base_u + S::kOffD);
+  }
+  // acc (+)= the MMAs of block u and half hf of tile t, one commit group
+  auto issue = [&](float (&a)[2 * kNb], int u, int t, int hf) {
+    if constexpr (kUDesc)
+      issue_half_mma_udesc<kE>(a, q_lo[u], d_lo + (t % kDStages) * (kDTileBytes >> 4) + hf * (kHalfBytes >> 4));
+    else
+      issue_block_mma<kE>(a, q_block(u), d_half(t, hf));
+  };
   float acc[2][2 * kNb];
   uint32_t mask_next = 0;
 
@@ -517,7 +566,7 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
     for (int u = 0; u < NB; ++u) {
       const bool last = u + 1 == NB;
       const int j = wg + u * kWgs;
-      issue_block_mma<kE>(acc[1], q_block(u), d_half(t, 1));
+      issue(acc[1], u, t, 1);
       wgmma_wait<1>();
       wgmma_fence_operands(acc[0]);
       // the reducer must have consumed the partial sums of tile t-2 before this buffer is reused
@@ -530,12 +579,12 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
         slot = fold_accumulator<kNb / 2, 1>(acc[0], mask & ((1u << kHalfGroups) - 1u), m[u], pend, init,
                                             lane_part_buf, partial_buf, j, wq, lane);
       if (!last) {
-        issue_block_mma<kE>(acc[0], q_block(u + 1), d_half(t, 0));
+        issue(acc[0], u + 1, t, 0);
         wgmma_wait<1>();
       } else if (kNext) {
         mbar_wait_inline(bars.d_full((t + 1) % kDStages), ((t + 1) / kDStages) & 1u, p.status, kDevTimeoutMma);
         mask_next = __ldg(p.tile_end_mask + tile_base + t + 1);
-        issue_block_mma<kE>(acc[0], q_block(0), d_half(t + 1, 0));
+        issue(acc[0], 0, t + 1, 0);
         wgmma_wait<1>();
       } else {
         wgmma_wait<0>();
@@ -559,7 +608,7 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
   if (n_tiles <= 0) return;
   mbar_wait(bars.d_full(0), 0u, p.status, kDevTimeoutMma);
   mask_next = __ldg(p.tile_end_mask + tile_base);
-  issue_block_mma<kE>(acc[0], q_block(0), d_half(0, 0));
+  issue(acc[0], 0, 0, 0);
   int t = 0;
   for (; t + 1 < n_tiles; ++t) tile(t, std::true_type{});
   tile(t, std::false_type{});
@@ -584,18 +633,22 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
 // kSplit = true (flmr_scan_split_kernel, three warpgroups) runs scan_split_consumer instead of scan_consumer; the
 // producer, the reducer, the barriers and the shared-memory layout are the same code.
 //
+// kUDesc = true (flmr_scan_udesc_kernel) runs the split consumer loop with its MMA descriptors built from warp-uniform
+// bases (scan_split_consumer's kUDesc); everything else is the split kernel's.
+//
 // kPlan = true (the listed kernels) scans a per-call plan instead of the corpus partition: CTA c's tiles are
 // cta_tile_base[c] .. cta_tile_base[c + 1] of the plan's arrays, tile i is loaded from stored row tile_row[i], and a
 // tile with kTileRunStart set resets the consumers' running maxima.  The fold, the reducer (its tombstone and allow
 // tests drop whatever the plan's tiles cover besides the listed passages) and the top-k are the same code, so every
 // score is bitwise the one the partition kernels compute.  A CTA without tiles publishes its empty top-k lists and
 // waits on no barrier.
-template <int kWgs, bool kPair, Elem kE, bool kSplit, bool kPlan = false>
+template <int kWgs, bool kPair, Elem kE, bool kSplit, bool kPlan = false, bool kUDesc = false>
 __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, const ScanParams& p) {
   static_assert(!(kPair && kE != Elem::kBF16), "the CTA-pair kernel is bf16 only");
   static_assert(!(kPair && kPlan), "plan mode has no CTA-pair kernel");
   constexpr bool kFp8 = kE == Elem::kE4M3;
   static_assert(!kSplit || (kWgs == 3 && !kPair), "the split consumer loop is written for three single-CTA warpgroups");
+  static_assert(!kUDesc || (kSplit && !kPlan), "uniform descriptors: the split consumer loop over the partition");
   using S = ScanSmem;
   constexpr int kConsumerWarps = kWgs * 4;
   constexpr int kWarpRed0 = kConsumerWarps;
@@ -842,9 +895,9 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
     const int nb = wg < n_blocks ? (n_blocks - wg + kWgs - 1) / kWgs : 0;
     if constexpr (kSplit) {
       if (nb == 1) {
-        scan_split_consumer<1, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+        scan_split_consumer<1, kE, kPlan, kUDesc>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
       } else if (nb == 2) {
-        scan_split_consumer<2, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+        scan_split_consumer<2, kE, kPlan, kUDesc>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
       }
     } else if (nb == 1) {
       scan_consumer<1, kWgs, kPair, kOverlap, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
@@ -876,8 +929,8 @@ flmr_scan_split_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanPar
 
 // The fp16 corpus (FLMR_CORPUS_FP16): the kernels above with wgmma .f16 in place of .bf16 — the same tiles, stages,
 // fold, reducer and top-k.  Their own names keep the bf16 and e4m3 kernels' symbols (and code) as they were.  There
-// is no CTA-pair fp16 kernel; launch_scan uses the two-warpgroup one below five occupied query blocks, the split one
-// from five up, and a forced variant without an fp16 instantiation is refused.
+// is no CTA-pair fp16 kernel; launch_scan uses the two-warpgroup one below five occupied query blocks, the split loop
+// (flmr_scan_udesc_kernel<Elem::kF16>) from five up, and a forced variant without an fp16 instantiation is refused.
 __global__ void __launch_bounds__(scan_threads(2), 1)
 flmr_scan_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
   scan_kernel_body<2, false, Elem::kF16, false>(tmap_d, p);
@@ -885,6 +938,15 @@ flmr_scan_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParam
 __global__ void __launch_bounds__(scan_threads(3), 1)
 flmr_scan_split_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
   scan_kernel_body<3, false, Elem::kF16, true>(tmap_d, p);
+}
+
+// The split kernel with warp-uniform MMA descriptors (scan_kernel_body's kUDesc), one instantiation per storage:
+// the same schedule, fold, reducer and top-k, so bit-identical to flmr_scan_split_kernel; only the instructions that
+// issue the MMAs differ.  Its own name keeps the split kernels' symbols and code as they were.
+template <Elem kE>
+__global__ void __launch_bounds__(scan_threads(3), 1)
+flmr_scan_udesc_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<3, false, kE, true, false, true>(tmap_d, p);
 }
 
 // Plan mode (flmr_maxsim_topk_listed / flmr_maxsim_scores_listed): the two kernels the product launches, over a plan
