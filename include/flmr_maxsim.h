@@ -506,9 +506,9 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* corpus, const void* d_q, 
  * warpgroups), normal passes only, 4 = CTA-pair passes (clusters of two CTAs stream one token
  * range, each D tile fetched once and TMA-multicast to both) whenever a call has enough queries, on any bf16 shard
  * (a search on an e4m3 corpus returns FLMR_ERR_UNSUPPORTED), 6 = flmr_scan_split_kernel (three warpgroups,
- * split-tile loop), 7 = flmr_scan_udesc_kernel (the split-tile loop with warp-uniform MMA descriptors; a listed search
- * under it returns FLMR_ERR_UNSUPPORTED) — so the parity suite can run against any of them at any shape.  An
- * FLMR_CORPUS_FP16 corpus has fp16 forms of variants 2, 6 and 7 only: a search on it under variant 3 or 4 returns
+ * split-tile loop with warp-uniform MMA descriptors; listed searches run its listed form) — so the parity suite can run
+ * against any of them at any shape.  Any other variant, 5 and 7 included, returns FLMR_ERR_INVALID_ARG.  An
+ * FLMR_CORPUS_FP16 corpus has fp16 forms of variants 2 and 6 only: a search on it under variant 3 or 4 returns
  * FLMR_ERR_UNSUPPORTED. */
 int flmr_debug_set_scan_variant(int variant);
 

@@ -1194,9 +1194,8 @@ constexpr int kNcclInt64 = 4, kNcclFloat32 = 7;   // ncclDataType_t values (nccl
 
 thread_local bool g_profiling = false;
 // which scan kernel a search on this thread launches: 0 = chosen per pass (pick_scan), 2 = flmr_scan_kernel<2> (two
-// consumer warpgroups), 3 = flmr_scan_kernel<3> (three), 4 = CTA-pair passes forced, 6 = flmr_scan_split_kernel
-// (three, split-tile loop; 5 stays unassigned), 7 = flmr_scan_udesc_kernel (the split-tile loop with warp-uniform MMA
-// descriptors); flmr_debug_set_scan_variant
+// consumer warpgroups), 3 = flmr_scan_kernel<3> (three), 4 = CTA-pair passes forced, 6 = flmr_scan_split_kernel or
+// flmr_scan_listed_split_kernel (three, split-tile loop; 5 and 7 stay unassigned); flmr_debug_set_scan_variant
 thread_local int g_scan_variant = 0;
 struct EventPair {
   cudaEvent_t a, b;
@@ -1480,18 +1479,16 @@ struct ScanKernels {
   ScanFn three;   // three, serial loop (variant 3)
   ScanFn split;   // three, split-tile loop
   ScanFn pair;    // clusters of two CTAs (variant 4)
-  ScanFn udesc;   // three, split-tile loop with warp-uniform MMA descriptors (variant 7)
-  bool udesc_from_5;   // variant 0 runs udesc instead of split from five occupied blocks up
 };
 constexpr ScanKernels kScanKernels[3][2] = {   // [Elem][listed]
-    {{flmr_scan_kernel<2>, flmr_scan_kernel<3>, flmr_scan_split_kernel<false>, flmr_scan_kernel<2, true>,
-      flmr_scan_udesc_kernel<Elem::kBF16>, true},
-     {flmr_scan_listed_kernel<false>, nullptr, flmr_scan_listed_split_kernel<false>, nullptr, nullptr, false}},
-    {{flmr_scan_f16_kernel, nullptr, flmr_scan_split_f16_kernel, nullptr, flmr_scan_udesc_kernel<Elem::kF16>, true},
-     {flmr_scan_listed_f16_kernel, nullptr, flmr_scan_listed_split_f16_kernel, nullptr, nullptr, false}},
-    {{flmr_scan_kernel<2, false, true>, flmr_scan_kernel<3, false, true>, flmr_scan_split_kernel<true>, nullptr,
-      flmr_scan_udesc_kernel<Elem::kE4M3>, true},
-     {flmr_scan_listed_kernel<true>, nullptr, flmr_scan_listed_split_kernel<true>, nullptr, nullptr, false}},
+    {{flmr_scan_kernel<2, Elem::kBF16>, flmr_scan_kernel<3, Elem::kBF16>, flmr_scan_split_kernel<Elem::kBF16>,
+      flmr_scan_kernel<2, Elem::kBF16, true>},
+     {flmr_scan_listed_kernel<Elem::kBF16>, nullptr, flmr_scan_listed_split_kernel<Elem::kBF16>, nullptr}},
+    {{flmr_scan_kernel<2, Elem::kF16>, nullptr, flmr_scan_split_kernel<Elem::kF16>, nullptr},
+     {flmr_scan_listed_kernel<Elem::kF16>, nullptr, flmr_scan_listed_split_kernel<Elem::kF16>, nullptr}},
+    {{flmr_scan_kernel<2, Elem::kE4M3>, flmr_scan_kernel<3, Elem::kE4M3>, flmr_scan_split_kernel<Elem::kE4M3>,
+      nullptr},
+     {flmr_scan_listed_kernel<Elem::kE4M3>, nullptr, flmr_scan_listed_split_kernel<Elem::kE4M3>, nullptr}},
 };
 
 struct ScanKernel {
@@ -1503,18 +1500,17 @@ struct ScanKernel {
 // the blocks: from five up (Nq = 320: five, a full row slice: six) three warpgroups with the split-tile loop (2 / 2 / 1
 // or 2 / 2 / 2 blocks, each warpgroup folding one half of a tile under the MMAs of the other), below that two (each
 // with two accumulators, its own MMAs overlapping its fold).  On an H100 80GB HBM3 (700 W, 200k x 180-token passages,
-// median of 5, DESIGN.md 4.1) 16 x Nq = 320 took 6.27 ms split, 6.72 ms with the serial three-warpgroup loop and
-// 7.98 ms with two warpgroups; 3 x Nq = 832 row slices 6.63 / 6.73 / 7.19 ms; a 4-block pass (4 x Nq = 256) 5.55 /
-// 5.91 / 5.46 ms.  e4m3 follows the same threshold (5 blocks: 3.95 ms split, 5.00 ms serial).  From five blocks up
-// every storage now runs the split loop with warp-uniform MMA descriptors (udesc_from_5).  Same card, limit and passages,
-// 4 x Nq = 320 / 384 (five / six blocks), median of 5: bf16 5.62 / 6.46 ms against 6.06 / 6.88 split, fp16 5.59 / 6.53
-// against 6.17 / 6.91, e4m3 3.78 / 4.29 against 3.93 / 4.46; the flagship bench went from 31.7 to 34.1 queries/s
-// (DESIGN.md 6).  Variants 2, 3, 4, 6 and 7 force a kernel.  Every kernel computes bit-identical results.
+// median of 5, DESIGN.md 4.1), with the split loop's MMA descriptors rebuilt in regular registers, 16 x Nq = 320 took
+// 6.27 ms split, 6.72 ms with the serial three-warpgroup loop and 7.98 ms with two warpgroups; 3 x Nq = 832 row slices
+// 6.63 / 6.73 / 7.19 ms; a 4-block pass (4 x Nq = 256) 5.55 / 5.91 / 5.46 ms; e4m3 at five blocks 3.95 ms split,
+// 5.00 ms serial.  With its descriptors in uniform registers, as here, the split loop took less again at five and six
+// blocks (4 x Nq = 320 / 384) for every storage: bf16 5.62 / 6.46 ms against 6.06 / 6.88, fp16 5.59 / 6.53 against
+// 6.17 / 6.91, e4m3 3.78 / 4.29 against 3.93 / 4.46.  Variants 2, 3, 4 and 6 force a kernel.  Every kernel computes
+// bit-identical results.
 ScanKernel pick_scan(Elem elem, bool listed, int variant, int blocks) {
   const ScanKernels& t = kScanKernels[static_cast<int>(elem)][listed];
   if (variant == 3) return {t.three, 3};
   if (variant == 4) return {t.pair, 2};
-  if (variant == 7 || (variant == 0 && blocks >= 5 && t.udesc_from_5)) return {t.udesc, 3};
   if (variant == 6 || (variant == 0 && blocks >= 5)) return {t.split, 3};
   return {t.two, 2};
 }
@@ -1881,7 +1877,7 @@ int build_layout(Elem elem, const __nv_bfloat16* d_tokens, const uint8_t* d_fp8,
                  const std::vector<int64_t>& poff, const int32_t* lens, int sm_total, SlotLayout* l) {
   // per-device function attributes of the storage's scan kernels (idempotent), set here rather than at launch time
   for (const ScanKernels& t : kScanKernels[static_cast<int>(elem)])
-    for (ScanFn fn : {t.two, t.three, t.split, t.pair, t.udesc}) {
+    for (ScanFn fn : {t.two, t.three, t.split, t.pair}) {
       const cudaError_t e =
           fn ? cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes) : cudaSuccess;
       if (e != cudaSuccess)
@@ -3313,9 +3309,9 @@ int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n
 }
 
 int flmr_debug_set_scan_variant(int variant) {
-  if (variant != 0 && variant != 2 && variant != 3 && variant != 4 && variant != 6 && variant != 7)
+  if (variant != 0 && variant != 2 && variant != 3 && variant != 4 && variant != 6)
     return fail(FLMR_ERR_INVALID_ARG, "variant must be 0 (default), 2 or 3 (epilogue warpgroups), 4 (CTA-pair "
-                "experiment), 6 (three warpgroups, split-tile loop) or 7 (split-tile loop, uniform descriptors)");
+                "experiment) or 6 (three warpgroups, split-tile loop)");
   g_scan_variant = variant;
   return FLMR_OK;
 }

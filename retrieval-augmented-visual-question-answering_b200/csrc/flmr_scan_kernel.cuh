@@ -307,11 +307,8 @@ __device__ __forceinline__ int fold_accumulator(const float (&acc)[4 * kCb], uin
 // acc = (64-row query block at q_block) . (D tile at d_stage)^T over K = 128, one commit group: bf16 or fp16, 8 x
 // wgmma.m64n96k16 over two 128-byte k-blocks; e4m3, 4 x wgmma.m64n96k32 over one.  Either way a k-step is 32
 // bytes along the row, and the accumulator fragment is the same.
-// A 24-register accumulator takes 48 tokens instead (m64n48, the split loop's tile halves): `d_stage` then points
-// 48 rows (6 KiB, whole swizzle atoms) into the stage for half 1, and the k-steps and their order are unchanged.
-template <Elem kE, int kAcc>
-__device__ __forceinline__ void issue_block_mma(float (&acc)[kAcc], uint32_t q_block, uint32_t d_stage) {
-  static_assert(kAcc == 4 * kNb || kAcc == 2 * kNb, "a whole 96-token tile or one 48-token half");
+template <Elem kE>
+__device__ __forceinline__ void issue_block_mma(float (&acc)[4 * kNb], uint32_t q_block, uint32_t d_stage) {
   // the query block's descriptors are loop-invariant: hidden from the compiler so that they are rebuilt here (a
   // few integer adds) rather than hoisted out of the tile loop into 16 registers per block
   asm volatile("" : "+r"(q_block));
@@ -321,10 +318,7 @@ __device__ __forceinline__ void issue_block_mma(float (&acc)[kAcc], uint32_t q_b
     for (int k = 0; k < kDim / 32; ++k) {
       const uint64_t a_desc = make_kmajor_sw128_desc(q_block + k * 32u);   // 32 elements along the 128-byte row
       const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + k * 32u);
-      if constexpr (kAcc == 4 * kNb)
-        wgmma_m64n96k32_e4m3(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
-      else
-        wgmma_m64n48k32_e4m3(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+      wgmma_m64n96k32_e4m3(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
     }
   } else {
 #pragma unroll
@@ -332,14 +326,10 @@ __device__ __forceinline__ void issue_block_mma(float (&acc)[kAcc], uint32_t q_b
       const uint32_t koff = (k & 3) * 32u;   // 16 elements along the 128-byte row
       const uint64_t a_desc = make_kmajor_sw128_desc(q_block + (k >> 2) * kQKBlockBytes + koff);
       const uint64_t b_desc = make_kmajor_sw128_desc(d_stage + (k >> 2) * kDKBlockBytes + koff);
-      if constexpr (kAcc == 4 * kNb && kE == Elem::kF16)
+      if constexpr (kE == Elem::kF16)
         wgmma_m64n96k16_f16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
-      else if constexpr (kAcc == 4 * kNb)
-        wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
-      else if constexpr (kE == Elem::kF16)
-        wgmma_m64n48k16_f16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
       else
-        wgmma_m64n48k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
+        wgmma_m64n96k16(acc, a_desc, b_desc, k > 0 ? 1u : 0u);
     }
   }
   wgmma_commit();
@@ -505,10 +495,10 @@ __device__ __forceinline__ void scan_consumer(const ScanParams& p, uint8_t* smem
 // last tile is peeled.  The fold carries the open passage's maxima and the passage-end slot from half 0 to half 1 in
 // the same thread: a passage's row maxima and chunk sums are the values, in the order, of the whole-tile fold (max is
 // exact, whatever order it is taken in), and the scores bitwise those of flmr_scan_kernel.
+// The MMAs take their descriptors from warp-uniform bases (issue_half_mma_udesc): the query blocks' once per
+// warpgroup, the half tile's once per tile.
 // kPlan: as scan_consumer's (the reset happens before half 0 of the tile is folded).
-// kUDesc (flmr_scan_udesc_kernel): the same loop, whose MMAs take their descriptors from warp-uniform bases
-// (issue_half_mma_udesc): the query blocks' once per warpgroup, the half tile's once per tile.
-template <int NB, Elem kE, bool kPlan = false, bool kUDesc = false>
+template <int NB, Elem kE, bool kPlan = false>
 __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t* smem, uint32_t smem_base,
                                                     ScanBars bars, int n_tiles, int64_t tile_base, int wg, int wq,
                                                     int lane) {
@@ -523,27 +513,19 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
   for (int u = 0; u < NB; ++u) m[u][0] = m[u][1] = init;
   float* const lane_part = reinterpret_cast<float*>(smem + S::kOffLanePart);
   float* const partial = reinterpret_cast<float*>(smem + S::kOffPartial);
-  const uint32_t q_smem = smem_base + S::kOffQ;
-  auto q_block = [&](int u) { return q_smem + (wg + u * kWgs) * 64 * 128; };
-  auto d_half = [&](int t, int hf) { return smem_base + S::kOffD + (t % kDStages) * kDTileBytes + hf * kHalfBytes; };
-  // kUDesc: descriptor low words.  The shuffles from lane 0 tell ptxas that the warpgroup, the shared-memory base and
-  // the tile count (hence every base below, and the tile index the D stage follows) are the same in all lanes, so it
-  // can keep them in uniform registers.
-  uint32_t q_lo[NB], d_lo = 0;
-  if constexpr (kUDesc) {
-    n_tiles = __shfl_sync(0xffffffffu, n_tiles, 0);
-    const int wg_u = __shfl_sync(0xffffffffu, wg, 0);
-    const uint32_t base_u = __shfl_sync(0xffffffffu, smem_base, 0);
+  // Descriptor low words.  The shuffles from lane 0 tell ptxas that the warpgroup, the shared-memory base and the tile
+  // count (hence every base below, and the tile index the D stage follows) are the same in all lanes, so it can keep
+  // them in uniform registers.
+  n_tiles = __shfl_sync(0xffffffffu, n_tiles, 0);
+  const int wg_u = __shfl_sync(0xffffffffu, wg, 0);
+  const uint32_t base_u = __shfl_sync(0xffffffffu, smem_base, 0);
+  uint32_t q_lo[NB];
 #pragma unroll
-    for (int u = 0; u < NB; ++u) q_lo[u] = sw128_desc_lo(base_u + S::kOffQ + (wg_u + u * kWgs) * 64 * 128);
-    d_lo = sw128_desc_lo(base_u + S::kOffD);
-  }
+  for (int u = 0; u < NB; ++u) q_lo[u] = sw128_desc_lo(base_u + S::kOffQ + (wg_u + u * kWgs) * 64 * 128);
+  const uint32_t d_lo = sw128_desc_lo(base_u + S::kOffD);
   // acc (+)= the MMAs of block u and half hf of tile t, one commit group
   auto issue = [&](float (&a)[2 * kNb], int u, int t, int hf) {
-    if constexpr (kUDesc)
-      issue_half_mma_udesc<kE>(a, q_lo[u], d_lo + (t % kDStages) * (kDTileBytes >> 4) + hf * (kHalfBytes >> 4));
-    else
-      issue_block_mma<kE>(a, q_block(u), d_half(t, hf));
+    issue_half_mma_udesc<kE>(a, q_lo[u], d_lo + (t % kDStages) * (kDTileBytes >> 4) + hf * (kHalfBytes >> 4));
   };
   float acc[2][2 * kNb];
   uint32_t mask_next = 0;
@@ -633,22 +615,18 @@ __device__ __forceinline__ void scan_split_consumer(const ScanParams& p, uint8_t
 // kSplit = true (flmr_scan_split_kernel, three warpgroups) runs scan_split_consumer instead of scan_consumer; the
 // producer, the reducer, the barriers and the shared-memory layout are the same code.
 //
-// kUDesc = true (flmr_scan_udesc_kernel) runs the split consumer loop with its MMA descriptors built from warp-uniform
-// bases (scan_split_consumer's kUDesc); everything else is the split kernel's.
-//
 // kPlan = true (the listed kernels) scans a per-call plan instead of the corpus partition: CTA c's tiles are
 // cta_tile_base[c] .. cta_tile_base[c + 1] of the plan's arrays, tile i is loaded from stored row tile_row[i], and a
 // tile with kTileRunStart set resets the consumers' running maxima.  The fold, the reducer (its tombstone and allow
 // tests drop whatever the plan's tiles cover besides the listed passages) and the top-k are the same code, so every
 // score is bitwise the one the partition kernels compute.  A CTA without tiles publishes its empty top-k lists and
 // waits on no barrier.
-template <int kWgs, bool kPair, Elem kE, bool kSplit, bool kPlan = false, bool kUDesc = false>
+template <int kWgs, bool kPair, Elem kE, bool kSplit, bool kPlan = false>
 __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, const ScanParams& p) {
   static_assert(!(kPair && kE != Elem::kBF16), "the CTA-pair kernel is bf16 only");
   static_assert(!(kPair && kPlan), "plan mode has no CTA-pair kernel");
   constexpr bool kFp8 = kE == Elem::kE4M3;
   static_assert(!kSplit || (kWgs == 3 && !kPair), "the split consumer loop is written for three single-CTA warpgroups");
-  static_assert(!kUDesc || (kSplit && !kPlan), "uniform descriptors: the split consumer loop over the partition");
   using S = ScanSmem;
   constexpr int kConsumerWarps = kWgs * 4;
   constexpr int kWarpRed0 = kConsumerWarps;
@@ -895,9 +873,9 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
     const int nb = wg < n_blocks ? (n_blocks - wg + kWgs - 1) / kWgs : 0;
     if constexpr (kSplit) {
       if (nb == 1) {
-        scan_split_consumer<1, kE, kPlan, kUDesc>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+        scan_split_consumer<1, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
       } else if (nb == 2) {
-        scan_split_consumer<2, kE, kPlan, kUDesc>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
+        scan_split_consumer<2, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
       }
     } else if (nb == 1) {
       scan_consumer<1, kWgs, kPair, kOverlap, kE, kPlan>(p, smem, smem_base, bars, n_tiles, tile_base, wg, wq, lane);
@@ -913,62 +891,33 @@ __device__ __forceinline__ void scan_kernel_body(const CUtensorMap& tmap_d, cons
   if constexpr (kPair) cluster_sync_all();   // no CTA leaves while its peer may still signal its barriers
 }
 
-template <int kWgs, bool kPair = false, bool kFp8 = false>
+// Every scan kernel is instantiated per storage type kE; there is no CTA-pair kernel for fp16 or e4m3, and no
+// three-warpgroup serial kernel for fp16 (launch_scan refuses a forced variant without an instantiation).
+template <int kWgs, Elem kE, bool kPair = false>
 __global__ void __launch_bounds__(scan_threads(kWgs), 1)
 flmr_scan_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<kWgs, kPair, kFp8 ? Elem::kE4M3 : Elem::kBF16, false>(tmap_d, p);
+  scan_kernel_body<kWgs, kPair, kE, false>(tmap_d, p);
 }
 
 // Three consumer warpgroups whose loop folds one half of each tile while the MMAs of the other half run
-// (scan_split_consumer); bit-identical to flmr_scan_kernel<3, false, kFp8>.
-template <bool kFp8>
-__global__ void __launch_bounds__(scan_threads(3), 1)
-flmr_scan_split_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<3, false, kFp8 ? Elem::kE4M3 : Elem::kBF16, true>(tmap_d, p);
-}
-
-// The fp16 corpus (FLMR_CORPUS_FP16): the kernels above with wgmma .f16 in place of .bf16 — the same tiles, stages,
-// fold, reducer and top-k.  Their own names keep the bf16 and e4m3 kernels' symbols (and code) as they were.  There
-// is no CTA-pair fp16 kernel; launch_scan uses the two-warpgroup one below five occupied query blocks, the split loop
-// (flmr_scan_udesc_kernel<Elem::kF16>) from five up, and a forced variant without an fp16 instantiation is refused.
-__global__ void __launch_bounds__(scan_threads(2), 1)
-flmr_scan_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<2, false, Elem::kF16, false>(tmap_d, p);
-}
-__global__ void __launch_bounds__(scan_threads(3), 1)
-flmr_scan_split_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<3, false, Elem::kF16, true>(tmap_d, p);
-}
-
-// The split kernel with warp-uniform MMA descriptors (scan_kernel_body's kUDesc), one instantiation per storage:
-// the same schedule, fold, reducer and top-k, so bit-identical to flmr_scan_split_kernel; only the instructions that
-// issue the MMAs differ.  Its own name keeps the split kernels' symbols and code as they were.
+// (scan_split_consumer); bit-identical to flmr_scan_kernel<kWgs, kE>.
 template <Elem kE>
 __global__ void __launch_bounds__(scan_threads(3), 1)
-flmr_scan_udesc_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<3, false, kE, true, false, true>(tmap_d, p);
+flmr_scan_split_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
+  scan_kernel_body<3, false, kE, true>(tmap_d, p);
 }
 
-// Plan mode (flmr_maxsim_topk_listed / flmr_maxsim_scores_listed): the two kernels the product launches, over a plan
-// of the listed passages' rows (see scan_kernel_body's kPlan).  Their own names keep the partition kernels' symbols
-// and code as they were.
-template <bool kFp8>
+// Plan mode (flmr_maxsim_topk_listed / flmr_maxsim_scores_listed): the two- and three-warpgroup loops over a plan of
+// the listed passages' rows (see scan_kernel_body's kPlan).
+template <Elem kE>
 __global__ void __launch_bounds__(scan_threads(2), 1)
 flmr_scan_listed_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<2, false, kFp8 ? Elem::kE4M3 : Elem::kBF16, false, true>(tmap_d, p);
+  scan_kernel_body<2, false, kE, false, true>(tmap_d, p);
 }
-template <bool kFp8>
+template <Elem kE>
 __global__ void __launch_bounds__(scan_threads(3), 1)
 flmr_scan_listed_split_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<3, false, kFp8 ? Elem::kE4M3 : Elem::kBF16, true, true>(tmap_d, p);
-}
-__global__ void __launch_bounds__(scan_threads(2), 1)
-flmr_scan_listed_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<2, false, Elem::kF16, false, true>(tmap_d, p);
-}
-__global__ void __launch_bounds__(scan_threads(3), 1)
-flmr_scan_listed_split_f16_kernel(const __grid_constant__ CUtensorMap tmap_d, const ScanParams p) {
-  scan_kernel_body<3, false, Elem::kF16, true, true>(tmap_d, p);
+  scan_kernel_body<3, false, kE, true, true>(tmap_d, p);
 }
 
 }  // namespace flmr

@@ -48,7 +48,9 @@ int main(void) {
     if (flmr_corpus_builder_finish(NULL, &corpus, NULL) != FLMR_ERR_INVALID_ARG) return 31;
     if (flmr_corpus_builder_destroy(NULL) != FLMR_OK) return 32;
   }
-  if (flmr_debug_set_scan_variant(5) != FLMR_ERR_INVALID_ARG || flmr_debug_set_scan_variant(0) != FLMR_OK) return 33;
+  if (flmr_debug_set_scan_variant(5) != FLMR_ERR_INVALID_ARG || flmr_debug_set_scan_variant(7) != FLMR_ERR_INVALID_ARG ||
+      flmr_debug_set_scan_variant(0) != FLMR_OK)
+    return 33;
   if (flmr_debug_set_argmax_path(7) != FLMR_ERR_INVALID_ARG || flmr_debug_set_argmax_path(0) != FLMR_OK) return 34;
   /* host-only helper: 5 passages over 2 CTAs */
   int32_t dl[5] = {100, 7, 96, 1, 50};

@@ -16,7 +16,7 @@ from ravqa_b200 import _cabi
 from helpers import ROOT
 
 SRC = os.path.join(ROOT, "retrieval-augmented-visual-question-answering_b200", "csrc", "flmr_maxsim.cu")
-SCAN = re.compile(r"flmr_scan_kernelILi(\d)ELb(\d)ELb(\d)E")
+SCAN = re.compile(r"flmr_scan_kernelILi(\d)ELNS_4ElemE([02])ELb(\d)E")   # bf16 and e4m3
 # registers of each scan instantiation (kWgs, kPair, kFp8) before the tombstone test was added: it must not raise them
 REGISTERS_BEFORE = {(2, 0, 0): 167, (3, 0, 0): 119, (2, 0, 1): 167, (3, 0, 1): 111, (2, 1, 0): 168}
 
@@ -152,7 +152,7 @@ def _sections(text, header):
     for line in text.splitlines():
         if re.search(header, line):
             m = SCAN.search(line)
-            cur = tuple(int(x) for x in m.groups()) if m else None
+            cur = (int(m.group(1)), int(m.group(3)), int(m.group(2) == "2")) if m else None
             if cur:
                 out[cur] = []
             continue

@@ -17,13 +17,13 @@ from helpers import ROOT
 
 SRC = os.path.join(ROOT, "retrieval-augmented-visual-question-answering_b200", "csrc", "flmr_maxsim.cu")
 # fp16 kernel -> its bf16 twin (the kernel the same launch runs on a bf16 corpus)
-F16_KERNELS = {"flmr_scan_f16_kernel": r"flmr_scan_kernelILi2ELb0ELb0E",
-               "flmr_scan_split_f16_kernel": r"flmr_scan_split_kernelILb0E"}
-# registers of every scan instantiation of the parent revision (kernel name pattern -> registers)
-REGISTERS_BEFORE = {r"flmr_scan_kernelILi2ELb0ELb0E": 167, r"flmr_scan_kernelILi3ELb0ELb0E": 119,
-                    r"flmr_scan_kernelILi2ELb0ELb1E": 167, r"flmr_scan_kernelILi3ELb0ELb1E": 109,
-                    r"flmr_scan_kernelILi2ELb1ELb0E": 168, r"flmr_scan_split_kernelILb0E": 106,
-                    r"flmr_scan_split_kernelILb1E": 102}
+F16_KERNELS = {r"flmr_scan_kernelILi2ELNS_4ElemE1ELb0E": r"flmr_scan_kernelILi2ELNS_4ElemE0ELb0E",
+               r"flmr_scan_split_kernelILNS_4ElemE1E": r"flmr_scan_split_kernelILNS_4ElemE0E"}
+# registers of every bf16 and e4m3 scan instantiation (kernel name pattern -> registers)
+REGISTERS_BEFORE = {r"flmr_scan_kernelILi2ELNS_4ElemE0ELb0E": 167, r"flmr_scan_kernelILi3ELNS_4ElemE0ELb0E": 119,
+                    r"flmr_scan_kernelILi2ELNS_4ElemE2ELb0E": 167, r"flmr_scan_kernelILi3ELNS_4ElemE2ELb0E": 109,
+                    r"flmr_scan_kernelILi2ELNS_4ElemE0ELb1E": 168, r"flmr_scan_split_kernelILNS_4ElemE0E": 109,
+                    r"flmr_scan_split_kernelILNS_4ElemE2E": 102}
 
 
 @pytest.fixture(scope="module")
@@ -71,7 +71,7 @@ def test_f16_kernels_no_spills_and_no_more_registers_than_bf16(ptxas_build):
     log, _ = ptxas_build
     kernels = _sections(log, r"Compiling entry function")
     for f16, twin in F16_KERNELS.items():
-        regs = _registers(_find(kernels, f16 + "E"))
+        regs = _registers(_find(kernels, f16))
         assert regs <= _registers(_find(kernels, twin)), (f16, regs)
 
 
@@ -85,8 +85,8 @@ def test_existing_scan_kernels_keep_their_registers(ptxas_build):
 def test_f16_kernels_issue_f16_hgmma_and_overlap_the_fold(ptxas_build):
     _, sass = ptxas_build
     kernels = _sections(sass, r"Function : ")
-    for f16, shape in (("flmr_scan_f16_kernel", "64x96x16"), ("flmr_scan_split_f16_kernel", "64x48x16")):
-        text = "\n".join(_find(kernels, f16 + "E"))
+    for f16, shape in zip(F16_KERNELS, ("64x96x16", "64x48x16")):
+        text = "\n".join(_find(kernels, f16))
         assert "HGMMA.%s.F32 " % shape in text, f16
         assert ".BF16" not in text and "QGMMA" not in text, f16      # no bf16 or e4m3 MMA in the fp16 kernels
         assert "WARPGROUP.DEPBAR.LE gsb0, 0x1" in text, f16

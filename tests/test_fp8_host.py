@@ -13,7 +13,7 @@ import fp8_oracle as F8
 from helpers import ROOT, golden_names, load_golden
 
 SRC = os.path.join(ROOT, "retrieval-augmented-visual-question-answering_b200", "csrc", "flmr_maxsim.cu")
-FP8_SCAN = re.compile(r"flmr_scan_kernelILi(\d)ELb0ELb1E")
+FP8_SCAN = re.compile(r"flmr_scan_kernelILi(\d)ELNS_4ElemE2ELb0E")
 
 
 @pytest.fixture(scope="module")

@@ -13,12 +13,12 @@ from ravqa_b200 import _cabi
 
 SRC = os.path.join(ROOT, "retrieval-augmented-visual-question-answering_b200", "csrc", "flmr_maxsim.cu")
 # plan-mode kernel (mangled-name pattern) -> registers ptxas gives it, and the MMA its SASS must hold
-LISTED_KERNELS = {r"23flmr_scan_listed_kernelILb0E": (167, "HGMMA.64x96x16.F32.BF16"),
-                  r"23flmr_scan_listed_kernelILb1E": (159, "QGMMA.64x96x32.F32.E4M3.E4M3"),
-                  r"27flmr_scan_listed_f16_kernelE": (167, "HGMMA.64x96x16.F32 "),
-                  r"29flmr_scan_listed_split_kernelILb0E": (108, "HGMMA.64x48x16.F32.BF16"),
-                  r"29flmr_scan_listed_split_kernelILb1E": (102, "QGMMA.64x48x32.F32.E4M3.E4M3"),
-                  r"33flmr_scan_listed_split_f16_kernelE": (108, "HGMMA.64x48x16.F32 ")}
+LISTED_KERNELS = {r"23flmr_scan_listed_kernelILNS_4ElemE0E": (167, "HGMMA.64x96x16.F32.BF16"),
+                  r"23flmr_scan_listed_kernelILNS_4ElemE2E": (159, "QGMMA.64x96x32.F32.E4M3.E4M3"),
+                  r"23flmr_scan_listed_kernelILNS_4ElemE1E": (167, "HGMMA.64x96x16.F32 "),
+                  r"29flmr_scan_listed_split_kernelILNS_4ElemE0E": (109, "HGMMA.64x48x16.F32.BF16"),
+                  r"29flmr_scan_listed_split_kernelILNS_4ElemE2E": (102, "QGMMA.64x48x32.F32.E4M3.E4M3"),
+                  r"29flmr_scan_listed_split_kernelILNS_4ElemE1E": (109, "HGMMA.64x48x16.F32 ")}
 
 
 @pytest.fixture(scope="module")
@@ -73,7 +73,7 @@ def test_listed_kernels_issue_their_mmas_and_overlap_the_fold(ptxas_build):
     for pattern, (_, mma) in LISTED_KERNELS.items():
         text = "\n".join(_find(kernels, pattern))
         assert mma in text, pattern
-        if "f16" in pattern:
+        if pattern.endswith("ElemE1E"):   # fp16
             assert ".BF16" not in text and "QGMMA" not in text, pattern
         assert "WARPGROUP.DEPBAR.LE gsb0, 0x1" in text, pattern
 

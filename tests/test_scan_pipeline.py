@@ -19,7 +19,9 @@ from oracle import maxsim_oracle as O
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "retrieval-augmented-visual-question-answering_b200")
 SRC = os.path.join(PKG, "csrc", "flmr_maxsim.cu")
-SCAN = re.compile(r"flmr_scan_kernelILi(\d)ELb(\d)E")
+SCAN = re.compile(r"flmr_scan_kernelILi(\d)ELNS_4ElemE(\d)ELb(\d)E")
+# (kWgs, Elem value, kPair) of every flmr_scan_kernel instantiation
+KERNELS = {(2, 0, False), (3, 0, False), (2, 0, True), (2, 1, False), (2, 2, False), (3, 2, False)}
 
 
 def _nvcc():
@@ -43,12 +45,12 @@ def ptxas_build(tmp_path_factory):
 
 
 def _per_scan_kernel(text, header):
-    """{(kWgs, kPair): lines} for the sections of `text` that start with a line matching `header`."""
+    """{(kWgs, Elem value, kPair): lines} for the sections of `text` that start with a line matching `header`."""
     sections, cur = {}, None
     for line in text.splitlines():
         if re.search(header, line):
             m = SCAN.search(line)
-            cur = (int(m.group(1)), bool(int(m.group(2)))) if m else None
+            cur = (int(m.group(1)), int(m.group(2)), bool(int(m.group(3)))) if m else None
             if cur:
                 sections[cur] = []
             continue
@@ -62,7 +64,7 @@ def test_ptxas_no_serialised_wgmma_and_no_spills(ptxas_build):
     assert "C7518" not in log and "C7517" not in log and "C7511" not in log and "C7512" not in log, \
         [l for l in log.splitlines() if "C75" in l]
     kernels = _per_scan_kernel(log, r"Compiling entry function")
-    assert set(kernels) == {(2, False), (3, False), (2, True)}
+    assert set(kernels) == KERNELS
     for key, lines in kernels.items():
         spill = next(l for l in lines if "spill stores" in l)
         assert "0 bytes spill stores, 0 bytes spill loads" in spill, (key, spill)
@@ -71,7 +73,7 @@ def test_ptxas_no_serialised_wgmma_and_no_spills(ptxas_build):
 def test_sass_overlaps_mma_with_fold(ptxas_build):
     _, sass = ptxas_build
     kernels = _per_scan_kernel(sass, r"Function : ")
-    assert set(kernels) == {(2, False), (3, False), (2, True)}
+    assert set(kernels) == KERNELS
     for key, lines in kernels.items():
         waits = [l for l in lines if "WARPGROUP.DEPBAR.LE gsb0" in l]
         overlapped = [l for l in waits if "gsb0, 0x1" in l]

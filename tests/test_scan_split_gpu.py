@@ -1,8 +1,9 @@
 """GPU: flmr_scan_split_kernel (scan variant 6, three consumer warpgroups folding one half of each tile while the other
-half's MMAs run) against flmr_scan_kernel<3> (variant 3): bitwise the same scores and fused top-k, and the default
-selection (variant 0) with them.
+half's MMAs run) against flmr_scan_kernel<3> (variant 3; fp16 corpora, which have no such kernel, against the
+two-warpgroup fp16 kernel of variant 2): bitwise the same scores and fused top-k, and the default selection (variant 0)
+with them.
 
-The cases cover both storages, relu on and off, passes of five and six occupied 64-row blocks (2/2/1 and 2/2/2 over
+The cases cover every storage, relu on and off, passes of five and six occupied 64-row blocks (2/2/1 and 2/2/2 over
 the warpgroups: Nq 288 / 320 / 321 / 384, the row slices of Nq 832, 10-12 queries of 32 rows per pass in the reducer's
 lane mode), passages of 1 token (24 ends per tile: slots past kFastSlots in both halves) to thousands (open across
 many tiles), ends on either side of the half boundary (4-token groups 11 and 12), corpora below, at and above 132
@@ -32,6 +33,10 @@ CASES = [
     ("bf16", False, 384, 1, "long", 2000),
     ("fp8", False, 321, 1, "ragged", 100),
     ("bf16", True, 320, 2, "halves", 2000),
+    ("fp16", False, 320, 3, "1", 2000),
+    ("fp16", True, 384, 2, "halves", 133),
+    ("fp16", False, 832, 2, "ragged", 2000),
+    ("fp16", False, 32, 12, "le4", 2000),
 ]
 
 
@@ -82,6 +87,7 @@ def test_split_kernel_is_bitwise_the_serial_kernel(R, ci):
     from ravqa_b200 import _cabi
     L = _cabi.lib()
     storage, relu, nq, B, kind, n = CASES[ci]
+    ref_variant = 2 if storage == "fp16" else 3
     seed = 7000 + ci
     dl = _doclens(kind, n, seed)
     if kind == "halves":
@@ -95,14 +101,14 @@ def test_split_kernel_is_bitwise_the_serial_kernel(R, ci):
     Qd = Q.cuda()
     corpus = R.FlatCorpus(D.to(torch.bfloat16), dl, device=0, storage=storage)
     try:
-        ref = _run(R, L, corpus, Qd, relu, 3)
+        ref = _run(R, L, corpus, Qd, relu, ref_variant)
         _same(ref, _run(R, L, corpus, Qd, relu, 6), "variant 6")
         _same(ref, _run(R, L, corpus, Qd, relu, 0), "variant 0")
         # tombstones and per-query allow bitmaps
         rng = np.random.default_rng(seed)
         corpus.delete(rng.choice(n, size=max(1, n // 10), replace=False))
         allow = corpus.allow_bitmaps([rng.choice(n, size=max(1, (7 * n) // 10), replace=False) for _ in range(B)])
-        ref = _run(R, L, corpus, Qd, relu, 3, allow)
+        ref = _run(R, L, corpus, Qd, relu, ref_variant, allow)
         _same(ref, _run(R, L, corpus, Qd, relu, 6, allow), "variant 6, filtered")
         _same(ref, _run(R, L, corpus, Qd, relu, 0, allow), "variant 0, filtered")
     finally:

@@ -10,7 +10,6 @@ query and five occupied 64-row query blocks per pass; --nq 384: six) with a bf16
   * skeleton n48 split loop    (skeleton library, flmr_scan_split_kernel, variant 6)
   * full n96 serial loop       (release library, variant 3: the kernel the product ran before the split loop)
   * full n48 split loop        (release library, variant 6)
-  * skeleton / full n48 udesc  (flmr_scan_udesc_kernel, variant 7: the split loop with warp-uniform MMA descriptors)
 
 fp16 has no serial three-warpgroup kernel: its variant-3 rows are n/a.
 
@@ -31,8 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "retrieval-augmented-visual-question-answering_b200")
 ND = 180
 ARMS = [("skeleton", 3, "skeleton n96 serial"), ("skeleton", 6, "skeleton n48 split"),
-        ("skeleton", 7, "skeleton n48 udesc"), ("release", 3, "full n96 serial"), ("release", 6, "full n48 split"),
-        ("release", 7, "full n48 udesc")]
+        ("release", 3, "full n96 serial"), ("release", 6, "full n48 split")]
 STORAGES = ("bf16", "fp16", "e4m3")
 
 
@@ -90,7 +88,7 @@ def main():
     ap.add_argument("--repeat", type=int, default=5)
     ap.add_argument("--out", default=None, help="directory for the skeleton library and the raw samples")
     ap.add_argument("--worker", action="store_true", help=argparse.SUPPRESS)
-    ap.add_argument("--variants", default="3,6,7", help=argparse.SUPPRESS)
+    ap.add_argument("--variants", default="3,6", help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.worker:
         worker(args)

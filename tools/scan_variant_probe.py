@@ -1,7 +1,6 @@
 """GPU: the scan kernel's variants — flmr_scan_kernel<2> (two consumer warpgroups), <3> (three), flmr_scan_split_kernel
-(three, split-tile loop), flmr_scan_udesc_kernel (the split loop with warp-uniform MMA descriptors) and CTA-pair
-passes — bit-identical results of <2>, <3>, the split and the udesc kernel over a spread of shapes, then timing of
-all five.
+(three, split-tile loop) and CTA-pair passes — bit-identical results of <2>, <3> and the split kernel over a spread of
+shapes, then timing of all four.
 
     python tools/scan_variant_probe.py [--passages 200000]
 """
@@ -43,7 +42,7 @@ def main():
             s2 = R.maxsim_scores(corpus, Qt, relu=relu)
             t2 = R.maxsim_topk(corpus, Qt, min(k, n), relu=relu)
             ok = True
-            for variant in (3, 6, 7, 4):
+            for variant in (3, 6, 4):
                 L.flmr_debug_set_scan_variant(variant)
                 s3 = R.maxsim_scores(corpus, Qt, relu=relu)
                 t3 = R.maxsim_topk(corpus, Qt, min(k, n), relu=relu)
@@ -71,7 +70,7 @@ def main():
           "|---|---|---:|---:|---:|---:|---:|")
     for (B, nq) in [(16, 320), (2, 320), (1, 320), (20, 32), (12, 32), (1, 32), (3, 832), (4, 256), (2, 128)]:
         Q = torch.nn.functional.normalize(torch.randn((B, nq, 128), device=dev, generator=g), dim=-1).bfloat16()
-        for variant in (2, 3, 6, 7, 4):
+        for variant in (2, 3, 6, 4):
             if variant == 4 and (B % 2 or nq > 384):   # pairs of whole queries that fit one pass
                 continue
             L.flmr_debug_set_scan_variant(variant)
@@ -97,7 +96,7 @@ def main():
             spread = max(x[1] for x in samples) - min(x[1] for x in samples)
             flops_call = 2.0 * B * nq * 128 * n_p * nd
             print("| B=%d Nq=%d | %s | %.3f | %.3f | %.0f | %.0f | %.1f |"
-                  % (B, nq, {2: "2 WGs", 3: "3 WGs", 6: "3 WGs, split", 7: "3 WGs, split, uniform descriptors", 4: "CTA pairs (multicast)"}[variant], ms_launch, spread,
+                  % (B, nq, {2: "2 WGs", 3: "3 WGs", 6: "3 WGs, split", 4: "CTA pairs (multicast)"}[variant], ms_launch, spread,
                      flops_call / scan_call / 1e9, n_p * nd * 256.0 / ms_launch / 1e6, B / ms_call * 1e3 * n_p / 1e6),
                   flush=True)
     # sustained (power-capped) A/B at the headline shape: alternate the two variants in blocks of ~2 s, three rounds
