@@ -45,6 +45,10 @@
  *   flmr_maxsim_topk_listed / flmr_maxsim_scores_listed
  *       the same restriction given as id lists, at the cost of the listed passages: the scan runs over a per-call
  *       plan of their rows (the reference's pipeline likewise scores only its candidates, CB/search/index_storage.py).
+ *   flmr_corpus_create_streamed / flmr_corpus_builder_create_streamed / flmr_corpus_residency
+ *       a corpus kept in pinned host memory and streamed through two HBM windows per search, for a shard that does not
+ *       fit beside what the GPU already holds (the reference builds its validation Searcher inside the training
+ *       process, src/executors/FLMR_executor.py:774-792).
  *   flmr_debug_maxsim_scores_simt
  *       test infrastructure: an independent plain-SIMT fp32 device kernel used by tests to
  *       cross-check the tensor-core kernel at sizes where the CPU oracle is too slow.
@@ -250,6 +254,41 @@ int flmr_corpus_builder_append(flmr_corpus_builder_t* b, const void* h_tokens_bf
 int flmr_corpus_builder_append_file(flmr_corpus_builder_t* b, const char* path, int64_t byte_offset, int64_t n_rows);
 int flmr_corpus_builder_finish(flmr_corpus_builder_t* b, flmr_corpus_t** out, double* host_fill_seconds);
 int flmr_corpus_builder_destroy(flmr_corpus_builder_t* b);
+
+/*
+ * A STREAMED corpus: the padded token rows live in a library-owned pinned host matrix (cudaHostAllocMapped |
+ * cudaHostAllocPortable) instead of HBM, so a shard may be larger than the memory a GPU has free — a corpus searched
+ * beside a training run, or one larger than the card.  At creation the slots are cut into WINDOWS: contiguous slot
+ * ranges whose stored rows fit window_bytes, each with its own CTA partition (row starts relative to the window,
+ * slots and ids absolute).  Each workspace holds two window buffers of the largest window's rows (one when the plan
+ * has one window) and a copy stream of
+ * its own; a search streams the corpus ONCE: window w is copied into buffer w % 2 while the scans of window w - 1 run,
+ * the scans of window w wait for its copy, and the copy of window w + 2 waits for the scans of window w.  Every call
+ * chunk is scanned over each window in turn and its running top-k merged with the window's per-CTA lists.  Everything
+ * is asynchronous on the caller's stream, with no host synchronisation.  The scan kernels, their fold and reducer are
+ * the resident corpus's, so every result is bitwise the one a resident corpus of the same rows returns.
+ *
+ * flmr_corpus_create_streamed   as flmr_corpus_create (tokens host or device, bf16, or fp16 with FLMR_CORPUS_FP16),
+ *                               plus window_bytes (>= one row).  FLMR_CORPUS_FP8, FLMR_CORPUS_ADOPT and a window
+ *                               smaller than the longest passage's stored rows give FLMR_ERR_UNSUPPORTED.
+ * flmr_corpus_builder_create_streamed   the index-load builder of a streamed corpus: flmr_corpus_builder_append(_file)
+ *                               read rows straight into the pinned matrix (through one pinned staging buffer when
+ *                               passages need padding), with no device copy; finish plans the windows.
+ * flmr_corpus_residency         *streamed = 1 for a streamed corpus (0 otherwise), *window_bytes its window_bytes and
+ *                               *host_bytes its pinned matrix (0 and 0 for a resident corpus).  Any output may be NULL.
+ *
+ * On a streamed corpus flmr_maxsim_scores, flmr_maxsim_topk, their _allowed forms, flmr_maxsim_topk_sharded(_allowed),
+ * flmr_corpus_delete / _deleted, flmr_corpus_gather and flmr_debug_maxsim_scores_simt work as on a resident one (the
+ * gather and the SIMT kernel read the mapped host rows); flmr_corpus_info's hbm_bytes counts no token rows.
+ * flmr_corpus_append, flmr_corpus_compact, the _listed calls and flmr_debug_listed_plan return FLMR_ERR_UNSUPPORTED and
+ * change nothing.  Searches on a streamed corpus are not capturable in a CUDA graph.
+ */
+int flmr_corpus_create_streamed(const void* tokens, const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                int64_t pid_base, unsigned flags, int64_t window_bytes, flmr_corpus_t** out);
+int flmr_corpus_builder_create_streamed(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                        int64_t pid_base, unsigned flags, int64_t window_bytes,
+                                        flmr_corpus_builder_t** out);
+int flmr_corpus_residency(const flmr_corpus_t* corpus, int* streamed, int64_t* window_bytes, int64_t* host_bytes);
 
 /* Scratch for searches on `corpus`.  max_queries (>= 1) sizes the per-CTA candidate buffer: a call with more
  * queries is processed in chunks of max_queries (each chunk: its scan passes + ONE merge launch).  max_nq
@@ -526,6 +565,18 @@ int flmr_debug_build_partition(const int32_t* h_doclens, int64_t n_passages, int
                                int32_t* cta_row_begin, int64_t* cta_tile_base,
                                uint32_t* tile_end_mask, int32_t* tile_first_pid,
                                int64_t tile_capacity, int64_t* n_tiles_out);
+
+/* Test infrastructure, host-only: the windows of a streamed corpus of these doclens (see flmr_corpus_create_streamed)
+ * for `n_ctas` SMs.  out_windows (may be NULL to query *n_windows_out) receives 6 int64 per window: first slot, end slot
+ * (exclusive), first stored row, stored rows, CTAs (min(n_ctas, slots of the window)), tiles.  The four partition
+ * arrays (all four or none) receive each window's flmr_debug_build_partition of its own passages, concatenated in
+ * window order, with cta_row_begin relative to the window and tile_first_pid ABSOLUTE slots; each holds up to
+ * tile_capacity entries (cta_row_begin / cta_tile_base take CTAs + 1 per window).  *n_tiles_out (may be NULL) = all
+ * windows' tiles.  A passage longer than a window gives FLMR_ERR_UNSUPPORTED. */
+int flmr_debug_window_plan(const int32_t* h_doclens, int64_t n_passages, int64_t window_bytes, int n_ctas,
+                           int64_t* out_windows, int64_t capacity, int64_t* n_windows_out, int32_t* cta_row_begin,
+                           int64_t* cta_tile_base, uint32_t* tile_end_mask, int32_t* tile_first_pid,
+                           int64_t tile_capacity, int64_t* n_tiles_out);
 
 /* Test infrastructure, host-only: the corpus passes flmr_maxsim_scores / flmr_maxsim_topk run for a batch of
  * `n_queries` queries of `nq` tokens (a pass = one scan-kernel launch with up to 384 query rows resident per CTA);

@@ -42,14 +42,17 @@ FP16_TRAIN_SYMBOLS = ("flmr_maxsim_argmax_fp16", "flmr_maxsim_backward_fp16", "f
                       "flmr_maxsim_backward_grouped_fp16")
 # restricted search over id lists at the cost of the listed passages (the scan's plan mode)
 LISTED_SYMBOLS = ("flmr_maxsim_topk_listed", "flmr_maxsim_scores_listed", "flmr_debug_listed_plan")
+# a corpus kept in pinned host memory and streamed through HBM windows
+STREAMED_SYMBOLS = ("flmr_corpus_create_streamed", "flmr_corpus_builder_create_streamed", "flmr_corpus_residency",
+                    "flmr_debug_window_plan")
 # symbols an earlier revision's library may lack (tools/scan_ab.py drives one through this binding)
 OPTIONAL_SYMBOLS = (UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS + FP16_TRAIN_SYMBOLS + COMPACT_SYMBOLS
-                    + LISTED_SYMBOLS)
+                    + LISTED_SYMBOLS + STREAMED_SYMBOLS)
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
     "flmr_corpus_create", "flmr_corpus_destroy", "flmr_corpus_info", "flmr_corpus_storage",
-    *UPDATE_SYMBOLS, *COMPACT_SYMBOLS,
+    *UPDATE_SYMBOLS, *COMPACT_SYMBOLS, *STREAMED_SYMBOLS,
     "flmr_workspace_create", "flmr_workspace_destroy", "flmr_workspace_status",
     "flmr_maxsim_scores", "flmr_maxsim_topk", "flmr_topk_merge", "flmr_topk_select", "flmr_plaid_decode",
     *FP16_SYMBOLS,
@@ -116,6 +119,12 @@ def lib() -> C.CDLL:
         L.flmr_maxsim_topk_listed.argtypes = [vp, vp, vp, i32, i32, i32, u32, vp, vp, vp, vp, vp]
         L.flmr_maxsim_scores_listed.argtypes = [vp, vp, vp, i32, i32, u32, vp, vp, vp, vp]
         L.flmr_debug_listed_plan.argtypes = [vp, vp, i32, i32, vp, vp, vp, i64, C.POINTER(i64)]
+    if hasattr(L, "flmr_corpus_create_streamed"):
+        L.flmr_corpus_create_streamed.argtypes = [vp, vp, i64, i32, i32, i64, u32, i64, C.POINTER(vp)]
+        L.flmr_corpus_builder_create_streamed.argtypes = [vp, i64, i32, i32, i64, u32, i64, C.POINTER(vp)]
+        L.flmr_corpus_residency.argtypes = [vp, C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
+        L.flmr_debug_window_plan.argtypes = [vp, i64, i64, i32, vp, i64, C.POINTER(i64), vp, vp, vp, vp, i64,
+                                             C.POINTER(i64)]
     L.flmr_workspace_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
     L.flmr_workspace_destroy.argtypes = [vp]
     L.flmr_workspace_status.argtypes = [vp, C.POINTER(i32)]

@@ -40,6 +40,24 @@ def element_dtype(storage: str) -> torch.dtype:
     return torch.float16 if storage == "fp16" else torch.bfloat16
 
 
+RESIDENCIES = ("device", "host")
+DEFAULT_WINDOW_BYTES = 1 << 30
+
+
+def _check_residency(residency: str, storage: str, window_bytes) -> None:
+    """The arguments of a corpus's residency: "device" (its rows in HBM) or "host" (a streamed corpus: its rows in
+    pinned host memory, copied through two HBM windows of at most ``window_bytes`` per search)."""
+    if residency not in RESIDENCIES:
+        raise ValueError("residency must be one of %s, got %r" % (RESIDENCIES, residency))
+    if residency == "host":
+        if storage == "fp8":
+            raise ValueError("residency='host' streams bf16 or fp16 rows; storage='fp8' is held in HBM only")
+        if isinstance(window_bytes, bool) or not isinstance(window_bytes, (int, np.integer)) \
+                or window_bytes < _cabi.DIM * 2:
+            raise ValueError("window_bytes must be an int of at least one row (%d bytes), got %r"
+                             % (_cabi.DIM * 2, window_bytes))
+
+
 def _read_storage(handle) -> str:
     code = C.c_int(0)
     _cabi.check(_cabi.lib().flmr_corpus_storage(handle, C.byref(code), None))
@@ -93,10 +111,18 @@ class FlatCorpus:
                and the scan runs fp16 MMAs, at the bytes and layout of bf16.  fp32 / bf16 sources are converted
                with torch's ``.half()`` as the reference does (beyond +-65504 they become +-inf); queries are
                converted to fp16 for the search, and ``gather_padded`` returns fp16 rows.
+    residency: "device" (default): the rows live in HBM.  "host": a STREAMED corpus — the rows live in pinned host
+               memory and every search copies them through two HBM windows of at most ``window_bytes`` (default
+               1 GiB) while it scans them, so the corpus takes no HBM for its rows; its results are bitwise those of
+               the same rows held in HBM.  For a shard that does not fit beside what the GPU already holds (a
+               validation corpus searched inside a training process), or one larger than the card.  bf16 or fp16
+               only; it cannot be appended to or compacted (``FlmrError``), and restricted searches test bitmaps.
     """
 
     def __init__(self, tokens: torch.Tensor, doclens, device: Optional[Union[int, torch.device]] = None,
-                 pid_base: int = 0, adopt: bool = True, storage: str = "bf16"):
+                 pid_base: int = 0, adopt: bool = True, storage: str = "bf16", residency: str = "device",
+                 window_bytes: int = DEFAULT_WINDOW_BYTES):
+        _check_residency(residency, storage, window_bytes)
         if not torch.cuda.is_available():
             raise RuntimeError("FlatCorpus needs a CUDA device: there is no CPU fallback for this path")
         sflag = _storage_flag(storage)
@@ -124,10 +150,16 @@ class FlatCorpus:
         if tokens.is_cuda:
             torch.cuda.current_stream(device).synchronize()  # producer kernels of `tokens` are done
         handle = C.c_void_p()
-        _cabi.check(L.flmr_corpus_create(C.c_void_p(tokens.data_ptr()),
-                                         self.doclens.ctypes.data_as(C.c_void_p),
-                                         int(self.doclens.shape[0]), _cabi.DIM, int(device.index),
-                                         int(pid_base), flags, C.byref(handle)))
+        if residency == "host":
+            _cabi.check(L.flmr_corpus_create_streamed(C.c_void_p(tokens.data_ptr()),
+                                                      self.doclens.ctypes.data_as(C.c_void_p),
+                                                      int(self.doclens.shape[0]), _cabi.DIM, int(device.index),
+                                                      int(pid_base), sflag, int(window_bytes), C.byref(handle)))
+        else:
+            _cabi.check(L.flmr_corpus_create(C.c_void_p(tokens.data_ptr()),
+                                             self.doclens.ctypes.data_as(C.c_void_p),
+                                             int(self.doclens.shape[0]), _cabi.DIM, int(device.index),
+                                             int(pid_base), flags, C.byref(handle)))
         self._h = handle
         info = _cabi.CorpusInfo()
         _cabi.check(L.flmr_corpus_info(self._h, C.byref(info)))
@@ -155,13 +187,25 @@ class FlatCorpus:
         return self
 
     @property
+    def residency(self) -> str:
+        """"host" for a streamed corpus (rows in pinned host memory), "device" for one whose rows are in HBM."""
+        return "host" if self.residency_info()["streamed"] else "device"
+
+    def residency_info(self) -> dict:
+        """``{"streamed", "window_bytes", "host_bytes"}`` of ``flmr_corpus_residency``."""
+        streamed, window, host = C.c_int(0), C.c_int64(0), C.c_int64(0)
+        _cabi.check(_cabi.lib().flmr_corpus_residency(self.handle, C.byref(streamed), C.byref(window), C.byref(host)))
+        return {"streamed": bool(streamed.value), "window_bytes": int(window.value), "host_bytes": int(host.value)}
+
+    @property
     def dtype(self) -> torch.dtype:
         """Element type of the rows this corpus takes (``append``) and gathers, and of its queries."""
         return element_dtype(self.storage)
 
     @classmethod
     def from_index(cls, path: str, device=None, rank: int = 0, world_size: int = 1,
-                   storage: Optional[str] = None) -> "FlatCorpus":
+                   storage: Optional[str] = None, residency: str = "device",
+                   window_bytes: int = DEFAULT_WINDOW_BYTES) -> "FlatCorpus":
         """Load a flat index (index_io.py) — or, with world_size > 1, only this rank's contiguous,
         token-balanced passage shard of it (SURVEY.md 8e) — into HBM.
 
@@ -173,16 +217,21 @@ class FlatCorpus:
         ``storage=None`` (default) keeps the index's own dtype: "fp16" for an fp16 index ("flmr-flat-f16"), "bf16"
         otherwise.  A storage of another element type converts the shard once on its way in (read on the host,
         ``.to()`` the storage's type) instead of streaming the files.
-        The deletions an index records (``deleted.npy``, format v2) are applied to the passages of this shard."""
+        The deletions an index records (``deleted.npy``, format v2) are applied to the passages of this shard.
+        ``residency="host"``: a streamed corpus (see the class); the files are read straight into its pinned host
+        matrix, with no device copy."""
         import time
         from .index_io import deleted_in_range, index_dtype, index_token_files, load_flat_index, read_deleted, \
             read_metadata
         from .sharded import shard_ranges
+        if storage is not None:
+            _check_residency(residency, storage, window_bytes)
         if not torch.cuda.is_available():
             raise RuntimeError("FlatCorpus needs a CUDA device: there is no CPU fallback for this path")
         disk_storage = "fp16" if index_dtype(read_metadata(path)) == "float16" else "bf16"
         storage = disk_storage if storage is None else storage
         flags = _storage_flag(storage)
+        _check_residency(residency, storage, window_bytes)
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device())
         device = torch.device(device) if not isinstance(device, torch.device) else device
@@ -195,7 +244,8 @@ class FlatCorpus:
         doclens = np.ascontiguousarray(all_doclens[p0:p1], dtype=np.int32)
         if element_dtype(storage) != element_dtype(disk_storage):
             tokens, _, _ = load_flat_index(path, (p0, p1))
-            self = cls(tokens, doclens, device=device, pid_base=p0, storage=storage)
+            self = cls(tokens, doclens, device=device, pid_base=p0, storage=storage, residency=residency,
+                       window_bytes=window_bytes)
             dead = deleted_in_range(read_deleted(path), p0, p1)
             if dead.size:
                 self.delete(dead)
@@ -203,8 +253,13 @@ class FlatCorpus:
         L = _cabi.lib()
         t0 = time.perf_counter()
         b = C.c_void_p()
-        _cabi.check(L.flmr_corpus_builder_create_ex(doclens.ctypes.data_as(C.c_void_p), len(doclens), _cabi.DIM,
-                                                    int(device.index), int(p0), flags, C.byref(b)))
+        if residency == "host":
+            _cabi.check(L.flmr_corpus_builder_create_streamed(doclens.ctypes.data_as(C.c_void_p), len(doclens),
+                                                              _cabi.DIM, int(device.index), int(p0), flags,
+                                                              int(window_bytes), C.byref(b)))
+        else:
+            _cabi.check(L.flmr_corpus_builder_create_ex(doclens.ctypes.data_as(C.c_void_p), len(doclens), _cabi.DIM,
+                                                        int(device.index), int(p0), flags, C.byref(b)))
         try:
             for fname, f0, fn, _rows in files:
                 a, e = max(p0, f0), min(p1, f0 + fn)
@@ -231,12 +286,28 @@ class FlatCorpus:
 
     @classmethod
     def from_plaid(cls, path: str, device=None, rank: int = 0, world_size: int = 1,
-                   storage: str = "bf16") -> "FlatCorpus":
+                   storage: str = "bf16", residency: str = "device",
+                   window_bytes: int = DEFAULT_WINDOW_BYTES) -> "FlatCorpus":
         """Decode a reference PLAID index directory on the GPU (plaid.py) and keep it resident — with
         world_size > 1 only this rank's contiguous, token-balanced passage shard (SURVEY.md 8e).  ``storage="fp16"``
-        decodes straight to fp16 (``flmr_plaid_decode_fp16``), the type the reference's codec decodes to."""
-        from .plaid import plaid_to_flat, read_plaid_doclens, read_plaid_metadata
+        decodes straight to fp16 (``flmr_plaid_decode_fp16``), the type the reference's codec decodes to.
+        ``residency="host"``: a streamed corpus (see the class), decoded on the GPU in bounded chunks
+        (``plaid_to_host_chunks``), each copied down into its pinned host matrix."""
+        from .plaid import plaid_to_flat, plaid_to_host_chunks, read_plaid_doclens, read_plaid_metadata
         from .sharded import shard_ranges
+        _storage_flag(storage)
+        _check_residency(residency, storage, window_bytes)
+        if residency == "host":
+            if world_size == 1:
+                p0, p1 = 0, None
+            else:
+                all_doclens = np.concatenate(read_plaid_doclens(path, read_plaid_metadata(path)["num_chunks"]))
+                p0, p1 = shard_ranges(all_doclens, world_size)[rank]
+                if p0 == p1:
+                    return None
+            return cls._streamed_from_chunks(plaid_to_host_chunks(path, device, passage_range=(p0, p1),
+                                                                  dtype=element_dtype(storage)),
+                                             device, p0, storage, window_bytes)
         if world_size == 1:
             tokens, doclens = plaid_to_flat(path, device, dtype=element_dtype(storage))
             return cls(tokens, doclens, device=tokens.device, storage=storage)
@@ -246,6 +317,28 @@ class FlatCorpus:
             return None
         tokens, doclens = plaid_to_flat(path, device, passage_range=(p0, p1), dtype=element_dtype(storage))
         return cls(tokens, doclens, device=tokens.device, pid_base=p0, storage=storage)
+
+    @classmethod
+    def _streamed_from_chunks(cls, chunks, device, pid_base: int, storage: str, window_bytes: int) -> "FlatCorpus":
+        """A streamed corpus built from ``chunks = (device, doclens, iterator of host token tensors in order)``
+        through the C-level builder, which copies each chunk into the pinned host matrix."""
+        device, doclens, pieces = chunks
+        doclens = np.ascontiguousarray(doclens, dtype=np.int32)
+        L = _cabi.lib()
+        b = C.c_void_p()
+        _cabi.check(L.flmr_corpus_builder_create_streamed(doclens.ctypes.data_as(C.c_void_p), len(doclens), _cabi.DIM,
+                                                          int(device.index), int(pid_base), _storage_flag(storage),
+                                                          int(window_bytes), C.byref(b)))
+        try:
+            for t in pieces:
+                _cabi.check(L.flmr_corpus_builder_append(b, C.c_void_p(t.data_ptr()), t.size(0)))
+            handle = C.c_void_p()
+            _cabi.check(L.flmr_corpus_builder_finish(b, C.byref(handle), None))
+            b = None
+        finally:
+            if b is not None:
+                L.flmr_corpus_builder_destroy(b)
+        return cls._from_handle(handle, doclens, device, pid_base)
 
     # -- properties ---------------------------------------------------------------------------
     @property

@@ -816,13 +816,16 @@ __global__ void __launch_bounds__(kMergeThreads)
 flmr_merge_kernel(const uint64_t* __restrict__ keys, const float* __restrict__ in_scores,
                   const int64_t* __restrict__ in_pids, int n_lists, int n_queries, int k_in,
                   int k_out, int64_t pid_base, const int64_t* __restrict__ slot_pid, float* __restrict__ out_scores,
-                  int64_t* __restrict__ out_pids, int q_offset) {
+                  int64_t* __restrict__ out_pids, int q_offset, bool merge_out = false) {
   __shared__ uint32_t s_ord[32];
   __shared__ int64_t s_pid[32];
   __shared__ uint32_t w_ord;
   __shared__ int64_t w_pid;
   const int b = q_offset + blockIdx.x;   // n_queries = stride of the per-list arrays; blocks cover [q_offset, q_offset + grid)
-  const int n = n_lists * k_in;
+  // merge_out: the k_out entries already in the output row (a streamed corpus's running top-k of earlier windows) are
+  // one more list.  Every thread loads its candidates before the first __syncthreads, and only then is a row written.
+  const int n_in = n_lists * k_in;
+  const int n = n_in + (merge_out ? k_out : 0);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   Cand c[kMergePer];
 #pragma unroll
@@ -830,7 +833,14 @@ flmr_merge_kernel(const uint64_t* __restrict__ keys, const float* __restrict__ i
     const int idx = threadIdx.x + i * kMergeThreads;
     c[i].ord = 0u;
     c[i].pid = kPidEmpty;
-    if (idx < n) {
+    if (idx >= n_in && idx < n) {
+      const int64_t g = static_cast<int64_t>(b) * k_out + (idx - n_in);
+      const int64_t pid = out_pids[g];
+      if (pid >= 0) {
+        c[i].ord = float_to_ordered(out_scores[g]);   // written by this kernel from an ordered key: the same key back
+        c[i].pid = pid;
+      }
+    } else if (idx < n) {
       const int l = idx / k_in, j = idx % k_in;
       const int64_t g = (static_cast<int64_t>(l) * n_queries + b) * k_in + j;
       if (keys) {
@@ -1053,6 +1063,16 @@ struct SlotLayout {
   int64_t bytes = 0;                   // HBM the device arrays above take
 };
 
+// One window of a streamed corpus: the slots [slot0, slot1), stored rows [row0, row0 + rows), scanned from a window
+// buffer that holds exactly those rows from its row 0.  Its partition's row starts are relative to the window; its
+// tiles' first slots are absolute, so candidate keys, tombstones, allow bitmaps and score rows are indexed as in a
+// resident corpus.
+struct Window {
+  int64_t slot0 = 0, slot1 = 0, row0 = 0, rows = 0;
+  int n_ctas = 0;                      // min(SMs, slots of the window)
+  Partition cta;
+};
+
 }  // namespace
 
 // ---- handles -----------------------------------------------------------------------------------------
@@ -1084,6 +1104,15 @@ struct flmr_corpus {
   std::vector<uint32_t> h_dead;
   int64_t n_deleted = 0;
   int sm_total = 0;                    // SMs of the device
+  // A streamed corpus (flmr_corpus_create_streamed): the padded rows live in h_stream (pinned, mapped; d_tokens is its
+  // device alias, which the gather and the SIMT kernel read) and searches copy them window by window into the
+  // workspace's two window buffers.  layout holds the offsets and lengths, but no partition and no tensor map.
+  bool streamed = false;
+  void* h_stream = nullptr;
+  int64_t window_bytes = 0;            // as requested at creation
+  int64_t window_rows = 0;             // rows of the largest window (each window buffer holds this many)
+  std::vector<Window> windows;
+  int64_t windows_bytes = 0;           // HBM of the windows' partitions
 };
 
 // Streaming corpus construction (index load): the padded token matrix is allocated once, packed rows arrive in
@@ -1119,6 +1148,14 @@ struct flmr_workspace {
   int* h_status = nullptr;             // pinned + mapped: readable by the host even after a device trap
   int* d_status = nullptr;             // device alias of h_status
   int dbg_lane_rbq = 4;  // -DFLMR_DEBUG builds: FLMR_LANE_RBQ, read once at creation
+  // streamed corpus only: two window buffers filled on a copy stream of the workspace's own, and the events that order
+  // the copies against the scans (see run_search)
+  __nv_bfloat16* d_win[2] = {nullptr, nullptr};
+  CUtensorMap tmap_win[2];
+  cudaStream_t copy_stream = nullptr;
+  cudaEvent_t fork_ev = nullptr;
+  cudaEvent_t copied_ev[2] = {nullptr, nullptr};
+  cudaEvent_t scanned_ev[2] = {nullptr, nullptr};
 };
 
 // NCCL is resolved at RUN time (dlopen): the library has no link dependency on it, loads on a box without
@@ -1211,11 +1248,11 @@ int64_t hbm_row_bytes(Elem elem) { return elem == Elem::kE4M3 ? kDim : kDim * 2;
 
 const char* elem_name(Elem elem) { return elem == Elem::kE4M3 ? "e4m3" : elem == Elem::kF16 ? "fp16" : "bf16"; }
 
-// HBM a corpus holds: its matrix (an adopted one is the caller's), its layout, its tombstones by slot and its
-// slot -> id map.
+// HBM a corpus holds: its matrix (an adopted one is the caller's, a streamed one is host memory), its layout, the
+// partitions of its windows, its tombstones by slot and its slot -> id map.
 int64_t hbm_bytes(const flmr_corpus* c) {
   const int64_t ns = slots(c);
-  return (c->adopted ? 0 : c->n_rows * hbm_row_bytes(c->elem)) + c->layout.bytes +
+  return (c->adopted || c->streamed ? 0 : c->n_rows * hbm_row_bytes(c->elem)) + c->layout.bytes + c->windows_bytes +
          (c->d_dead ? (ns + 31) / 32 * 4 : 0) + (c->d_slot_pid ? ns * 8 : 0);
 }
 
@@ -1384,6 +1421,37 @@ void build_partition(const std::vector<int64_t>& poff, int n_ctas, int tile_n,
   }
 }
 
+// ---- window planning of a streamed corpus (pure host logic; exported for tests as flmr_debug_window_plan) ----------
+// The slots cut into contiguous ranges, each taking as many slots as fit window_rows stored rows (poff: stored-row
+// offsets of the slots).  *out receives (first slot, end slot) pairs.  A slot longer than a window cannot be scanned
+// from one: FLMR_ERR_UNSUPPORTED.
+int plan_windows(const std::vector<int64_t>& poff, int64_t window_rows, std::vector<std::pair<int64_t, int64_t>>* out) {
+  out->clear();
+  const int64_t n = static_cast<int64_t>(poff.size()) - 1;
+  for (int64_t s0 = 0; s0 < n;) {
+    const int64_t s1 = std::upper_bound(poff.begin() + s0, poff.end(), poff[s0] + window_rows) - poff.begin() - 1;
+    if (s1 <= s0)
+      return fail(FLMR_ERR_UNSUPPORTED, "passage %lld has %lld stored rows (%lld B), more than a window of %lld rows "
+                  "holds", (long long)s0, (long long)(poff[s0 + 1] - poff[s0]),
+                  (long long)((poff[s0 + 1] - poff[s0]) * kDim * 2), (long long)window_rows);
+    out->emplace_back(s0, s1);
+    s0 = s1;
+  }
+  return FLMR_OK;
+}
+
+// The partition of one window [s0, s1) for min(sm_total, s1 - s0) CTAs: build_partition over the window's own row
+// offsets, its tiles' first slots made absolute.
+void window_partition(const std::vector<int64_t>& poff, int64_t s0, int64_t s1, int sm_total, int* n_ctas,
+                      std::vector<int32_t>* rb, std::vector<int64_t>* tb, std::vector<uint32_t>* em,
+                      std::vector<int32_t>* fp) {
+  std::vector<int64_t> wpoff(poff.begin() + s0, poff.begin() + s1 + 1);
+  for (int64_t& r : wpoff) r -= poff[s0];
+  *n_ctas = static_cast<int>(std::min<int64_t>(sm_total, s1 - s0));
+  build_partition(wpoff, *n_ctas, kTileN, rb, tb, em, fp);
+  for (int32_t& f : *fp) f += static_cast<int32_t>(s0);
+}
+
 // ---- pass planning (pure host logic; exported for tests as flmr_debug_plan_passes) -------------------
 // One pass = one launch of the scan kernel over the whole shard with up to kRbMax 32-row blocks of
 // queries resident (kNqMax queries at most).
@@ -1516,19 +1584,20 @@ ScanKernel pick_scan(Elem elem, bool listed, int variant, int blocks) {
 }
 
 // One scan pass.  pair: a CTA-pair pass (planned only under variant 4).  listed: p holds a listed search's plan
-// (run_search's ListedArgs).
-int launch_scan(const flmr_corpus* c, ScanParams p, bool pair, bool listed, cudaStream_t st) {
+// (run_search's ListedArgs).  win (a streamed corpus): the pass scans that window from the buffer win_map describes.
+int launch_scan(const flmr_corpus* c, ScanParams p, bool pair, bool listed, cudaStream_t st,
+                const Window* win = nullptr, const CUtensorMap* win_map = nullptr) {
   const SlotLayout& l = c->layout;
   // the passes variant 4 leaves to single CTAs run the two-warpgroup kernel
   const int variant = g_scan_variant == 4 && !pair ? 2 : g_scan_variant;
   const ScanKernel k = pick_scan(c->elem, listed, variant, scan_blocks(p.nq_pass, p.rbq));
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(pair ? 2 * l.n_pairs : l.n_ctas));
+  cfg.gridDim = dim3(static_cast<unsigned>(win ? win->n_ctas : pair ? 2 * l.n_pairs : l.n_ctas));
   cfg.blockDim = dim3(scan_threads(k.wgs));
   cfg.dynamicSmemBytes = ScanSmem::kBytes;
   cfg.stream = st;
   if (!listed) {   // a listed pass brings its plan's tiles
-    const Partition& part = pair ? l.pair : l.cta;
+    const Partition& part = win ? win->cta : pair ? l.pair : l.cta;
     p.cta_row_begin = part.row_begin;
     p.cta_tile_base = part.tile_base;
     p.tile_end_mask = part.end_mask;
@@ -1542,7 +1611,7 @@ int launch_scan(const flmr_corpus* c, ScanParams p, bool pair, bool listed, cuda
     cfg.attrs = &cluster;
     cfg.numAttrs = 1;
   }
-  void* args[] = {const_cast<CUtensorMap*>(pair ? &l.tmap_half : &l.tmap_d), &p};
+  void* args[] = {const_cast<CUtensorMap*>(win ? win_map : pair ? &l.tmap_half : &l.tmap_d), &p};
   EventPair ev{};
   if (g_profiling) {
     FLMR_CUDA(cudaEventCreate(&ev.a));
@@ -1574,14 +1643,16 @@ int stage_queries(flmr_workspace* ws, const void* d_q, int nq, const StageParams
 
 // Queries [q0, q0 + nq) of a chunk of `stride` queries; `n_lists` = candidate lists per query (CTAs, or CTA pairs
 // for queries that went through pair passes).  d_out_* point at the chunk's first query.
+// merge_out: the output rows already hold a running top-k (a streamed corpus's earlier windows), merged in as one more
+// list.
 int launch_merge_keys(const flmr_corpus* c, flmr_workspace* ws, int n_lists, int stride, int q0, int nq, int k,
-                      float* d_out_scores, int64_t* d_out_pids, cudaStream_t st) {
+                      float* d_out_scores, int64_t* d_out_pids, cudaStream_t st, bool merge_out = false) {
   if (nq <= 0) return FLMR_OK;
-  if (static_cast<int64_t>(n_lists) * k > kMergeThreads * kMergePer)
+  if ((static_cast<int64_t>(n_lists) + merge_out) * k > kMergeThreads * kMergePer)
     return fail(FLMR_ERR_UNSUPPORTED, "n_lists*k = %lld exceeds merge capacity %d",
-                (long long)n_lists * k, kMergeThreads * kMergePer);
+                (long long)(n_lists + merge_out) * k, kMergeThreads * kMergePer);
   flmr_merge_kernel<<<nq, kMergeThreads, 0, st>>>(ws->d_cand_keys, nullptr, nullptr, n_lists, stride, k, k,
-                                                  c->pid_base, c->d_slot_pid, d_out_scores, d_out_pids, q0);
+                                                  c->pid_base, c->d_slot_pid, d_out_scores, d_out_pids, q0, merge_out);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
   return FLMR_OK;
@@ -1774,87 +1845,120 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   // within a chunk: every pass's scan, then the merge over the chunk's queries (one launch per kind of pass)
   std::vector<PassPlan> plan;
   std::vector<int> slot;
-  for (int c0 = 0; c0 < n_queries; c0 += ws->max_queries) {
-    const int nqc = std::min(ws->max_queries, n_queries - c0);
-    const __nv_bfloat16* d_qc = static_cast<const __nv_bfloat16*>(d_q) + static_cast<int64_t>(c0) * nq * kDim;
-    float* d_all_c = d_slot_scores ? d_slot_scores
-                                   : d_all_scores ? d_all_scores + static_cast<int64_t>(c0) * c->n_passages : nullptr;
-    int group = 1, n_pair_q = 0;
-    plan_passes(nqc, nq, allow_pair, &plan, &group, &n_pair_q);
-    if (!d_all_c && nq > kRbMax * 32 && (rc = ensure_acc(ws, static_cast<int64_t>(group) * ns)))
-      return rc;
-    p.cand_q_stride = nqc;
-    ListedChunkPlan lp;
-    if (listed && (rc = plan_listed_chunk(c, ws, plan, c0, nqc, *listed, st, &lp))) return rc;
-    slot.assign(plan.size(), 0);
-    size_t staged_until = 0;                    // passes [0, staged_until) have their queries staged
-    for (size_t pi = 0; pi < plan.size(); ++pi) {
-      if (pi == staged_until) {
-        // the query blocks of as many of the next passes as fit the staging buffer (a pair pass takes two slots:
-        // one block per CTA of a pair) are staged by ONE launch, ahead of their scans
-        StageParams sp{};
-        int used = 0;
-        while (staged_until < plan.size()) {
-          const PassPlan& q = plan[staged_until];
-          const int need = (q.flags & kPassPair) ? 2 : 1;
-          if (used + need > kStageMaxPasses) break;
-          slot[staged_until] = used;
-          for (int r = 0; r < need; ++r)
-            sp.pass[used++] = {q.q_first + r * q.n_q, q.n_q, q.row0, q.rows, q.rbq, q.n_mtiles * kTileM};
-          ++staged_until;
+  // A streamed corpus is scanned window by window, each window once per call: the windows are the outer loop, the call
+  // chunks the inner one, and each chunk's top-k rows carry the running top-k from window to window (the merge of a
+  // window's per-CTA lists takes the rows as one more list).  Window w is copied into buffer w & 1 on the workspace's
+  // copy stream; its scans wait for that copy, and the copy of window w + 2 into the same buffer waits for them.  The
+  // copy stream first waits for the call's stream, and every copy is waited for by a scan on it, so the call is
+  // ordered on `st` like any other.
+  const int n_windows = c->streamed ? static_cast<int>(c->windows.size()) : 1;
+  auto copy_window = [&](int w) -> int {
+    const Window& win = c->windows[w];
+    const int b = w & 1;
+    if (w >= 2) FLMR_CUDA(cudaStreamWaitEvent(ws->copy_stream, ws->scanned_ev[b], 0));
+    FLMR_CUDA(cudaMemcpyAsync(ws->d_win[b], static_cast<const char*>(c->h_stream) + win.row0 * kDim * 2,
+                              static_cast<size_t>(win.rows) * kDim * 2, cudaMemcpyHostToDevice, ws->copy_stream));
+    FLMR_CUDA(cudaEventRecord(ws->copied_ev[b], ws->copy_stream));
+    return FLMR_OK;
+  };
+  if (c->streamed) {
+    if (listed) return fail(FLMR_ERR_UNSUPPORTED, "a streamed corpus has no listed scan");
+    FLMR_CUDA(cudaEventRecord(ws->fork_ev, st));
+    FLMR_CUDA(cudaStreamWaitEvent(ws->copy_stream, ws->fork_ev, 0));
+    for (int w = 0; w < std::min(n_windows, 2); ++w)
+      if ((rc = copy_window(w))) return rc;
+  }
+  for (int w = 0; w < n_windows; ++w) {
+    const Window* win = c->streamed ? &c->windows[w] : nullptr;
+    const CUtensorMap* win_map = win ? &ws->tmap_win[w & 1] : nullptr;
+    const int n_lists = win ? win->n_ctas : l.n_ctas;
+    if (win) FLMR_CUDA(cudaStreamWaitEvent(st, ws->copied_ev[w & 1], 0));
+    for (int c0 = 0; c0 < n_queries; c0 += ws->max_queries) {
+      const int nqc = std::min(ws->max_queries, n_queries - c0);
+      const __nv_bfloat16* d_qc = static_cast<const __nv_bfloat16*>(d_q) + static_cast<int64_t>(c0) * nq * kDim;
+      float* d_all_c = d_slot_scores ? d_slot_scores
+                                     : d_all_scores ? d_all_scores + static_cast<int64_t>(c0) * c->n_passages : nullptr;
+      int group = 1, n_pair_q = 0;
+      plan_passes(nqc, nq, allow_pair, &plan, &group, &n_pair_q);
+      if (!d_all_c && nq > kRbMax * 32 && (rc = ensure_acc(ws, static_cast<int64_t>(group) * ns)))
+        return rc;
+      p.cand_q_stride = nqc;
+      ListedChunkPlan lp;
+      if (listed && (rc = plan_listed_chunk(c, ws, plan, c0, nqc, *listed, st, &lp))) return rc;
+      slot.assign(plan.size(), 0);
+      size_t staged_until = 0;                    // passes [0, staged_until) have their queries staged
+      for (size_t pi = 0; pi < plan.size(); ++pi) {
+        if (pi == staged_until) {
+          // the query blocks of as many of the next passes as fit the staging buffer (a pair pass takes two slots:
+          // one block per CTA of a pair) are staged by ONE launch, ahead of their scans
+          StageParams sp{};
+          int used = 0;
+          while (staged_until < plan.size()) {
+            const PassPlan& q = plan[staged_until];
+            const int need = (q.flags & kPassPair) ? 2 : 1;
+            if (used + need > kStageMaxPasses) break;
+            slot[staged_until] = used;
+            for (int r = 0; r < need; ++r)
+              sp.pass[used++] = {q.q_first + r * q.n_q, q.n_q, q.row0, q.rows, q.rbq, q.n_mtiles * kTileM};
+            ++staged_until;
+          }
+          if ((rc = stage_queries(ws, d_qc, nq, sp, used, st))) return rc;
         }
-        if ((rc = stage_queries(ws, d_qc, nq, sp, used, st))) return rc;
+        const PassPlan& pp = plan[pi];
+        // partial / final scores of query (group_first + acc_slot + i) live in row i of `acc`
+        float* acc = d_all_c
+                         ? d_all_c + static_cast<int64_t>(pp.group_first + pp.acc_slot) * ns
+                         : (ws->d_acc ? ws->d_acc + static_cast<int64_t>(pp.acc_slot) * ns : nullptr);
+        p.q_pad = reinterpret_cast<const uint4*>(ws->d_qpad) + static_cast<int64_t>(slot[pi]) * (kMtMax * kTileM * 16);
+        p.n_mtiles = pp.n_mtiles;
+        p.nq_pass = pp.n_q;
+        p.rbq = pp.rbq;
+        p.acc_in = (pp.flags & kPassAccIn) ? acc : nullptr;
+        p.acc_out = ((pp.flags & kPassAccOut) || ((pp.flags & kPassFinal) && d_all_c)) ? acc : nullptr;
+        p.k = (pp.flags & kPassFinal) ? k : 0;
+        p.cand_q_first = pp.q_first;
+        p.allow = allow ? allow + static_cast<int64_t>(c0 + pp.q_first) * allow_stride : nullptr;
+        p.allow_stride = allow_stride;
+        if (listed) {   // the pass's plan, and its queries' slot bitmaps
+          const ListedPass& lpp = lp.passes[pi];
+          p.cta_row_begin = nullptr;
+          p.cta_tile_base = lp.cta_tile_base + lpp.c_off;
+          p.tile_end_mask = lp.tile_mask + lpp.t_off;
+          p.tile_first_pid = lp.tile_first + lpp.t_off;
+          p.tile_row = lp.tile_row + lpp.t_off;
+          p.allow = lp.allow + static_cast<int64_t>(pp.q_first) * lp.words;
+          p.allow_stride = lp.words;
+        }
+        if ((rc = launch_scan(c, p, (pp.flags & kPassPair) != 0, listed != nullptr, st, win, win_map))) return rc;
       }
-      const PassPlan& pp = plan[pi];
-      // partial / final scores of query (group_first + acc_slot + i) live in row i of `acc`
-      float* acc = d_all_c
-                       ? d_all_c + static_cast<int64_t>(pp.group_first + pp.acc_slot) * ns
-                       : (ws->d_acc ? ws->d_acc + static_cast<int64_t>(pp.acc_slot) * ns : nullptr);
-      p.q_pad = reinterpret_cast<const uint4*>(ws->d_qpad) + static_cast<int64_t>(slot[pi]) * (kMtMax * kTileM * 16);
-      p.n_mtiles = pp.n_mtiles;
-      p.nq_pass = pp.n_q;
-      p.rbq = pp.rbq;
-      p.acc_in = (pp.flags & kPassAccIn) ? acc : nullptr;
-      p.acc_out = ((pp.flags & kPassAccOut) || ((pp.flags & kPassFinal) && d_all_c)) ? acc : nullptr;
-      p.k = (pp.flags & kPassFinal) ? k : 0;
-      p.cand_q_first = pp.q_first;
-      p.allow = allow ? allow + static_cast<int64_t>(c0 + pp.q_first) * allow_stride : nullptr;
-      p.allow_stride = allow_stride;
-      if (listed) {   // the pass's plan, and its queries' slot bitmaps
-        const ListedPass& lpp = lp.passes[pi];
-        p.cta_row_begin = nullptr;
-        p.cta_tile_base = lp.cta_tile_base + lpp.c_off;
-        p.tile_end_mask = lp.tile_mask + lpp.t_off;
-        p.tile_first_pid = lp.tile_first + lpp.t_off;
-        p.tile_row = lp.tile_row + lpp.t_off;
-        p.allow = lp.allow + static_cast<int64_t>(pp.q_first) * lp.words;
-        p.allow_stride = lp.words;
-      }
-      if ((rc = launch_scan(c, p, (pp.flags & kPassPair) != 0, listed != nullptr, st))) return rc;
-    }
-    if (listed && d_slot_scores) {
-      const int64_t n = listed->h_off[c0 + nqc] - listed->h_off[c0];
-      if (n > 0) {
-        flmr_listed_scores_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
-            listed->d_pids, listed->d_off + c0, nqc, c->d_slot_pid, ns, c->pid_base, c->n_passages, d_slot_scores,
-            listed->d_scores);
+      if (listed && d_slot_scores) {
+        const int64_t n = listed->h_off[c0 + nqc] - listed->h_off[c0];
+        if (n > 0) {
+          flmr_listed_scores_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
+              listed->d_pids, listed->d_off + c0, nqc, c->d_slot_pid, ns, c->pid_base, c->n_passages, d_slot_scores,
+              listed->d_scores);
+          FLMR_CUDA(cudaGetLastError());
+          ++g_launches;
+        }
+      } else if (d_slot_scores) {
+        const int64_t n = static_cast<int64_t>(nqc) * c->n_passages;
+        flmr_expand_slot_scores_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
+            d_slot_scores, ns, c->d_slot_pid, c->pid_base, c->n_passages, nqc,
+            d_all_scores + static_cast<int64_t>(c0) * c->n_passages);
         FLMR_CUDA(cudaGetLastError());
         ++g_launches;
       }
-    } else if (d_slot_scores) {
-      const int64_t n = static_cast<int64_t>(nqc) * c->n_passages;
-      flmr_expand_slot_scores_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
-          d_slot_scores, ns, c->d_slot_pid, c->pid_base, c->n_passages, nqc,
-          d_all_scores + static_cast<int64_t>(c0) * c->n_passages);
-      FLMR_CUDA(cudaGetLastError());
-      ++g_launches;
+      if (k > 0) {
+        float* os = d_topk_scores + static_cast<int64_t>(c0) * k;
+        int64_t* op = d_topk_pids + static_cast<int64_t>(c0) * k;
+        // queries of pair passes have one candidate list per CTA PAIR, the others one per CTA
+        if ((rc = launch_merge_keys(c, ws, l.n_pairs, nqc, 0, n_pair_q, k, os, op, st))) return rc;
+        if ((rc = launch_merge_keys(c, ws, n_lists, nqc, n_pair_q, nqc - n_pair_q, k, os, op, st, w > 0))) return rc;
+      }
     }
-    if (k > 0) {
-      float* os = d_topk_scores + static_cast<int64_t>(c0) * k;
-      int64_t* op = d_topk_pids + static_cast<int64_t>(c0) * k;
-      // queries of pair passes have one candidate list per CTA PAIR, the others one per CTA
-      if ((rc = launch_merge_keys(c, ws, l.n_pairs, nqc, 0, n_pair_q, k, os, op, st))) return rc;
-      if ((rc = launch_merge_keys(c, ws, l.n_ctas, nqc, n_pair_q, nqc - n_pair_q, k, os, op, st))) return rc;
+    if (win) {
+      FLMR_CUDA(cudaEventRecord(ws->scanned_ev[w & 1], st));
+      if (w + 2 < n_windows && (rc = copy_window(w + 2))) return rc;
     }
   }
   return FLMR_OK;
@@ -1920,6 +2024,65 @@ int build_layout(Elem elem, const __nv_bfloat16* d_tokens, const uint8_t* d_fp8,
   }
   if (rc) free_layout(l);
   return rc;
+}
+
+// The layout of a streamed corpus from its slots' offsets and lengths: the offsets and lengths on the device (for the
+// gather and the SIMT kernel), and the windows of c->window_bytes with their partitions.  layout.n_ctas is the most
+// CTAs a window launches (it sizes a workspace's candidate lists), layout.cta.n_tiles the tiles of all windows.
+int build_streamed_layout(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_t* lens) {
+  SlotLayout* l = &c->layout;
+  const int64_t ns = static_cast<int64_t>(poff.size()) - 1;
+  std::vector<std::pair<int64_t, int64_t>> ranges;
+  if (int rc = plan_windows(poff, c->window_bytes / (kDim * 2), &ranges)) return rc;
+  l->h_poff = poff;
+  l->h_doclen.assign(lens, lens + ns);
+  for (int64_t s = 0; s < ns; ++s) l->max_rows = std::max(l->max_rows, poff[s + 1] - poff[s]);
+  int rc = dev_upload(&l->d_poff, l->h_poff, &l->bytes);
+  if (!rc) rc = dev_upload(&l->d_doclen, l->h_doclen, &l->bytes);
+  c->windows.resize(ranges.size());
+  for (size_t w = 0; w < ranges.size() && !rc; ++w) {
+    Window& win = c->windows[w];
+    win.slot0 = ranges[w].first;
+    win.slot1 = ranges[w].second;
+    win.row0 = poff[win.slot0];
+    win.rows = poff[win.slot1] - win.row0;
+    c->window_rows = std::max(c->window_rows, win.rows);
+    std::vector<int32_t> rb, fp;
+    std::vector<int64_t> tb;
+    std::vector<uint32_t> em;
+    window_partition(poff, win.slot0, win.slot1, c->sm_total, &win.n_ctas, &rb, &tb, &em, &fp);
+    win.cta.n_tiles = static_cast<int64_t>(em.size());
+    l->n_ctas = std::max(l->n_ctas, win.n_ctas);
+    l->cta.n_tiles += win.cta.n_tiles;
+    rc = dev_upload(&win.cta.row_begin, rb, &c->windows_bytes);
+    if (!rc) rc = dev_upload(&win.cta.tile_base, tb, &c->windows_bytes);
+    if (!rc) rc = dev_upload(&win.cta.end_mask, em, &c->windows_bytes);
+    if (!rc) rc = dev_upload(&win.cta.first_pid, fp, &c->windows_bytes);
+  }
+  // the scan kernels' shared-memory limit, which build_layout sets for a resident corpus
+  for (const ScanKernels& t : kScanKernels[static_cast<int>(c->elem)])
+    for (ScanFn fn : {t.two, t.three, t.split, t.pair}) {
+      const cudaError_t e =
+          fn && !rc ? cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes)
+                    : cudaSuccess;
+      if (e != cudaSuccess)
+        rc = fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s", ScanSmem::kBytes,
+                  cudaGetErrorString(e));
+    }
+  return rc;
+}
+
+// The pinned, mapped host matrix of a new streamed corpus (n_rows set); d_tokens becomes its device alias.
+int alloc_stream_matrix(flmr_corpus* c) {
+  const size_t bytes = static_cast<size_t>(c->n_rows) * kDim * 2;
+  if (const cudaError_t e = cudaHostAlloc(&c->h_stream, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+      e != cudaSuccess) {
+    c->h_stream = nullptr;
+    return fail(FLMR_ERR_OOM, "cudaHostAlloc(%zu B) for the streamed token matrix failed: %s", bytes,
+                cudaGetErrorString(e));
+  }
+  FLMR_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&c->d_tokens), c->h_stream, 0));
+  return FLMR_OK;
 }
 
 // The token matrix of a new corpus (n_rows set): bf16 in HBM, or (e4m3) the e4m3 copy in HBM plus the bf16 master
@@ -1992,6 +2155,23 @@ cudaError_t pack_passages(const void* tokens, bool is_device_ptr, const std::vec
   cudaFree(d_soff);
   cudaFree(d_poff);
   return e;
+}
+
+// The host twin of flmr_scatter_rows_kernel, for a streamed corpus's host matrix: packed rows [s0, s0 + n) at src go to
+// their place in the padded layout at dst, a passage's last token also over its padding rows.
+void host_scatter_rows(const char* src, const std::vector<int64_t>& soff, const std::vector<int64_t>& poff, int64_t s0,
+                       int64_t n, char* dst) {
+  constexpr int64_t kRow = kDim * 2;
+  int64_t p = std::upper_bound(soff.begin(), soff.end(), s0) - soff.begin() - 1;
+  for (int64_t r = s0; r < s0 + n; ++p) {
+    const int64_t take = std::min(soff[p + 1], s0 + n) - r;   // rows of passage p in this chunk
+    char* d = dst + (poff[p] + (r - soff[p])) * kRow;
+    memcpy(d, src + (r - s0) * kRow, static_cast<size_t>(take * kRow));
+    r += take;
+    if (r == soff[p + 1])
+      for (int64_t j = poff[p] + (soff[p + 1] - soff[p]); j < poff[p + 1]; ++j)
+        memcpy(dst + j * kRow, src + (r - 1 - s0) * kRow, kRow);
+  }
 }
 
 // ---- compaction schedule (pure host logic; exported for tests as flmr_debug_compact_plan) ----------------------
@@ -2157,11 +2337,79 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
   return FLMR_OK;
 }
 
+int flmr_corpus_create_streamed(const void* tokens, const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                int64_t pid_base, unsigned flags, int64_t window_bytes, flmr_corpus_t** out) {
+  if (!out) return fail(FLMR_ERR_INVALID_ARG, "out is null");
+  *out = nullptr;
+  if (flags & ~FLMR_CORPUS_FP16)
+    return fail(FLMR_ERR_UNSUPPORTED, "flags 0x%x: a streamed corpus is bf16 or FLMR_CORPUS_FP16, and is never adopted",
+                flags);
+  if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
+  if (n_passages <= 0 || !tokens || !h_doclens)
+    return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null tokens/doclens");
+  if (window_bytes < kDim * 2) return fail(FLMR_ERR_INVALID_ARG, "window_bytes=%lld holds no row", (long long)window_bytes);
+  std::vector<int64_t> soff, poff;
+  int rc;
+  if ((rc = passage_offsets(h_doclens, n_passages, &soff, &poff, nullptr))) return rc;
+  const int64_t n_rows = poff[n_passages];
+  if (n_rows + kTileN >= (1ll << 31))
+    return fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
+                (long long)n_rows);
+  {   // refused before anything is allocated
+    std::vector<std::pair<int64_t, int64_t>> ranges;
+    if ((rc = plan_windows(poff, window_bytes / (kDim * 2), &ranges))) return rc;
+  }
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
+  int sm_count;
+  bool is_device_ptr;
+  if ((rc = sm90_count(device, &sm_count)) || (rc = token_source(tokens, device, &is_device_ptr))) return rc;
+  flmr_corpus* c = new (std::nothrow) flmr_corpus();
+  if (!c) return fail(FLMR_ERR_OOM, "host allocation failed");
+  c->device = device;
+  c->n_passages = n_passages;
+  c->n_tokens = soff[n_passages];
+  c->n_rows = n_rows;
+  c->pid_base = pid_base;
+  c->elem = (flags & FLMR_CORPUS_FP16) ? Elem::kF16 : Elem::kBF16;
+  c->sm_total = sm_count;
+  c->streamed = true;
+  c->window_bytes = window_bytes;
+  auto bail = [&](int code) {
+    flmr_corpus_destroy(c);
+    return code;
+  };
+  if ((rc = alloc_stream_matrix(c))) return bail(rc);
+  if (is_device_ptr) {   // the repack kernel writes the host matrix through its device alias
+    const cudaError_t e = pack_passages(tokens, true, soff, poff, h_doclens, n_passages,
+                                        reinterpret_cast<uint4*>(c->d_tokens), nullptr);
+    if (e != cudaSuccess) return bail(fail(FLMR_ERR_CUDA, "corpus repack failed: %s", cudaGetErrorString(e)));
+  } else {
+    host_scatter_rows(static_cast<const char*>(tokens), soff, poff, 0, c->n_tokens, static_cast<char*>(c->h_stream));
+  }
+  if ((rc = build_streamed_layout(c, poff, h_doclens))) return bail(rc);
+  *out = c;
+  return FLMR_OK;
+}
+
+int flmr_corpus_residency(const flmr_corpus_t* c, int* streamed, int64_t* window_bytes, int64_t* host_bytes) {
+  if (!c) return fail(FLMR_ERR_INVALID_ARG, "null corpus");
+  if (streamed) *streamed = c->streamed ? 1 : 0;
+  if (window_bytes) *window_bytes = c->streamed ? c->window_bytes : 0;
+  if (host_bytes) *host_bytes = c->streamed ? c->n_rows * kDim * 2 : 0;
+  return FLMR_OK;
+}
+
 int flmr_corpus_destroy(flmr_corpus_t* c) {
   if (!c) return FLMR_OK;
   DeviceGuard guard(c->device);
-  if (c->vm_tokens.base || c->vm_fp8.base) cudaDeviceSynchronize();   // no search still reads the matrices
+  if (c->vm_tokens.base || c->vm_fp8.base || c->h_stream) cudaDeviceSynchronize();   // no search still reads them
   if (c->h_master) cudaFreeHost(c->h_master);   // d_tokens is its device alias
+  if (c->h_stream) cudaFreeHost(c->h_stream);   // likewise
+  for (Window& w : c->windows)
+    for (void* q : {static_cast<void*>(w.cta.row_begin), static_cast<void*>(w.cta.tile_base),
+                    static_cast<void*>(w.cta.end_mask), static_cast<void*>(w.cta.first_pid)})
+      cudaFree(q);
   gm_free(&c->vm_tokens);                       // (an adopted matrix is the caller's and has no mapping here)
   gm_free(&c->vm_fp8);
   free_layout(&c->layout);
@@ -2176,10 +2424,16 @@ int flmr_corpus_builder_create(const int32_t* h_doclens, int64_t n_passages, int
   return flmr_corpus_builder_create_ex(h_doclens, n_passages, dim, device, pid_base, FLMR_CORPUS_COPY, out);
 }
 
-int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
-                                  int64_t pid_base, unsigned flags, flmr_corpus_builder_t** out) {
+extern "C++" {
+namespace {
+// flmr_corpus_builder_create_ex (window_bytes = 0) and flmr_corpus_builder_create_streamed (window_bytes > 0).
+int builder_create(const int32_t* h_doclens, int64_t n_passages, int dim, int device, int64_t pid_base, unsigned flags,
+                   int64_t window_bytes, flmr_corpus_builder_t** out) {
   if (!out) return fail(FLMR_ERR_INVALID_ARG, "out is null");
   *out = nullptr;
+  const bool streamed = window_bytes > 0;
+  if (streamed && (flags & ~FLMR_CORPUS_FP16))
+    return fail(FLMR_ERR_UNSUPPORTED, "builder flags 0x%x: a streamed corpus is bf16 or FLMR_CORPUS_FP16", flags);
   if (flags & ~(FLMR_CORPUS_FP8 | FLMR_CORPUS_FP16))
     return fail(FLMR_ERR_INVALID_ARG, "builder flags 0x%x: only FLMR_CORPUS_FP8 or FLMR_CORPUS_FP16 applies to a "
                 "streamed load", flags);
@@ -2199,6 +2453,10 @@ int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, 
   if (n_rows + kTileN >= (1ll << 31))
     return bail(fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
                      (long long)n_rows));
+  if (streamed) {   // refused before anything is allocated
+    std::vector<std::pair<int64_t, int64_t>> ranges;
+    if (int rc = plan_windows(b->poff, window_bytes / (kDim * 2), &ranges)) return bail(rc);
+  }
   DeviceGuard guard(device);
   if (!guard.ok) return bail(fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device));
   int sm_count;
@@ -2213,6 +2471,22 @@ int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, 
   c->pid_base = pid_base;
   c->elem = elem;
   c->sm_total = sm_count;
+  if (streamed) {
+    // rows are read (or copied) straight into the host matrix, or, when passages need padding, through one pinned
+    // staging buffer from which host_scatter_rows puts them in place; the device is not involved
+    c->streamed = true;
+    c->window_bytes = window_bytes;
+    if (int rc = alloc_stream_matrix(c)) return bail(rc);
+    const size_t buf_bytes = static_cast<size_t>(flmr_corpus_builder::kBufRows) * kDim * 2;
+    if (!b->aligned) {
+      if (const cudaError_t e = cudaHostAlloc(&b->h_pin[0], buf_bytes, cudaHostAllocDefault); e != cudaSuccess) {
+        b->h_pin[0] = nullptr;
+        return bail(fail(FLMR_ERR_OOM, "staging buffer: %s", cudaGetErrorString(e)));
+      }
+    }
+    *out = b;
+    return FLMR_OK;
+  }
   if (int rc = alloc_token_matrix(c)) return bail(rc);
   // an e4m3 corpus always goes through the scatter kernel, which writes the master and the e4m3 copy
   const bool scatter = !b->aligned || elem == Elem::kE4M3;
@@ -2234,6 +2508,23 @@ int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, 
   *out = b;
   return FLMR_OK;
 }
+}  // namespace
+}  // extern "C++"
+
+int flmr_corpus_builder_create_ex(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                  int64_t pid_base, unsigned flags, flmr_corpus_builder_t** out) {
+  return builder_create(h_doclens, n_passages, dim, device, pid_base, flags, 0, out);
+}
+
+int flmr_corpus_builder_create_streamed(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                        int64_t pid_base, unsigned flags, int64_t window_bytes,
+                                        flmr_corpus_builder_t** out) {
+  if (window_bytes < kDim * 2) {
+    if (out) *out = nullptr;
+    return fail(FLMR_ERR_INVALID_ARG, "window_bytes=%lld holds no row", (long long)window_bytes);
+  }
+  return builder_create(h_doclens, n_passages, dim, device, pid_base, flags, window_bytes, out);
+}
 
 extern "C++" {
 namespace {
@@ -2247,6 +2538,22 @@ int builder_feed(flmr_corpus_builder* b, int64_t n_rows, Fill fill) {
                 (long long)n_rows, (long long)c->n_tokens, (long long)b->rows_done);
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
+  if (c->streamed) {   // straight into the host matrix (aligned), or through the staging buffer and host_scatter_rows
+    char* matrix = static_cast<char*>(c->h_stream);
+    for (int64_t r0 = 0; r0 < n_rows; r0 += flmr_corpus_builder::kBufRows) {
+      const int64_t rows = std::min<int64_t>(flmr_corpus_builder::kBufRows, n_rows - r0);
+      void* dst = b->aligned ? matrix + b->rows_done * kDim * 2 : b->h_pin[0];
+      timespec t0, t1;
+      clock_gettime(CLOCK_MONOTONIC, &t0);
+      if (int rc = fill(dst, r0, rows)) return rc;
+      clock_gettime(CLOCK_MONOTONIC, &t1);
+      b->fill_s += (t1.tv_sec - t0.tv_sec) + 1e-9 * (t1.tv_nsec - t0.tv_nsec);
+      if (!b->aligned) host_scatter_rows(static_cast<const char*>(b->h_pin[0]), b->soff, b->poff, b->rows_done, rows,
+                                         matrix);
+      b->rows_done += rows;
+    }
+    return FLMR_OK;
+  }
   for (int64_t r0 = 0; r0 < n_rows; r0 += flmr_corpus_builder::kBufRows) {
     const int64_t rows = std::min<int64_t>(flmr_corpus_builder::kBufRows, n_rows - r0);
     const int i = b->next;
@@ -2328,10 +2635,14 @@ int flmr_corpus_builder_finish(flmr_corpus_builder_t* b, flmr_corpus_t** out, do
                 (long long)c->n_tokens);
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
-  FLMR_CUDA(cudaStreamSynchronize(b->stream));
-  if (int rc = build_layout(c->elem, c->d_tokens, c->d_fp8, c->n_rows, b->poff, b->doclens.data(), c->sm_total,
-                            &c->layout))
-    return rc;
+  if (c->streamed) {
+    if (int rc = build_streamed_layout(c, b->poff, b->doclens.data())) return rc;
+  } else {
+    FLMR_CUDA(cudaStreamSynchronize(b->stream));
+    if (int rc = build_layout(c->elem, c->d_tokens, c->d_fp8, c->n_rows, b->poff, b->doclens.data(), c->sm_total,
+                              &c->layout))
+      return rc;
+  }
   if (host_fill_seconds) *host_fill_seconds = b->fill_s;
   b->corpus = nullptr;     // ownership passes to the caller
   flmr_corpus_builder_destroy(b);
@@ -2381,6 +2692,7 @@ int flmr_corpus_storage(const flmr_corpus_t* c, int* storage, int64_t* host_byte
 int flmr_corpus_append(flmr_corpus_t* c, const void* tokens, const int32_t* h_doclens, int64_t n_passages,
                        int64_t* first_pid) {
   if (!c || !tokens || !h_doclens) return fail(FLMR_ERR_INVALID_ARG, "null argument");
+  if (c->streamed) return fail(FLMR_ERR_UNSUPPORTED, "a streamed corpus cannot be appended to");
   if (n_passages <= 0) return fail(FLMR_ERR_INVALID_ARG, "n_passages=%lld must be >= 1", (long long)n_passages);
   const int64_t old_n = c->n_passages, old_rows = c->n_rows;
   // the new passages, relative to their first: packed (soff) and padded (poff) row offsets
@@ -2536,6 +2848,7 @@ int flmr_corpus_compact(flmr_corpus_t* c, int64_t* n_removed, int64_t* bytes_rel
   if (n_removed) *n_removed = 0;
   if (bytes_released) *bytes_released = 0;
   if (!c) return fail(FLMR_ERR_INVALID_ARG, "null corpus");
+  if (c->streamed) return fail(FLMR_ERR_UNSUPPORTED, "a streamed corpus cannot be compacted");
   const int64_t ns = slots(c);
   // --- 1. which slots stay: their ids, offsets and lengths in the compacted corpus ---
   std::vector<char> keep(ns, 1);
@@ -2698,6 +3011,25 @@ int flmr_workspace_create(const flmr_corpus_t* c, int max_queries, int max_nq,
     return bail(fail(FLMR_ERR_CUDA, "workspace allocation failed: %s", cudaGetErrorString(e)));
   ws->cand_lists = c->layout.n_ctas;
   *ws->h_status = 0;
+  if (c->streamed) {   // the window buffers (two, or one for a one-window plan; zeroed: rows a tile reads past its
+                       // window's end are finite), their tensor maps, the copy stream and its events
+    const size_t wbytes = static_cast<size_t>(c->window_rows) * kDim * 2;
+    const int n_bufs = c->windows.size() > 1 ? 2 : 1;
+    for (int i = 0; i < n_bufs; ++i) {
+      if ((e = cudaMalloc(reinterpret_cast<void**>(&ws->d_win[i]), wbytes)) != cudaSuccess ||
+          (e = cudaMemset(ws->d_win[i], 0, wbytes)) != cudaSuccess ||
+          (e = cudaEventCreateWithFlags(&ws->copied_ev[i], cudaEventDisableTiming)) != cudaSuccess ||
+          (e = cudaEventCreateWithFlags(&ws->scanned_ev[i], cudaEventDisableTiming)) != cudaSuccess)
+        return bail(fail(e == cudaErrorMemoryAllocation ? FLMR_ERR_OOM : FLMR_ERR_CUDA,
+                         "window buffers: %s", cudaGetErrorString(e)));
+      if (int rc = encode_rows_map(&ws->tmap_win[i], ws->d_win[i], static_cast<uint64_t>(c->window_rows), kTileN,
+                                   c->elem))
+        return bail(rc);
+    }
+    if ((e = cudaStreamCreateWithFlags(&ws->copy_stream, cudaStreamNonBlocking)) != cudaSuccess ||
+        (e = cudaEventCreateWithFlags(&ws->fork_ev, cudaEventDisableTiming)) != cudaSuccess)
+      return bail(fail(FLMR_ERR_CUDA, "copy stream: %s", cudaGetErrorString(e)));
+  }
   if (max_nq > kRbMax * 32) {   // row-sliced queries expected: size their partial-score rows now
     std::vector<PassPlan> plan;
     int group = 1;
@@ -2719,6 +3051,14 @@ int flmr_workspace_destroy(flmr_workspace_t* ws) {
   cudaFree(ws->d_acc);
   cudaFree(ws->d_plan);
   if (ws->h_status) cudaFreeHost(ws->h_status);
+  if (ws->copy_stream) cudaStreamSynchronize(ws->copy_stream);
+  for (int i = 0; i < 2; ++i) {
+    cudaFree(ws->d_win[i]);   // waits for the scans still reading it
+    if (ws->copied_ev[i]) cudaEventDestroy(ws->copied_ev[i]);
+    if (ws->scanned_ev[i]) cudaEventDestroy(ws->scanned_ev[i]);
+  }
+  if (ws->fork_ev) cudaEventDestroy(ws->fork_ev);
+  if (ws->copy_stream) cudaStreamDestroy(ws->copy_stream);
   delete ws;
   return FLMR_OK;
 }
@@ -2765,6 +3105,7 @@ int run_listed(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
                int k, const int64_t* h_off, const int64_t* d_pids, float* d_scores, float* d_topk_scores,
                int64_t* d_topk_pids, cudaStream_t st) {
   if (!c || !ws) return fail(FLMR_ERR_INVALID_ARG, "null corpus / workspace");
+  if (c->streamed) return fail(FLMR_ERR_UNSUPPORTED, "a streamed corpus has no listed scan; use the _allowed calls");
   if (n_queries < 0) return fail(FLMR_ERR_INVALID_ARG, "bad n_queries=%d", n_queries);
   if (!h_off) return fail(FLMR_ERR_INVALID_ARG, "h_list_offsets is null");
   if (h_off[0] < 0) return fail(FLMR_ERR_INVALID_ARG, "h_list_offsets[0] = %lld < 0", (long long)h_off[0]);
@@ -2810,6 +3151,7 @@ int flmr_debug_listed_plan(const flmr_corpus_t* c, flmr_workspace_t* ws, int n_q
   if (!c || !ws || !h_list_offsets || !n_out || n_queries < 1 || nq < 1)
     return fail(FLMR_ERR_INVALID_ARG, "bad argument");
   if (ws->corpus != c) return fail(FLMR_ERR_INVALID_ARG, "workspace belongs to a different corpus");
+  if (c->streamed) return fail(FLMR_ERR_UNSUPPORTED, "a streamed corpus has no listed scan");
   if (n_queries > ws->max_queries)
     return fail(FLMR_ERR_INVALID_ARG, "n_queries=%d > the workspace's max_queries=%d", n_queries, ws->max_queries);
   for (int b = 0; b < n_queries; ++b)
@@ -3343,6 +3685,55 @@ int flmr_debug_build_partition(const int32_t* h_doclens, int64_t n_passages, int
       return fail(FLMR_ERR_INVALID_ARG, "tile_capacity %lld < %zu tiles", (long long)tile_capacity, em.size());
     std::copy(em.begin(), em.end(), tile_end_mask);
     std::copy(fp.begin(), fp.end(), tile_first_pid);
+  }
+  return FLMR_OK;
+}
+
+int flmr_debug_window_plan(const int32_t* h_doclens, int64_t n_passages, int64_t window_bytes, int n_ctas,
+                           int64_t* out_windows, int64_t capacity, int64_t* n_windows_out, int32_t* cta_row_begin,
+                           int64_t* cta_tile_base, uint32_t* tile_end_mask, int32_t* tile_first_pid,
+                           int64_t tile_capacity, int64_t* n_tiles_out) {
+  if (!h_doclens || n_passages <= 0 || n_ctas < 1 || !n_windows_out) return fail(FLMR_ERR_INVALID_ARG, "bad argument");
+  if (window_bytes < kDim * 2) return fail(FLMR_ERR_INVALID_ARG, "window_bytes=%lld holds no row", (long long)window_bytes);
+  std::vector<int64_t> poff;
+  if (int rc = passage_offsets(h_doclens, n_passages, nullptr, &poff, nullptr)) return rc;
+  std::vector<std::pair<int64_t, int64_t>> ranges;
+  if (int rc = plan_windows(poff, window_bytes / (kDim * 2), &ranges)) return rc;
+  const int64_t nw = static_cast<int64_t>(ranges.size());
+  *n_windows_out = nw;
+  if (!out_windows) return FLMR_OK;
+  if (capacity < nw) return fail(FLMR_ERR_INVALID_ARG, "capacity %lld < %lld windows", (long long)capacity, (long long)nw);
+  std::vector<int32_t> all_rb, all_fp;
+  std::vector<int64_t> all_tb;
+  std::vector<uint32_t> all_em;
+  for (int64_t w = 0; w < nw; ++w) {
+    const int64_t s0 = ranges[w].first, s1 = ranges[w].second;
+    int nc = 0;
+    std::vector<int32_t> rb, fp;
+    std::vector<int64_t> tb;
+    std::vector<uint32_t> em;
+    window_partition(poff, s0, s1, n_ctas, &nc, &rb, &tb, &em, &fp);
+    int64_t* o = out_windows + 6 * w;
+    o[0] = s0;
+    o[1] = s1;
+    o[2] = poff[s0];
+    o[3] = poff[s1] - poff[s0];
+    o[4] = nc;
+    o[5] = static_cast<int64_t>(em.size());
+    all_rb.insert(all_rb.end(), rb.begin(), rb.end());
+    all_tb.insert(all_tb.end(), tb.begin(), tb.end());
+    all_em.insert(all_em.end(), em.begin(), em.end());
+    all_fp.insert(all_fp.end(), fp.begin(), fp.end());
+  }
+  if (n_tiles_out) *n_tiles_out = static_cast<int64_t>(all_em.size());
+  if (cta_row_begin && cta_tile_base && tile_end_mask && tile_first_pid) {
+    if (static_cast<int64_t>(all_em.size()) > tile_capacity || static_cast<int64_t>(all_rb.size()) > tile_capacity)
+      return fail(FLMR_ERR_INVALID_ARG, "tile_capacity %lld < %zu tiles or %zu CTA entries", (long long)tile_capacity,
+                  all_em.size(), all_rb.size());
+    std::copy(all_rb.begin(), all_rb.end(), cta_row_begin);
+    std::copy(all_tb.begin(), all_tb.end(), cta_tile_base);
+    std::copy(all_em.begin(), all_em.end(), tile_end_mask);
+    std::copy(all_fp.begin(), all_fp.end(), tile_first_pid);
   }
   return FLMR_OK;
 }

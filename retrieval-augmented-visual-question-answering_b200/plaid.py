@@ -60,11 +60,9 @@ def read_plaid_doclens(path: str, num_chunks: int):
     return out
 
 
-def plaid_to_flat(path: str, device=None, passage_range: Optional[Tuple[int, int]] = None,
-                  dtype: torch.dtype = torch.bfloat16) -> Tuple[torch.Tensor, np.ndarray]:
-    """Decode a PLAID index — all of it, or the passages ``[p0, p1)`` only (one GPU's shard: only the chunks
-    that overlap are read) — into (tokens ``[n_tokens, 128]`` of ``dtype``, bf16 or fp16, on the GPU, doclens
-    int32)."""
+def _plaid_pieces(path: str, device, passage_range: Optional[Tuple[int, int]]):
+    """What a decode of the passages ``[p0, p1)`` of a PLAID index reads: (device, metadata, centroids and bucket
+    weights on the device, pieces ``(chunk, first token row, one-past-last row, doclens slice, chunk rows)``)."""
     if not torch.cuda.is_available():
         raise RuntimeError("PLAID decode runs on the GPU; there is no CPU fallback")
     device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -79,6 +77,7 @@ def plaid_to_flat(path: str, device=None, passage_range: Optional[Tuple[int, int
     chunk_doclens = read_plaid_doclens(path, meta["num_chunks"])
     n_total = int(sum(len(d) for d in chunk_doclens))
     p0, p1 = (0, n_total) if passage_range is None else passage_range
+    p1 = n_total if p1 is None else p1
     if not 0 <= p0 <= p1 <= n_total:
         raise ValueError("passage_range %s outside [0, %d]" % (passage_range, n_total))
     pieces, c0 = [], 0                       # (chunk, first token row, one-past-last row, doclens slice)
@@ -88,14 +87,56 @@ def plaid_to_flat(path: str, device=None, passage_range: Optional[Tuple[int, int
             off = np.concatenate([[0], np.cumsum(dl)])
             pieces.append((c, int(off[a]), int(off[b]), dl[a:b], int(off[-1])))
         c0 += len(dl)
+    return device, meta, centroids, weights, pieces
+
+
+def _load_piece(path: str, c: int, n_chunk: int):
+    codes = torch.load(os.path.join(path, "%d.codes.pt" % c), map_location="cpu")
+    residuals = torch.load(os.path.join(path, "%d.residuals.pt" % c), map_location="cpu")
+    if codes.numel() != n_chunk:
+        raise ValueError("chunk %d holds %d codes but its doclens sum to %d" % (c, codes.numel(), n_chunk))
+    return codes, residuals
+
+
+def _piece_doclens(pieces) -> np.ndarray:
+    doclens = np.concatenate([p[3] for p in pieces]) if pieces else np.empty(0, dtype=np.int64)
+    return doclens.astype(np.int32)
+
+
+def plaid_to_flat(path: str, device=None, passage_range: Optional[Tuple[int, int]] = None,
+                  dtype: torch.dtype = torch.bfloat16) -> Tuple[torch.Tensor, np.ndarray]:
+    """Decode a PLAID index — all of it, or the passages ``[p0, p1)`` only (one GPU's shard: only the chunks
+    that overlap are read) — into (tokens ``[n_tokens, 128]`` of ``dtype``, bf16 or fp16, on the GPU, doclens
+    int32)."""
+    device, meta, centroids, weights, pieces = _plaid_pieces(path, device, passage_range)
     tokens = torch.empty((sum(p[2] - p[1] for p in pieces), _cabi.DIM), dtype=dtype, device=device)
     row = 0
     for c, r0, r1, _, n_chunk in pieces:
-        codes = torch.load(os.path.join(path, "%d.codes.pt" % c), map_location="cpu")
-        residuals = torch.load(os.path.join(path, "%d.residuals.pt" % c), map_location="cpu")
-        if codes.numel() != n_chunk:
-            raise ValueError("chunk %d holds %d codes but its doclens sum to %d" % (c, codes.numel(), n_chunk))
+        codes, residuals = _load_piece(path, c, n_chunk)
         decode_chunk(codes[r0:r1], residuals[r0:r1], centroids, weights, meta["nbits"], tokens[row:row + r1 - r0])
         row += r1 - r0
-    doclens = np.concatenate([p[3] for p in pieces]) if pieces else np.empty(0, dtype=np.int64)
-    return tokens, doclens.astype(np.int32)
+    return tokens, _piece_doclens(pieces)
+
+
+# token rows one decode step of plaid_to_host_chunks holds on the GPU (32 MiB of bf16 rows)
+HOST_DECODE_ROWS = 1 << 17
+
+
+def plaid_to_host_chunks(path: str, device=None, passage_range: Optional[Tuple[int, int]] = None,
+                         dtype: torch.dtype = torch.bfloat16, rows_per_step: int = HOST_DECODE_ROWS):
+    """The decode of ``plaid_to_flat`` for a corpus kept in host memory: (device, doclens int32, an iterator of host
+    token tensors ``[rows, 128]`` of ``dtype`` that concatenate to ``plaid_to_flat``'s tokens).  Each step decodes at
+    most ``rows_per_step`` rows on the GPU, with the same kernels, and copies them down; the GPU never holds more."""
+    device, meta, centroids, weights, pieces = _plaid_pieces(path, device, passage_range)
+
+    def steps():
+        buf = torch.empty((min(rows_per_step, max((p[2] - p[1] for p in pieces), default=1)), _cabi.DIM),
+                          dtype=dtype, device=device)
+        for c, r0, r1, _, n_chunk in pieces:
+            codes, residuals = _load_piece(path, c, n_chunk)
+            for a in range(r0, r1, rows_per_step):
+                b = min(r1, a + rows_per_step)
+                out = buf[:b - a]
+                decode_chunk(codes[a:b], residuals[a:b], centroids, weights, meta["nbits"], out)
+                yield out.cpu()
+    return device, _piece_doclens(pieces), steps()

@@ -23,6 +23,15 @@ query).  ``shard_across_ranks=True`` (an extension; needs an initialised ``torch
 only this rank's passage shard resident and merges the per-shard top-k with one all-gather, where the
 reference repeats the whole search on every rank (FLMR_executor.py:778-781).
 
+``residency="host"`` (with ``window_bytes``) opens an index path as a streamed corpus: pinned host memory, copied
+through two HBM windows per library call (``FlatCorpus``), for validation inside a training process, where the corpus
+does not fit beside the model and optimizer state.  Results are bitwise those of the corpus held in HBM.  Each library
+call copies the corpus once, so on a streamed corpus an unrestricted top-k search (k <= 128) hands the whole batch to
+one call, and searches with per-query score rows or bitmaps (``filter_fn``, k > 128, ``pids=`` / ``qid_to_pids=``)
+take as many queries per call as keep that scratch within ``STREAMED_SCRATCH_BYTES``.  ``residency`` and
+``window_bytes`` choose how an index path is loaded; with a ``FlatCorpus`` given, a ``residency`` other than its own
+and any ``window_bytes`` are refused.
+
 ``storage="fp8"`` keeps the corpus as e4m3 in HBM (half the bytes; the exact bf16 rows stay in pinned host memory)
 and searches in two stages, as PLAID does (colbert/search/index_storage.py:160-177): the exhaustive e4m3 scan
 shortlists ``ndocs / 4`` candidates per query (the reference's exact-scoring depth, filter_pids.cpp:148), which are
@@ -52,6 +61,12 @@ RERANK_GATHER_BYTES = 1 << 30
 # above it.  tools/listed_scan_probe.py brackets the crossover between 0.12 and 1.2 of this measure on an H100
 # (profiles/r09_listed_scan_probe.md).
 LISTED_SCAN_MAX_ROW_FRACTION = 0.5
+
+# A streamed corpus (residency="host") copies all of its rows over PCIe once per library call, so its searches hand the
+# library as many queries per call as they can: the fused top-k takes a whole batch (the library chunks it by the
+# workspace's max_queries inside its window loop), and calls whose per-query scratch grows with the shard (a score row,
+# an allow bitmap and the byte per passage it is built from) take as many queries as keep that scratch within this bound.
+STREAMED_SCRATCH_BYTES = 1 << 30
 
 
 def _default_knobs(k: int) -> Tuple[int, float, int]:
@@ -206,7 +221,7 @@ class Searcher:
                  disable_gpu: bool = True, device: Optional[Union[int, torch.device]] = None,
                  encode_fn: Optional[Callable] = None, index_root: Optional[str] = None,
                  query_batch: int = 64, shard_across_ranks: bool = False, group=None,
-                 storage: Optional[str] = None):
+                 storage: Optional[str] = None, residency: Optional[str] = None, window_bytes: Optional[int] = None):
         # `disable_gpu` is part of the reference signature (default True) but dead there: colbert/searcher.py:23
         # never reads it, the device is chosen by config.total_visible_gpus (:40-43), which FLMR_executor.py:778-781
         # zeroes under DDP to force CPU search.  Here the search always runs on the GPU (no CPU path exists);
@@ -224,6 +239,11 @@ class Searcher:
         if isinstance(index, FlatCorpus):
             if storage is not None and storage != index.storage:
                 raise ValueError("storage=%r, but the corpus given is stored as %r" % (storage, index.storage))
+            if residency is not None and residency != index.residency:
+                raise ValueError("residency=%r, but the corpus given has residency %r" % (residency, index.residency))
+            if window_bytes is not None:
+                raise ValueError("window_bytes applies to an index path opened with residency='host'; the corpus given "
+                                 "was created with its own")
             self.corpus = index
             self.index = None
             self.index_kind = "resident"
@@ -241,8 +261,17 @@ class Searcher:
             load = FlatCorpus.from_index if self.index_kind == "flat" else FlatCorpus.from_plaid
             # storage None: a flat index keeps its own dtype (fp16 for an "flmr-flat-f16" index), PLAID decodes to bf16
             extra = {"storage": storage} if storage is not None else {}
+            if window_bytes is not None and residency != "host":
+                raise ValueError("window_bytes=%r applies to residency='host' only" % (window_bytes,))
+            if residency is not None:   # "host": a streamed corpus (FlatCorpus residency="host")
+                extra["residency"] = residency
+                if window_bytes is not None:
+                    extra["window_bytes"] = window_bytes
             self.corpus = load(self.index, device=device, rank=rank, world_size=world, **extra)
         self.storage = getattr(self.corpus, "storage", None) or storage or "bf16"
+        # every rank of a sharded Searcher gets the same residency argument, so ranks without a shard batch their
+        # collectives as the others do
+        self.residency = getattr(self.corpus, "residency", None) or residency or "device"
         self._last_depth = None
         # searcher.py:35: checkpoint config < index config < (config + Run().config); kept for callers that
         # read searcher.config — none of its PLAID knobs influence the exhaustive scan.
@@ -345,6 +374,15 @@ class Searcher:
         order = torch.argsort((~live).to(torch.int8), dim=1, stable=True)[:, :max(n_live, 1)]
         return torch.gather(Q, 1, order.unsqueeze(-1).expand(-1, -1, Q.size(2)))
 
+    def _batch(self, scratch_bytes_per_query: int = 0) -> int:
+        """Queries per library call: ``query_batch``, or on a streamed corpus (one copy of its rows per call) as many
+        as keep per-query scratch of this size within STREAMED_SCRATCH_BYTES (no bound: every query in one call)."""
+        if self.residency != "host":
+            return self.query_batch
+        if scratch_bytes_per_query <= 0:
+            return 1 << 30
+        return max(self.query_batch, STREAMED_SCRATCH_BYTES // int(scratch_bytes_per_query))
+
     def _local_topk(self, Q: torch.Tensor, kk: int, keep: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
         """Top-``kk`` of this shard: (scores [B, kk'], global pids [B, kk']), kk' = min(kk, candidates)."""
         corpus = self.corpus
@@ -356,8 +394,9 @@ class Searcher:
         if keep is None and kk <= _cabi.MAX_K:
             kq = min(kk, _n_live(corpus))                # deleted passages are never offered to the fused top-k
             outs, outp = [], []
-            for b0 in range(0, Q.size(0), self.query_batch):
-                s, p = maxsim_topk(corpus, Q[b0:b0 + self.query_batch], kq, relu=self._relu)
+            step = self._batch()
+            for b0 in range(0, Q.size(0), step):
+                s, p = maxsim_topk(corpus, Q[b0:b0 + step], kq, relu=self._relu)
                 outs.append(s)
                 outp.append(p)
             return torch.cat(outs), torch.cat(outp)
@@ -369,8 +408,9 @@ class Searcher:
         if kq == 0:
             return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=corpus.device),
                     torch.empty((Q.size(0), 0), dtype=torch.int64, device=corpus.device))
-        for b0 in range(0, Q.size(0), self.query_batch):
-            s = maxsim_scores(corpus, Q[b0:b0 + self.query_batch], relu=self._relu)
+        step = self._batch(4 * corpus.n_passages)               # one fp32 score row per query
+        for b0 in range(0, Q.size(0), step):
+            s = maxsim_scores(corpus, Q[b0:b0 + step], relu=self._relu)
             if keep is not None:
                 s = s[:, keep]
             if kq <= _cabi.SELECT_MAX_K:
@@ -462,10 +502,13 @@ class Searcher:
         # the C-level sharded search (scan + exchange in one call) takes bf16 shards; the others exchange below
         c_level = self._nccl is not None and corpus is not None and self.storage != "fp8"
         parts = []
+        # per query: the allow bitmap, and the byte per passage allow_bitmaps builds it from; sized by the whole index,
+        # so that every rank of a sharded search (one without a shard included) makes the same calls and collectives
+        step = self._batch(self._index_size() * 9 // 8 + 1)
         if corpus is not None:
-            for b0 in range(0, B, self.query_batch):
-                Qb = Q[b0:b0 + self.query_batch]
-                lb = lists[b0:b0 + self.query_batch]
+            for b0 in range(0, B, step):
+                Qb = Q[b0:b0 + step]
+                lb = lists[b0:b0 + step]
                 if self._listed_is_cheaper(Qb, lb):
                     # the scan streams the listed passages' rows only; on the C-level sharded path the exchange that
                     # flmr_maxsim_topk_sharded_allowed would make follows, so every rank makes the same collectives
@@ -493,8 +536,7 @@ class Searcher:
             # one exchange per query batch, as the ranks on the C-level path make (a rank without a shard takes this
             # branch while the others may not)
             ex = self._nccl or self._sharded
-            merged = [ex.exchange(s[b0:b0 + self.query_batch], p[b0:b0 + self.query_batch], k)
-                      for b0 in range(0, B, self.query_batch)]
+            merged = [ex.exchange(s[b0:b0 + step], p[b0:b0 + step], k) for b0 in range(0, B, step)]
             s, p = torch.cat([m[0] for m in merged]), torch.cat([m[1] for m in merged])
         n_valid = int((p >= 0).sum(dim=1).max()) if p.numel() else 0
         return s[:, :n_valid], p[:, :n_valid]
@@ -505,6 +547,8 @@ class Searcher:
         shard's rows once per scan pass; a pass holds up to 12 queries of at most 32 tokens, fewer of longer ones)."""
         corpus = self.corpus
         if corpus is None or any(ids is None for ids in lists):
+            return False
+        if getattr(corpus, "residency", "device") == "host":   # a streamed corpus has no listed scan
             return False
         rbq = (Q.size(1) + 31) // 32
         per_pass = max(1, min(12, 12 // rbq)) if rbq <= 12 else 1
@@ -638,8 +682,9 @@ class Searcher:
         if self._nccl is not None and keep is None and corpus is not None and self.storage != "fp8":
             # the C-level sharded search: scan + one grouped all-gather + merge per call, no torch glue
             # (fp8 shards re-rank their shortlists first, then exchange exact scores below)
-            outs = [self._nccl.search(corpus, Q[b0:b0 + self.query_batch], int(k), relu=self._relu)
-                    for b0 in range(0, Q.size(0), self.query_batch)]
+            step = self._batch()
+            outs = [self._nccl.search(corpus, Q[b0:b0 + step], int(k), relu=self._relu)
+                    for b0 in range(0, Q.size(0), step)]
             s, p = torch.cat([o[0] for o in outs]), torch.cat([o[1] for o in outs])
             n_valid = int((p[0] >= 0).sum()) if p.numel() else 0
             return s[:, :n_valid], p[:, :n_valid]
@@ -725,7 +770,7 @@ class Searcher:
     def _search_all_Q(self, queries, Q: torch.Tensor, k: int, filter_fn=None, progress: bool = True,
                       remove_zero_tensors: bool = False, qid_to_pids=None) -> Ranking:
         """searcher.py:73-89, batched: one fused scan per ``query_batch`` queries instead of a Python
-        loop of per-query ``dense_search`` calls.
+        loop of per-query ``dense_search`` calls (on a streamed corpus: one per call, see the module docstring).
 
         ``qid_to_pids`` (later ColBERT's argument) maps every qid to the global ids its query may return (None: the
         whole index); a qid missing from it raises KeyError.  Queries may then return fewer than k hits."""
