@@ -250,17 +250,9 @@ class FlatCorpus:
             if dead.size:
                 self.delete(dead)
             return self
-        L = _cabi.lib()
         t0 = time.perf_counter()
-        b = C.c_void_p()
-        if residency == "host":
-            _cabi.check(L.flmr_corpus_builder_create_streamed(doclens.ctypes.data_as(C.c_void_p), len(doclens),
-                                                              _cabi.DIM, int(device.index), int(p0), flags,
-                                                              int(window_bytes), C.byref(b)))
-        else:
-            _cabi.check(L.flmr_corpus_builder_create_ex(doclens.ctypes.data_as(C.c_void_p), len(doclens), _cabi.DIM,
-                                                        int(device.index), int(p0), flags, C.byref(b)))
-        try:
+
+        def feed(L, b):
             for fname, f0, fn, _rows in files:
                 a, e = max(p0, f0), min(p1, f0 + fn)
                 if a >= e:
@@ -268,19 +260,14 @@ class FlatCorpus:
                 row_a = int(all_doclens[f0:a].sum())
                 rows = int(all_doclens[a:e].sum())
                 _cabi.check(L.flmr_corpus_builder_append_file(b, fname.encode(), row_a * _cabi.DIM * 2, rows))
-            handle, fill_s = C.c_void_p(), C.c_double(0)
-            _cabi.check(L.flmr_corpus_builder_finish(b, C.byref(handle), C.byref(fill_s)))
-            b = None
-        finally:
-            if b is not None:
-                L.flmr_corpus_builder_destroy(b)
-        self = cls._from_handle(handle, doclens, device, p0)
+
+        self, fill_s = cls._build(doclens, device, p0, flags, residency, window_bytes, feed)
         dead = deleted_in_range(read_deleted(path), p0, p1)    # this shard's share of the index's deletions
         if dead.size:
             self.delete(dead)
         dt = time.perf_counter() - t0
         gb = float(doclens.sum()) * _cabi.DIM * 2 / 1e9
-        self.load_stats = {"seconds": dt, "gigabytes": gb, "gb_per_s": gb / dt, "host_fill_seconds": fill_s.value,
+        self.load_stats = {"seconds": dt, "gigabytes": gb, "gb_per_s": gb / dt, "host_fill_seconds": fill_s,
                            "rank": rank, "world_size": world_size}
         return self
 
@@ -305,9 +292,15 @@ class FlatCorpus:
                 p0, p1 = shard_ranges(all_doclens, world_size)[rank]
                 if p0 == p1:
                     return None
-            return cls._streamed_from_chunks(plaid_to_host_chunks(path, device, passage_range=(p0, p1),
-                                                                  dtype=element_dtype(storage)),
-                                             device, p0, storage, window_bytes)
+            device, doclens, pieces = plaid_to_host_chunks(path, device, passage_range=(p0, p1),
+                                                           dtype=element_dtype(storage))
+
+            def feed(L, b):
+                for t in pieces:
+                    _cabi.check(L.flmr_corpus_builder_append(b, C.c_void_p(t.data_ptr()), t.size(0)))
+
+            return cls._build(np.ascontiguousarray(doclens, dtype=np.int32), device, p0, _storage_flag(storage),
+                              residency, window_bytes, feed)[0]
         if world_size == 1:
             tokens, doclens = plaid_to_flat(path, device, dtype=element_dtype(storage))
             return cls(tokens, doclens, device=tokens.device, storage=storage)
@@ -319,26 +312,28 @@ class FlatCorpus:
         return cls(tokens, doclens, device=tokens.device, pid_base=p0, storage=storage)
 
     @classmethod
-    def _streamed_from_chunks(cls, chunks, device, pid_base: int, storage: str, window_bytes: int) -> "FlatCorpus":
-        """A streamed corpus built from ``chunks = (device, doclens, iterator of host token tensors in order)``
-        through the C-level builder, which copies each chunk into the pinned host matrix."""
-        device, doclens, pieces = chunks
-        doclens = np.ascontiguousarray(doclens, dtype=np.int32)
+    def _build(cls, doclens: np.ndarray, device: torch.device, pid_base: int, flags: int, residency: str,
+               window_bytes: int, feed) -> tuple:
+        """A corpus of ``doclens`` (int32) built through the C-level builder of ``residency``: ``feed(L, builder)``
+        appends every packed row in order (``L``: the library).  Returns the corpus and the host fill seconds."""
         L = _cabi.lib()
         b = C.c_void_p()
-        _cabi.check(L.flmr_corpus_builder_create_streamed(doclens.ctypes.data_as(C.c_void_p), len(doclens), _cabi.DIM,
-                                                          int(device.index), int(pid_base), _storage_flag(storage),
-                                                          int(window_bytes), C.byref(b)))
+        if residency == "host":
+            _cabi.check(L.flmr_corpus_builder_create_streamed(doclens.ctypes.data_as(C.c_void_p), len(doclens),
+                                                              _cabi.DIM, int(device.index), int(pid_base), flags,
+                                                              int(window_bytes), C.byref(b)))
+        else:
+            _cabi.check(L.flmr_corpus_builder_create_ex(doclens.ctypes.data_as(C.c_void_p), len(doclens), _cabi.DIM,
+                                                        int(device.index), int(pid_base), flags, C.byref(b)))
         try:
-            for t in pieces:
-                _cabi.check(L.flmr_corpus_builder_append(b, C.c_void_p(t.data_ptr()), t.size(0)))
-            handle = C.c_void_p()
-            _cabi.check(L.flmr_corpus_builder_finish(b, C.byref(handle), None))
+            feed(L, b)
+            handle, fill_s = C.c_void_p(), C.c_double(0)
+            _cabi.check(L.flmr_corpus_builder_finish(b, C.byref(handle), C.byref(fill_s)))
             b = None
         finally:
             if b is not None:
                 L.flmr_corpus_builder_destroy(b)
-        return cls._from_handle(handle, doclens, device, pid_base)
+        return cls._from_handle(handle, doclens, device, pid_base), fill_s.value
 
     # -- properties ---------------------------------------------------------------------------
     @property

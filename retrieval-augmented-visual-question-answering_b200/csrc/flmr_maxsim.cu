@@ -1044,6 +1044,16 @@ struct Partition {
   int32_t* first_pid = nullptr;   // [n_tiles]
 };
 
+// One window of a corpus: the slots [slot0, slot1), stored rows [row0, row0 + rows), scanned from a buffer that holds
+// exactly those rows from its row 0 (a resident corpus: its one window, the token matrix).  Its partition's row starts
+// are relative to the window; its tiles' first slots are absolute, so candidate keys, tombstones, allow bitmaps and
+// score rows are indexed alike in every window.
+struct Window {
+  int64_t slot0 = 0, slot1 = 0, row0 = 0, rows = 0;
+  int n_ctas = 0;                      // min(SMs, slots of the window)
+  Partition cta;
+};
+
 // Everything build_layout derives from the stored passages' (the slots') offsets: what the scan, the SIMT kernel and
 // the gather read.  An append or a compaction builds a new one and swaps it in whole (free_layout frees one).
 struct SlotLayout {
@@ -1052,25 +1062,16 @@ struct SlotLayout {
   int64_t* d_poff = nullptr;           // device copies of the two above
   int32_t* d_doclen = nullptr;
   int64_t max_rows = 0;                // stored rows of the longest slot (bounds a listed search's plan)
-  int n_ctas = 0;                      // min(sm_total, slots)
-  Partition cta;
+  int n_ctas = 0;                      // the most CTAs a window launches (sizes a workspace's candidate lists)
+  std::vector<Window> windows;         // a resident corpus has one, over every slot
+  int64_t window_rows = 0;             // rows of the largest window (a streamed corpus's window buffers hold this many)
+  // resident corpus only: the token matrix's tensor map, and the CTA-pair experiment (flmr_debug_set_scan_variant(4),
+  // bf16 only): n_pairs ranges, and a tensor map with a half-tile box
   CUtensorMap tmap_d;
-  // CTA-pair experiment (flmr_debug_set_scan_variant(4), bf16 only): n_pairs ranges, and a tensor map with a
-  // half-tile box
   int n_pairs = 0;
   Partition pair;
   CUtensorMap tmap_half;
   int64_t bytes = 0;                   // HBM the device arrays above take
-};
-
-// One window of a streamed corpus: the slots [slot0, slot1), stored rows [row0, row0 + rows), scanned from a window
-// buffer that holds exactly those rows from its row 0.  Its partition's row starts are relative to the window; its
-// tiles' first slots are absolute, so candidate keys, tombstones, allow bitmaps and score rows are indexed as in a
-// resident corpus.
-struct Window {
-  int64_t slot0 = 0, slot1 = 0, row0 = 0, rows = 0;
-  int n_ctas = 0;                      // min(SMs, slots of the window)
-  Partition cta;
 };
 
 }  // namespace
@@ -1106,13 +1107,10 @@ struct flmr_corpus {
   int sm_total = 0;                    // SMs of the device
   // A streamed corpus (flmr_corpus_create_streamed): the padded rows live in h_stream (pinned, mapped; d_tokens is its
   // device alias, which the gather and the SIMT kernel read) and searches copy them window by window into the
-  // workspace's two window buffers.  layout holds the offsets and lengths, but no partition and no tensor map.
+  // workspace's two window buffers.  Its layout has no tensor map of the matrix and no CTA-pair partition.
   bool streamed = false;
   void* h_stream = nullptr;
   int64_t window_bytes = 0;            // as requested at creation
-  int64_t window_rows = 0;             // rows of the largest window (each window buffer holds this many)
-  std::vector<Window> windows;
-  int64_t windows_bytes = 0;           // HBM of the windows' partitions
 };
 
 // Streaming corpus construction (index load): the padded token matrix is allocated once, packed rows arrive in
@@ -1248,11 +1246,11 @@ int64_t hbm_row_bytes(Elem elem) { return elem == Elem::kE4M3 ? kDim : kDim * 2;
 
 const char* elem_name(Elem elem) { return elem == Elem::kE4M3 ? "e4m3" : elem == Elem::kF16 ? "fp16" : "bf16"; }
 
-// HBM a corpus holds: its matrix (an adopted one is the caller's, a streamed one is host memory), its layout, the
-// partitions of its windows, its tombstones by slot and its slot -> id map.
+// HBM a corpus holds: its matrix (an adopted one is the caller's, a streamed one is host memory), its layout, its
+// tombstones by slot and its slot -> id map.
 int64_t hbm_bytes(const flmr_corpus* c) {
   const int64_t ns = slots(c);
-  return (c->adopted || c->streamed ? 0 : c->n_rows * hbm_row_bytes(c->elem)) + c->layout.bytes + c->windows_bytes +
+  return (c->adopted || c->streamed ? 0 : c->n_rows * hbm_row_bytes(c->elem)) + c->layout.bytes +
          (c->d_dead ? (ns + 31) / 32 * 4 : 0) + (c->d_slot_pid ? ns * 8 : 0);
 }
 
@@ -1421,7 +1419,7 @@ void build_partition(const std::vector<int64_t>& poff, int n_ctas, int tile_n,
   }
 }
 
-// ---- window planning of a streamed corpus (pure host logic; exported for tests as flmr_debug_window_plan) ----------
+// ---- window planning (pure host logic; exported for tests as flmr_debug_window_plan) ------------------------------
 // The slots cut into contiguous ranges, each taking as many slots as fit window_rows stored rows (poff: stored-row
 // offsets of the slots).  *out receives (first slot, end slot) pairs.  A slot longer than a window cannot be scanned
 // from one: FLMR_ERR_UNSUPPORTED.
@@ -1583,21 +1581,22 @@ ScanKernel pick_scan(Elem elem, bool listed, int variant, int blocks) {
   return {t.two, 2};
 }
 
-// One scan pass.  pair: a CTA-pair pass (planned only under variant 4).  listed: p holds a listed search's plan
-// (run_search's ListedArgs).  win (a streamed corpus): the pass scans that window from the buffer win_map describes.
-int launch_scan(const flmr_corpus* c, ScanParams p, bool pair, bool listed, cudaStream_t st,
-                const Window* win = nullptr, const CUtensorMap* win_map = nullptr) {
+// One scan pass over window `win`, whose rows the tensor map `rows` describes.  pair: a CTA-pair pass (planned only
+// under variant 4), which scans the resident matrix through the layout's pair partition and half-tile map instead.
+// listed: p holds a listed search's plan (run_search's ListedArgs).
+int launch_scan(const flmr_corpus* c, ScanParams p, bool pair, bool listed, const Window& win, const CUtensorMap& rows,
+                cudaStream_t st) {
   const SlotLayout& l = c->layout;
   // the passes variant 4 leaves to single CTAs run the two-warpgroup kernel
   const int variant = g_scan_variant == 4 && !pair ? 2 : g_scan_variant;
   const ScanKernel k = pick_scan(c->elem, listed, variant, scan_blocks(p.nq_pass, p.rbq));
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(win ? win->n_ctas : pair ? 2 * l.n_pairs : l.n_ctas));
+  cfg.gridDim = dim3(static_cast<unsigned>(pair ? 2 * l.n_pairs : win.n_ctas));
   cfg.blockDim = dim3(scan_threads(k.wgs));
   cfg.dynamicSmemBytes = ScanSmem::kBytes;
   cfg.stream = st;
   if (!listed) {   // a listed pass brings its plan's tiles
-    const Partition& part = win ? win->cta : pair ? l.pair : l.cta;
+    const Partition& part = pair ? l.pair : win.cta;
     p.cta_row_begin = part.row_begin;
     p.cta_tile_base = part.tile_base;
     p.tile_end_mask = part.end_mask;
@@ -1611,7 +1610,7 @@ int launch_scan(const flmr_corpus* c, ScanParams p, bool pair, bool listed, cuda
     cfg.attrs = &cluster;
     cfg.numAttrs = 1;
   }
-  void* args[] = {const_cast<CUtensorMap*>(win ? win_map : pair ? &l.tmap_half : &l.tmap_d), &p};
+  void* args[] = {const_cast<CUtensorMap*>(pair ? &l.tmap_half : &rows), &p};
   EventPair ev{};
   if (g_profiling) {
     FLMR_CUDA(cudaEventCreate(&ev.a));
@@ -1845,15 +1844,15 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   // within a chunk: every pass's scan, then the merge over the chunk's queries (one launch per kind of pass)
   std::vector<PassPlan> plan;
   std::vector<int> slot;
-  // A streamed corpus is scanned window by window, each window once per call: the windows are the outer loop, the call
-  // chunks the inner one, and each chunk's top-k rows carry the running top-k from window to window (the merge of a
-  // window's per-CTA lists takes the rows as one more list).  Window w is copied into buffer w & 1 on the workspace's
-  // copy stream; its scans wait for that copy, and the copy of window w + 2 into the same buffer waits for them.  The
-  // copy stream first waits for the call's stream, and every copy is waited for by a scan on it, so the call is
-  // ordered on `st` like any other.
-  const int n_windows = c->streamed ? static_cast<int>(c->windows.size()) : 1;
+  // The corpus is scanned window by window, each window once per call (a resident corpus has one): the windows are
+  // the outer loop, the call chunks the inner one, and each chunk's top-k rows carry the running top-k from window to
+  // window (the merge of a window's per-CTA lists takes the rows as one more list).  A streamed corpus's window w is
+  // copied into buffer w & 1 on the workspace's copy stream; its scans wait for that copy, and the copy of window
+  // w + 2 into the same buffer waits for them.  The copy stream first waits for the call's stream, and every copy is
+  // waited for by a scan on it, so the call is ordered on `st` like any other.
+  const int n_windows = static_cast<int>(l.windows.size());
   auto copy_window = [&](int w) -> int {
-    const Window& win = c->windows[w];
+    const Window& win = l.windows[w];
     const int b = w & 1;
     if (w >= 2) FLMR_CUDA(cudaStreamWaitEvent(ws->copy_stream, ws->scanned_ev[b], 0));
     FLMR_CUDA(cudaMemcpyAsync(ws->d_win[b], static_cast<const char*>(c->h_stream) + win.row0 * kDim * 2,
@@ -1869,10 +1868,9 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
       if ((rc = copy_window(w))) return rc;
   }
   for (int w = 0; w < n_windows; ++w) {
-    const Window* win = c->streamed ? &c->windows[w] : nullptr;
-    const CUtensorMap* win_map = win ? &ws->tmap_win[w & 1] : nullptr;
-    const int n_lists = win ? win->n_ctas : l.n_ctas;
-    if (win) FLMR_CUDA(cudaStreamWaitEvent(st, ws->copied_ev[w & 1], 0));
+    const Window& win = l.windows[w];
+    const CUtensorMap& rows = c->streamed ? ws->tmap_win[w & 1] : l.tmap_d;
+    if (c->streamed) FLMR_CUDA(cudaStreamWaitEvent(st, ws->copied_ev[w & 1], 0));
     for (int c0 = 0; c0 < n_queries; c0 += ws->max_queries) {
       const int nqc = std::min(ws->max_queries, n_queries - c0);
       const __nv_bfloat16* d_qc = static_cast<const __nv_bfloat16*>(d_q) + static_cast<int64_t>(c0) * nq * kDim;
@@ -1929,7 +1927,7 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
           p.allow = lp.allow + static_cast<int64_t>(pp.q_first) * lp.words;
           p.allow_stride = lp.words;
         }
-        if ((rc = launch_scan(c, p, (pp.flags & kPassPair) != 0, listed != nullptr, st, win, win_map))) return rc;
+        if ((rc = launch_scan(c, p, (pp.flags & kPassPair) != 0, listed != nullptr, win, rows, st))) return rc;
       }
       if (listed && d_slot_scores) {
         const int64_t n = listed->h_off[c0 + nqc] - listed->h_off[c0];
@@ -1953,10 +1951,11 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
         int64_t* op = d_topk_pids + static_cast<int64_t>(c0) * k;
         // queries of pair passes have one candidate list per CTA PAIR, the others one per CTA
         if ((rc = launch_merge_keys(c, ws, l.n_pairs, nqc, 0, n_pair_q, k, os, op, st))) return rc;
-        if ((rc = launch_merge_keys(c, ws, n_lists, nqc, n_pair_q, nqc - n_pair_q, k, os, op, st, w > 0))) return rc;
+        if ((rc = launch_merge_keys(c, ws, win.n_ctas, nqc, n_pair_q, nqc - n_pair_q, k, os, op, st, w > 0)))
+          return rc;
       }
     }
-    if (win) {
+    if (c->streamed) {
       FLMR_CUDA(cudaEventRecord(ws->scanned_ev[w & 1], st));
       if (w + 2 < n_windows && (rc = copy_window(w + 2))) return rc;
     }
@@ -1967,20 +1966,24 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
 void free_layout(SlotLayout* l) {
   cudaFree(l->d_poff);
   cudaFree(l->d_doclen);
-  for (const Partition& q : {l->cta, l->pair})
+  auto free_partition = [](const Partition& q) {
     for (void* p : {static_cast<void*>(q.row_begin), static_cast<void*>(q.tile_base), static_cast<void*>(q.end_mask),
                     static_cast<void*>(q.first_pid)})
       cudaFree(p);
+  };
+  for (const Window& w : l->windows) free_partition(w.cta);
+  free_partition(l->pair);
   *l = SlotLayout();
 }
 
-// The layout of a corpus of storage `elem` whose stored passages (the slots: all of them until a compaction) have row
-// offsets poff and lengths lens, over the token matrix d_tokens (and the e4m3 copy d_fp8 of an e4m3 corpus) of n_rows
-// rows, into the empty layout *l.  On failure nothing stays allocated.
-int build_layout(Elem elem, const __nv_bfloat16* d_tokens, const uint8_t* d_fp8, int64_t n_rows,
-                 const std::vector<int64_t>& poff, const int32_t* lens, int sm_total, SlotLayout* l) {
+// The layout of corpus c whose stored passages (the slots: all of them until a compaction) have row offsets poff and
+// lengths lens, over the token matrix d_tokens of n_rows rows (and c's e4m3 copy d_fp8 of an e4m3 corpus), into the
+// empty layout *l.  A streamed corpus's windows hold c->window_bytes each; a resident corpus is one window of every
+// slot, scanned straight from the matrix.  On failure nothing stays allocated.
+int build_layout(const flmr_corpus* c, const __nv_bfloat16* d_tokens, int64_t n_rows, const std::vector<int64_t>& poff,
+                 const int32_t* lens, SlotLayout* l) {
   // per-device function attributes of the storage's scan kernels (idempotent), set here rather than at launch time
-  for (const ScanKernels& t : kScanKernels[static_cast<int>(elem)])
+  for (const ScanKernels& t : kScanKernels[static_cast<int>(c->elem)])
     for (ScanFn fn : {t.two, t.three, t.split, t.pair}) {
       const cudaError_t e =
           fn ? cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes) : cudaSuccess;
@@ -1988,88 +1991,88 @@ int build_layout(Elem elem, const __nv_bfloat16* d_tokens, const uint8_t* d_fp8,
         return fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s", ScanSmem::kBytes,
                     cudaGetErrorString(e));
     }
+  std::vector<std::pair<int64_t, int64_t>> ranges;
+  if (int rc = plan_windows(poff, c->streamed ? c->window_bytes / (kDim * 2) : n_rows, &ranges)) return rc;
   const int64_t ns = static_cast<int64_t>(poff.size()) - 1;
   l->h_poff = poff;
   l->h_doclen.assign(lens, lens + ns);
   for (int64_t s = 0; s < ns; ++s) l->max_rows = std::max(l->max_rows, poff[s + 1] - poff[s]);
-  int n_ctas = sm_total;
+  int max_ctas = c->sm_total;
 #ifdef FLMR_DEBUG
-  if (const char* e = getenv("FLMR_NUM_CTAS")) n_ctas = std::max(1, atoi(e));
+  if (const char* e = getenv("FLMR_NUM_CTAS")) max_ctas = std::max(1, atoi(e));
 #endif
-  l->n_ctas = static_cast<int>(std::min<int64_t>(n_ctas, ns));
-  auto partition = [&](int n, Partition* q) {   // the slots split into n ranges, uploaded
-    std::vector<int32_t> rb, fp;
-    std::vector<int64_t> tb;
-    std::vector<uint32_t> em;
-    build_partition(poff, n, kTileN, &rb, &tb, &em, &fp);
+  // a partition's arrays, uploaded into *q
+  auto upload = [&](const std::vector<int32_t>& rb, const std::vector<int64_t>& tb, const std::vector<uint32_t>& em,
+                    const std::vector<int32_t>& fp, Partition* q) {
     q->n_tiles = static_cast<int64_t>(em.size());
     int rc = dev_upload(&q->row_begin, rb, &l->bytes);
     if (!rc) rc = dev_upload(&q->tile_base, tb, &l->bytes);
     if (!rc) rc = dev_upload(&q->end_mask, em, &l->bytes);
     return rc ? rc : dev_upload(&q->first_pid, fp, &l->bytes);
   };
+  std::vector<int32_t> rb, fp;
+  std::vector<int64_t> tb;
+  std::vector<uint32_t> em;
   int rc = dev_upload(&l->d_poff, l->h_poff, &l->bytes);
   if (!rc) rc = dev_upload(&l->d_doclen, l->h_doclen, &l->bytes);
-  if (!rc) rc = partition(l->n_ctas, &l->cta);
-  if (!rc)
-    rc = encode_rows_map(&l->tmap_d, elem == Elem::kE4M3 ? static_cast<const void*>(d_fp8) : d_tokens,
-                         static_cast<uint64_t>(n_rows), kTileN, elem);
+  l->windows.resize(ranges.size());
+  for (size_t w = 0; w < ranges.size() && !rc; ++w) {
+    Window& win = l->windows[w];
+    win.slot0 = ranges[w].first;
+    win.slot1 = ranges[w].second;
+    win.row0 = poff[win.slot0];
+    win.rows = poff[win.slot1] - win.row0;
+    l->window_rows = std::max(l->window_rows, win.rows);
+    window_partition(poff, win.slot0, win.slot1, max_ctas, &win.n_ctas, &rb, &tb, &em, &fp);
+    l->n_ctas = std::max(l->n_ctas, win.n_ctas);
+    rc = upload(rb, tb, em, fp, &win.cta);
+  }
+  if (!rc && !c->streamed)
+    rc = encode_rows_map(&l->tmap_d, c->elem == Elem::kE4M3 ? static_cast<const void*>(c->d_fp8) : d_tokens,
+                         static_cast<uint64_t>(n_rows), kTileN, c->elem);
   // CTA-pair passes: their own partition + half-tile tensor map.  The product never plans pair passes (see
   // run_search); these few KB per corpus are built so flmr_debug_set_scan_variant(4) can hold the cluster kernel
-  // against the single-CTA kernels on any bf16 corpus.
-  if (!rc && elem == Elem::kBF16 && l->n_ctas >= 2) {
+  // against the single-CTA kernels on any resident bf16 corpus.
+  if (!rc && !c->streamed && c->elem == Elem::kBF16 && l->n_ctas >= 2) {
     l->n_pairs = l->n_ctas / 2;
-    rc = partition(l->n_pairs, &l->pair);
+    build_partition(poff, l->n_pairs, kTileN, &rb, &tb, &em, &fp);
+    rc = upload(rb, tb, em, fp, &l->pair);
     if (!rc) rc = encode_rows_map(&l->tmap_half, d_tokens, static_cast<uint64_t>(n_rows), kTileN / 2);
   }
   if (rc) free_layout(l);
   return rc;
 }
 
-// The layout of a streamed corpus from its slots' offsets and lengths: the offsets and lengths on the device (for the
-// gather and the SIMT kernel), and the windows of c->window_bytes with their partitions.  layout.n_ctas is the most
-// CTAs a window launches (it sizes a workspace's candidate lists), layout.cta.n_tiles the tiles of all windows.
-int build_streamed_layout(flmr_corpus* c, const std::vector<int64_t>& poff, const int32_t* lens) {
-  SlotLayout* l = &c->layout;
-  const int64_t ns = static_cast<int64_t>(poff.size()) - 1;
+// The packed (*soff) and stored (*poff) row offsets of a new corpus's passages (*aligned: as passage_offsets), refused
+// when a corpus cannot hold them: a zero-length passage, 2^31 stored rows, or (window_bytes > 0: a streamed corpus) a
+// passage longer than a window.
+int corpus_offsets(const int32_t* h_doclens, int64_t n_passages, int64_t window_bytes, std::vector<int64_t>* soff,
+                   std::vector<int64_t>* poff, bool* aligned) {
+  if (int rc = passage_offsets(h_doclens, n_passages, soff, poff, aligned)) return rc;
+  const int64_t n_rows = (*poff)[n_passages];
+  if (n_rows + kTileN >= (1ll << 31))
+    return fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
+                (long long)n_rows);
   std::vector<std::pair<int64_t, int64_t>> ranges;
-  if (int rc = plan_windows(poff, c->window_bytes / (kDim * 2), &ranges)) return rc;
-  l->h_poff = poff;
-  l->h_doclen.assign(lens, lens + ns);
-  for (int64_t s = 0; s < ns; ++s) l->max_rows = std::max(l->max_rows, poff[s + 1] - poff[s]);
-  int rc = dev_upload(&l->d_poff, l->h_poff, &l->bytes);
-  if (!rc) rc = dev_upload(&l->d_doclen, l->h_doclen, &l->bytes);
-  c->windows.resize(ranges.size());
-  for (size_t w = 0; w < ranges.size() && !rc; ++w) {
-    Window& win = c->windows[w];
-    win.slot0 = ranges[w].first;
-    win.slot1 = ranges[w].second;
-    win.row0 = poff[win.slot0];
-    win.rows = poff[win.slot1] - win.row0;
-    c->window_rows = std::max(c->window_rows, win.rows);
-    std::vector<int32_t> rb, fp;
-    std::vector<int64_t> tb;
-    std::vector<uint32_t> em;
-    window_partition(poff, win.slot0, win.slot1, c->sm_total, &win.n_ctas, &rb, &tb, &em, &fp);
-    win.cta.n_tiles = static_cast<int64_t>(em.size());
-    l->n_ctas = std::max(l->n_ctas, win.n_ctas);
-    l->cta.n_tiles += win.cta.n_tiles;
-    rc = dev_upload(&win.cta.row_begin, rb, &c->windows_bytes);
-    if (!rc) rc = dev_upload(&win.cta.tile_base, tb, &c->windows_bytes);
-    if (!rc) rc = dev_upload(&win.cta.end_mask, em, &c->windows_bytes);
-    if (!rc) rc = dev_upload(&win.cta.first_pid, fp, &c->windows_bytes);
-  }
-  // the scan kernels' shared-memory limit, which build_layout sets for a resident corpus
-  for (const ScanKernels& t : kScanKernels[static_cast<int>(c->elem)])
-    for (ScanFn fn : {t.two, t.three, t.split, t.pair}) {
-      const cudaError_t e =
-          fn && !rc ? cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ScanSmem::kBytes)
-                    : cudaSuccess;
-      if (e != cudaSuccess)
-        rc = fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit to %d bytes: %s", ScanSmem::kBytes,
-                  cudaGetErrorString(e));
-    }
-  return rc;
+  return window_bytes > 0 ? plan_windows(*poff, window_bytes / (kDim * 2), &ranges) : FLMR_OK;
+}
+
+// A new corpus handle, with no matrix and no layout yet: streamed when window_bytes > 0.
+int new_corpus(int device, int64_t n_passages, const std::vector<int64_t>& soff, const std::vector<int64_t>& poff,
+               int64_t pid_base, Elem elem, int sm_total, int64_t window_bytes, flmr_corpus** out) {
+  flmr_corpus* c = new (std::nothrow) flmr_corpus();
+  if (!c) return fail(FLMR_ERR_OOM, "host allocation failed");
+  c->device = device;
+  c->n_passages = n_passages;
+  c->n_tokens = soff[n_passages];
+  c->n_rows = poff[n_passages];
+  c->pid_base = pid_base;
+  c->elem = elem;
+  c->sm_total = sm_total;
+  c->streamed = window_bytes > 0;
+  c->window_bytes = window_bytes;
+  *out = c;
+  return FLMR_OK;
 }
 
 // The pinned, mapped host matrix of a new streamed corpus (n_rows set); d_tokens becomes its device alias.
@@ -2277,23 +2280,29 @@ extern "C" {
 const char* flmr_last_error(void) { return g_last_error.c_str(); }
 int flmr_abi_version(void) { return FLMR_ABI_VERSION; }
 
-int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_passages, int dim,
-                       int device, int64_t pid_base, unsigned flags, flmr_corpus_t** out) {
+extern "C++" {
+namespace {
+// flmr_corpus_create (window_bytes 0) and flmr_corpus_create_streamed (window_bytes as the caller passed it: a streamed
+// call's window of no bytes is refused in its place among the checks, not taken for a resident corpus).
+int corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                  int64_t pid_base, unsigned flags, bool streamed, int64_t window_bytes, flmr_corpus_t** out) {
   if (!out) return fail(FLMR_ERR_INVALID_ARG, "out is null");
   *out = nullptr;
+  if (streamed && (flags & ~FLMR_CORPUS_FP16))
+    return fail(FLMR_ERR_UNSUPPORTED, "flags 0x%x: a streamed corpus is bf16 or FLMR_CORPUS_FP16, and is never adopted",
+                flags);
   if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
   if (n_passages <= 0 || !tokens || !h_doclens)
     return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null tokens/doclens");
+  if (streamed && window_bytes < kDim * 2)
+    return fail(FLMR_ERR_INVALID_ARG, "window_bytes=%lld holds no row", (long long)window_bytes);
   Elem elem;
   std::vector<int64_t> soff, poff;
   bool aligned;
   int rc;
-  if ((rc = storage_from_flags(flags, &elem)) || (rc = passage_offsets(h_doclens, n_passages, &soff, &poff, &aligned)))
+  if ((rc = storage_from_flags(flags, &elem)) ||
+      (rc = corpus_offsets(h_doclens, n_passages, window_bytes, &soff, &poff, &aligned)))   // before any allocation
     return rc;
-  const int64_t n_rows = poff[n_passages];
-  if (n_rows + kTileN >= (1ll << 31))
-    return fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
-                (long long)n_rows);
 
   DeviceGuard guard(device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
@@ -2303,93 +2312,48 @@ int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_p
   if ((flags & FLMR_CORPUS_ADOPT) && !is_device_ptr)
     return fail(FLMR_ERR_INVALID_ARG, "FLMR_CORPUS_ADOPT requires a device pointer");
 
-  flmr_corpus* c = new (std::nothrow) flmr_corpus();
-  if (!c) return fail(FLMR_ERR_OOM, "host allocation failed");
-  c->device = device;
-  c->n_passages = n_passages;
-  c->n_tokens = soff[n_passages];
-  c->n_rows = n_rows;
-  c->pid_base = pid_base;
-  c->elem = elem;
-  c->sm_total = sm_count;
+  flmr_corpus* c;
+  if ((rc = new_corpus(device, n_passages, soff, poff, pid_base, elem, sm_count, window_bytes, &c))) return rc;
   auto bail = [&](int code) {
     flmr_corpus_destroy(c);
     return code;
   };
 
-  // --- token matrix residency ---
-  if ((flags & FLMR_CORPUS_ADOPT) && aligned &&
-      (reinterpret_cast<uintptr_t>(tokens) % 16 == 0)) {
+  // --- token matrix residency: pinned host memory (streamed), the caller's buffer (adopted) or library HBM ---
+  if (streamed) {
+    rc = alloc_stream_matrix(c);
+  } else if ((flags & FLMR_CORPUS_ADOPT) && aligned && (reinterpret_cast<uintptr_t>(tokens) % 16 == 0)) {
     c->d_tokens = static_cast<__nv_bfloat16*>(const_cast<void*>(tokens));
     c->adopted = true;
   } else {
-    if ((rc = alloc_token_matrix(c))) return bail(rc);
+    rc = alloc_token_matrix(c);
+  }
+  if (rc) return bail(rc);
+  if (streamed && !is_device_ptr) {
+    host_scatter_rows(static_cast<const char*>(tokens), soff, poff, 0, c->n_tokens, static_cast<char*>(c->h_stream));
+  } else if (!c->adopted) {   // the repack kernel writes a streamed corpus's host matrix through its device alias
     const cudaError_t e = pack_passages(tokens, is_device_ptr, soff, poff, h_doclens, n_passages,
                                         reinterpret_cast<uint4*>(c->d_tokens),
-                                        reinterpret_cast<uint2*>(c->d_fp8));   // d_fp8: null for a bf16 corpus
+                                        reinterpret_cast<uint2*>(c->d_fp8));   // d_fp8: null but for an e4m3 corpus
     if (e != cudaSuccess)
       return bail(fail(FLMR_ERR_CUDA, "corpus repack failed: %s", cudaGetErrorString(e)));
   }
 
-  if ((rc = build_layout(elem, c->d_tokens, c->d_fp8, n_rows, poff, h_doclens, sm_count, &c->layout)))
-    return bail(rc);
+  if ((rc = build_layout(c, c->d_tokens, c->n_rows, poff, h_doclens, &c->layout))) return bail(rc);
   *out = c;
   return FLMR_OK;
+}
+}  // namespace
+}  // extern "C++"
+
+int flmr_corpus_create(const void* tokens, const int32_t* h_doclens, int64_t n_passages, int dim,
+                       int device, int64_t pid_base, unsigned flags, flmr_corpus_t** out) {
+  return corpus_create(tokens, h_doclens, n_passages, dim, device, pid_base, flags, false, 0, out);
 }
 
 int flmr_corpus_create_streamed(const void* tokens, const int32_t* h_doclens, int64_t n_passages, int dim, int device,
                                 int64_t pid_base, unsigned flags, int64_t window_bytes, flmr_corpus_t** out) {
-  if (!out) return fail(FLMR_ERR_INVALID_ARG, "out is null");
-  *out = nullptr;
-  if (flags & ~FLMR_CORPUS_FP16)
-    return fail(FLMR_ERR_UNSUPPORTED, "flags 0x%x: a streamed corpus is bf16 or FLMR_CORPUS_FP16, and is never adopted",
-                flags);
-  if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
-  if (n_passages <= 0 || !tokens || !h_doclens)
-    return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null tokens/doclens");
-  if (window_bytes < kDim * 2) return fail(FLMR_ERR_INVALID_ARG, "window_bytes=%lld holds no row", (long long)window_bytes);
-  std::vector<int64_t> soff, poff;
-  int rc;
-  if ((rc = passage_offsets(h_doclens, n_passages, &soff, &poff, nullptr))) return rc;
-  const int64_t n_rows = poff[n_passages];
-  if (n_rows + kTileN >= (1ll << 31))
-    return fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
-                (long long)n_rows);
-  {   // refused before anything is allocated
-    std::vector<std::pair<int64_t, int64_t>> ranges;
-    if ((rc = plan_windows(poff, window_bytes / (kDim * 2), &ranges))) return rc;
-  }
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
-  int sm_count;
-  bool is_device_ptr;
-  if ((rc = sm90_count(device, &sm_count)) || (rc = token_source(tokens, device, &is_device_ptr))) return rc;
-  flmr_corpus* c = new (std::nothrow) flmr_corpus();
-  if (!c) return fail(FLMR_ERR_OOM, "host allocation failed");
-  c->device = device;
-  c->n_passages = n_passages;
-  c->n_tokens = soff[n_passages];
-  c->n_rows = n_rows;
-  c->pid_base = pid_base;
-  c->elem = (flags & FLMR_CORPUS_FP16) ? Elem::kF16 : Elem::kBF16;
-  c->sm_total = sm_count;
-  c->streamed = true;
-  c->window_bytes = window_bytes;
-  auto bail = [&](int code) {
-    flmr_corpus_destroy(c);
-    return code;
-  };
-  if ((rc = alloc_stream_matrix(c))) return bail(rc);
-  if (is_device_ptr) {   // the repack kernel writes the host matrix through its device alias
-    const cudaError_t e = pack_passages(tokens, true, soff, poff, h_doclens, n_passages,
-                                        reinterpret_cast<uint4*>(c->d_tokens), nullptr);
-    if (e != cudaSuccess) return bail(fail(FLMR_ERR_CUDA, "corpus repack failed: %s", cudaGetErrorString(e)));
-  } else {
-    host_scatter_rows(static_cast<const char*>(tokens), soff, poff, 0, c->n_tokens, static_cast<char*>(c->h_stream));
-  }
-  if ((rc = build_streamed_layout(c, poff, h_doclens))) return bail(rc);
-  *out = c;
-  return FLMR_OK;
+  return corpus_create(tokens, h_doclens, n_passages, dim, device, pid_base, flags, true, window_bytes, out);
 }
 
 int flmr_corpus_residency(const flmr_corpus_t* c, int* streamed, int64_t* window_bytes, int64_t* host_bytes) {
@@ -2406,10 +2370,6 @@ int flmr_corpus_destroy(flmr_corpus_t* c) {
   if (c->vm_tokens.base || c->vm_fp8.base || c->h_stream) cudaDeviceSynchronize();   // no search still reads them
   if (c->h_master) cudaFreeHost(c->h_master);   // d_tokens is its device alias
   if (c->h_stream) cudaFreeHost(c->h_stream);   // likewise
-  for (Window& w : c->windows)
-    for (void* q : {static_cast<void*>(w.cta.row_begin), static_cast<void*>(w.cta.tile_base),
-                    static_cast<void*>(w.cta.end_mask), static_cast<void*>(w.cta.first_pid)})
-      cudaFree(q);
   gm_free(&c->vm_tokens);                       // (an adopted matrix is the caller's and has no mapping here)
   gm_free(&c->vm_fp8);
   free_layout(&c->layout);
@@ -2448,34 +2408,18 @@ int builder_create(const int32_t* h_doclens, int64_t n_passages, int dim, int de
     return code;
   };
   b->doclens.assign(h_doclens, h_doclens + n_passages);
-  if (int rc = passage_offsets(h_doclens, n_passages, &b->soff, &b->poff, &b->aligned)) return bail(rc);
-  const int64_t n_rows = b->poff[n_passages];
-  if (n_rows + kTileN >= (1ll << 31))
-    return bail(fail(FLMR_ERR_UNSUPPORTED, "%lld stored token rows exceed the 2^31 per-shard limit; shard the corpus",
-                     (long long)n_rows));
-  if (streamed) {   // refused before anything is allocated
-    std::vector<std::pair<int64_t, int64_t>> ranges;
-    if (int rc = plan_windows(b->poff, window_bytes / (kDim * 2), &ranges)) return bail(rc);
-  }
+  if (int rc = corpus_offsets(h_doclens, n_passages, window_bytes, &b->soff, &b->poff, &b->aligned)) return bail(rc);
   DeviceGuard guard(device);
   if (!guard.ok) return bail(fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device));
   int sm_count;
   if (int rc = sm90_count(device, &sm_count)) return bail(rc);
-  flmr_corpus* c = new (std::nothrow) flmr_corpus();
-  if (!c) return bail(fail(FLMR_ERR_OOM, "host allocation failed"));
+  flmr_corpus* c;
+  if (int rc = new_corpus(device, n_passages, b->soff, b->poff, pid_base, elem, sm_count, window_bytes, &c))
+    return bail(rc);
   b->corpus = c;
-  c->device = device;
-  c->n_passages = n_passages;
-  c->n_tokens = b->soff[n_passages];
-  c->n_rows = n_rows;
-  c->pid_base = pid_base;
-  c->elem = elem;
-  c->sm_total = sm_count;
   if (streamed) {
     // rows are read (or copied) straight into the host matrix, or, when passages need padding, through one pinned
     // staging buffer from which host_scatter_rows puts them in place; the device is not involved
-    c->streamed = true;
-    c->window_bytes = window_bytes;
     if (int rc = alloc_stream_matrix(c)) return bail(rc);
     const size_t buf_bytes = static_cast<size_t>(flmr_corpus_builder::kBufRows) * kDim * 2;
     if (!b->aligned) {
@@ -2635,14 +2579,8 @@ int flmr_corpus_builder_finish(flmr_corpus_builder_t* b, flmr_corpus_t** out, do
                 (long long)c->n_tokens);
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
-  if (c->streamed) {
-    if (int rc = build_streamed_layout(c, b->poff, b->doclens.data())) return rc;
-  } else {
-    FLMR_CUDA(cudaStreamSynchronize(b->stream));
-    if (int rc = build_layout(c->elem, c->d_tokens, c->d_fp8, c->n_rows, b->poff, b->doclens.data(), c->sm_total,
-                              &c->layout))
-      return rc;
-  }
+  if (b->stream) FLMR_CUDA(cudaStreamSynchronize(b->stream));   // a streamed load wrote the host matrix itself
+  if (int rc = build_layout(c, c->d_tokens, c->n_rows, b->poff, b->doclens.data(), &c->layout)) return rc;
   if (host_fill_seconds) *host_fill_seconds = b->fill_s;
   b->corpus = nullptr;     // ownership passes to the caller
   flmr_corpus_builder_destroy(b);
@@ -2676,7 +2614,8 @@ int flmr_corpus_info(const flmr_corpus_t* c, flmr_corpus_info_t* out) {
   out->device = c->device;
   out->n_ctas = c->layout.n_ctas;
   out->adopted = c->adopted ? 1 : 0;
-  out->n_tiles = c->layout.cta.n_tiles;
+  out->n_tiles = 0;
+  for (const Window& w : c->layout.windows) out->n_tiles += w.cta.n_tiles;
   out->hbm_bytes = hbm_bytes(c);
   return FLMR_OK;
 }
@@ -2776,7 +2715,7 @@ int flmr_corpus_append(flmr_corpus_t* c, const void* tokens, const int32_t* h_do
   if (!rc && c->d_dead)   // d_dead exists once anything is deleted, except right after a compaction
     rc = dev_upload(&d_dead, compacted ? dead_by_slot(slot_pid, c->pid_base, dead) : dead, nullptr);
   SlotLayout layout;
-  if (!rc) rc = build_layout(c->elem, c->d_tokens, c->d_fp8, new_rows, all_poff, all_len.data(), c->sm_total, &layout);
+  if (!rc) rc = build_layout(c, c->d_tokens, new_rows, all_poff, all_len.data(), &layout);
   if (rc) {
     cudaFree(d_dead);
     cudaFree(d_slot_pid);
@@ -2931,7 +2870,7 @@ int flmr_corpus_compact(flmr_corpus_t* c, int64_t* n_removed, int64_t* bytes_rel
     }
   }
   if ((rc = dev_upload(&d_slot_pid, slot_pid, nullptr)) ||
-      (rc = build_layout(c->elem, d_tokens, c->d_fp8, new_rows, poff, lens.data(), c->sm_total, &layout)))
+      (rc = build_layout(c, d_tokens, new_rows, poff, lens.data(), &layout)))
     return release(rc);
 
   // --- 3. the rows move: the HBM matrix on the device, the pinned bf16 master of an e4m3 corpus on the host ---
@@ -3013,8 +2952,8 @@ int flmr_workspace_create(const flmr_corpus_t* c, int max_queries, int max_nq,
   *ws->h_status = 0;
   if (c->streamed) {   // the window buffers (two, or one for a one-window plan; zeroed: rows a tile reads past its
                        // window's end are finite), their tensor maps, the copy stream and its events
-    const size_t wbytes = static_cast<size_t>(c->window_rows) * kDim * 2;
-    const int n_bufs = c->windows.size() > 1 ? 2 : 1;
+    const size_t wbytes = static_cast<size_t>(c->layout.window_rows) * kDim * 2;
+    const int n_bufs = c->layout.windows.size() > 1 ? 2 : 1;
     for (int i = 0; i < n_bufs; ++i) {
       if ((e = cudaMalloc(reinterpret_cast<void**>(&ws->d_win[i]), wbytes)) != cudaSuccess ||
           (e = cudaMemset(ws->d_win[i], 0, wbytes)) != cudaSuccess ||
@@ -3022,8 +2961,8 @@ int flmr_workspace_create(const flmr_corpus_t* c, int max_queries, int max_nq,
           (e = cudaEventCreateWithFlags(&ws->scanned_ev[i], cudaEventDisableTiming)) != cudaSuccess)
         return bail(fail(e == cudaErrorMemoryAllocation ? FLMR_ERR_OOM : FLMR_ERR_CUDA,
                          "window buffers: %s", cudaGetErrorString(e)));
-      if (int rc = encode_rows_map(&ws->tmap_win[i], ws->d_win[i], static_cast<uint64_t>(c->window_rows), kTileN,
-                                   c->elem))
+      if (int rc = encode_rows_map(&ws->tmap_win[i], ws->d_win[i], static_cast<uint64_t>(c->layout.window_rows),
+                                   kTileN, c->elem))
         return bail(rc);
     }
     if ((e = cudaStreamCreateWithFlags(&ws->copy_stream, cudaStreamNonBlocking)) != cudaSuccess ||

@@ -76,6 +76,32 @@ def test_argument_validation_without_gpu():
     assert rc == 1 and b"zero-length" in L.flmr_last_error()
     # null pointers
     assert L.flmr_corpus_create(None, dl.ctypes.data, 2, 128, 0, 0, 0, C.byref(h)) == 1
+    # a streamed corpus and its builder: each refused before any device call, with its code and, where two checks
+    # could trip, in its order (the corpus checks its flags before dim and the window, the builder its window first)
+    row, fp8 = _cabi.DIM * 2, _cabi.CORPUS_FP8
+    for args, rc, msg in (((tok.ctypes.data, dl.ctypes.data, 2, 64, 0, 0, 0, 1 << 20), 3, b"dim"),
+                          ((None, dl.ctypes.data, 2, 128, 0, 0, 0, 1 << 20), 1, None),
+                          ((tok.ctypes.data, None, 2, 128, 0, 0, 0, 1 << 20), 1, None),
+                          ((tok.ctypes.data, dl0.ctypes.data, 2, 128, 0, 0, 0, 1 << 20), 1, b"zero-length"),
+                          ((tok.ctypes.data, dl.ctypes.data, 2, 128, 0, 0, 0, row - 1), 1, b"holds no row"),
+                          ((tok.ctypes.data, dl.ctypes.data, 2, 128, 0, 0, 0, 0), 1, b"holds no row"),
+                          ((tok.ctypes.data, dl.ctypes.data, 2, 128, 0, 0, fp8, 1 << 20), 3, b"flags"),
+                          ((tok.ctypes.data, dl.ctypes.data, 2, 128, 0, 0, _cabi.CORPUS_ADOPT, 1 << 20), 3, b"flags"),
+                          ((tok.ctypes.data, dl.ctypes.data, 2, 128, 0, 0, 0, 3 * row), 3, b"window"),
+                          ((tok.ctypes.data, dl.ctypes.data, 2, 64, 0, 0, fp8, 0), 3, b"flags")):
+        assert L.flmr_corpus_create_streamed(*args, C.byref(h)) == rc and not h.value, args
+        assert msg is None or msg in L.flmr_last_error(), (args, L.flmr_last_error())
+    b = C.c_void_p()
+    for args, rc, msg in (((dl.ctypes.data, 2, 64, 0, 0, 0, 1 << 20), 3, b"dim"),
+                          ((None, 2, 128, 0, 0, 0, 1 << 20), 1, None),
+                          ((dl0.ctypes.data, 2, 128, 0, 0, 0, 1 << 20), 1, b"zero-length"),
+                          ((dl.ctypes.data, 2, 128, 0, 0, 0, row - 1), 1, b"holds no row"),
+                          ((dl.ctypes.data, 2, 128, 0, 0, 0, 0), 1, b"holds no row"),
+                          ((dl.ctypes.data, 2, 128, 0, 0, fp8, 1 << 20), 3, b"flags"),
+                          ((dl.ctypes.data, 2, 128, 0, 0, 0, 3 * row), 3, b"window"),
+                          ((dl.ctypes.data, 2, 64, 0, 0, fp8, 0), 1, b"holds no row")):
+        assert L.flmr_corpus_builder_create_streamed(*args, C.byref(b)) == rc and not b.value, args
+        assert msg is None or msg in L.flmr_last_error(), (args, L.flmr_last_error())
     assert L.flmr_topk_merge(None, None, 1, 1, 1, 1, None, None, 0, None) == 1
     assert L.flmr_maxsim_topk(None, None, None, 1, 32, 5, 0, None, None, None) == 1
     assert L.flmr_corpus_destroy(None) == 0 and L.flmr_workspace_destroy(None) == 0

@@ -94,6 +94,40 @@ def _windows(L, dl, window_bytes):
     return table
 
 
+def _want_info(L, dl, storage, window_bytes, sms):
+    """(n_ctas, n_tiles, hbm_bytes) flmr_corpus_info reports for a new library-owned corpus of doclens dl: resident
+    (window_bytes 0: its rows, one partition and, bf16, the CTA-pair partition) or streamed (its windows' partitions),
+    each beside the offsets and lengths.  Every device array takes 4 or 8 B per entry."""
+    dl = np.ascontiguousarray(dl, np.int32)
+    n, rows = len(dl), int(((dl.astype(np.int64) + 3) // 4 * 4).sum())
+
+    def tiles(n_ctas):
+        nt = C.c_int64()
+        rb, tb = np.zeros(n_ctas + 1, np.int32), np.zeros(n_ctas + 1, np.int64)
+        assert L.flmr_debug_build_partition(dl.ctypes.data, n, n_ctas, rb.ctypes.data, tb.ctypes.data, None, None, 0,
+                                            C.byref(nt)) == 0
+        return nt.value
+
+    def partition_bytes(n_ctas, n_tiles):
+        return (n_ctas + 1) * (4 + 8) + n_tiles * (4 + 4)
+
+    meta = (n + 1) * 8 + n * 4
+    if window_bytes:
+        nw = C.c_int64()
+        assert L.flmr_debug_window_plan(dl.ctypes.data, n, window_bytes, sms, None, 0, C.byref(nw), None, None, None,
+                                        None, 0, None) == 0
+        table = np.zeros((nw.value, 6), np.int64)
+        assert L.flmr_debug_window_plan(dl.ctypes.data, n, window_bytes, sms, table.ctypes.data, nw.value,
+                                        C.byref(nw), None, None, None, None, 0, None) == 0
+        return (int(table[:, 4].max()), int(table[:, 5].sum()),
+                meta + sum(partition_bytes(int(w[4]), int(w[5])) for w in table))
+    nc = min(sms, n)
+    hbm = rows * ROW + meta + partition_bytes(nc, tiles(nc))
+    if storage == "bf16" and nc >= 2:
+        hbm += partition_bytes(nc // 2, tiles(nc // 2))
+    return nc, tiles(nc), hbm
+
+
 # storage, relu, Nq, B, windows (24: more than 20), pid_base, deletions, allow bitmaps.  B = 70 exceeds the default
 # workspace's 64 queries, so such a call scans each window in two chunks; Nq = 832 is row-sliced (partial scores by slot).
 FACTORS = (("bf16", "fp16"), (False, True), (1, 32, 320, 832), (1, 5, 13, 70), (1, 2, 3, 24), (0, 1000),
@@ -144,6 +178,10 @@ def test_streamed_is_bitwise_resident(R, L, storage, relu, nq, B, n_windows, pid
     assert (len(table) == n_windows) if n_windows < 20 else (len(table) > 20)
     assert st.residency == "host" and res.residency == "device"
     assert st.residency_info()["window_bytes"] == wb and st.residency_info()["host_bytes"] == st.info.n_rows * ROW
+    assert res.residency_info() == {"streamed": False, "window_bytes": 0, "host_bytes": 0}
+    sms = torch.cuda.get_device_properties(st.device).multi_processor_count
+    for c, w in ((res, 0), (st, wb)):
+        assert (c.info.n_ctas, c.info.n_tiles, c.info.hbm_bytes) == _want_info(L, dl, storage, w, sms), c.residency
     rng = np.random.default_rng(B)
     if dels != "none":
         dead = rng.choice(n, size=n // 10, replace=False)

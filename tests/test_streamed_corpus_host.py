@@ -122,6 +122,9 @@ def _cases():
     dl = np.array([10, 20, 64, 3, 5, 64, 7, 8, 9, 64], np.int32)
     yield "edges", dl, 64 * ROW, 132
     yield "odd-bytes", rng.integers(1, 100, 700).astype(np.int32), 100 * ROW + 255, 7
+    # one window of exactly every row, as a resident corpus plans it
+    dl = rng.integers(1, 300, 900).astype(np.int32)
+    yield "exact", dl, int(_poff(dl)[-1]) * ROW, 7
 
 
 @pytest.mark.parametrize("name,doclens,window_bytes,n_ctas", list(_cases()), ids=[c[0] for c in _cases()])
@@ -149,6 +152,18 @@ def test_window_plan_matches_numpy(name, doclens, window_bytes, n_ctas):
         sizes = table[:, 1] - table[:, 0]
         assert 1 in sizes[:-1] and sizes[-1] == 1
         assert (table[:, 3] == 64).any()
+    if window_bytes >= poff[-1] * ROW:
+        # one window of every slot, whose partition is exactly flmr_debug_build_partition's: the resident corpus's
+        assert len(table) == 1
+        L, dl, nt = _cabi.lib(), np.ascontiguousarray(doclens, np.int32), C.c_int64()
+        nc = min(n_ctas, len(dl))
+        want = (np.zeros(nc + 1, np.int32), np.zeros(nc + 1, np.int64), np.zeros(len(got[3]), np.uint32),
+                np.zeros(len(got[3]), np.int32))
+        _cabi.check(L.flmr_debug_build_partition(dl.ctypes.data, len(dl), n_ctas, *(a.ctypes.data for a in want),
+                                                 len(got[3]), C.byref(nt)))
+        assert table[0, 4] == nc and nt.value == len(got[3])
+        for a, b in zip(got[1:], want):
+            assert np.array_equal(a, b)
 
 
 def test_window_plan_refuses_a_passage_longer_than_the_window():
