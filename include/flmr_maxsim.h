@@ -49,6 +49,10 @@
  *       a corpus kept in pinned host memory and streamed through two HBM windows per search, for a shard that does not
  *       fit beside what the GPU already holds (the reference builds its validation Searcher inside the training
  *       process, src/executors/FLMR_executor.py:774-792).
+ *   flmr_corpus_builder_create_plaid / flmr_corpus_builder_append_plaid / flmr_corpus_codec
+ *       a streamed corpus kept in a PLAID index's compressed form (centroid codes and packed residuals) and decoded
+ *       window by window on the GPU before the scan: 20 to 132 B of pinned host memory and PCIe traffic per token
+ *       instead of 256.
  *   flmr_debug_maxsim_scores_simt
  *       test infrastructure: an independent plain-SIMT fp32 device kernel used by tests to
  *       cross-check the tensor-core kernel at sizes where the CPU oracle is too slow.
@@ -289,6 +293,44 @@ int flmr_corpus_builder_create_streamed(const int32_t* h_doclens, int64_t n_pass
                                         int64_t pid_base, unsigned flags, int64_t window_bytes,
                                         flmr_corpus_builder_t** out);
 int flmr_corpus_residency(const flmr_corpus_t* corpus, int* streamed, int64_t* window_bytes, int64_t* host_bytes);
+
+/*
+ * A PLAID-CODED streamed corpus: a streamed corpus that keeps a PLAID index's compressed form in pinned host memory,
+ * a 4-byte centroid code and 16 * nbits bytes of packed residual per stored row, instead of 256-byte rows.  Each search
+ * copies a window's codes and residuals and decodes them on the GPU into one HBM window buffer, which the unchanged
+ * scan kernels read.  Decoding does exactly what flmr_plaid_decode (normalize = 1), or flmr_plaid_decode_fp16 with
+ * FLMR_CORPUS_FP16, does to each row, so every result is bitwise that of a resident corpus of those decoded rows.
+ *
+ * flmr_corpus_builder_create_plaid   as flmr_corpus_builder_create_streamed, plus the codec: nbits (1, 2, 4 or 8),
+ *                               the fp32 centroids [n_centroids, 128] and the fp32 bucket weights [2^nbits] (host
+ *                               pointers, copied).  window_bytes bounds a window's DECODED rows (256 B each).  Refusals,
+ *                               in this order: window_bytes < one row (FLMR_ERR_INVALID_ARG), flags other than
+ *                               FLMR_CORPUS_FP16 (FLMR_ERR_UNSUPPORTED), dim != 128 (FLMR_ERR_UNSUPPORTED), no passage
+ *                               or null doclens, nbits outside {1, 2, 4, 8}, null tables or n_centroids < 1
+ *                               (FLMR_ERR_INVALID_ARG), a passage longer than a window (FLMR_ERR_UNSUPPORTED).
+ * flmr_corpus_builder_append_plaid   the next n_rows packed token rows, in order and in any split: codes int32 [n_rows]
+ *                               and residuals uint8 [n_rows, 16 * nbits], as an index's chunks hold them.  The library
+ *                               stores them in the padded row layout (each passage's last row repeated up to a multiple
+ *                               of 4 rows).  A code outside [0, n_centroids) gives FLMR_ERR_INVALID_ARG and stores
+ *                               nothing.  flmr_corpus_builder_append(_file) refuse this builder, and this call any other
+ *                               (FLMR_ERR_INVALID_ARG).  flmr_corpus_builder_finish copies the tables to HBM (counted in
+ *                               hbm_bytes) and plans the windows; flmr_corpus_builder_destroy abandons the build.
+ * flmr_corpus_codec             *nbits = the codec's bits of a PLAID-coded corpus, 0 for any other corpus.
+ *
+ * Each workspace holds one decoded window buffer and two staging buffers of compressed rows (one of each for a
+ * one-window plan).  A search copies window w's compressed rows into staging buffer w % 2 on the workspace's copy stream;
+ * the caller's stream waits for that copy and decodes the window, and the copy of window w + 2 waits for that decode.
+ * On this corpus flmr_corpus_residency gives *streamed = 1 and *host_bytes = its compressed arrays; the calls that work
+ * on a streamed corpus work, flmr_corpus_gather decodes the requested rows from the mapped host arrays (and stays
+ * capturable), and flmr_debug_maxsim_scores_simt returns FLMR_ERR_UNSUPPORTED, as do the calls a streamed corpus refuses.
+ */
+int flmr_corpus_builder_create_plaid(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                     int64_t pid_base, unsigned flags, int64_t window_bytes, int nbits,
+                                     const float* h_centroids, int64_t n_centroids, const float* h_bucket_weights,
+                                     flmr_corpus_builder_t** out);
+int flmr_corpus_builder_append_plaid(flmr_corpus_builder_t* b, const int32_t* h_codes, const uint8_t* h_residuals,
+                                     int64_t n_rows);
+int flmr_corpus_codec(const flmr_corpus_t* corpus, int* nbits);
 
 /* Scratch for searches on `corpus`.  max_queries (>= 1) sizes the per-CTA candidate buffer: a call with more
  * queries is processed in chunks of max_queries (each chunk: its scan passes + ONE merge launch).  max_nq

@@ -45,14 +45,16 @@ LISTED_SYMBOLS = ("flmr_maxsim_topk_listed", "flmr_maxsim_scores_listed", "flmr_
 # a corpus kept in pinned host memory and streamed through HBM windows
 STREAMED_SYMBOLS = ("flmr_corpus_create_streamed", "flmr_corpus_builder_create_streamed", "flmr_corpus_residency",
                     "flmr_debug_window_plan")
+# a streamed corpus kept in a PLAID index's compressed form and decoded window by window on the GPU
+PLAID_STREAMED_SYMBOLS = ("flmr_corpus_builder_create_plaid", "flmr_corpus_builder_append_plaid", "flmr_corpus_codec")
 # symbols an earlier revision's library may lack (tools/scan_ab.py drives one through this binding)
 OPTIONAL_SYMBOLS = (UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS + FP16_TRAIN_SYMBOLS + COMPACT_SYMBOLS
-                    + LISTED_SYMBOLS + STREAMED_SYMBOLS)
+                    + LISTED_SYMBOLS + STREAMED_SYMBOLS + PLAID_STREAMED_SYMBOLS)
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
     "flmr_corpus_create", "flmr_corpus_destroy", "flmr_corpus_info", "flmr_corpus_storage",
-    *UPDATE_SYMBOLS, *COMPACT_SYMBOLS, *STREAMED_SYMBOLS,
+    *UPDATE_SYMBOLS, *COMPACT_SYMBOLS, *STREAMED_SYMBOLS, *PLAID_STREAMED_SYMBOLS,
     "flmr_workspace_create", "flmr_workspace_destroy", "flmr_workspace_status",
     "flmr_maxsim_scores", "flmr_maxsim_topk", "flmr_topk_merge", "flmr_topk_select", "flmr_plaid_decode",
     *FP16_SYMBOLS,
@@ -125,6 +127,11 @@ def lib() -> C.CDLL:
         L.flmr_corpus_residency.argtypes = [vp, C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
         L.flmr_debug_window_plan.argtypes = [vp, i64, i64, i32, vp, i64, C.POINTER(i64), vp, vp, vp, vp, i64,
                                              C.POINTER(i64)]
+    if hasattr(L, "flmr_corpus_builder_create_plaid"):
+        L.flmr_corpus_builder_create_plaid.argtypes = [vp, i64, i32, i32, i64, u32, i64, i32, vp, i64, vp,
+                                                       C.POINTER(vp)]
+        L.flmr_corpus_builder_append_plaid.argtypes = [vp, vp, vp, i64]
+        L.flmr_corpus_codec.argtypes = [vp, C.POINTER(i32)]
     L.flmr_workspace_create.argtypes = [vp, i32, i32, C.POINTER(vp)]
     L.flmr_workspace_destroy.argtypes = [vp]
     L.flmr_workspace_status.argtypes = [vp, C.POINTER(i32)]

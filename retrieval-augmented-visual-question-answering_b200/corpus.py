@@ -198,6 +198,14 @@ class FlatCorpus:
         return {"streamed": bool(streamed.value), "window_bytes": int(window.value), "host_bytes": int(host.value)}
 
     @property
+    def codec_nbits(self) -> int:
+        """The PLAID codec's bits per dimension of a PLAID-coded streamed corpus (``from_plaid(..., compressed=True)``),
+        0 for any other corpus."""
+        nbits = C.c_int(0)
+        _cabi.check(_cabi.lib().flmr_corpus_codec(self.handle, C.byref(nbits)))
+        return int(nbits.value)
+
+    @property
     def dtype(self) -> torch.dtype:
         """Element type of the rows this corpus takes (``append``) and gathers, and of its queries."""
         return element_dtype(self.storage)
@@ -274,16 +282,25 @@ class FlatCorpus:
     @classmethod
     def from_plaid(cls, path: str, device=None, rank: int = 0, world_size: int = 1,
                    storage: str = "bf16", residency: str = "device",
-                   window_bytes: int = DEFAULT_WINDOW_BYTES) -> "FlatCorpus":
+                   window_bytes: int = DEFAULT_WINDOW_BYTES, compressed: bool = False) -> "FlatCorpus":
         """Decode a reference PLAID index directory on the GPU (plaid.py) and keep it resident — with
         world_size > 1 only this rank's contiguous, token-balanced passage shard (SURVEY.md 8e).  ``storage="fp16"``
         decodes straight to fp16 (``flmr_plaid_decode_fp16``), the type the reference's codec decodes to.
         ``residency="host"``: a streamed corpus (see the class), decoded on the GPU in bounded chunks
-        (``plaid_to_host_chunks``), each copied down into its pinned host matrix."""
-        from .plaid import plaid_to_flat, plaid_to_host_chunks, read_plaid_doclens, read_plaid_metadata
+        (``plaid_to_host_chunks``), each copied down into its pinned host matrix.
+        ``residency="host", compressed=True``: a PLAID-coded streamed corpus.  Nothing is decoded at load time: the
+        pinned host memory holds each token's centroid code and packed residual (4 + 16 nbits bytes instead of 256),
+        and every search copies a window's compressed rows and decodes them on the GPU before scanning them.  Its
+        results are bitwise those of the resident ``from_plaid`` corpus of the same storage.  bf16 or fp16 only."""
+        from .plaid import plaid_compressed_chunks, plaid_to_flat, plaid_to_host_chunks, read_plaid_doclens, \
+            read_plaid_metadata
         from .sharded import shard_ranges
         _storage_flag(storage)
         _check_residency(residency, storage, window_bytes)
+        if not isinstance(compressed, bool):
+            raise ValueError("compressed must be a bool, got %r" % (compressed,))
+        if compressed and residency != "host":
+            raise ValueError("compressed=True streams a PLAID index's compressed form and needs residency='host'")
         if residency == "host":
             if world_size == 1:
                 p0, p1 = 0, None
@@ -292,6 +309,22 @@ class FlatCorpus:
                 p0, p1 = shard_ranges(all_doclens, world_size)[rank]
                 if p0 == p1:
                     return None
+            if compressed:
+                if not torch.cuda.is_available():
+                    raise RuntimeError("FlatCorpus needs a CUDA device: there is no CPU fallback for this path")
+                device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+                if device.index is None:
+                    device = torch.device("cuda", torch.cuda.current_device())
+                nbits, centroids, weights, doclens, chunks = plaid_compressed_chunks(path, passage_range=(p0, p1))
+
+                def feed_codes(L, b):
+                    for codes, residuals in chunks:
+                        _cabi.check(L.flmr_corpus_builder_append_plaid(b, C.c_void_p(codes.data_ptr()),
+                                                                       C.c_void_p(residuals.data_ptr()),
+                                                                       codes.numel()))
+
+                return cls._build(np.ascontiguousarray(doclens, dtype=np.int32), device, p0, _storage_flag(storage),
+                                  residency, window_bytes, feed_codes, codec=(nbits, centroids, weights))[0]
             device, doclens, pieces = plaid_to_host_chunks(path, device, passage_range=(p0, p1),
                                                            dtype=element_dtype(storage))
 
@@ -313,12 +346,22 @@ class FlatCorpus:
 
     @classmethod
     def _build(cls, doclens: np.ndarray, device: torch.device, pid_base: int, flags: int, residency: str,
-               window_bytes: int, feed) -> tuple:
+               window_bytes: int, feed, codec=None) -> tuple:
         """A corpus of ``doclens`` (int32) built through the C-level builder of ``residency``: ``feed(L, builder)``
-        appends every packed row in order (``L``: the library).  Returns the corpus and the host fill seconds."""
+        appends every packed row in order (``L``: the library).  ``codec = (nbits, centroids, bucket weights)`` (fp32
+        CPU tensors) builds a PLAID-coded streamed corpus.  Returns the corpus and the host fill seconds."""
         L = _cabi.lib()
         b = C.c_void_p()
-        if residency == "host":
+        if codec is not None:
+            nbits, centroids, weights = codec
+            centroids = centroids.float().contiguous()
+            weights = weights.float().contiguous()
+            _cabi.check(L.flmr_corpus_builder_create_plaid(doclens.ctypes.data_as(C.c_void_p), len(doclens),
+                                                           _cabi.DIM, int(device.index), int(pid_base), flags,
+                                                           int(window_bytes), int(nbits),
+                                                           C.c_void_p(centroids.data_ptr()), centroids.size(0),
+                                                           C.c_void_p(weights.data_ptr()), C.byref(b)))
+        elif residency == "host":
             _cabi.check(L.flmr_corpus_builder_create_streamed(doclens.ctypes.data_as(C.c_void_p), len(doclens),
                                                               _cabi.DIM, int(device.index), int(pid_base), flags,
                                                               int(window_bytes), C.byref(b)))

@@ -736,7 +736,8 @@ __global__ void flmr_simt_maxsim_kernel(const void* __restrict__ d_any, const in
 // :51-73 reversed_bit_map, :77-93 lookup table; decode loop decompress_residuals.cpp:27-78), then the
 // row is L2-normalised (index_storage.py:173) and stored as bf16 (kF16: fp16, the reference's own decode type,
 // residual.py:273), rounded once from fp32.  HBM-bound byte work: one warp per token, lane = 4 dims, centroid rows
-// come from L2, bucket weights from shared memory.
+// come from L2, bucket weights from shared memory.  The per-token arithmetic is flmr_plaid_decode_row.cuh, which the
+// window decode and the gather of a PLAID-coded streamed corpus include too.
 template <bool kF16>
 __global__ void flmr_plaid_decode_kernel(const int32_t* __restrict__ codes,
                                          const uint8_t* __restrict__ residuals,
@@ -764,36 +765,82 @@ __global__ void flmr_plaid_decode_kernel(const int32_t* __restrict__ codes,
     }
     const float4 c = __ldg(reinterpret_cast<const float4*>(centroids + static_cast<int64_t>(code) * kDim) + lane);
     const uint8_t* row = residuals + t * packed_dim;
-    float v[4] = {c.x, c.y, c.z, c.w};
-#pragma unroll
-    for (int dd = 0; dd < 4; ++dd) {
-      const int i = 4 * lane + dd;
-      const uint32_t byte = __ldg(row + i / keys);
-      const uint32_t field = (byte >> (8 - nbits * (i % keys + 1))) & mask;
-      v[dd] += s_w[__brev(field) >> (32 - nbits)];
-    }
-    if (normalize) {
-      float ss = v[0] * v[0] + v[1] * v[1] + v[2] * v[2] + v[3] * v[3];
-#pragma unroll
-      for (int off = 16; off >= 1; off >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
-      const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);   // torch.nn.functional.normalize eps
-#pragma unroll
-      for (int dd = 0; dd < 4; ++dd) v[dd] *= inv;
-    }
-    uint2 w;
-    if constexpr (kF16) {
-      __half2 lo = __floats2half2_rn(v[0], v[1]);
-      __half2 hi = __floats2half2_rn(v[2], v[3]);
-      w.x = *reinterpret_cast<uint32_t*>(&lo);
-      w.y = *reinterpret_cast<uint32_t*>(&hi);
-    } else {
-      __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]);
-      __nv_bfloat162 hi = __floats2bfloat162_rn(v[2], v[3]);
-      w.x = *reinterpret_cast<uint32_t*>(&lo);
-      w.y = *reinterpret_cast<uint32_t*>(&hi);
-    }
+#include "flmr_plaid_decode_row.cuh"
     out[t * 32 + lane] = w;
   }
+}
+
+// The window decode of a PLAID-coded streamed corpus: the staged compressed rows of one window (codes [rows], packed
+// residuals [rows, 16 nbits], in the padded row layout, so rows is a multiple of kGroup) into the window buffer, in
+// bf16 or (kF16) fp16, always L2-normalised as a PLAID index's embeddings are.  The codes were checked when the corpus
+// was built.  A warp decodes kGroup consecutive rows per step and issues their code and centroid loads before the
+// first row's arithmetic, so it keeps four tokens' loads in flight rather than one.
+template <bool kF16>
+__global__ void __launch_bounds__(256)
+flmr_plaid_window_decode_kernel(const int32_t* __restrict__ codes, const uint8_t* __restrict__ residuals,
+                                const float* __restrict__ centroids, const float* __restrict__ bucket_weights,
+                                int nbits, int64_t rows, uint2* __restrict__ out) {
+  __shared__ float s_w[256];
+  for (int i = threadIdx.x; i < (1 << nbits); i += blockDim.x) s_w[i] = bucket_weights[i];
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int64_t n_warps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
+  const int keys = 8 / nbits;
+  const int packed_dim = kDim * nbits / 8;
+  const uint32_t mask = (1u << nbits) - 1u;
+  const int normalize = 1;
+  for (int64_t t0 = warp0 * kGroup; t0 < rows; t0 += n_warps * kGroup) {
+    float4 cg[kGroup];
+#pragma unroll
+    for (int g = 0; g < kGroup; ++g)
+      cg[g] = __ldg(reinterpret_cast<const float4*>(centroids + static_cast<int64_t>(__ldg(codes + t0 + g)) * kDim) +
+                    lane);
+#pragma unroll
+    for (int g = 0; g < kGroup; ++g) {
+      const float4 c = cg[g];
+      const uint8_t* row = residuals + (t0 + g) * packed_dim;
+#include "flmr_plaid_decode_row.cuh"
+      out[(t0 + g) * 32 + lane] = w;
+    }
+  }
+}
+
+// The gather of a PLAID-coded streamed corpus: flmr_gather_kernel's batch (one warp per (id, token) of the
+// [n_pids, nd_max, 128] output; an all-masked zero row for an id outside the shard, a deleted id and every token past
+// the passage's length), each row decoded from the corpus's mapped host arrays as the window decode decodes it.
+template <bool kF16>
+__global__ void flmr_plaid_gather_kernel(const int32_t* __restrict__ codes, const uint8_t* __restrict__ residuals,
+                                         const float* __restrict__ centroids,
+                                         const float* __restrict__ bucket_weights, int nbits,
+                                         const int64_t* __restrict__ poff, const int32_t* __restrict__ doclen,
+                                         const uint32_t* __restrict__ dead, const int64_t* __restrict__ pids,
+                                         int64_t n_pids, int nd_max, int64_t n_passages, int64_t pid_base,
+                                         uint2* __restrict__ out, uint8_t* __restrict__ mask_out) {
+  __shared__ float s_w[256];
+  for (int i = threadIdx.x; i < (1 << nbits); i += blockDim.x) s_w[i] = bucket_weights[i];
+  __syncthreads();
+  const int64_t wi = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (wi >= n_pids * nd_max) return;
+  const int keys = 8 / nbits;
+  const uint32_t mask = (1u << nbits) - 1u;
+  const int normalize = 1;
+  const int64_t slot = wi / nd_max;
+  const int j = static_cast<int>(wi % nd_max);
+  const int64_t p = pids[slot] - pid_base;
+  uint2 o = make_uint2(0u, 0u);
+  bool real = false;
+  if (p >= 0 && p < n_passages && j < doclen[p] && !(dead && ((dead[p >> 5] >> (p & 31)) & 1u))) {   // warp-uniform
+    const int64_t r = poff[p] + j;
+    const float4 c = __ldg(reinterpret_cast<const float4*>(centroids + static_cast<int64_t>(codes[r]) * kDim) + lane);
+    const uint8_t* row = residuals + r * (kDim * nbits / 8);
+#include "flmr_plaid_decode_row.cuh"
+    o = w;
+    real = true;
+  }
+  out[wi * 32 + lane] = o;
+  if (mask_out && lane == 0) mask_out[wi] = real ? 1 : 0;
 }
 
 // Candidate merge: per query, select the k_out best of n candidates by (score desc, pid asc).
@@ -1111,6 +1158,19 @@ struct flmr_corpus {
   bool streamed = false;
   void* h_stream = nullptr;
   int64_t window_bytes = 0;            // as requested at creation
+  // A PLAID-coded streamed corpus (flmr_corpus_builder_create_plaid; codec_nbits > 0): no row matrix at all (h_stream
+  // and d_tokens stay null).  h_codes [n_rows] and h_residuals [n_rows, 16 nbits] hold each stored row's centroid code
+  // and packed residual in the padded row layout, in one pinned, mapped allocation (d_codes / d_residuals: its device
+  // aliases, which the gather reads); searches copy a window's compressed rows and decode them on the GPU.
+  int codec_nbits = 0;
+  int32_t* h_codes = nullptr;
+  uint8_t* h_residuals = nullptr;
+  const int32_t* d_codes = nullptr;
+  const uint8_t* d_residuals = nullptr;
+  float* d_centroids = nullptr;        // fp32 [n_centroids, 128], in HBM
+  float* d_bucket_weights = nullptr;   // fp32 [2^nbits], in HBM
+  int64_t n_centroids = 0;
+  int64_t codec_hbm_bytes = 0;         // the two arrays above
 };
 
 // Streaming corpus construction (index load): the padded token matrix is allocated once, packed rows arrive in
@@ -1130,6 +1190,8 @@ struct flmr_corpus_builder {
   int64_t *d_soff = nullptr, *d_poff = nullptr;
   int next = 0;
   double fill_s = 0.0;                  // host time spent filling the pinned buffers (read / memcpy)
+  // a PLAID-coded corpus (corpus->codec_nbits > 0): the codec tables, copied to HBM by finish
+  std::vector<float> centroids, bucket_weights;
 };
 
 struct flmr_workspace {
@@ -1154,6 +1216,11 @@ struct flmr_workspace {
   cudaEvent_t fork_ev = nullptr;
   cudaEvent_t copied_ev[2] = {nullptr, nullptr};
   cudaEvent_t scanned_ev[2] = {nullptr, nullptr};
+  // PLAID-coded streamed corpus only: d_win[0] is the one decoded window buffer; a window's compressed rows are copied
+  // into staging buffer w % 2 (codes, then residuals from byte window_rows * 4), and decoded_ev[w % 2] marks the
+  // decode that read it
+  uint8_t* d_cstage[2] = {nullptr, nullptr};
+  cudaEvent_t decoded_ev[2] = {nullptr, nullptr};
 };
 
 // NCCL is resolved at RUN time (dlopen): the library has no link dependency on it, loads on a box without
@@ -1247,12 +1314,15 @@ int64_t hbm_row_bytes(Elem elem) { return elem == Elem::kE4M3 ? kDim : kDim * 2;
 const char* elem_name(Elem elem) { return elem == Elem::kE4M3 ? "e4m3" : elem == Elem::kF16 ? "fp16" : "bf16"; }
 
 // HBM a corpus holds: its matrix (an adopted one is the caller's, a streamed one is host memory), its layout, its
-// tombstones by slot and its slot -> id map.
+// tombstones by slot and its slot -> id map (and a PLAID-coded corpus's centroids and bucket weights).
 int64_t hbm_bytes(const flmr_corpus* c) {
   const int64_t ns = slots(c);
   return (c->adopted || c->streamed ? 0 : c->n_rows * hbm_row_bytes(c->elem)) + c->layout.bytes +
-         (c->d_dead ? (ns + 31) / 32 * 4 : 0) + (c->d_slot_pid ? ns * 8 : 0);
+         (c->d_dead ? (ns + 31) / 32 * 4 : 0) + (c->d_slot_pid ? ns * 8 : 0) + c->codec_hbm_bytes;
 }
+
+// Bytes per stored row of a PLAID-coded corpus's compressed arrays: a 4-byte code and 16 nbits bytes of residual.
+int64_t codec_row_bytes(int nbits) { return 4 + kDim * nbits / 8; }
 
 // The storage a corpus's flags select (FLMR_CORPUS_ADOPT reaches here only from flmr_corpus_create).
 int storage_from_flags(unsigned flags, Elem* elem) {
@@ -1764,6 +1834,22 @@ int plan_listed_chunk(const flmr_corpus* c, flmr_workspace* ws, const std::vecto
 
 // Shared driver of flmr_maxsim_scores / flmr_maxsim_topk (and their _allowed forms: `allow` null = unrestricted,
 // else query b's bitmap starts at allow + b * allow_stride; and their _listed forms: `listed` non-null, `allow` null).
+// Decode the compressed rows of window `win` of a PLAID-coded corpus, staged in ws->d_cstage[b], into the workspace's
+// decoded window buffer, on `st`: one grid-stride launch of at most 8 blocks of 256 threads per SM (one wave).
+int decode_window(const flmr_corpus* c, flmr_workspace* ws, const Window& win, int b, cudaStream_t st) {
+  const int threads = 256;
+  const int64_t want = (win.rows / kGroup + threads / 32 - 1) / (threads / 32);
+  const unsigned blocks = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(want, 8ll * c->sm_total)));
+  const int32_t* codes = reinterpret_cast<const int32_t*>(ws->d_cstage[b]);
+  const uint8_t* residuals = ws->d_cstage[b] + c->layout.window_rows * 4;
+  auto* kernel = c->elem == Elem::kF16 ? flmr_plaid_window_decode_kernel<true> : flmr_plaid_window_decode_kernel<false>;
+  kernel<<<blocks, threads, 0, st>>>(codes, residuals, c->d_centroids, c->d_bucket_weights, c->codec_nbits, win.rows,
+                                     reinterpret_cast<uint2*>(ws->d_win[0]));
+  FLMR_CUDA(cudaGetLastError());
+  ++g_launches;
+  return FLMR_OK;
+}
+
 int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_queries, int nq,
                unsigned flags, int k, const uint32_t* allow, int64_t allow_stride, float* d_all_scores,
                float* d_topk_scores, int64_t* d_topk_pids, cudaStream_t st, const ListedArgs* listed = nullptr) {
@@ -1850,10 +1936,25 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   // copied into buffer w & 1 on the workspace's copy stream; its scans wait for that copy, and the copy of window
   // w + 2 into the same buffer waits for them.  The copy stream first waits for the call's stream, and every copy is
   // waited for by a scan on it, so the call is ordered on `st` like any other.
+  // A PLAID-coded corpus copies window w's codes and residuals into staging buffer w & 1 instead; `st` waits for that
+  // copy, decodes the window into the one decoded buffer and records decoded_ev[w & 1], and the copy of window w + 2
+  // waits for that decode, not for the scans.  Decode and scans are serial on `st` (the scan occupies every SM), so
+  // one decoded buffer suffices.
   const int n_windows = static_cast<int>(l.windows.size());
+  const int nbits = c->codec_nbits;
   auto copy_window = [&](int w) -> int {
     const Window& win = l.windows[w];
     const int b = w & 1;
+    if (nbits) {
+      const int64_t pb = kDim * nbits / 8;
+      if (w >= 2) FLMR_CUDA(cudaStreamWaitEvent(ws->copy_stream, ws->decoded_ev[b], 0));
+      FLMR_CUDA(cudaMemcpyAsync(ws->d_cstage[b], c->h_codes + win.row0, static_cast<size_t>(win.rows) * 4,
+                                cudaMemcpyHostToDevice, ws->copy_stream));
+      FLMR_CUDA(cudaMemcpyAsync(ws->d_cstage[b] + l.window_rows * 4, c->h_residuals + win.row0 * pb,
+                                static_cast<size_t>(win.rows * pb), cudaMemcpyHostToDevice, ws->copy_stream));
+      FLMR_CUDA(cudaEventRecord(ws->copied_ev[b], ws->copy_stream));
+      return FLMR_OK;
+    }
     if (w >= 2) FLMR_CUDA(cudaStreamWaitEvent(ws->copy_stream, ws->scanned_ev[b], 0));
     FLMR_CUDA(cudaMemcpyAsync(ws->d_win[b], static_cast<const char*>(c->h_stream) + win.row0 * kDim * 2,
                               static_cast<size_t>(win.rows) * kDim * 2, cudaMemcpyHostToDevice, ws->copy_stream));
@@ -1869,8 +1970,13 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
   }
   for (int w = 0; w < n_windows; ++w) {
     const Window& win = l.windows[w];
-    const CUtensorMap& rows = c->streamed ? ws->tmap_win[w & 1] : l.tmap_d;
+    const CUtensorMap& rows = nbits ? ws->tmap_win[0] : c->streamed ? ws->tmap_win[w & 1] : l.tmap_d;
     if (c->streamed) FLMR_CUDA(cudaStreamWaitEvent(st, ws->copied_ev[w & 1], 0));
+    if (nbits) {
+      if ((rc = decode_window(c, ws, win, w & 1, st))) return rc;
+      FLMR_CUDA(cudaEventRecord(ws->decoded_ev[w & 1], st));
+      if (w + 2 < n_windows && (rc = copy_window(w + 2))) return rc;
+    }
     for (int c0 = 0; c0 < n_queries; c0 += ws->max_queries) {
       const int nqc = std::min(ws->max_queries, n_queries - c0);
       const __nv_bfloat16* d_qc = static_cast<const __nv_bfloat16*>(d_q) + static_cast<int64_t>(c0) * nq * kDim;
@@ -1955,7 +2061,7 @@ int run_search(const flmr_corpus* c, flmr_workspace* ws, const void* d_q, int n_
           return rc;
       }
     }
-    if (c->streamed) {
+    if (c->streamed && !nbits) {
       FLMR_CUDA(cudaEventRecord(ws->scanned_ev[w & 1], st));
       if (w + 2 < n_windows && (rc = copy_window(w + 2))) return rc;
     }
@@ -2161,10 +2267,10 @@ cudaError_t pack_passages(const void* tokens, bool is_device_ptr, const std::vec
 }
 
 // The host twin of flmr_scatter_rows_kernel, for a streamed corpus's host matrix: packed rows [s0, s0 + n) at src go to
-// their place in the padded layout at dst, a passage's last token also over its padding rows.
+// their place in the padded layout at dst, a passage's last token also over its padding rows.  kRow: bytes per row
+// (a PLAID-coded corpus scatters its codes and its residuals this way too).
 void host_scatter_rows(const char* src, const std::vector<int64_t>& soff, const std::vector<int64_t>& poff, int64_t s0,
-                       int64_t n, char* dst) {
-  constexpr int64_t kRow = kDim * 2;
+                       int64_t n, char* dst, int64_t kRow = kDim * 2) {
   int64_t p = std::upper_bound(soff.begin(), soff.end(), s0) - soff.begin() - 1;
   for (int64_t r = s0; r < s0 + n; ++p) {
     const int64_t take = std::min(soff[p + 1], s0 + n) - r;   // rows of passage p in this chunk
@@ -2360,21 +2466,32 @@ int flmr_corpus_residency(const flmr_corpus_t* c, int* streamed, int64_t* window
   if (!c) return fail(FLMR_ERR_INVALID_ARG, "null corpus");
   if (streamed) *streamed = c->streamed ? 1 : 0;
   if (window_bytes) *window_bytes = c->streamed ? c->window_bytes : 0;
-  if (host_bytes) *host_bytes = c->streamed ? c->n_rows * kDim * 2 : 0;
+  if (host_bytes)
+    *host_bytes = !c->streamed ? 0 : c->n_rows * (c->codec_nbits ? codec_row_bytes(c->codec_nbits) : kDim * 2);
+  return FLMR_OK;
+}
+
+int flmr_corpus_codec(const flmr_corpus_t* c, int* nbits) {
+  if (!c || !nbits) return fail(FLMR_ERR_INVALID_ARG, "null argument");
+  *nbits = c->codec_nbits;
   return FLMR_OK;
 }
 
 int flmr_corpus_destroy(flmr_corpus_t* c) {
   if (!c) return FLMR_OK;
   DeviceGuard guard(c->device);
-  if (c->vm_tokens.base || c->vm_fp8.base || c->h_stream) cudaDeviceSynchronize();   // no search still reads them
+  // no search still reads them
+  if (c->vm_tokens.base || c->vm_fp8.base || c->h_stream || c->h_codes) cudaDeviceSynchronize();
   if (c->h_master) cudaFreeHost(c->h_master);   // d_tokens is its device alias
   if (c->h_stream) cudaFreeHost(c->h_stream);   // likewise
+  if (c->h_codes) cudaFreeHost(c->h_codes);     // h_residuals lies in the same allocation
   gm_free(&c->vm_tokens);                       // (an adopted matrix is the caller's and has no mapping here)
   gm_free(&c->vm_fp8);
   free_layout(&c->layout);
   cudaFree(c->d_dead);
   cudaFree(c->d_slot_pid);
+  cudaFree(c->d_centroids);
+  cudaFree(c->d_bucket_weights);
   delete c;
   return FLMR_OK;
 }
@@ -2386,9 +2503,18 @@ int flmr_corpus_builder_create(const int32_t* h_doclens, int64_t n_passages, int
 
 extern "C++" {
 namespace {
-// flmr_corpus_builder_create_ex (window_bytes = 0) and flmr_corpus_builder_create_streamed (window_bytes > 0).
+// The codec of a PLAID-coded streamed corpus, as flmr_corpus_builder_create_plaid receives it.
+struct PlaidCodec {
+  int nbits;
+  const float* centroids;   // host fp32 [n_centroids, 128]
+  int64_t n_centroids;
+  const float* bucket_weights;   // host fp32 [2^nbits]
+};
+
+// flmr_corpus_builder_create_ex (window_bytes = 0), flmr_corpus_builder_create_streamed (window_bytes > 0) and
+// flmr_corpus_builder_create_plaid (window_bytes > 0 and a codec).
 int builder_create(const int32_t* h_doclens, int64_t n_passages, int dim, int device, int64_t pid_base, unsigned flags,
-                   int64_t window_bytes, flmr_corpus_builder_t** out) {
+                   int64_t window_bytes, flmr_corpus_builder_t** out, const PlaidCodec* codec = nullptr) {
   if (!out) return fail(FLMR_ERR_INVALID_ARG, "out is null");
   *out = nullptr;
   const bool streamed = window_bytes > 0;
@@ -2401,6 +2527,13 @@ int builder_create(const int32_t* h_doclens, int64_t n_passages, int dim, int de
   if (int rc = storage_from_flags(flags, &elem)) return rc;
   if (dim != kDim) return fail(FLMR_ERR_UNSUPPORTED, "dim=%d (only %d is supported)", dim, kDim);
   if (n_passages <= 0 || !h_doclens) return fail(FLMR_ERR_INVALID_ARG, "empty corpus or null doclens");
+  if (codec) {
+    const int nb = codec->nbits;
+    if (nb != 1 && nb != 2 && nb != 4 && nb != 8)
+      return fail(FLMR_ERR_INVALID_ARG, "nbits=%d (the PLAID codec packs 1, 2, 4 or 8 bits per dim)", nb);
+    if (!codec->centroids || !codec->bucket_weights || codec->n_centroids < 1)
+      return fail(FLMR_ERR_INVALID_ARG, "null centroids / bucket weights or no centroid");
+  }
   flmr_corpus_builder* b = new (std::nothrow) flmr_corpus_builder();
   if (!b) return fail(FLMR_ERR_OOM, "host allocation failed");
   auto bail = [&](int code) {
@@ -2417,6 +2550,28 @@ int builder_create(const int32_t* h_doclens, int64_t n_passages, int dim, int de
   if (int rc = new_corpus(device, n_passages, b->soff, b->poff, pid_base, elem, sm_count, window_bytes, &c))
     return bail(rc);
   b->corpus = c;
+  if (codec) {
+    // the compressed arrays in the padded row layout, filled by flmr_corpus_builder_append_plaid; the tables wait for
+    // finish
+    const size_t bytes = static_cast<size_t>(c->n_rows) * codec_row_bytes(codec->nbits);
+    void* h = nullptr;
+    if (const cudaError_t e = cudaHostAlloc(&h, bytes, cudaHostAllocMapped | cudaHostAllocPortable); e != cudaSuccess)
+      return bail(fail(FLMR_ERR_OOM, "cudaHostAlloc(%zu B) for the compressed rows failed: %s", bytes,
+                       cudaGetErrorString(e)));
+    c->codec_nbits = codec->nbits;
+    c->n_centroids = codec->n_centroids;
+    c->h_codes = static_cast<int32_t*>(h);
+    c->h_residuals = static_cast<uint8_t*>(h) + c->n_rows * 4;
+    void* d = nullptr;
+    if (const cudaError_t e = cudaHostGetDevicePointer(&d, h, 0); e != cudaSuccess)
+      return bail(fail(FLMR_ERR_CUDA, "cudaHostGetDevicePointer: %s", cudaGetErrorString(e)));
+    c->d_codes = static_cast<const int32_t*>(d);
+    c->d_residuals = static_cast<const uint8_t*>(d) + c->n_rows * 4;
+    b->centroids.assign(codec->centroids, codec->centroids + codec->n_centroids * kDim);
+    b->bucket_weights.assign(codec->bucket_weights, codec->bucket_weights + (1 << codec->nbits));
+    *out = b;
+    return FLMR_OK;
+  }
   if (streamed) {
     // rows are read (or copied) straight into the host matrix, or, when passages need padding, through one pinned
     // staging buffer from which host_scatter_rows puts them in place; the device is not involved
@@ -2470,6 +2625,43 @@ int flmr_corpus_builder_create_streamed(const int32_t* h_doclens, int64_t n_pass
   return builder_create(h_doclens, n_passages, dim, device, pid_base, flags, window_bytes, out);
 }
 
+int flmr_corpus_builder_create_plaid(const int32_t* h_doclens, int64_t n_passages, int dim, int device,
+                                     int64_t pid_base, unsigned flags, int64_t window_bytes, int nbits,
+                                     const float* h_centroids, int64_t n_centroids, const float* h_bucket_weights,
+                                     flmr_corpus_builder_t** out) {
+  if (window_bytes < kDim * 2) {
+    if (out) *out = nullptr;
+    return fail(FLMR_ERR_INVALID_ARG, "window_bytes=%lld holds no row", (long long)window_bytes);
+  }
+  const PlaidCodec codec{nbits, h_centroids, n_centroids, h_bucket_weights};
+  return builder_create(h_doclens, n_passages, dim, device, pid_base, flags, window_bytes, out, &codec);
+}
+
+int flmr_corpus_builder_append_plaid(flmr_corpus_builder_t* b, const int32_t* h_codes, const uint8_t* h_residuals,
+                                     int64_t n_rows) {
+  if (!b || !h_codes || !h_residuals) return fail(FLMR_ERR_INVALID_ARG, "null argument");
+  flmr_corpus* c = b->corpus;
+  if (!c->codec_nbits)
+    return fail(FLMR_ERR_INVALID_ARG, "flmr_corpus_builder_append_plaid feeds the builder of a PLAID-coded corpus only");
+  if (n_rows < 0 || b->rows_done + n_rows > c->n_tokens)
+    return fail(FLMR_ERR_INVALID_ARG, "append of %lld rows overruns the %lld rows the doclens announce (%lld done)",
+                (long long)n_rows, (long long)c->n_tokens, (long long)b->rows_done);
+  for (int64_t i = 0; i < n_rows; ++i)   // every code, before any row is stored: a search never checks them
+    if (h_codes[i] < 0 || h_codes[i] >= c->n_centroids)
+      return fail(FLMR_ERR_INVALID_ARG, "code %d of row %lld is outside [0, %lld)", h_codes[i],
+                  (long long)(b->rows_done + i), (long long)c->n_centroids);
+  timespec t0, t1;
+  clock_gettime(CLOCK_MONOTONIC, &t0);
+  host_scatter_rows(reinterpret_cast<const char*>(h_codes), b->soff, b->poff, b->rows_done, n_rows,
+                    reinterpret_cast<char*>(c->h_codes), 4);
+  host_scatter_rows(reinterpret_cast<const char*>(h_residuals), b->soff, b->poff, b->rows_done, n_rows,
+                    reinterpret_cast<char*>(c->h_residuals), kDim * c->codec_nbits / 8);
+  clock_gettime(CLOCK_MONOTONIC, &t1);
+  b->fill_s += (t1.tv_sec - t0.tv_sec) + 1e-9 * (t1.tv_nsec - t0.tv_nsec);
+  b->rows_done += n_rows;
+  return FLMR_OK;
+}
+
 extern "C++" {
 namespace {
 // Feed `n_rows` packed rows through the staging ring; `fill(dst, row0, rows)` writes rows [row0, row0 + rows) of
@@ -2477,6 +2669,8 @@ namespace {
 template <typename Fill>
 int builder_feed(flmr_corpus_builder* b, int64_t n_rows, Fill fill) {
   flmr_corpus* c = b->corpus;
+  if (c->codec_nbits)
+    return fail(FLMR_ERR_INVALID_ARG, "the builder of a PLAID-coded corpus takes flmr_corpus_builder_append_plaid");
   if (n_rows < 0 || b->rows_done + n_rows > c->n_tokens)
     return fail(FLMR_ERR_INVALID_ARG, "append of %lld rows overruns the %lld rows the doclens announce (%lld done)",
                 (long long)n_rows, (long long)c->n_tokens, (long long)b->rows_done);
@@ -2580,6 +2774,18 @@ int flmr_corpus_builder_finish(flmr_corpus_builder_t* b, flmr_corpus_t** out, do
   DeviceGuard guard(c->device);
   if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", c->device);
   if (b->stream) FLMR_CUDA(cudaStreamSynchronize(b->stream));   // a streamed load wrote the host matrix itself
+  if (c->codec_nbits && !c->d_centroids) {   // a PLAID-coded corpus: its codec tables go to HBM
+    int64_t bytes = 0;
+    int rc = dev_upload(&c->d_centroids, b->centroids, &bytes);
+    if (!rc) rc = dev_upload(&c->d_bucket_weights, b->bucket_weights, &bytes);
+    if (rc) {
+      cudaFree(c->d_centroids);
+      cudaFree(c->d_bucket_weights);
+      c->d_centroids = c->d_bucket_weights = nullptr;
+      return rc;
+    }
+    c->codec_hbm_bytes = bytes;
+  }
   if (int rc = build_layout(c, c->d_tokens, c->n_rows, b->poff, b->doclens.data(), &c->layout)) return rc;
   if (host_fill_seconds) *host_fill_seconds = b->fill_s;
   b->corpus = nullptr;     // ownership passes to the caller
@@ -2954,13 +3160,20 @@ int flmr_workspace_create(const flmr_corpus_t* c, int max_queries, int max_nq,
                        // window's end are finite), their tensor maps, the copy stream and its events
     const size_t wbytes = static_cast<size_t>(c->layout.window_rows) * kDim * 2;
     const int n_bufs = c->layout.windows.size() > 1 ? 2 : 1;
+    // a PLAID-coded corpus: one decoded window buffer, and n_bufs staging buffers of compressed rows
+    const bool coded = c->codec_nbits > 0;
+    const size_t sbytes = coded ? static_cast<size_t>(c->layout.window_rows * codec_row_bytes(c->codec_nbits)) : 0;
     for (int i = 0; i < n_bufs; ++i) {
-      if ((e = cudaMalloc(reinterpret_cast<void**>(&ws->d_win[i]), wbytes)) != cudaSuccess ||
-          (e = cudaMemset(ws->d_win[i], 0, wbytes)) != cudaSuccess ||
+      const bool win_buf = !coded || i == 0;
+      if ((win_buf && (e = cudaMalloc(reinterpret_cast<void**>(&ws->d_win[i]), wbytes)) != cudaSuccess) ||
+          (win_buf && (e = cudaMemset(ws->d_win[i], 0, wbytes)) != cudaSuccess) ||
+          (coded && (e = cudaMalloc(reinterpret_cast<void**>(&ws->d_cstage[i]), sbytes)) != cudaSuccess) ||
+          (coded && (e = cudaEventCreateWithFlags(&ws->decoded_ev[i], cudaEventDisableTiming)) != cudaSuccess) ||
           (e = cudaEventCreateWithFlags(&ws->copied_ev[i], cudaEventDisableTiming)) != cudaSuccess ||
           (e = cudaEventCreateWithFlags(&ws->scanned_ev[i], cudaEventDisableTiming)) != cudaSuccess)
         return bail(fail(e == cudaErrorMemoryAllocation ? FLMR_ERR_OOM : FLMR_ERR_CUDA,
                          "window buffers: %s", cudaGetErrorString(e)));
+      if (!win_buf) continue;
       if (int rc = encode_rows_map(&ws->tmap_win[i], ws->d_win[i], static_cast<uint64_t>(c->layout.window_rows),
                                    kTileN, c->elem))
         return bail(rc);
@@ -2993,8 +3206,10 @@ int flmr_workspace_destroy(flmr_workspace_t* ws) {
   if (ws->copy_stream) cudaStreamSynchronize(ws->copy_stream);
   for (int i = 0; i < 2; ++i) {
     cudaFree(ws->d_win[i]);   // waits for the scans still reading it
+    cudaFree(ws->d_cstage[i]);
     if (ws->copied_ev[i]) cudaEventDestroy(ws->copied_ev[i]);
     if (ws->scanned_ev[i]) cudaEventDestroy(ws->scanned_ev[i]);
+    if (ws->decoded_ev[i]) cudaEventDestroy(ws->decoded_ev[i]);
   }
   if (ws->fork_ev) cudaEventDestroy(ws->fork_ev);
   if (ws->copy_stream) cudaStreamDestroy(ws->copy_stream);
@@ -3261,6 +3476,16 @@ int flmr_corpus_gather(const flmr_corpus_t* c, const int64_t* d_pids, int64_t n_
     FLMR_CUDA(cudaGetLastError());
     ++g_launches;
     d_pids = slot_ids;
+  }
+  if (c->codec_nbits) {   // a PLAID-coded corpus: decoded from its mapped host arrays
+    auto* kernel = c->elem == Elem::kF16 ? flmr_plaid_gather_kernel<true> : flmr_plaid_gather_kernel<false>;
+    kernel<<<static_cast<unsigned>(blocks), threads, 0, st>>>(
+        c->d_codes, c->d_residuals, c->d_centroids, c->d_bucket_weights, c->codec_nbits, c->layout.d_poff,
+        c->layout.d_doclen, c->d_dead, d_pids, n_pids, nd_max, slots(c), c->pid_base, static_cast<uint2*>(d_out_bf16),
+        d_mask);
+    FLMR_CUDA(cudaGetLastError());
+    ++g_launches;
+    return FLMR_OK;
   }
   flmr_gather_kernel<<<static_cast<unsigned>(blocks), threads, 0, st>>>(
       reinterpret_cast<const uint2*>(c->d_tokens), c->layout.d_poff, c->layout.d_doclen, c->d_dead, d_pids, n_pids,
@@ -3544,6 +3769,7 @@ int flmr_maxsim_backward_grouped_fp16(const void* d_q, int n_queries, int nq, co
 int flmr_debug_maxsim_scores_simt(const flmr_corpus_t* c, const void* d_q, int n_queries, int nq,
                                   unsigned flags, float* d_out_scores, void* stream) {
   if (!c || !d_q || !d_out_scores) return fail(FLMR_ERR_INVALID_ARG, "null argument");
+  if (c->codec_nbits) return fail(FLMR_ERR_UNSUPPORTED, "a PLAID-coded corpus holds no rows for the SIMT kernel");
   if (n_queries <= 0 || nq <= 0) return fail(FLMR_ERR_INVALID_ARG, "bad shape");
   if (c->n_passages > 0x7fffffffll || n_queries > 65535)
     return fail(FLMR_ERR_UNSUPPORTED, "SIMT cross-check grid too large");

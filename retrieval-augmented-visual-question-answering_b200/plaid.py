@@ -68,12 +68,19 @@ def _plaid_pieces(path: str, device, passage_range: Optional[Tuple[int, int]]):
     device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     if device.index is None:
         device = torch.device("cuda", torch.cuda.current_device())
+    meta, centroids, weights, pieces = _plaid_plan(path, passage_range)
+    return device, meta, centroids.to(device), weights.to(device), pieces
+
+
+def _plaid_plan(path: str, passage_range: Optional[Tuple[int, int]]):
+    """(metadata, centroids and bucket weights as fp32 CPU tensors, the pieces of ``_plaid_pieces``) of the passages
+    ``[p0, p1)`` of a PLAID index."""
     meta = read_plaid_metadata(path)
     if meta["dim"] != _cabi.DIM:
         raise ValueError("dim=%d (only %d is supported)" % (meta["dim"], _cabi.DIM))
-    centroids = torch.load(os.path.join(path, "centroids.pt"), map_location="cpu").float().to(device).contiguous()
+    centroids = torch.load(os.path.join(path, "centroids.pt"), map_location="cpu").float().contiguous()
     _cutoffs, weights = torch.load(os.path.join(path, "buckets.pt"), map_location="cpu")
-    weights = weights.float().to(device).contiguous()
+    weights = weights.float().contiguous()
     chunk_doclens = read_plaid_doclens(path, meta["num_chunks"])
     n_total = int(sum(len(d) for d in chunk_doclens))
     p0, p1 = (0, n_total) if passage_range is None else passage_range
@@ -87,7 +94,7 @@ def _plaid_pieces(path: str, device, passage_range: Optional[Tuple[int, int]]):
             off = np.concatenate([[0], np.cumsum(dl)])
             pieces.append((c, int(off[a]), int(off[b]), dl[a:b], int(off[-1])))
         c0 += len(dl)
-    return device, meta, centroids, weights, pieces
+    return meta, centroids, weights, pieces
 
 
 def _load_piece(path: str, c: int, n_chunk: int):
@@ -140,3 +147,22 @@ def plaid_to_host_chunks(path: str, device=None, passage_range: Optional[Tuple[i
                 decode_chunk(codes[a:b], residuals[a:b], centroids, weights, meta["nbits"], out)
                 yield out.cpu()
     return device, _piece_doclens(pieces), steps()
+
+
+def plaid_compressed_chunks(path: str, passage_range: Optional[Tuple[int, int]] = None):
+    """The compressed form of the passages ``[p0, p1)`` of a PLAID index, read on the host with nothing decoded:
+    (nbits, centroids fp32 ``[K, 128]``, bucket weights fp32 ``[2^nbits]``, doclens int32, an iterator of
+    (codes int32 ``[n]``, residuals uint8 ``[n, 16 nbits]``) CPU tensors, one per chunk the range overlaps, that
+    concatenate to the range's packed token rows)."""
+    meta, centroids, weights, pieces = _plaid_plan(path, passage_range)
+    nbits = meta["nbits"]
+
+    def steps():
+        for c, r0, r1, _, n_chunk in pieces:
+            codes, residuals = _load_piece(path, c, n_chunk)
+            codes = codes[r0:r1].to(torch.int32).contiguous()
+            residuals = residuals[r0:r1].to(torch.uint8).contiguous()
+            if residuals.shape != (r1 - r0, _cabi.DIM * nbits // 8):
+                raise ValueError("chunk %d: residuals of shape %s for nbits=%d" % (c, tuple(residuals.shape), nbits))
+            yield codes, residuals
+    return nbits, centroids, weights, _piece_doclens(pieces), steps()

@@ -30,7 +30,10 @@ call copies the corpus once, so on a streamed corpus an unrestricted top-k searc
 one call, and searches with per-query score rows or bitmaps (``filter_fn``, k > 128, ``pids=`` / ``qid_to_pids=``)
 take as many queries per call as keep that scratch within ``STREAMED_SCRATCH_BYTES``.  ``residency`` and
 ``window_bytes`` choose how an index path is loaded; with a ``FlatCorpus`` given, a ``residency`` other than its own
-and any ``window_bytes`` are refused.
+and any ``window_bytes`` are refused.  ``compressed=True`` (with ``residency="host"``, on a PLAID index path) keeps the
+index in its compressed form, a centroid code and a packed residual per token, and decodes each window on the GPU
+before the scan (``FlatCorpus.from_plaid``); results stay bitwise those of the decoded corpus.  With a ``FlatCorpus``
+given, a ``compressed`` that disagrees with it is refused.
 
 ``storage="fp8"`` keeps the corpus as e4m3 in HBM (half the bytes; the exact bf16 rows stay in pinned host memory)
 and searches in two stages, as PLAID does (colbert/search/index_storage.py:160-177): the exhaustive e4m3 scan
@@ -221,7 +224,8 @@ class Searcher:
                  disable_gpu: bool = True, device: Optional[Union[int, torch.device]] = None,
                  encode_fn: Optional[Callable] = None, index_root: Optional[str] = None,
                  query_batch: int = 64, shard_across_ranks: bool = False, group=None,
-                 storage: Optional[str] = None, residency: Optional[str] = None, window_bytes: Optional[int] = None):
+                 storage: Optional[str] = None, residency: Optional[str] = None, window_bytes: Optional[int] = None,
+                 compressed: Optional[bool] = None):
         # `disable_gpu` is part of the reference signature (default True) but dead there: colbert/searcher.py:23
         # never reads it, the device is chosen by config.total_visible_gpus (:40-43), which FLMR_executor.py:778-781
         # zeroes under DDP to force CPU search.  Here the search always runs on the GPU (no CPU path exists);
@@ -244,6 +248,9 @@ class Searcher:
             if window_bytes is not None:
                 raise ValueError("window_bytes applies to an index path opened with residency='host'; the corpus given "
                                  "was created with its own")
+            if compressed is not None and bool(compressed) != (index.codec_nbits > 0):
+                raise ValueError("compressed=%r, but the corpus given %s a PLAID-coded corpus"
+                                 % (compressed, "is" if index.codec_nbits else "is not"))
             self.corpus = index
             self.index = None
             self.index_kind = "resident"
@@ -267,6 +274,11 @@ class Searcher:
                 extra["residency"] = residency
                 if window_bytes is not None:
                     extra["window_bytes"] = window_bytes
+            if compressed:   # a PLAID index kept in its compressed form (FlatCorpus.from_plaid compressed=True)
+                if self.index_kind != "plaid":
+                    raise ValueError("compressed=True streams a PLAID index's compressed form; %s is a flat index"
+                                     % self.index)
+                extra["compressed"] = True
             self.corpus = load(self.index, device=device, rank=rank, world_size=world, **extra)
         self.storage = getattr(self.corpus, "storage", None) or storage or "bf16"
         # every rank of a sharded Searcher gets the same residency argument, so ranks without a shard batch their
