@@ -53,6 +53,11 @@
  *       a streamed corpus kept in a PLAID index's compressed form (centroid codes and packed residuals) and decoded
  *       window by window on the GPU before the scan: 20 to 132 B of pinned host memory and PCIe traffic per token
  *       instead of 256.
+ *   flmr_plaid_encode
+ *       writes a PLAID index's codes and packed residuals: replaces ResidualCodec.compress_into_codes and compress
+ *       (CB/indexing/codecs/residual.py:169-222), which materialise a [K, batch] score matrix and an [n, dim]
+ *       residual matrix in HBM, by one wgmma kernel that keeps both in registers; its assignment-only mode is the
+ *       assignment step of the k-means the Python Indexer runs instead of faiss.
  *   flmr_debug_maxsim_scores_simt
  *       test infrastructure: an independent plain-SIMT fp32 device kernel used by tests to
  *       cross-check the tensor-core kernel at sizes where the CPU oracle is too slow.
@@ -67,7 +72,7 @@
  *     header needs no CUDA include; NULL = default stream);
  *   - CUDA graph capture: flmr_maxsim_scores, flmr_maxsim_topk and their _allowed forms (every storage, compacted
  *     corpora included), flmr_topk_select, flmr_topk_merge, flmr_corpus_gather, flmr_maxsim_argmax /
- *     flmr_maxsim_backward with their _grouped and _fp16 forms (either arg-max kernel) and flmr_ib_loss may be captured
+ *     flmr_maxsim_backward with their _grouped and _fp16 forms (either arg-max kernel) and flmr_ib_loss and flmr_plaid_encode may be captured
  *     on the stream they are given and replayed with new contents in the same buffers, once a call of the same shape
  *     has run outside the capture on the same workspace (it sizes the workspace's buffers), and while the corpus does
  *     not change.  The _listed calls are not capturable: their host offsets size the plan when the call is made, and
@@ -486,6 +491,27 @@ int flmr_plaid_decode(const int32_t* d_codes, const uint8_t* d_residuals, int64_
 int flmr_plaid_decode_fp16(const int32_t* d_codes, const uint8_t* d_residuals, int64_t n_tokens,
                            const float* d_centroids, int64_t n_centroids, const float* d_bucket_weights,
                            int nbits, int dim, int normalize, void* d_out_fp16, int device, void* stream);
+
+/*
+ * Encode token embeddings against PLAID centroids: what ResidualCodec.compress computes (CB/indexing/codecs/
+ * residual.py:169-222), with neither its score matrix nor its residual matrix ever written.  Asynchronous on `stream`,
+ * no host synchronisation, capturable in a CUDA graph.
+ *   d_x          fp16  [n, 128]              token embeddings (16-byte aligned)
+ *   d_centroids  fp16  [K, 128]              (centroids.pt; 16-byte aligned)
+ *   d_cutoffs    fp32  [2^nbits - 1]         non-decreasing bucket cutoffs (buckets.pt[0]); NULL when d_residuals is
+ *   d_codes      int32 [n]                   argmax_c <x_t, C_c>, fp32 accumulation, the lowest c on exact ties
+ *   d_residuals  uint8 [n, 16 * nbits]       or NULL (assignment only; 4-byte aligned): with r = fp16(float(x_t) -
+ *                                            float(C_code)) per dim and bucket = #{j : cutoffs[j] < float(r)}, bit j
+ *                                            of dim d's bucket is element d * nbits + j of the row's bit string,
+ *                                            packed MSB-first (np.packbits): flmr_plaid_decode (normalize = 0) of
+ *                                            the output is C_code + bucket_weights[bucket] exactly
+ *   d_best       fp32  [n]                   the winning score, or NULL
+ * Refused before any CUDA call: a null d_x / d_centroids / d_codes, or d_residuals without d_cutoffs, nbits not in
+ * {1, 2, 4, 8}, K < 1, n < 0 and misaligned pointers (FLMR_ERR_INVALID_ARG); n >= 2^31 - 256 (FLMR_ERR_UNSUPPORTED).
+ * n == 0 does nothing.
+ */
+int flmr_plaid_encode(const void* d_x, int64_t n, const void* d_centroids, int K, const float* d_cutoffs, int nbits,
+                      int32_t* d_codes, uint8_t* d_residuals, float* d_best, int device, void* stream);
 
 /*
  * Gather retrieved passages out of the resident corpus into a padded batch — the operand of the RAG

@@ -34,6 +34,7 @@
 #include "flmr_scan_kernel.cuh"
 #include "flmr_train_kernels.cuh"
 #include "flmr_train_tc_kernel.cuh"
+#include "flmr_plaid_encode_kernel.cuh"
 
 namespace {
 
@@ -3438,6 +3439,54 @@ int flmr_plaid_decode_fp16(const int32_t* d_codes, const uint8_t* d_residuals, i
                            int nbits, int dim, int normalize, void* d_out_fp16, int device, void* stream) {
   return plaid_decode<true>(d_codes, d_residuals, n_tokens, d_centroids, n_centroids, d_bucket_weights, nbits, dim,
                             normalize, d_out_fp16, device, stream);
+}
+
+// PLAID encode (flmr_plaid_encode_kernel.cuh): one persistent CTA per SM over 256-row token tiles, nothing
+// synchronised, so the call can be captured in a CUDA graph.
+int flmr_plaid_encode(const void* d_x, int64_t n, const void* d_centroids, int K, const float* d_cutoffs, int nbits,
+                      int32_t* d_codes, uint8_t* d_residuals, float* d_best, int device, void* stream) {
+  if (!d_x || !d_centroids || !d_codes || (d_residuals && !d_cutoffs)) return fail(FLMR_ERR_INVALID_ARG, "null pointer");
+  if (nbits != 1 && nbits != 2 && nbits != 4 && nbits != 8)
+    return fail(FLMR_ERR_INVALID_ARG, "nbits=%d (the PLAID codec packs 1, 2, 4 or 8 bits per dim)", nbits);
+  if (K < 1) return fail(FLMR_ERR_INVALID_ARG, "K=%d: at least one centroid is needed", K);
+  if (n < 0) return fail(FLMR_ERR_INVALID_ARG, "n=%lld", (long long)n);
+  if ((reinterpret_cast<uintptr_t>(d_x) | reinterpret_cast<uintptr_t>(d_centroids)) & 15u)
+    return fail(FLMR_ERR_INVALID_ARG, "d_x and d_centroids must be 16-byte aligned");
+  if (d_residuals && (reinterpret_cast<uintptr_t>(d_residuals) & 3u))
+    return fail(FLMR_ERR_INVALID_ARG, "d_residuals must be 4-byte aligned");
+  if (n == 0) return FLMR_OK;
+  if (n + kEncRows >= (1ll << 31)) return fail(FLMR_ERR_UNSUPPORTED, "n=%lld tokens: split the call below 2^31", (long long)n);
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
+  CUtensorMap tmap_x, tmap_c;
+  if (int rc = encode_rows_map(&tmap_x, d_x, static_cast<uint64_t>(n), 128, Elem::kF16)) return rc;
+  if (int rc = encode_rows_map(&tmap_c, d_centroids, static_cast<uint64_t>(K), kEncTileC, Elem::kF16)) return rc;
+  static std::once_flag attr_once[64];
+  cudaError_t attr_err = cudaSuccess;
+  std::call_once(attr_once[device & 63], [&]() {
+    attr_err = cudaFuncSetAttribute(flmr_plaid_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kEncSmemBytes);
+  });
+  if (attr_err != cudaSuccess)
+    return fail(FLMR_ERR_CUDA, "cannot raise the dynamic shared memory limit: %s", cudaGetErrorString(attr_err));
+  int sms = 0;
+  FLMR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  PlaidEncodeParams prm{};
+  prm.centroids = static_cast<const __half*>(d_centroids);
+  prm.cutoffs = d_cutoffs;
+  prm.codes = d_codes;
+  prm.residuals = d_residuals;
+  prm.best = d_best;
+  prm.n = n;
+  prm.K = K;
+  prm.nbits = nbits;
+  prm.n_tiles = static_cast<int32_t>((n + kEncRows - 1) / kEncRows);
+  prm.status = nullptr;
+  const unsigned grid = static_cast<unsigned>(std::min<int64_t>(prm.n_tiles, sms));
+  flmr_plaid_encode_kernel<<<grid, kEncThreads, kEncSmemBytes, static_cast<cudaStream_t>(stream)>>>(tmap_x, tmap_c, prm);
+  cudaError_t e = cudaGetLastError();
+  ++g_launches;
+  if (e != cudaSuccess) return fail(FLMR_ERR_CUDA, "flmr_plaid_encode_kernel launch failed: %s", cudaGetErrorString(e));
+  return FLMR_OK;
 }
 
 int flmr_topk_select(const float* d_scores, int n_queries, int64_t n, int k, int64_t pid_base,

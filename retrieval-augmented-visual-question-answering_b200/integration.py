@@ -20,6 +20,8 @@ What is replaced (reference -> here):
 
     colbert.Indexer (opt-in: ``patch_colbert(indexer=True)``)            -> ravqa_b200.Indexer
         (indexer.py:16-84, caller FLMR_executor.py:601-617: flat bf16 store instead of the PLAID build)
+    colbert.Indexer (opt-in: ``patch_colbert(indexer="plaid")``)         -> ravqa_b200.indexer.PlaidIndexer
+        (the same call lines write a PLAID directory, built on the GPU: k-means, codes, residuals and IVF)
 
 Nothing of the reference is modified on disk; ``unpatch_colbert()`` restores the originals.  Encoders, data
 pipeline, executors and (unless opted out of as above) the PLAID index *build* stay the reference's own.
@@ -99,7 +101,7 @@ def _rebind_everywhere(old, new) -> int:
     return n
 
 
-def patch_colbert(searcher: bool = True, scoring: bool = True, ib_loss: bool = True, indexer: bool = False
+def patch_colbert(searcher: bool = True, scoring: bool = True, ib_loss: bool = True, indexer=False
                   ) -> Dict[str, int]:
     """Install the replacements listed in the module docstring into the loaded ``colbert`` package (imports it
     if needed: ``third_party/ColBERT`` must be on ``sys.path`` as the reference arranges).  Returns how many
@@ -108,16 +110,21 @@ def patch_colbert(searcher: bool = True, scoring: bool = True, ib_loss: bool = T
     ``indexer=True`` (opt-in) also replaces ``colbert.Indexer`` (indexer.py:16, called at FLMR_executor.py:601-617)
     by ``ravqa_b200.Indexer``: same constructor and ``index(name, collection, overwrite)``, the reference's own
     ``Checkpoint`` as document encoder, but the embeddings are stored flat in bf16 — no k-means, residual codec or
-    IVF — where the reference would put its PLAID directory; ``Searcher`` opens either kind."""
+    IVF — where the reference would put its PLAID directory; ``Searcher`` opens either kind.  ``indexer="plaid"``
+    replaces it by ``indexer.PlaidIndexer`` instead, which writes the PLAID directory itself (``nbits`` from the
+    config the executor passes), built on the GPU."""
     import colbert                                      # noqa: F401  (the reference's vendored package)
     import colbert.modeling.colbert as M
     import colbert.searcher as S
     done: Dict[str, int] = {}
+    if indexer not in (False, True, "plaid"):
+        raise ValueError("patch_colbert(indexer=...) takes False, True (flat store) or 'plaid', got %r" % (indexer,))
     if indexer:
         import colbert.indexer as IX
-        from .indexer import Indexer
-        if IX.Indexer is not Indexer:
-            done["Indexer"] = _rebind_everywhere(IX.Indexer, Indexer)
+        from .indexer import Indexer, PlaidIndexer
+        ours = PlaidIndexer if indexer == "plaid" else Indexer
+        if IX.Indexer is not ours:
+            done["Indexer"] = _rebind_everywhere(IX.Indexer, ours)
     if searcher and S.Searcher is not Searcher:
         done["Searcher"] = _rebind_everywhere(S.Searcher, Searcher)
     if scoring:
