@@ -23,6 +23,9 @@
  *   flmr_topk_merge
  *       the only exchange step of the sharded path (SURVEY.md §8e): merges per-shard top-k lists
  *       (gathered by the host with one NCCL all-gather) into the global top-k.
+ *   flmr_topk_merge_devices
+ *       the same exchange for shards one process holds on several devices: the merge kernel reads every shard's
+ *       lists on the home device, through peer access, with no collective and no host synchronisation.
  *   FLMR_CORPUS_FP8, flmr_corpus_storage
  *       an e4m3 corpus: the scan reads half the bytes per token and runs fp8 MMAs, so its scores are
  *       APPROXIMATE; the exact bf16 rows stay in pinned host memory for flmr_corpus_gather.  The first stage of
@@ -430,6 +433,24 @@ int flmr_topk_merge(const float* d_in_scores, const int64_t* d_in_pids, int n_li
                     void* stream);
 
 /*
+ * The exchange of shards held by ONE process on several devices: merge lists that live on different devices into
+ * one top-k on the device of `stream` (the home device), in flmr_topk_merge's order (score descending, then the lower
+ * pid on exact ties; pid < 0 marks an empty entry; short results end in (-inf, -1)).
+ *   d_scores[i] fp32 / d_pids[i] int64 [n_queries, k_in]: list i, on device devices[i], written by work on
+ *   src_streams[i] (a cudaStream_t of devices[i]; NULL = that device's default stream)
+ *   d_out_*  [n_queries, k_out] on the home device; k_out <= FLMR_MAX_K, k_out <= n_lists * k_in,
+ *   n_lists * k_in <= 20480, n_lists <= 128 (FLMR_ERR_UNSUPPORTED above either)
+ * Asynchronous: an event recorded on each source stream is waited for on `stream`, and the host never waits.  One
+ * kernel on the home device reads each list where it lives: in place on the home device, through peer access where
+ * cudaDeviceCanAccessPeer allows it (enabled by the first call for each device pair), else after a
+ * cudaMemcpyPeerAsync into a stream-ordered staging buffer on the home device.  A device may hold several lists.
+ * Argument errors (null arrays or lists, the shapes above) are refused before any CUDA call.
+ */
+int flmr_topk_merge_devices(const float* const* d_scores, const int64_t* const* d_pids, const int* devices,
+                            void* const* src_streams, int n_lists, int n_queries, int k_in, int k_out,
+                            float* d_out_scores, int64_t* d_out_pids, void* stream);
+
+/*
  * The sharded search at the C boundary (SURVEY.md 8e; the reference has no counterpart: under DDP every rank
  * repeats the whole CPU search, src/executors/FLMR_executor.py:778-781).  Each rank holds a contiguous passage
  * shard (flmr_corpus_create with its pid_base); ONE exchange step — an NCCL all-gather of every rank's [B, k]
@@ -623,6 +644,12 @@ int flmr_debug_set_scan_variant(int variant);
  * size (the product behaviour), 1 = the warp-MMA kernel, 2 = the wgmma kernel, for bf16 and fp16 operands alike — so
  * tests can hold either against the other and the oracle at any shape. */
 int flmr_debug_set_argmax_path(int path);
+
+/* Test infrastructure: how flmr_topk_merge_devices reads its lists on the calling thread — 0 = in place or through
+ * peer access where the devices allow it (the product behaviour), 1 = every list copied into the home staging buffer
+ * first, those on the home device included — so tests reach the staged copy on a node whose devices all read each
+ * other. */
+int flmr_debug_set_merge_path(int path);
 
 /* Test infrastructure, host-only (no GPU needed): the token-balanced CTA partition + per-tile
  * passage-end metadata the scan kernel consumes, for `n_ctas` persistent CTAs and

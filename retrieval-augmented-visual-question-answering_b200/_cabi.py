@@ -49,9 +49,12 @@ STREAMED_SYMBOLS = ("flmr_corpus_create_streamed", "flmr_corpus_builder_create_s
 PLAID_STREAMED_SYMBOLS = ("flmr_corpus_builder_create_plaid", "flmr_corpus_builder_append_plaid", "flmr_corpus_codec")
 # the encode of a PLAID index build: nearest-centroid codes and packed residuals
 PLAID_ENCODE_SYMBOLS = ("flmr_plaid_encode",)
+# the merge of shards one process holds on several devices, read by the home device through peer access
+MULTI_DEVICE_SYMBOLS = ("flmr_topk_merge_devices", "flmr_debug_set_merge_path")
 # symbols an earlier revision's library may lack (tools/scan_ab.py drives one through this binding)
 OPTIONAL_SYMBOLS = (UPDATE_SYMBOLS + ALLOWED_SYMBOLS + FP16_SYMBOLS + FP16_TRAIN_SYMBOLS + COMPACT_SYMBOLS
-                    + LISTED_SYMBOLS + STREAMED_SYMBOLS + PLAID_STREAMED_SYMBOLS + PLAID_ENCODE_SYMBOLS)
+                    + LISTED_SYMBOLS + STREAMED_SYMBOLS + PLAID_STREAMED_SYMBOLS + PLAID_ENCODE_SYMBOLS
+                    + MULTI_DEVICE_SYMBOLS)
 # every symbol include/flmr_maxsim.h declares (tests check the .so exports all of them)
 SYMBOLS = [
     "flmr_last_error", "flmr_abi_version",
@@ -59,7 +62,7 @@ SYMBOLS = [
     *UPDATE_SYMBOLS, *COMPACT_SYMBOLS, *STREAMED_SYMBOLS, *PLAID_STREAMED_SYMBOLS,
     "flmr_workspace_create", "flmr_workspace_destroy", "flmr_workspace_status",
     "flmr_maxsim_scores", "flmr_maxsim_topk", "flmr_topk_merge", "flmr_topk_select", "flmr_plaid_decode",
-    *FP16_SYMBOLS, *PLAID_ENCODE_SYMBOLS,
+    *FP16_SYMBOLS, *PLAID_ENCODE_SYMBOLS, *MULTI_DEVICE_SYMBOLS,
     "flmr_maxsim_argmax", "flmr_maxsim_backward", "flmr_corpus_gather",
     "flmr_maxsim_argmax_grouped", "flmr_maxsim_backward_grouped", "flmr_ib_loss", *FP16_TRAIN_SYMBOLS,
     "flmr_corpus_builder_create", "flmr_corpus_builder_create_ex", "flmr_corpus_builder_append", "flmr_corpus_builder_append_file",
@@ -141,6 +144,9 @@ def lib() -> C.CDLL:
     L.flmr_maxsim_topk.argtypes = [vp, vp, vp, i32, i32, i32, u32, vp, vp, vp]
     L.flmr_topk_merge.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, i32, vp]
     L.flmr_topk_select.argtypes = [vp, i32, i64, i32, i64, vp, vp, i32, vp]
+    if hasattr(L, "flmr_topk_merge_devices"):
+        L.flmr_topk_merge_devices.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp]
+        L.flmr_debug_set_merge_path.argtypes = [i32]
     L.flmr_plaid_decode.argtypes = [vp, vp, i64, vp, i64, vp, i32, i32, i32, vp, i32, vp]
     if hasattr(L, "flmr_plaid_decode_fp16"):
         L.flmr_plaid_decode_fp16.argtypes = [vp, vp, i64, vp, i64, vp, i32, i32, i32, vp, i32, vp]

@@ -959,6 +959,100 @@ flmr_merge_kernel(const uint64_t* __restrict__ keys, const float* __restrict__ i
   }
 }
 
+// The merge of flmr_topk_merge_devices: list l is its own [n_queries, k_in] array, read where it lives (on this device,
+// through peer access, or in the home staging buffer).  The pointer tables are kernel parameters (__grid_constant__), so
+// indexing them by list reads the parameter bank with no local copy.  Each candidate is read once: its ordered score
+// stays in a register and its pid goes to shared memory, where the selection reads it only to break an exact tie and to
+// publish a thread's best; so the selection order is flmr_merge_kernel's (score desc, pid asc), and the kernel holds
+// kMergePer candidates per thread without spilling.
+constexpr int kMergeMaxLists = 128;
+struct MergeLists {
+  const float* scores[kMergeMaxLists];
+  const int64_t* pids[kMergeMaxLists];
+};
+
+__global__ void __launch_bounds__(kMergeThreads)
+flmr_merge_lists_kernel(const __grid_constant__ MergeLists lists, int n_lists, int k_in, int k_out,
+                        float* __restrict__ out_scores, int64_t* __restrict__ out_pids) {
+  extern __shared__ int64_t s_cand_pid[];   // [n_lists * k_in]
+  __shared__ uint32_t s_ord[32];
+  __shared__ int64_t s_pid[32];
+  __shared__ uint32_t w_ord;
+  __shared__ int64_t w_pid;
+  const int b = blockIdx.x;
+  const int n = n_lists * k_in;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint32_t ord[kMergePer];   // candidate threadIdx.x + i * kMergeThreads; 0 = empty
+#pragma unroll
+  for (int i = 0; i < kMergePer; ++i) {
+    const int idx = threadIdx.x + i * kMergeThreads;
+    ord[i] = 0u;
+    if (idx < n) {
+      const int l = idx / k_in;
+      const int64_t g = static_cast<int64_t>(b) * k_in + (idx - l * k_in);
+      const int64_t pid = lists.pids[l][g];
+      s_cand_pid[idx] = pid;
+      if (pid >= 0) ord[i] = float_to_ordered(lists.scores[l][g] + 0.0f);   // -0 -> +0, as in flmr_merge_kernel
+    }
+  }
+  __syncthreads();
+  for (int r = 0; r < k_out; ++r) {
+    Cand best;
+    best.ord = 0u;
+    best.pid = kPidEmpty;
+#pragma unroll
+    for (int i = 0; i < kMergePer; ++i) {
+      if (ord[i] != 0u && ord[i] >= best.ord) {
+        const int64_t pid = s_cand_pid[threadIdx.x + i * kMergeThreads];
+        if (ord[i] > best.ord || pid < best.pid) {
+          best.ord = ord[i];
+          best.pid = pid;
+        }
+      }
+    }
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) {
+      Cand o;
+      o.ord = __shfl_xor_sync(0xffffffffu, best.ord, off);
+      o.pid = __shfl_xor_sync(0xffffffffu, best.pid, off);
+      if (cand_better(o, best)) best = o;
+    }
+    if (lane == 0) {
+      s_ord[warp] = best.ord;
+      s_pid[warp] = best.pid;
+    }
+    __syncthreads();
+    if (warp == 0) {
+      Cand x;
+      x.ord = s_ord[lane];
+      x.pid = s_pid[lane];
+#pragma unroll
+      for (int off = 16; off >= 1; off >>= 1) {
+        Cand o;
+        o.ord = __shfl_xor_sync(0xffffffffu, x.ord, off);
+        o.pid = __shfl_xor_sync(0xffffffffu, x.pid, off);
+        if (cand_better(o, x)) x = o;
+      }
+      if (lane == 0) {
+        w_ord = x.ord;
+        w_pid = x.pid;
+        const bool empty = (x.ord == 0u);
+        out_scores[static_cast<int64_t>(b) * k_out + r] = empty ? -INFINITY : ordered_to_float(x.ord);
+        out_pids[static_cast<int64_t>(b) * k_out + r] = empty ? -1 : x.pid;
+      }
+    }
+    __syncthreads();
+    const uint32_t wo = w_ord;
+    const int64_t wp = w_pid;
+    if (wo != 0u) {   // every copy of the winner leaves, as in flmr_merge_kernel
+#pragma unroll
+      for (int i = 0; i < kMergePer; ++i)
+        if (ord[i] == wo && s_cand_pid[threadIdx.x + i * kMergeThreads] == wp) ord[i] = 0u;
+    }
+    // (w_ord/w_pid are rewritten only after the next round's first __syncthreads)
+  }
+}
+
 // Top-k selection over a dense score row for k beyond the fused capacity (SURVEY 8a a10:
 // Searcher.dense_search accepts any k).  One 1024-thread block per query:
 //   1. 4-pass MSB radix select (8 bits per pass, 256-bin histogram in shared memory) over the
@@ -3380,6 +3474,142 @@ int flmr_topk_merge(const float* d_in_scores, const int64_t* d_in_pids, int n_li
       nullptr, d_in_scores, d_in_pids, n_lists, n_queries, k_in, k_out, 0, nullptr, d_out_scores, d_out_pids, 0);
   FLMR_CUDA(cudaGetLastError());
   ++g_launches;
+  return FLMR_OK;
+}
+
+extern "C++" {
+namespace {
+thread_local int g_merge_path = 0;   // 0 = by peer capability, 1 = stage every list (flmr_debug_set_merge_path)
+
+// How the home device reads lists on `peer`: 1 through peer access (enabled here the first time), 0 through a staged
+// copy.  Decided once per ordered device pair for the process, under a lock.
+int peer_readable(int home, int peer, int n_dev, bool* out) {
+  static std::mutex mu;
+  static std::vector<signed char> state;   // [home * n_dev + peer]: -1 undecided, 0 staged, 1 peer reads
+  std::lock_guard<std::mutex> lock(mu);
+  if (state.size() < static_cast<size_t>(n_dev) * n_dev) state.assign(static_cast<size_t>(n_dev) * n_dev, -1);
+  signed char& s = state[static_cast<size_t>(home) * n_dev + peer];
+  if (s < 0) {
+    int can = 0;
+    FLMR_CUDA(cudaDeviceCanAccessPeer(&can, home, peer));
+    if (can) {
+      DeviceGuard guard(home);
+      if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", home);
+      const cudaError_t e = cudaDeviceEnablePeerAccess(peer, 0);
+      if (e == cudaErrorPeerAccessAlreadyEnabled) {
+        cudaGetLastError();   // enabled earlier by someone else in this process: not an error, and not left behind
+      } else if (e != cudaSuccess) {
+        return fail(FLMR_ERR_CUDA, "cudaDeviceEnablePeerAccess(%d -> %d) failed: %s", home, peer, cudaGetErrorString(e));
+      }
+    }
+    s = can ? 1 : 0;
+  }
+  *out = s == 1;
+  return FLMR_OK;
+}
+
+// One event per device and host thread, recorded on a source stream and waited for at once, so one suffices.
+int device_event(int device, cudaEvent_t* out) {
+  thread_local std::vector<cudaEvent_t> events;
+  if (events.size() <= static_cast<size_t>(device)) events.resize(device + 1, nullptr);
+  if (!events[device]) {
+    DeviceGuard guard(device);
+    if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", device);
+    FLMR_CUDA(cudaEventCreateWithFlags(&events[device], cudaEventDisableTiming));
+  }
+  *out = events[device];
+  return FLMR_OK;
+}
+}  // namespace
+}  // extern "C++"
+
+int flmr_topk_merge_devices(const float* const* d_scores, const int64_t* const* d_pids, const int* devices,
+                            void* const* src_streams, int n_lists, int n_queries, int k_in, int k_out,
+                            float* d_out_scores, int64_t* d_out_pids, void* stream) {
+  if (!d_scores || !d_pids || !devices || !src_streams || !d_out_scores || !d_out_pids)
+    return fail(FLMR_ERR_INVALID_ARG, "null array or output pointer");
+  if (n_lists < 1 || n_queries < 0 || k_in < 1 || k_out < 1 || k_out > kMaxK)
+    return fail(FLMR_ERR_INVALID_ARG, "bad merge shape n_lists=%d n_queries=%d k_in=%d k_out=%d",
+                n_lists, n_queries, k_in, k_out);
+  if (static_cast<int64_t>(k_out) > static_cast<int64_t>(n_lists) * k_in)
+    return fail(FLMR_ERR_INVALID_ARG, "k_out=%d exceeds the n_lists*k_in = %lld entries merged", k_out,
+                (long long)n_lists * k_in);
+  if (n_lists > kMergeMaxLists)
+    return fail(FLMR_ERR_UNSUPPORTED, "n_lists=%d exceeds %d lists", n_lists, kMergeMaxLists);
+  if (static_cast<int64_t>(n_lists) * k_in > kMergeThreads * kMergePer)
+    return fail(FLMR_ERR_UNSUPPORTED, "n_lists*k_in = %lld exceeds merge capacity %d",
+                (long long)n_lists * k_in, kMergeThreads * kMergePer);
+  for (int i = 0; i < n_lists; ++i) {
+    if (!d_scores[i] || !d_pids[i]) return fail(FLMR_ERR_INVALID_ARG, "list %d is null", i);
+    if (devices[i] < 0) return fail(FLMR_ERR_INVALID_ARG, "list %d: device %d", i, devices[i]);
+  }
+  if (n_queries == 0) return FLMR_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int n_dev = 0, home = 0;
+  FLMR_CUDA(cudaGetDeviceCount(&n_dev));
+  for (int i = 0; i < n_lists; ++i)
+    if (devices[i] >= n_dev) return fail(FLMR_ERR_INVALID_ARG, "list %d: device %d of %d", i, devices[i], n_dev);
+  FLMR_CUDA(cudaStreamGetDevice(st, &home));
+  DeviceGuard guard(home);
+  if (!guard.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", home);
+  // the merge reads list i once src_streams[i] has produced it: its event, waited for on `stream`
+  for (int i = 0; i < n_lists; ++i) {
+    cudaStream_t src = static_cast<cudaStream_t>(src_streams[i]);
+    if (src == st && devices[i] == home) continue;
+    cudaEvent_t ev = nullptr;
+    if (int rc = device_event(devices[i], &ev)) return rc;
+    {
+      DeviceGuard on_src(devices[i]);
+      if (!on_src.ok) return fail(FLMR_ERR_CUDA, "cudaSetDevice(%d) failed", devices[i]);
+      FLMR_CUDA(cudaEventRecord(ev, src));
+    }
+    FLMR_CUDA(cudaStreamWaitEvent(st, ev, 0));
+  }
+  // lists on the home device are read in place, lists on a peer the home device can read through peer access;
+  // the others are copied into one stream-ordered staging buffer on the home device first
+  MergeLists lists;
+  std::vector<int> staged;
+  for (int i = 0; i < n_lists; ++i) {
+    lists.scores[i] = d_scores[i];
+    lists.pids[i] = d_pids[i];
+    bool direct = devices[i] == home;
+    if (!direct)
+      if (int rc = peer_readable(home, devices[i], n_dev, &direct)) return rc;
+    if (g_merge_path == 1 || !direct) staged.push_back(i);
+  }
+  const size_t list_elems = static_cast<size_t>(n_queries) * k_in;
+  char* stage = nullptr;
+  if (!staged.empty()) {
+    const size_t bytes = staged.size() * list_elems * (sizeof(float) + sizeof(int64_t));
+    FLMR_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&stage), bytes, st));
+    int64_t* sp = reinterpret_cast<int64_t*>(stage);
+    float* ss = reinterpret_cast<float*>(sp + staged.size() * list_elems);
+    for (size_t j = 0; j < staged.size(); ++j) {
+      const int i = staged[j];
+      FLMR_CUDA(cudaMemcpyPeerAsync(ss + j * list_elems, home, d_scores[i], devices[i], list_elems * sizeof(float), st));
+      FLMR_CUDA(cudaMemcpyPeerAsync(sp + j * list_elems, home, d_pids[i], devices[i], list_elems * sizeof(int64_t), st));
+      lists.scores[i] = ss + j * list_elems;
+      lists.pids[i] = sp + j * list_elems;
+    }
+  }
+  const size_t smem = static_cast<size_t>(n_lists) * k_in * sizeof(int64_t);   // the candidates' pids
+  cudaError_t launched = cudaFuncSetAttribute(flmr_merge_lists_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              static_cast<int>(smem));
+  if (launched == cudaSuccess) {
+    flmr_merge_lists_kernel<<<n_queries, kMergeThreads, smem, st>>>(lists, n_lists, k_in, k_out, d_out_scores,
+                                                                    d_out_pids);
+    launched = cudaGetLastError();
+  }
+  if (stage) FLMR_CUDA(cudaFreeAsync(stage, st));   // stream-ordered: released after the kernel has read it
+  if (launched != cudaSuccess) return fail(FLMR_ERR_CUDA, "merge launch failed: %s", cudaGetErrorString(launched));
+  ++g_launches;
+  return FLMR_OK;
+}
+
+int flmr_debug_set_merge_path(int path) {
+  if (path < 0 || path > 1)
+    return fail(FLMR_ERR_INVALID_ARG, "path must be 0 (by peer capability) or 1 (stage every list)");
+  g_merge_path = path;
   return FLMR_OK;
 }
 

@@ -35,6 +35,15 @@ index in its compressed form, a centroid code and a packed residual per token, a
 before the scan (``FlatCorpus.from_plaid``); results stay bitwise those of the decoded corpus.  With a ``FlatCorpus``
 given, a ``compressed`` that disagrees with it is refused.
 
+``devices=[0, 1, ...]`` (or ``"all"``, every visible device) holds the index in this one process as one token-balanced
+shard per device (``sharded.shard_ranges``; shard i loaded on ``devices[i]``, all shards at once, one host thread each),
+for a corpus larger than one card searched without a launcher or a process group.  Every search runs each shard's own
+top-k, as a one-device Searcher would on that shard, on a stream of the shard's device, and merges the lists on the
+home device ``devices[0]`` with one kernel that reads them over peer access (``flmr_topk_merge_devices``); results are
+those of the one-device Searcher and come back on the home device.  A device may hold several shards (``[0, 0]``).  It
+loads an index path only, resident (``residency="host"`` and ``compressed=True`` are refused), and excludes ``device=``
+and ``shard_across_ranks``.  ``corpus`` is the first shard, ``shards`` lists them all.
+
 ``storage="fp8"`` keeps the corpus as e4m3 in HBM (half the bytes; the exact bf16 rows stay in pinned host memory)
 and searches in two stages, as PLAID does (colbert/search/index_storage.py:160-177): the exhaustive e4m3 scan
 shortlists ``ndocs / 4`` candidates per query (the reference's exact-scoring depth, filter_pids.cpp:148), which are
@@ -43,8 +52,10 @@ search only where the exact top-k was not inside the shortlist.
 """
 from __future__ import annotations
 
+import copy
 import json
 import os
+from concurrent.futures import ThreadPoolExecutor
 from typing import Callable, Dict, List, Optional, Tuple, Union
 
 import numpy as np
@@ -225,21 +236,36 @@ class Searcher:
                  encode_fn: Optional[Callable] = None, index_root: Optional[str] = None,
                  query_batch: int = 64, shard_across_ranks: bool = False, group=None,
                  storage: Optional[str] = None, residency: Optional[str] = None, window_bytes: Optional[int] = None,
-                 compressed: Optional[bool] = None):
+                 compressed: Optional[bool] = None, devices=None):
         # `disable_gpu` is part of the reference signature (default True) but dead there: colbert/searcher.py:23
         # never reads it, the device is chosen by config.total_visible_gpus (:40-43), which FLMR_executor.py:778-781
         # zeroes under DDP to force CPU search.  Here the search always runs on the GPU (no CPU path exists);
         # FlatCorpus raises when CUDA is absent.
         del disable_gpu
+        if devices is not None:
+            if isinstance(index, FlatCorpus):
+                raise ValueError("devices= loads the shards of an index path on their devices; a FlatCorpus given "
+                                 "lives on one device")
+            if shard_across_ranks:
+                raise ValueError("devices= shards the index across the devices of this process; it excludes "
+                                 "shard_across_ranks=True, which shards it across ranks")
+            if device is not None:
+                raise ValueError("devices= places every shard; it excludes device=")
+            if residency not in (None, "device") or compressed:
+                raise ValueError("devices= keeps every shard resident in HBM; residency=%r, compressed=%r are not "
+                                 "supported with it" % (residency, compressed))
         self.checkpoint = checkpoint
         self.collection = collection
         self.encode_fn = encode_fn
         self.query_batch = int(query_batch)
         self._sharded = None
+        self._sharded_index_size = None
+        self._devices = None        # a multi-device Searcher's DeviceShardedSearcher
         self._nccl = None
         self._checkpoint_model = None
         self.index_config = None
         run_cfg = active_run_config(config)
+        shards = None
         if isinstance(index, FlatCorpus):
             if storage is not None and storage != index.storage:
                 raise ValueError("storage=%r, but the corpus given is stored as %r" % (storage, index.storage))
@@ -279,7 +305,21 @@ class Searcher:
                     raise ValueError("compressed=True streams a PLAID index's compressed form; %s is a flat index"
                                      % self.index)
                 extra["compressed"] = True
-            self.corpus = load(self.index, device=device, rank=rank, world_size=world, **extra)
+            if devices is not None:
+                from .sharded import resolve_devices
+                devs = resolve_devices(devices)
+                _cabi.lib()                              # loaded (built if stale) once, before the loader threads
+
+                def load_shard(i):
+                    return load(self.index, device=devs[i], rank=i, world_size=len(devs), **extra)
+                with ThreadPoolExecutor(len(devs)) as pool:
+                    # a shard is None when there are more devices than passages
+                    shards = [c for c in pool.map(load_shard, range(len(devs))) if c is not None]
+                self.corpus = shards[0]
+            else:
+                self.corpus = load(self.index, device=device, rank=rank, world_size=world, **extra)
+        # the shards this process holds
+        self.shards = shards if shards is not None else ([self.corpus] if self.corpus is not None else [])
         self.storage = getattr(self.corpus, "storage", None) or storage or "bf16"
         # every rank of a sharded Searcher gets the same residency argument, so ranks without a shard batch their
         # collectives as the others do
@@ -320,6 +360,10 @@ class Searcher:
             t = torch.tensor([n], dtype=torch.int64, device=self.device if self._want_nccl else "cpu")
             dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self._group)
             self._sharded_index_size = int(t.item())
+        if shards is not None:
+            from .sharded import DeviceShardedSearcher
+            self._devices = DeviceShardedSearcher([c.device.index for c in self.shards], self._shard_search)
+            self._sharded_index_size = self.shards[-1].pid_base + self.shards[-1].n_passages
         self._relu = False
 
     # -- reference-compatible surface ------------------------------------------------------------
@@ -484,7 +528,7 @@ class Searcher:
 
     def _index_size(self) -> int:
         """Passages of the whole index (every shard, deleted ones included): ids a search may name are below it."""
-        if self._sharded is not None:
+        if self._sharded_index_size is not None:
             return self._sharded_index_size
         return self.corpus.pid_base + self.corpus.n_passages
 
@@ -682,6 +726,12 @@ class Searcher:
             Q = Q.unsqueeze(0)
         if remove_zero_tensors:
             Q = self._drop_zero_rows(Q)
+        if self._devices is not None:
+            # every shard's own search, then one merge on the home device; rows end in (-inf, -1) past their hits
+            self._last_depth = None
+            s, p = self._devices.search(Q, int(k), filter_fn=filter_fn, pid_lists=pid_lists)
+            n_valid = int((p >= 0).sum(dim=1).max()) if p.numel() else 0
+            return s[:, :n_valid], p[:, :n_valid]
         if pid_lists is not None:
             return self._restricted_tensors(Q, int(k), filter_fn, pid_lists)
         corpus = self.corpus
@@ -714,6 +764,40 @@ class Searcher:
             s, p = s[:, :n_valid], p[:, :n_valid]
         return s, p
 
+    def _shard_search(self, i: int, Q: torch.Tensor, k: int, filter_fn=None, pid_lists: Optional[List] = None
+                      ) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``_search_tensors`` of shard i of a multi-device Searcher: this Searcher's own code on a view of it that
+        holds that shard alone (ids are still checked against the whole index)."""
+        view = copy.copy(self)
+        view.corpus, view.device, view._devices = self.shards[i], self.shards[i].device, None
+        out = view._search_tensors(Q, k, filter_fn, False, pid_lists)
+        if view._last_depth is not None:
+            self._last_depth = max(self._last_depth or 0, view._last_depth)
+        return out
+
+    def _gather_padded(self, p: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``FlatCorpus.gather_padded`` of global ids ``p`` from the shards that own them, on the home device: each
+        shard gathers its own hits on its device (``flmr_corpus_gather``) and they are copied over."""
+        if len(self.shards) == 1:
+            return self.corpus.gather_padded(p)
+        ids = p.cpu().numpy()
+        nd_max = 1
+        for c in self.shards:
+            local = ids[(ids >= c.pid_base) & (ids < c.pid_base + c.n_passages)] - c.pid_base
+            if local.size:
+                nd_max = max(nd_max, int(c.doclens[local].max()))
+        D = mask = None
+        for c in self.shards:
+            own = (p >= c.pid_base) & (p < c.pid_base + c.n_passages)
+            Dc, mc = c.gather_padded(torch.where(own, p, -1), nd_max)
+            Dc, mc = Dc.to(self.device), mc.to(self.device)
+            if D is None:
+                D, mask = Dc, mc
+            else:
+                D = torch.where(own[..., None, None], Dc, D)
+                mask = torch.where(own[..., None, None], mc, mask)
+        return D, mask
+
     def retrieve_and_rescore(self, Q: torch.Tensor, n_docs: int, generator: Optional[torch.Generator] = None):
         """The retrieval block of ``RagModelForBlip.main_retrieve`` (src/models/rag/rag_model_blip.py:388-443)
         in one call: search ``max(5, n_docs)`` passages per query (:392-397), keep ``n_docs`` of them (a random
@@ -732,8 +816,9 @@ class Searcher:
         if self._sharded is not None:
             raise RuntimeError("retrieve_and_rescore gathers embeddings from the local shard only; "
                                "use an unsharded Searcher for the RAG block")
-        if _n_live(self.corpus) < n_docs:
-            raise ValueError("the corpus holds %d live passages, fewer than n_docs=%d" % (_n_live(self.corpus), n_docs))
+        n_live = sum(_n_live(c) for c in self.shards)
+        if n_live < n_docs:
+            raise ValueError("the corpus holds %d live passages, fewer than n_docs=%d" % (n_live, n_docs))
         n_retrieve = max(5, int(n_docs))
         Qd = Q.to(self.corpus.device)
         s, p = self._search_tensors(Qd.detach(), n_retrieve)
@@ -742,7 +827,7 @@ class Searcher:
         if s.size(1) != n_docs:
             pick = torch.rand(s.shape, generator=generator, device="cpu").argsort(dim=1)[:, :n_docs].to(s.device)
             s, p = s.gather(1, pick), p.gather(1, pick)
-        D, mask = self.corpus.gather_padded(p)                               # [B, n_docs, Nd, d]
+        D, mask = self._gather_padded(p)                                     # [B, n_docs, Nd, d]
         # one block-diagonal launch: question b against ITS n_docs passages only
         doc_scores = grouped_maxsim(Qd, D.flatten(0, 1), mask.flatten(0, 1), n_docs)
         return {"doc_scores": doc_scores, "retrieved_doc_ids": p.cpu().numpy(), "search_scores": s,
@@ -800,9 +885,9 @@ class Searcher:
                 "config": self.config.export() if hasattr(self.config, "export") else None,
                 "backend": "ravqa_b200 exhaustive fused scan", "index": self.index,
                 "index_kind": self.index_kind, "exhaustive": True,
-                "n_passages": self.corpus.n_passages if self.corpus is not None else 0,
-                "n_live": _n_live(self.corpus) if self.corpus is not None else 0,
-                "n_deleted": getattr(self.corpus, "n_deleted", 0) if self.corpus is not None else 0,
+                "n_passages": sum(c.n_passages for c in self.shards),
+                "n_live": sum(_n_live(c) for c in self.shards),
+                "n_deleted": sum(getattr(c, "n_deleted", 0) for c in self.shards),
                 "storage": self.storage, "restricted": qid_to_pids is not None}
         if self.storage == "fp8":
             prov["shortlist_depth"] = self._last_depth

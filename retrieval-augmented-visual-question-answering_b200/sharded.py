@@ -155,3 +155,100 @@ class ShardedSearcher:
             dist.all_gather(list(gathered.unbind(0)), payload, group=self.group)
         gs = gathered[:, 0].to(torch.int32).view(torch.float32)
         return self.merge(gs, gathered[:, 1], k)
+
+
+def resolve_devices(devices) -> List[int]:
+    """The device ordinals of ``Searcher(devices=...)``: ``"all"`` (every visible device) or a non-empty sequence of
+    ordinals or CUDA devices, in shard order; a device may repeat (several shards on one GPU)."""
+    if isinstance(devices, str):
+        if devices != "all":
+            raise ValueError("devices must be 'all' or a sequence of CUDA devices, got %r" % (devices,))
+        n = torch.cuda.device_count()
+        if n == 0:
+            raise RuntimeError("devices='all' found no CUDA device")
+        return list(range(n))
+    out = []
+    for d in devices:
+        d = torch.device("cuda", d) if isinstance(d, int) else torch.device(d)
+        if d.type != "cuda" or d.index is None:
+            raise ValueError("devices takes CUDA device ordinals, got %r" % (d,))
+        out.append(d.index)
+    if not out:
+        raise ValueError("devices needs at least one device")
+    return out
+
+
+def merge_device_lists(lists: List[Tuple[torch.Tensor, torch.Tensor]], streams: List[torch.cuda.Stream], k: int,
+                       home: torch.device) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The exchange of shards held on several devices of this process, on the current stream of ``home``: list i,
+    (scores fp32, pids int64) ``[B, k]`` on its own device, was written on ``streams[i]``.  k <= MAX_K: one
+    ``flmr_topk_merge_devices`` call (its kernel reads the lists in place or over peer access, after waiting for each
+    stream's event).  Larger k: the lists, copied to ``home``, are concatenated in shard order and selected by score;
+    the shards hold ascending id ranges and each list is sorted with ties on the lower id, so the lower column is the
+    lower id on every exact tie, as in the merge kernel."""
+    import ctypes as C
+    from . import _cabi
+    from .maxsim import topk_select
+    caller = torch.cuda.current_stream(home)
+    B = lists[0][0].size(0)
+    for s, p in lists:
+        s.record_stream(caller)                    # read on the home stream after the shard's own stream is done
+        p.record_stream(caller)
+    if k <= _cabi.MAX_K:
+        n = len(lists)
+        out_s = torch.empty((B, k), dtype=torch.float32, device=home)
+        out_p = torch.empty((B, k), dtype=torch.int64, device=home)
+        sp = (C.c_void_p * n)(*[s.data_ptr() for s, _ in lists])
+        pp = (C.c_void_p * n)(*[p.data_ptr() for _, p in lists])
+        dev = (C.c_int * n)(*[s.device.index for s, _ in lists])
+        sts = (C.c_void_p * n)(*[st.cuda_stream for st in streams])
+        with torch.cuda.device(home):
+            _cabi.check(_cabi.lib().flmr_topk_merge_devices(sp, pp, dev, sts, n, B, k, k, C.c_void_p(out_s.data_ptr()),
+                                                           C.c_void_p(out_p.data_ptr()),
+                                                           C.c_void_p(caller.cuda_stream)))
+        return out_s, out_p
+    for st in streams:
+        caller.wait_stream(st)
+    s = torch.cat([s.to(home) for s, _ in lists], dim=1)
+    p = torch.cat([p.to(home) for _, p in lists], dim=1)
+    if k <= _cabi.SELECT_MAX_K:
+        vals, col = topk_select(s, k)
+    else:
+        vals, col = torch.sort(s, dim=1, descending=True, stable=True)
+        vals, col = vals[:, :k], col[:, :k]
+    return vals, p.gather(1, col).masked_fill(vals == float("-inf"), -1)
+
+
+class DeviceShardedSearcher:
+    """The single-process counterpart of ``ShardedSearcher``, with the same two parts: shard i of one index lives on
+    ``devices[i]`` of this process, ``local_topk(i, Q, k, **kw) -> (scores [B, k_i], global pids [B, k_i])`` searches
+    it (on the current stream of its device), and ``merge(lists, streams, k, home)`` merges the per-shard lists on the
+    home device ``devices[0]`` (``merge_device_lists``).  There is no collective and no host synchronisation between
+    the shards: each shard runs on a stream of its own, ordered after the caller's stream on the home device."""
+
+    def __init__(self, devices: Sequence[int], local_topk: Callable, merge: Callable = merge_device_lists):
+        self.devices = [torch.device("cuda", int(d)) for d in devices]
+        self.home = self.devices[0]
+        self.local_topk = local_topk
+        self.merge = merge
+        self.streams = [torch.cuda.Stream(device=d) for d in self.devices]
+
+    def search(self, Q: torch.Tensor, k: int, **kw) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(scores [B, k], global pids [B, k]) of the merged ranking, on the home device's current stream; entries past
+        the candidates are (-inf, -1).  Each shard's stream receives a copy of ``Q`` and the shard's top-k, padded to
+        ``k``; for k beyond the merge kernel the padded lists are copied to the home device on that stream."""
+        from . import _cabi
+        caller = torch.cuda.current_stream(self.home)
+        lists = []
+        for i, (dev, st) in enumerate(zip(self.devices, self.streams)):
+            st.wait_stream(caller)
+            with torch.cuda.device(dev), torch.cuda.stream(st):
+                s, p = self.local_topk(i, Q.to(dev, non_blocking=True), k, **kw)
+                if s.size(1) < k:                        # short shard: pad with empty entries
+                    s = torch.cat([s, s.new_full((s.size(0), k - s.size(1)), float("-inf"))], dim=1)
+                    p = torch.cat([p, p.new_full((p.size(0), k - p.size(1)), -1)], dim=1)
+                s, p = s.contiguous(), p.contiguous()
+                if k > _cabi.MAX_K:
+                    s, p = s.to(self.home), p.to(self.home)
+            lists.append((s, p))
+        return self.merge(lists, self.streams, k, self.home)

@@ -32,6 +32,9 @@ class IndexUpdater:
         if searcher._sharded is not None:
             raise NotImplementedError("updating a corpus sharded across ranks is not supported; update an unsharded "
                                       "Searcher and persist it, then load the index sharded")
+        if searcher._devices is not None:
+            raise NotImplementedError("updating a corpus sharded across devices (Searcher(devices=...)) is not "
+                                      "supported; update a one-device Searcher and persist it, then load it sharded")
         if searcher.corpus is None:
             raise ValueError("the searcher holds no corpus")
         self.searcher = searcher
