@@ -40,7 +40,10 @@ shard per device (``sharded.shard_ranges``; shard i loaded on ``devices[i]``, al
 for a corpus larger than one card searched without a launcher or a process group.  Every search runs each shard's own
 top-k, as a one-device Searcher would on that shard, on a stream of the shard's device, and merges the lists on the
 home device ``devices[0]`` with one kernel that reads them over peer access (``flmr_topk_merge_devices``); results are
-those of the one-device Searcher and come back on the home device.  A device may hold several shards (``[0, 0]``).  It
+those of the one-device Searcher and come back on the home device.  An fp8 search keeps the one-device shortlist: each
+shard hands its e4m3 top-depth to the home device, which selects the global top-depth (the depth and allowed counts
+taken over the whole index) and re-ranks those candidates with the one-device code, gathering their bf16 rows from the
+shards that own them.  A device may hold several shards (``[0, 0]``).  It
 loads an index path only, resident (``residency="host"`` and ``compressed=True`` are refused), and excludes ``device=``
 and ``shard_across_ranks``.  ``corpus`` is the first shard, ``shards`` lists them all.
 
@@ -48,7 +51,8 @@ and ``shard_across_ranks``.  ``corpus`` is the first shard, ``shards`` lists the
 and searches in two stages, as PLAID does (colbert/search/index_storage.py:160-177): the exhaustive e4m3 scan
 shortlists ``ndocs / 4`` candidates per query (the reference's exact-scoring depth, filter_pids.cpp:148), which are
 gathered from the bf16 master and re-scored exactly.  Returned scores are exact; an id can differ from the bf16
-search only where the exact top-k was not inside the shortlist.
+search only where the exact top-k was not inside the shortlist.  With ``shard_across_ranks`` every rank shortlists and
+re-ranks its own shard, so its fp8 results need not be those of one device.
 """
 from __future__ import annotations
 
@@ -109,6 +113,23 @@ def _live_pids(corpus) -> torch.Tensor:
     if hasattr(corpus, "live_pids"):
         return corpus.live_pids()
     return torch.arange(corpus.n_passages, device=corpus.device) + corpus.pid_base
+
+
+def _allowed_live_counts(shards, lists: List) -> np.ndarray:
+    """Per query, the live passages of ``shards`` its list of global ids admits, each id counted once (None: every live
+    passage): what a restricted fp8 search's shortlist depth follows."""
+    out = np.zeros(len(lists), dtype=np.int64)
+    for c in shards:
+        dead = c.deleted_pids() if hasattr(c, "deleted_pids") else np.empty(0, dtype=np.int64)
+        lo, hi = c.pid_base, c.pid_base + c.n_passages
+        for b, ids in enumerate(lists):
+            if ids is None:
+                out[b] += _n_live(c)
+                continue
+            u = np.unique(torch.as_tensor(ids).reshape(-1).cpu().numpy())
+            u = u[(u >= lo) & (u < hi)]
+            out[b] += u.size - int(np.isin(u, dead).sum())
+    return out
 
 
 def _popcount_rows(words: torch.Tensor) -> torch.Tensor:
@@ -494,31 +515,55 @@ class Searcher:
         outs, outp = [], []
         for b0 in range(0, Q.size(0), self.query_batch):
             Qb = Q[b0:b0 + self.query_batch].to(corpus.device).to(torch.bfloat16)
-            s = maxsim_scores(corpus, Qb, relu=self._relu)
+            vals, pids = self._rerank(Qb, self._shortlist(Qb, depth, keep=keep)[1], kq)
+            outs.append(vals)
+            outp.append(pids)
+        return torch.cat(outs), torch.cat(outp)
+
+    def _shortlist(self, Q: torch.Tensor, depth: int, keep: Optional[torch.Tensor] = None,
+                   allow: Optional[torch.Tensor] = None, lists: Optional[List] = None
+                   ) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The e4m3 stage of an fp8 search on this shard: (scores, global pids) ``[B, min(depth, columns)]``, the top
+        ``depth`` e4m3 scores of the bf16 queries ``Q`` (ties: the lower pid) among the passages ``keep`` (local ids, in
+        ascending order), ``allow`` (bitmaps) or ``lists`` (global id lists, on the listed scan) admit.  An entry with a
+        -inf score (a deleted or disallowed passage, or padding) has pid -1."""
+        corpus = self.corpus
+        if lists is not None:
+            s, ids = self._listed_scores(Q, lists)          # ids ascend along a row
+        else:
+            s = maxsim_scores(corpus, Q, relu=self._relu, allow=allow)
             if keep is not None:
                 s = s[:, keep]
-            _, idx = topk_select(s, depth)
-            cand = keep[idx] if keep is not None else idx
-            # candidates in pid order, so that the select below breaks exact ties towards the lower pid
-            cand = torch.sort(cand, dim=1).values + corpus.pid_base
-            exact = self._exact_scores(Qb, cand)
-            vals, col = topk_select(exact, kq)
-            outs.append(vals)
-            outp.append(cand.gather(1, col))
-        return torch.cat(outs), torch.cat(outp)
+        d = min(depth, s.size(1))
+        if d == 0:
+            return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=corpus.device),
+                    torch.empty((Q.size(0), 0), dtype=torch.int64, device=corpus.device))
+        vals, col = topk_select(s, d)
+        if lists is not None:
+            pids = ids.gather(1, col.clamp_min(0))
+        else:
+            pids = (keep[col] if keep is not None else col) + corpus.pid_base
+        return vals, pids.masked_fill(vals == float("-inf"), -1)
+
+    def _rerank(self, Q: torch.Tensor, cand: torch.Tensor, kq: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The exact stage of an fp8 search: the top ``kq`` (scores, global pids) of the candidates ``cand`` (global
+        pids, -1: none) by their MaxSim over the bf16 rows, ties on the lower pid; short rows end in (-inf, -1)."""
+        cand = torch.sort(cand, dim=1).values        # pid order: the select below breaks exact ties by lower pid
+        exact = self._exact_scores(Q, cand).masked_fill(cand < 0, float("-inf"))
+        vals, col = topk_select(exact, kq)
+        return vals, cand.gather(1, col).masked_fill(vals == float("-inf"), -1)
 
     def _exact_scores(self, Q: torch.Tensor, cand: torch.Tensor) -> torch.Tensor:
         """Exact MaxSim ``[B, depth]`` of query b against its candidates ``cand[b]`` (global pids), from the bf16
-        rows of the corpus; the gather is split by queries to hold at most RERANK_GATHER_BYTES of tokens."""
-        corpus = self.corpus
+        rows of the shards that own them; the gather is split by queries to hold at most RERANK_GATHER_BYTES of
+        tokens."""
         depth = cand.size(1)
-        c = cand[cand >= 0]                              # (-1: an empty entry, gathered as an all-masked row)
-        nd_max = int(corpus.doclens[(c - corpus.pid_base).cpu().numpy()].max()) if c.numel() else 1
+        nd_max = self._longest(cand)
         per_query = depth * nd_max * _cabi.DIM * 2
         step = max(1, RERANK_GATHER_BYTES // per_query)
         out = []
         for q0 in range(0, Q.size(0), step):
-            D, mask = corpus.gather_padded(cand[q0:q0 + step], nd_max)          # [b, depth, nd_max, d]
+            D, mask = self._gather_padded(cand[q0:q0 + step], nd_max)          # [b, depth, nd_max, d]
             _, rowmax = maxsim_argmax_grouped(Q[q0:q0 + step], D.flatten(0, 1), mask.flatten(0, 1), depth,
                                               return_rowmax=True)
             if self._relu:
@@ -537,24 +582,11 @@ class Searcher:
         """``_search_tensors`` with query b restricted to the SET of global ids ``pid_lists[b]`` (None: the whole
         index).  The whole batch is checked before anything is searched.  Each query's allowed ids become a bitmap
         the scan's reducer tests, so there is no score matrix on the fused path.  Rows are padded with (-inf, -1)."""
-        n_index = self._index_size()
-        lists = []
-        for ids in pid_lists:
-            if ids is not None:
-                ids = torch.as_tensor(ids, dtype=torch.int64).reshape(-1).cpu()
-                if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= n_index):
-                    raise ValueError("passage id %d outside the index [0, %d)"
-                                     % (int(ids.min()) if int(ids.min()) < 0 else int(ids.max()), n_index))
-            lists.append(ids)
+        lists = self._pid_lists(pid_lists, filter_fn)
         if self._sharded is not None and k > _cabi.MAX_K:
             raise ValueError("sharded search merges at most k=%d results per query" % _cabi.MAX_K)
         corpus = self.corpus
         B = Q.size(0)
-        if filter_fn is not None:
-            # applied to each query's own list, as the reference applies it to the pids it was given
-            everything = _live_pids(corpus) if corpus is not None else torch.empty(0, dtype=torch.int64)
-            lists = [torch.as_tensor(filter_fn(ids.to(everything.device) if ids is not None else everything)).long()
-                     for ids in lists]
         # the C-level sharded search (scan + exchange in one call) takes bf16 shards; the others exchange below
         c_level = self._nccl is not None and corpus is not None and self.storage != "fp8"
         parts = []
@@ -596,6 +628,26 @@ class Searcher:
             s, p = torch.cat([m[0] for m in merged]), torch.cat([m[1] for m in merged])
         n_valid = int((p >= 0).sum(dim=1).max()) if p.numel() else 0
         return s[:, :n_valid], p[:, :n_valid]
+
+    def _pid_lists(self, pid_lists: List, filter_fn) -> List:
+        """The id lists of a restricted search, checked against the whole index before anything is searched, with
+        ``filter_fn`` applied to each query's own list (to every live passage of this Searcher's shards for a query
+        without one), as the reference applies it to the pids it was given."""
+        n_index = self._index_size()
+        lists = []
+        for ids in pid_lists:
+            if ids is not None:
+                ids = torch.as_tensor(ids, dtype=torch.int64).reshape(-1).cpu()
+                if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= n_index):
+                    raise ValueError("passage id %d outside the index [0, %d)"
+                                     % (int(ids.min()) if int(ids.min()) < 0 else int(ids.max()), n_index))
+            lists.append(ids)
+        if filter_fn is not None:
+            everything = (torch.cat([_live_pids(c).to(self.device) for c in self.shards]) if self.shards
+                          else torch.empty(0, dtype=torch.int64))
+            lists = [torch.as_tensor(filter_fn(ids.to(everything.device) if ids is not None else everything)).long()
+                     for ids in lists]
+        return lists
 
     def _listed_is_cheaper(self, Q: torch.Tensor, lists: List) -> bool:
         """Whether a batch's restricted search takes the listed scan: every query has a list, and the rows of the
@@ -643,10 +695,7 @@ class Searcher:
         kq = min(k, _n_live(corpus))
         n_allowed = None
         if self.storage == "fp8" and kq > 0:
-            dead = set(corpus.deleted_pids().tolist()) if hasattr(corpus, "deleted_pids") else set()
-            lo, hi = corpus.pid_base, corpus.pid_base + corpus.n_passages
-            n_allowed = max([len([i for i in set(ids.cpu().tolist()) if lo <= i < hi and i not in dead])
-                             for ids in lists], default=0)
+            n_allowed = int(_allowed_live_counts([corpus], lists).max(initial=0))
             kq = min(kq, n_allowed)
         if kq == 0:
             return (torch.empty((Q.size(0), 0), dtype=torch.float32, device=corpus.device),
@@ -657,14 +706,8 @@ class Searcher:
             depth = shortlist_depth(kq, getattr(self.config, "ndocs", None), n_allowed)
             self._last_depth = depth
             Qb = Q.to(corpus.device).to(torch.bfloat16)
-            s, ids = self._listed_scores(Qb, lists)
-            vals, col = topk_select(s, depth)
             # a -inf e4m3 score is a deleted passage or padding: it never reaches the exact re-rank
-            cand = torch.where(vals == float("-inf"), -1, ids.gather(1, col.clamp_min(0)))
-            cand = torch.sort(cand, dim=1).values        # pid order: the select below breaks exact ties by lower pid
-            exact = self._exact_scores(Qb, cand).masked_fill(cand < 0, float("-inf"))
-            vals, col = topk_select(exact, kq)
-            pids = cand.gather(1, col)
+            return self._rerank(Qb, self._shortlist(Qb, depth, lists=lists)[1], kq)
         else:
             s, ids = self._listed_scores(Q, lists)
             if s.size(1) < kq:                           # fewer listed passages than kq in every row
@@ -698,13 +741,8 @@ class Searcher:
             depth = shortlist_depth(kq, getattr(self.config, "ndocs", None), n_allowed)
             self._last_depth = depth
             Qb = Q.to(corpus.device).to(torch.bfloat16)
-            vals, idx = topk_select(maxsim_scores(corpus, Qb, relu=self._relu, allow=allow), depth)
             # a -inf e4m3 score is a disallowed or deleted passage: it never reaches the exact re-rank
-            cand = torch.where(vals == float("-inf"), -1, idx + corpus.pid_base)
-            cand = torch.sort(cand, dim=1).values        # pid order: the select below breaks exact ties by lower pid
-            exact = self._exact_scores(Qb, cand).masked_fill(cand < 0, float("-inf"))
-            vals, col = topk_select(exact, kq)
-            pids = cand.gather(1, col)
+            return self._rerank(Qb, self._shortlist(Qb, depth, allow=allow)[1], kq)
         elif kq <= _cabi.MAX_K:
             return maxsim_topk(corpus, Q, kq, relu=self._relu, allow=allow)
         else:
@@ -727,9 +765,12 @@ class Searcher:
         if remove_zero_tensors:
             Q = self._drop_zero_rows(Q)
         if self._devices is not None:
-            # every shard's own search, then one merge on the home device; rows end in (-inf, -1) past their hits
-            self._last_depth = None
-            s, p = self._devices.search(Q, int(k), filter_fn=filter_fn, pid_lists=pid_lists)
+            # every shard's own search, then one merge on the home device (fp8: every shard's shortlist, then one
+            # re-rank on the home device); rows end in (-inf, -1) past their hits
+            if self.storage == "fp8":
+                s, p = self._devices_fp8_tensors(Q, int(k), filter_fn, pid_lists)
+            else:
+                s, p = self._devices.search(Q, int(k), filter_fn=filter_fn, pid_lists=pid_lists)
             n_valid = int((p >= 0).sum(dim=1).max()) if p.numel() else 0
             return s[:, :n_valid], p[:, :n_valid]
         if pid_lists is not None:
@@ -768,24 +809,93 @@ class Searcher:
                       ) -> Tuple[torch.Tensor, torch.Tensor]:
         """``_search_tensors`` of shard i of a multi-device Searcher: this Searcher's own code on a view of it that
         holds that shard alone (ids are still checked against the whole index)."""
+        return self._shard_view(i)._search_tensors(Q, k, filter_fn, False, pid_lists)
+
+    def _shard_view(self, i: int) -> "Searcher":
         view = copy.copy(self)
         view.corpus, view.device, view._devices = self.shards[i], self.shards[i].device, None
-        out = view._search_tensors(Q, k, filter_fn, False, pid_lists)
-        if view._last_depth is not None:
-            self._last_depth = max(self._last_depth or 0, view._last_depth)
-        return out
+        view.shards = [self.shards[i]]
+        return view
 
-    def _gather_padded(self, p: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``FlatCorpus.gather_padded`` of global ids ``p`` from the shards that own them, on the home device: each
-        shard gathers its own hits on its device (``flmr_corpus_gather``) and they are copied over."""
-        if len(self.shards) == 1:
-            return self.corpus.gather_padded(p)
+    def _shard_shortlist(self, i: int, Q: torch.Tensor, depth: int, keep: Optional[torch.Tensor] = None,
+                         lists: Optional[List] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``_shortlist`` of shard i of a multi-device Searcher, on its device: ``keep`` (global ids, ascending) cut to
+        the shard, or the id ``lists`` on the listed scan or as bitmaps, as the one-device search would scan them."""
+        view = self._shard_view(i)
+        c = view.corpus
+        if lists is not None:
+            if view._listed_is_cheaper(Q, lists):
+                return view._shortlist(Q, depth, lists=lists)
+            return view._shortlist(Q, depth, allow=c.allow_bitmaps(lists))
+        if keep is not None:
+            keep = keep.to(c.device)
+            keep = keep[(keep >= c.pid_base) & (keep < c.pid_base + c.n_passages)] - c.pid_base
+        return view._shortlist(Q, depth, keep=keep)
+
+    def _devices_fp8_tensors(self, Q: torch.Tensor, k: int, filter_fn, pid_lists: Optional[List]
+                             ) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The fp8 search of a multi-device Searcher, ranked as the one-device Searcher ranks it: the shortlist depth
+        (and the allowed count it follows) over the whole index, every shard's e4m3 top-depth, the global top-depth
+        selected from them on the home device, and the one-device re-rank of those candidates, with the same query
+        batches, gathered from the shards that own them.  Rows end in (-inf, -1) past their hits."""
+        B = Q.size(0)
+        n_live = sum(_n_live(c) for c in self.shards)
+        ndocs = getattr(self.config, "ndocs", None)
+        lists = keep = None
+        if pid_lists is not None:
+            lists = self._pid_lists(pid_lists, filter_fn)
+        else:
+            if filter_fn is not None:
+                everything = torch.cat([_live_pids(c).to(self.device) for c in self.shards])
+                keep = torch.as_tensor(filter_fn(everything), device=self.device).long()
+            n_cand = n_live if keep is None else int(keep.numel())
+            kq = min(k, n_cand)
+            if kq > 0:
+                depth = shortlist_depth(k, ndocs, n_cand)
+        parts = []
+        for b0 in range(0, B, self.query_batch):
+            Qb = Q[b0:b0 + self.query_batch].to(self.device).to(torch.bfloat16)
+            lb = None
+            if lists is not None:
+                lb = lists[b0:b0 + self.query_batch]
+                n_allowed = int(_allowed_live_counts(self.shards, lb).max(initial=0))
+                kq = min(k, n_live, n_allowed)
+                if kq > 0:
+                    depth = shortlist_depth(kq, ndocs, n_allowed)
+            if kq == 0:
+                parts.append((Qb.new_empty((Qb.size(0), 0), dtype=torch.float32),
+                              Qb.new_empty((Qb.size(0), 0), dtype=torch.int64)))
+                continue
+            self._last_depth = depth
+            _, cand = self._devices.shortlist(self._shard_shortlist, Qb, depth, keep=keep, lists=lb)
+            parts.append(self._rerank(Qb, cand, kq))
+        width = max([ps.size(1) for ps, _ in parts], default=0)
+        s = torch.full((B, width), float("-inf"), dtype=torch.float32, device=self.device)
+        p = torch.full((B, width), -1, dtype=torch.int64, device=self.device)
+        b0 = 0
+        for ps, pp in parts:
+            s[b0:b0 + ps.size(0), :ps.size(1)] = ps
+            p[b0:b0 + pp.size(0), :pp.size(1)] = pp
+            b0 += ps.size(0)
+        return s, p
+
+    def _longest(self, p: torch.Tensor) -> int:
+        """The most tokens of a passage among global ids ``p`` (-1: none; 1 if there is none)."""
         ids = p.cpu().numpy()
         nd_max = 1
         for c in self.shards:
             local = ids[(ids >= c.pid_base) & (ids < c.pid_base + c.n_passages)] - c.pid_base
             if local.size:
                 nd_max = max(nd_max, int(c.doclens[local].max()))
+        return nd_max
+
+    def _gather_padded(self, p: torch.Tensor, nd_max: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``FlatCorpus.gather_padded`` of global ids ``p`` from the shards that own them, on the home device: each
+        shard gathers its own hits on its device (``flmr_corpus_gather``) and they are copied over."""
+        if len(self.shards) == 1:
+            return self.corpus.gather_padded(p, nd_max)
+        if nd_max is None:
+            nd_max = self._longest(p)
         D = mask = None
         for c in self.shards:
             own = (p >= c.pid_base) & (p < c.pid_base + c.n_passages)

@@ -179,13 +179,13 @@ def resolve_devices(devices) -> List[int]:
 
 
 def merge_device_lists(lists: List[Tuple[torch.Tensor, torch.Tensor]], streams: List[torch.cuda.Stream], k: int,
-                       home: torch.device) -> Tuple[torch.Tensor, torch.Tensor]:
+                       home: torch.device, select: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
     """The exchange of shards held on several devices of this process, on the current stream of ``home``: list i,
     (scores fp32, pids int64) ``[B, k]`` on its own device, was written on ``streams[i]``.  k <= MAX_K: one
     ``flmr_topk_merge_devices`` call (its kernel reads the lists in place or over peer access, after waiting for each
-    stream's event).  Larger k: the lists, copied to ``home``, are concatenated in shard order and selected by score;
-    the shards hold ascending id ranges and each list is sorted with ties on the lower id, so the lower column is the
-    lower id on every exact tie, as in the merge kernel."""
+    stream's event).  Larger k, or ``select``: the lists, copied to ``home``, are concatenated in shard order and
+    selected by score; the shards hold ascending id ranges and each list is sorted with ties on the lower id, so the
+    lower column is the lower id on every exact tie, as in the merge kernel."""
     import ctypes as C
     from . import _cabi
     from .maxsim import topk_select
@@ -194,7 +194,7 @@ def merge_device_lists(lists: List[Tuple[torch.Tensor, torch.Tensor]], streams: 
     for s, p in lists:
         s.record_stream(caller)                    # read on the home stream after the shard's own stream is done
         p.record_stream(caller)
-    if k <= _cabi.MAX_K:
+    if k <= _cabi.MAX_K and not select:
         n = len(lists)
         out_s = torch.empty((B, k), dtype=torch.float32, device=home)
         out_p = torch.empty((B, k), dtype=torch.int64, device=home)
@@ -238,17 +238,26 @@ class DeviceShardedSearcher:
         the candidates are (-inf, -1).  Each shard's stream receives a copy of ``Q`` and the shard's top-k, padded to
         ``k``; for k beyond the merge kernel the padded lists are copied to the home device on that stream."""
         from . import _cabi
+        return self.merge(self._lists(self.local_topk, Q, k, k > _cabi.MAX_K, kw), self.streams, k, self.home)
+
+    def shortlist(self, local: Callable, Q: torch.Tensor, depth: int, **kw) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The global top-``depth`` (scores [B, depth], global pids [B, depth]) of the shards' own top-``depth`` lists
+        ``local(i, Q, depth, **kw)``, selected on the home device by score with ties on the lower id at every depth
+        (``merge_device_lists(select=True)``): the first stage of a two-stage search, as one device would select it."""
+        return merge_device_lists(self._lists(local, Q, depth, True, kw), self.streams, depth, self.home, select=True)
+
+    def _lists(self, local: Callable, Q: torch.Tensor, k: int, to_home: bool, kw: dict) -> List:
         caller = torch.cuda.current_stream(self.home)
         lists = []
         for i, (dev, st) in enumerate(zip(self.devices, self.streams)):
             st.wait_stream(caller)
             with torch.cuda.device(dev), torch.cuda.stream(st):
-                s, p = self.local_topk(i, Q.to(dev, non_blocking=True), k, **kw)
+                s, p = local(i, Q.to(dev, non_blocking=True), k, **kw)
                 if s.size(1) < k:                        # short shard: pad with empty entries
                     s = torch.cat([s, s.new_full((s.size(0), k - s.size(1)), float("-inf"))], dim=1)
                     p = torch.cat([p, p.new_full((p.size(0), k - p.size(1)), -1)], dim=1)
                 s, p = s.contiguous(), p.contiguous()
-                if k > _cabi.MAX_K:
+                if to_home:
                     s, p = s.to(self.home), p.to(self.home)
             lists.append((s, p))
-        return self.merge(lists, self.streams, k, self.home)
+        return lists

@@ -44,8 +44,8 @@ def L(R):
 
 
 def _ragged():
-    """240 passages (the fp8 shortlist covers each of them, so fp8 results are exact on one device and on shards alike):
-    short ones around a run of long ones that holds the token-balanced shard boundaries of 2 and 3 shards."""
+    """240 passages: short ones around a run of long ones that holds the token-balanced shard boundaries of 2 and 3
+    shards."""
     rng = np.random.default_rng(11)
     dl = rng.integers(1, 31, size=240).astype(np.int32)
     dl[90:150] = rng.integers(120, 181, size=60)
